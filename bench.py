@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark: image-pairs/sec of the Patch2Pix correlate-and-refine hot path at 640x480,
 ptmax=400, panc=8 (BASELINE.json configs[2]; training-loop forward sequence under eval,
-train_patch2pix.py:97-118), on N B200s of one node.
+train_patch2pix.py:97-118), on N H100s of one node.
 
     python bench.py --gpus 1 --steps 20 --warmup 3
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
@@ -57,7 +57,6 @@ def parse():
     ap.add_argument('--seg-len', type=int, default=None)
     ap.add_argument('--mid-band', type=int, default=None)
     ap.add_argument('--fuse-gather', type=int, default=None)
-    ap.add_argument('--gemm-pair', type=int, default=None, help='bitmask of GEMM launches on the CTA-pair kernel')
     ap.add_argument('--nc-impl', type=int, default=None, help='1: tensor-core NeighConsensus (default), 0: fp32 CUDA-core kernels')
     ap.add_argument('--backbone-fp32', action='store_true', help='keep cuDNN TF32 off in the e2e backbone')
     ap.add_argument('--no-cpu-baseline', action='store_true')
@@ -69,6 +68,9 @@ def parse():
     ap.add_argument('--depth', type=int, default=3, help='pairs in flight per GPU (coarse stages enqueued ahead of the host sync)')
     ap.add_argument('--legacy-workload', action='store_true', help="round-1 generator (13-17 mutual matches per pair)")
     ap.add_argument('--cpu-sample-patches', type=int, default=200)
+    ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                    help='after the timed steps, write the last timed step\'s outputs (fine matches, their probabilities, '
+                         'the coarse matches they refine) to DIR/<name>.npy, for comparing two builds output for output')
     return ap.parse_args()
 
 
@@ -80,16 +82,6 @@ def model_config(device, panc):
                      weights_dict=None, change_stride=True, regressor_config=rc)
 
 
-def load_traffic():
-    """DRAM bytes (read + write) per launch from the committed `ncu --set full` capture of the round
-    (profiles/r02_traffic.json: kernel kind -> bytes), or {}."""
-    p = os.path.join(ROOT, 'profiles', 'r02_traffic.json')
-    if os.path.exists(p):
-        with open(p) as f:
-            return json.load(f)
-    return {}
-
-
 def load_peaks():
     """Burst peak for a kernel whose timed region is short (clocks near max), sustained for seconds-long regions."""
     p = os.path.join(ROOT, 'MEASURED_PEAKS.json')
@@ -98,7 +90,8 @@ def load_peaks():
             d = json.load(f)
         return {'hbm_gbs': d['hbm_gbs'], 'tflops_burst': d['bf16_tflops'],
                 'tflops_sustained': d.get('bf16_tflops_sustained', d['bf16_tflops']), 'src': 'measured'}
-    return {'hbm_gbs': 6650.0, 'tflops_burst': 1590.0, 'tflops_sustained': 1400.0, 'src': 'fallback'}
+    # NVIDIA's H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense fp16 -- an upper bound, not a measurement
+    return {'hbm_gbs': 3350.0, 'tflops_burst': 989.0, 'tflops_sustained': 989.0, 'src': 'H100 SXM data sheet'}
 
 
 _SAMPLER_SRC = r"""
@@ -206,6 +199,15 @@ class ClockSampler:
 # cannot travel to the GPU box).  One step = the full coarse stage of one pair + the two refine
 # stages on a bounded subset of the 3200 patches, extrapolated to the full pair.
 # --------------------------------------------------------------------------------------------------
+def dump_outputs(d, outs):
+    """Writes each output as DIR/<name>.npy: float tensors as float32, integer ones as float64 (exact)."""
+    os.makedirs(d, exist_ok=True)
+    for name, t in outs.items():
+        a = t.detach().cpu()
+        a = a.double() if not a.is_floating_point() else a.float()
+        np.save(os.path.join(d, name + '.npy'), a.numpy())
+
+
 def cpu_threads():
     """Threads for the CPU arm: every host core up to 32 (torch's CPU kernels for this path -- hundreds of
     small conv3d / index ops -- get slower, not faster, beyond that; measured on the 128-core GPU box).
@@ -332,11 +334,11 @@ def run_ours(args):
     net = Patch2PixB200(cfg)
     for key, v in (('mid_passes', args.mid_passes), ('fine_passes', args.fine_passes), ('corr_passes', args.corr_passes),
                    ('seg_len', args.seg_len), ('mid_band', args.mid_band), ('fuse_gather', args.fuse_gather),
-                   ('gemm_pair', args.gemm_pair), ('nc_impl', args.nc_impl)):
+                   ('nc_impl', args.nc_impl)):
         if v is not None:
             net.set_option(key, v)
     opts = {k: net._handle.get_option(k) for k in ('mid_passes', 'fine_passes', 'corr_passes', 'seg_len', 'mid_band', 'fuse_gather',
-                                                    'gemm_pair', 'nc_impl')}
+                                                    'nc_impl')}
 
     # pair indices: rank 0 decides, NCCL broadcasts (the "scatter pair indices" step); global pair p -> rank p % world
     total_steps = K + Wm
@@ -370,11 +372,14 @@ def run_ours(args):
     step_events = [torch.cuda.Event(enable_timing=True) for _ in range(max(K, 1))]   # created before the timed region
 
     host_stamps = [0.0] * max(K, 1)
+    last_out = {}                                          # --dump-outputs: what the last recorded step returned
 
     def hot_finish(tk, out_slot=None, keep=None, stamp=False):
         i, ticket = tk
         np.random.seed(mine[i] % (2 ** 31))               # the reference's global numpy RNG, seeded per pair
         fine, fine_p, cm = net.finish_match(ticket, 0.0, args.ptmax)
+        if out_slot is not None and args.dump_outputs:
+            last_out.update(fine_matches=fine[0], fine_probs=fine_p[0], coarse_matches=cm[0])
         if out_slot is not None:
             results[out_slot, :, :4] = fine[0]
             results[out_slot, :, 4] = fine_p[0]
@@ -472,6 +477,8 @@ def run_ours(args):
             sharder.gather_results(results)              # NCCL gather of the matches (inside the timed region)
         ms_hot = timed(hot_region, K, sampler)
         launches = net._handle.launch_count() - l0
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, last_out)
         clocks = sampler.finish() if sampler else None
         nst = min(K, n_mine)
         step_raw = [step_events[j].elapsed_time(step_events[j + 1]) for j in range(nst - 1)]
@@ -581,13 +588,9 @@ def run_ours(args):
         if dom:
             ach = kern[dom]['algorithmic_tflops']
             gemm_ms = sum(kern[k]['ms_per_launch'] * kern[k]['launches'] for k in gemm_names)
-            kname = ('umma_conv1_tma_kernel' if opts['fuse_gather'] == 3 else 'umma_conv1_fused_kernel') if (dom.startswith('conv1') and not dom.endswith('band') and opts['fuse_gather'] in (1, 3)) \
-                else 'umma_gemm_kernel'
-            traffic = load_traffic().get(dom if kname == 'umma_gemm_kernel' else 'conv1_fused')
-            roofline = {'kernel': f'{kname} ({dom})', 'bound': 'tensor', 'achieved': ach, 'peak': peak,
-                        'unit': 'TFLOP/s', 'frac': ach / peak, 'traffic': traffic,
-                        'traffic_unit': 'bytes of DRAM read+write per launch (ncu --set full, profiles/)',
-                        'peak_source': f"{peaks['src']} cuBLAS bf16 {'sustained' if sustained else 'burst'} (fp16 runs at the same "
+            roofline = {'kernel': f'umma_gemm_kernel ({dom})', 'bound': 'tensor', 'achieved': ach, 'peak': peak,
+                        'unit': 'TFLOP/s', 'frac': ach / peak,
+                        'peak_source': f"{peaks['src']} bf16 {'sustained' if sustained else 'burst'} (fp16 runs at the same "
                                        f"tensor rate); timed region {ms_hot / 1e3:.2f} s -> {'sustained' if sustained else 'burst'} denominator",
                         'frac_vs_burst': ach / peaks['tflops_burst'], 'frac_vs_sustained': ach / peaks['tflops_sustained'],
                         'tensor_passes': kern[dom]['tensor_passes'],
@@ -639,7 +642,7 @@ def run_ours(args):
                                               'p90': step_ms[(len(step_ms) * 9) // 10], 'max': step_ms[-1],
                                               'slowest_step': worst_step} if step_ms else None),
                        'l2': f'{len(imgs)} distinct pairs cycled per rank; per-step working set (~3 GB of scratch written and '
-                             f're-read) >> 126 MB L2',
+                             f're-read) >> 50 MB L2',
                        'pipelining': f'{depth} pairs in flight per GPU (the coarse stages of the next pairs are enqueued before the host sync of the oldest)',
                        'options': opts},
             'e2e': e2e, 'gpu_launches': launches, 'roofline': roofline, 'kernels': kern, 'clocks': clocks,

@@ -1,4 +1,4 @@
-/* libp2p_b200.so -- C ABI of the B200-native Patch2Pix correlate-and-refine path.
+/* libp2p_b200.so -- C ABI of the H100-native (sm_90a) Patch2Pix correlate-and-refine path.
  *
  * The reference (GrumpyZhou/patch2pix) has no FFI / operator registry: its boundary for this path
  * is the Python method surface of `networks.patch2pix.Patch2Pix` (SURVEY.md s8b).  Each entry point
@@ -72,10 +72,10 @@ P2P_API int p2p_set_regressor_weights(p2p_handle_t h, int which, const p2p_regre
 
 /* Options: "mid_passes"/"fine_passes" (1 = fp16 operands, 3 = fp16 hi/lo split, fp32-grade),
  * "corr_passes" (0 = CUDA-core fp32 correlation, 1/3 = tensor-core), "seg_len" (k-steps per
- * TMEM accumulation segment, 0 = whole K), "gemm_impl" (0 = tcgen05, 1 = CUDA-core checker),
+ * tensor-core accumulation segment, 0 = whole K), "gemm_impl" (0 = wgmma, 1 = CUDA-core checker),
  * "num_sms" (persistent grid size, 0 = all), "profile" (1 = record per-kernel CUDA events),
  * "mid_band" (thousandths of a pixel, default 26 = 2x the largest 1-pass/3-pass difference measured over 125k DISTINCT
- * coordinates, profiles/r02_band_stats.json; with mid_passes = 3 every row is first computed 1-pass and
+ * coordinates; with mid_passes = 3 every row is first computed 1-pass and
  * only rows with a coordinate within the band of an integer -- where trunc(mid) could differ from the
  * reference -- are re-computed 3-pass; 0 = 3-pass for every row), "fuse_gather" (conv1 A operand of the 1-pass launches; default 3 = per-image window map + strided TMA boxes, no
  * producer warps; 1 = gathered in producer warps; 2 = first-generation fused kernel; 0 = separate gather kernel + TMA
@@ -84,10 +84,7 @@ P2P_API int p2p_set_regressor_weights(p2p_handle_t h, int which, const p2p_regre
  * "nc_l2_mode" (layout of NC layer 2's block of hidden lines: 0 = chosen per shape, 1 = one haloed block per tile,
  * 2 = one block per column tap; bit-identical results), "unique_impl" (default 1: rank sort over the whole GPU for lists of
  * up to 8192 rows; 0: single-block bitonic network; identical results), "fc_impl" (default 1: the 512-512 and 512-256 Linear layers run on
- * the tensor cores, 3-pass; 0: fp32 CUDA-core FC kernel), "gemm_pair" (bitmask of GEMM launches that run
- * on the CTA-pair kernel -- tcgen05.mma.cta_group::2, one M=256 tile over the two SMs of a TPC, bit-identical
- * results: 1 = 1-pass convs, 2 = 3-pass convs, 4 = FC, 8 = correlation, 16 = p2p_test_gemm, 32 = fused-gather conv1;
- * default 35 = all conv launches). */
+ * the tensor cores, 3-pass; 0: fp32 CUDA-core FC kernel). */
 P2P_API int p2p_set_option(p2p_handle_t h, const char* key, int value);
 P2P_API int p2p_get_option(p2p_handle_t h, const char* key, int* value);
 /* Number of kernel launches enqueued by this handle since creation (bench.py's gpu_launches). */
@@ -193,7 +190,7 @@ P2P_API int p2p_finalize_matches(p2p_handle_t h, const float* fine, const float*
 P2P_API int p2p_preprocess_image(p2p_handle_t h, const uint8_t* rgb_hwc, int ho, int wo, int ht, int wt, float* out_chw,
                          uint8_t* resized_hwc_out, void* stream);
 
-/* ---- bring-up / accuracy probe: C[M,N] = alpha * A[M,K] B[N,K]^T on the tcgen05 path with the
+/* ---- bring-up / accuracy probe: C[M,N] = alpha * A[M,K] B[N,K]^T on the wgmma path with the
  * same operand format as the hot path (fp32 inputs are split to fp16 hi/lo on the device).
  * a, b, c are DEVICE fp32; K % 64 == 0. */
 P2P_API int p2p_test_gemm(p2p_handle_t h, const float* a, const float* b, float* c, int M, int N, int K, int passes,

@@ -95,13 +95,13 @@ class Handle:
     def __init__(self, device):
         device = torch.device(device)
         if device.type != 'cuda':
-            raise RuntimeError('patch2pix_b200 runs on CUDA (sm_100a) devices only; got device ' + str(device))
+            raise RuntimeError('patch2pix_b200 runs on CUDA (sm_90a) devices only; got device ' + str(device))
         self.device = torch.device('cuda', device.index if device.index is not None else torch.cuda.current_device())
         self.lib = load()
         h = C.c_void_p()
         check(self.lib.p2p_create(self.device.index, C.byref(h)))
         self.h = h
-        # P2P_OPTIONS="nc_impl=0,mid_band=0": option overrides for A/B measurements (tools/, bench.py)
+        # P2P_OPTIONS="nc_impl=0,mid_band=0": option overrides for A/B measurements (bench.py)
         for kv in filter(None, os.environ.get('P2P_OPTIONS', '').split(',')):
             k, _, v = kv.partition('=')
             self.set_option(k.strip(), int(v))

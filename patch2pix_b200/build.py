@@ -1,4 +1,4 @@
-"""Build libp2p_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libp2p_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
     python -m patch2pix_b200.build [--force] [--verbose]
 """
@@ -11,7 +11,7 @@ CSRC = os.path.join(HERE, 'csrc')
 OUT = os.path.join(HERE, 'libp2p_b200.so')
 SOURCES = ['api.cu', 'coarse.cu', 'refine.cu', 'umma_gemm.cu', 'nc_umma.cu', 'preprocess.cu']
 HEADERS = ['common.cuh', 'kernels.h', 'umma_gemm.h', 'umma_ptx.cuh', os.path.join('..', '..', 'include', 'p2p_b200.h')]
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
               '-Xcompiler', '-fPIC,-O2,-fvisibility=hidden', '--threads', '4']
 
 
@@ -49,7 +49,7 @@ def build(force=False, verbose=False):
         failed |= p.returncode != 0
     if failed:
         raise RuntimeError('nvcc failed building libp2p_b200.so')
-    cmd = [_nvcc(), '-shared', '-o', OUT] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a']
+    cmd = [_nvcc(), '-shared', '-o', OUT] + objs + ['-gencode', 'arch=compute_90a,code=sm_90a']
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError('link failed:\n' + r.stdout)

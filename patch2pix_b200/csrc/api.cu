@@ -83,24 +83,21 @@ using namespace p2p;
 
 struct p2p_handle_s {
   int device = 0;
-  int num_sms = 148;
+  int num_sms = 132;
   int opt_mid_passes = 3, opt_fine_passes = 1, opt_corr_passes = 3, opt_seg_len = 3, opt_gemm_impl = 0, opt_num_sms = 0;
-  int opt_mid_band = 26;  // thousandths of a pixel (2x the largest 1-pass/3-pass mid difference over 125k distinct coordinates,
-                          // profiles/r02_band_stats.json); 0 = pure 3-pass mid stage
-  int opt_gemm_pair = 35;   // bitmask of launches that use the CTA-pair (cta_group::2) GEMM kernel:
-                            // 1: 1-pass convs, 2: 3-pass convs, 4: FC, 8: correlation, 16: p2p_test_gemm,
-                            // 32: fused-gather conv1
+  int opt_mid_band = 26;  // thousandths of a pixel (2x the largest 1-pass/3-pass mid difference over 125k distinct coordinates);
+                          // 0 = pure 3-pass mid stage
   int opt_fc_impl = 1;      // 1: the two big Linear layers on the tensor cores (3-pass); 0: CUDA-core FC kernel
   int opt_fuse_gather = 3;  // conv1 A operand of the 1-pass launches: 3 (default): strided TMA boxes of a per-image window map
-                            // (umma_conv1_tma_kernel); 1: gathered by producer warps (128x512 tiles, lookup tables); 2: first-
-                            // generation fused kernel (128x256 tiles); 0: separate gather kernel + TMA of the patch tensor
+                            // (AMODE_WINDOW); 1 or 2: gathered by producer warps (AMODE_GATHER); 0: separate gather kernel +
+                            // TMA of the patch tensor
   const int* last_band_count = nullptr;  // device counter of the last risk-band subset
   unsigned long long* band_totals = nullptr;   // device: {band rows, rows} summed over mid-stage calls
   bool nc_set = false;
   float *nc_w1p = nullptr, *nc_b1p = nullptr, *nc_w2p = nullptr;
   float nc_b2 = 0.f;
   NcUmmaWeights ncw;            // tensor-core NC operand images
-  void* dbg_nc[4] = {nullptr, nullptr, nullptr, nullptr};   // scratch of the last p2p_neigh_consensus call (tools/nc_debug.py)
+  void* dbg_nc[4] = {nullptr, nullptr, nullptr, nullptr};   // scratch of the last p2p_neigh_consensus call (debug hook below)
   int opt_unique_impl = 1;      // 1: rank sort over the whole GPU for lists <= 8192 rows; 0: single-block bitonic network
   int* uniq_rank = nullptr;     // zeroed scratch of the rank-sort path
   int opt_nc_l2_mode = 0;       // NC layer 2 block layout: 0 auto, 1 one haloed block per tile, 2 one block per column tap
@@ -390,8 +387,8 @@ int p2p_create(int device, p2p_handle_t* out) {
   P2P_REQUIRE(device >= 0 && device < ndev, "device index out of range");
   cudaDeviceProp prop;
   P2P_CUDA_OK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
-    set_last_error(std::string("libp2p_b200 targets sm_100a (B200) only; device is sm_") + std::to_string(prop.major) +
+  if (prop.major != 9 || prop.minor != 0) {
+    set_last_error(std::string("libp2p_b200 targets sm_90a (H100) only; device is sm_") + std::to_string(prop.major) +
                    std::to_string(prop.minor));
     return -2;
   }
@@ -486,7 +483,6 @@ static int* option_slot(p2p_handle_t h, const char* key) {
   if (!strcmp(key, "mid_band")) return &h->opt_mid_band;
   if (!strcmp(key, "fuse_gather")) return &h->opt_fuse_gather;
   if (!strcmp(key, "fc_impl")) return &h->opt_fc_impl;
-  if (!strcmp(key, "gemm_pair")) return &h->opt_gemm_pair;
   if (!strcmp(key, "nc_impl")) return &h->opt_nc_impl;
   if (!strcmp(key, "nc_l2_mode")) return &h->opt_nc_l2_mode;
   if (!strcmp(key, "unique_impl")) return &h->opt_unique_impl;
@@ -574,8 +570,7 @@ static int corr_umma(p2p_handle_s* h, const __half* a_hi, const __half* a_lo, co
   const uint32_t ab[5] = {64, 1, 1, 1, 128};
   const uint64_t bd[2] = {(uint64_t)C, (uint64_t)n2pad};
   const uint64_t bs[1] = {(uint64_t)C * 2};
-  p.pair = (h->opt_gemm_pair & 8) ? 1 : 0;
-  const uint32_t bb[2] = {64, p.pair ? 128u : 256u};
+  const uint32_t bb[2] = {64, 128};
   int rc;
   if ((rc = make_tmap_fp16(&p.a_main_hi, a_hi, 5, ad, as, ab))) return rc;
   if ((rc = make_tmap_fp16(&p.b_hi, b_hi, 2, bd, bs, bb))) return rc;
@@ -765,7 +760,7 @@ int p2p_neigh_consensus(p2p_handle_t h, const float* in, int hA, int wA, int hB,
   return launch_neigh_consensus(in, hA, wA, hB, wB, h->nc_w1p, h->nc_b1p, h->nc_w2p, h->nc_b2, hidden, out, st);
 }
 
-// Development hook (tools/nc_debug.py; not part of include/p2p_b200.h): copies `bytes` of an intermediate of the last
+// Development hook (not part of include/p2p_b200.h): copies `bytes` of an intermediate of the last
 // p2p_neigh_consensus call to the host -- which = 0 hidden [V][64] fp16, 1 partial [18][V] f32, 2 xp (padded hi|lo
 // words), 3 xmax word.
 P2P_API int p2p_debug_nc_scratch(p2p_handle_t h, int which, void* host_dst, size_t bytes) {
@@ -928,10 +923,7 @@ int run_regressor(p2p_handle_s* h, Regressor& R, int which, int passes, const Re
     UmmaGemmParams p;
     memset(&p, 0, sizeof(p));
     const uint32_t abox[5] = {64, 8, 8, 1, 2};
-    const int pair = fused ? ((h->opt_gemm_pair & 32) && h->opt_fuse_gather == 1 ? 1 : 0)      // 32: fused conv1
-                           : ((h->opt_gemm_pair & (lo ? 2 : 1)) ? 1 : 0);
-    const int pair2 = (h->opt_gemm_pair & (lo ? 2 : 1)) ? 1 : 0;       // conv2 never runs fused
-    uint32_t bbox[2] = {64, pair ? 128u : 256u};
+    const uint32_t bbox[2] = {64, 128};
     const uint64_t npad = (uint64_t)B.npad;
     {  // conv1
       const uint64_t ad[5] = {512, 8, 8, 4, npad};
@@ -946,7 +938,6 @@ int run_regressor(p2p_handle_s* h, Regressor& R, int which, int passes, const Re
       if ((rc = make_tmap_fp16(&p.a_main_lo, lo ? B.p_lo : B.p_hi, 5, ad, as, abox))) return rc;
       if ((rc = make_tmap_fp16(&p.a_rgb_lo, lo ? B.r_lo : B.r_hi, 5, rd, rs, abox))) return rc;
       if ((rc = make_tmap_fp16(&p.b_lo, R.w1_lo, 2, bd, bs, bbox))) return rc;
-      p.pair = pair;
       p.nsteps = kConv1Steps;
       memcpy(p.steps, R.steps1, sizeof(R.steps1));
       p.m_tiles = (n + 1) / 2;
@@ -971,43 +962,31 @@ int run_regressor(p2p_handle_s* h, Regressor& R, int which, int passes, const Re
         }
         p.fg.matches = matches_in;
         p.fg.is_float = is_float;
-        p.fg.generation = h->opt_fuse_gather == 2 ? 1 : 2;
       }
       ProfScope ps(h, kb + 1, st);
       if (mapped) {
-        Conv1TmaParams q;
-        memset(&q, 0, sizeof(q));
-        const uint32_t wbox[2] = {64, 128};
-        if ((rc = make_tmap_fp16(&q.b_hi, R.w1_hi, 2, bd, bs, wbox))) return rc;
         for (int s2 = 0; s2 < 2; ++s2) {
           const uint64_t Wp = (uint64_t)h->pf[s2].W + 2 * kMapPad, Hp = (uint64_t)h->pf[s2].H + 2 * kMapPad;
           const uint64_t md[3] = {256, Wp, Hp};
           const uint64_t ms[2] = {512, Wp * 512};
           const uint32_t mb[3] = {64, 16, 16};       // 8 elements at traversal stride 2 (box = N * stride)
           const uint32_t me[3] = {1, 2, 2};
-          if ((rc = make_tmap_fp16(&q.wm.map[s2], h->pf[s2].wmap, 3, md, ms, mb, me))) return rc;
-          q.wm.rgbn[s2] = h->pf[s2].rgbn;
-          q.wm.H[s2] = h->pf[s2].H;
-          q.wm.W[s2] = h->pf[s2].W;
+          if ((rc = make_tmap_fp16(&p.wm.map[s2], h->pf[s2].wmap, 3, md, ms, mb, me))) return rc;
+          p.wm.rgbn[s2] = h->pf[s2].rgbn;
+          p.wm.H[s2] = h->pf[s2].H;
+          p.wm.W[s2] = h->pf[s2].W;
         }
-        q.wm.matches = matches_in;
-        q.wm.is_float = is_float;
-        q.nsteps = kConv1Steps;
-        memcpy(q.steps, R.steps1, sizeof(R.steps1));
-        q.m_tiles = (n + 1) / 2;
-        q.epi = p.epi;
-        if ((rc = launch_conv1_tma(q, sms(h), st))) return rc;
-      } else if ((rc = launch_umma_gemm(p, EPI_CONV1, passes, sms(h), st, fused))) {
-        return rc;
+        p.wm.matches = matches_in;
+        p.wm.is_float = is_float;
       }
+      const int amode = mapped ? AMODE_WINDOW : (fused ? AMODE_GATHER : AMODE_TMA);
+      if ((rc = launch_umma_gemm(p, EPI_CONV1, passes, sms(h), st, amode))) return rc;
     }
     {  // conv2
       const uint64_t ad[5] = {512, 8, 8, 1, npad};
       const uint64_t as[4] = {1024, 8192, 65536, 65536};
       const uint64_t bd[2] = {(uint64_t)kConv2Steps * 64, 512};
       const uint64_t bs[1] = {(uint64_t)kConv2Steps * 64 * 2};
-      p.pair = pair2;
-      bbox[1] = pair2 ? 128u : 256u;
       if ((rc = make_tmap_fp16(&p.a_main_hi, B.y_hi, 5, ad, as, abox))) return rc;
       if ((rc = make_tmap_fp16(&p.a_main_lo, lo ? B.y_lo : B.y_hi, 5, ad, as, abox))) return rc;
       if ((rc = make_tmap_fp16(&p.b_hi, R.w2_hi, 2, bd, bs, bbox))) return rc;
@@ -1031,11 +1010,10 @@ int run_regressor(p2p_handle_s* h, Regressor& R, int which, int passes, const Re
   if ((rc = launch_pooled_split(B.pooled, n, B.q_hi, B.q_lo, d_count, st))) return rc;
   const uint64_t m128 = align_up(n, 128);
   const uint32_t abx[5] = {64, 1, 1, 1, 128};
-  const uint32_t bbx[2] = {64, (h->opt_gemm_pair & 4) ? 128u : 256u};
+  const uint32_t bbx[2] = {64, 128};
   for (int layer = 0; layer < 2; ++layer) {
     UmmaGemmParams p;
     memset(&p, 0, sizeof(p));
-    p.pair = (h->opt_gemm_pair & 4) ? 1 : 0;
     const int nout = layer == 0 ? 512 : 256;
     const uint64_t ad[5] = {512, 1, 1, 1, m128};
     const uint64_t as[4] = {1024, 1024, 1024, 1024};
@@ -1194,8 +1172,7 @@ int p2p_test_gemm(p2p_handle_t h, const float* a, const float* b, float* c, int 
   const uint32_t abx[5] = {64, 1, 1, 1, 128};
   const uint64_t bd[2] = {(uint64_t)K, (uint64_t)npad};
   const uint64_t bs[1] = {(uint64_t)K * 2};
-  p.pair = (h->opt_gemm_pair & 16) ? 1 : 0;
-  const uint32_t bbx[2] = {64, p.pair ? 128u : 256u};
+  const uint32_t bbx[2] = {64, 128};
   if ((rc = make_tmap_fp16(&p.a_main_hi, a_hi, 5, ad, as, abx))) return rc;
   if ((rc = make_tmap_fp16(&p.a_main_lo, a_lo, 5, ad, as, abx))) return rc;
   if ((rc = make_tmap_fp16(&p.b_hi, b_hi, 2, bd, bs, bbx))) return rc;

@@ -122,7 +122,7 @@ __global__ void __launch_bounds__(256) corr_pool_kernel(const float* __restrict_
   }
 }
 
-// K-major fp16 hi/lo output for the tcgen05 correlation.  Block = 32 consecutive output positions x all channels:
+// K-major fp16 hi/lo output for the tensor-core correlation.  Block = 32 consecutive output positions x all channels:
 // coalesced reads along the positions (NCHW input), transposed through shared memory, 64-byte row segments out.
 // Both images in one launch (blockIdx.y).
 struct L2NormArgs {
@@ -711,7 +711,7 @@ int launch_neigh_consensus(const float* x, int hA, int wA, int hB, int wB, const
     const size_t smem = sizeof(float) * (81 * 32 + 8 * PH * PW + 16);
     P2P_REQUIRE(smem <= 200 * 1024, "NC layer 2: pooled B grid does not fit shared memory");
     // A cells per block: the choice with the least wave-quantisation waste on this device
-    int JB = 2, nsm = 148;
+    int JB = 2, nsm = 132;
     {
       int dev = 0;
       cudaGetDevice(&dev);

@@ -123,7 +123,7 @@ struct KStep {
   int bk;                         // K coordinate in the weight matrix
 };
 
-// CUDA-core debug GEMM over exactly the tensors the tcgen05 kernel consumes (bring-up checker;
+// CUDA-core debug GEMM over exactly the tensors the wgmma kernel consumes (bring-up checker;
 // not a product path: selected only by p2p_set_option("gemm_impl", 1)).
 struct GemmOperands {
   const __half *a_hi, *a_lo;      // main A tensor [N][planes][8][8][512]

@@ -1,4 +1,4 @@
-// NeighConsensus (symmetric 2-layer Conv4d 1 -> 16 -> 1, k = 3, ReLU after each layer) on the tcgen05 tensor cores.
+// NeighConsensus (symmetric 2-layer Conv4d 1 -> 16 -> 1, k = 3, ReLU after each layer) on the Hopper tensor cores (wgmma).
 //
 // Reference semantics (file:line relative to the reference repo):
 //   NeighConsensus.forward   networks/ncn/model.py:145-155   conv(x) + conv(x^T)^T, shared weights
@@ -7,7 +7,7 @@
 // conv(x) + conv(x^T)^T equals two independent nets on the SAME input, the second with tap axes (a,b) <-> (d,e)
 // swapped (api.cu packs both: w1p / w2p [81 taps][32 = 16 ch of net 0 | 16 ch of net 1]).
 //
-// Both layers are skinny GEMMs on tcgen05; nothing but x, the hidden tensor and the partial maps touches HBM and no
+// Both layers are skinny GEMMs on wgmma; nothing but x, the hidden tensor and the partial maps touches HBM and no
 // FMA-pipe inner loop is left:
 //
 //   pad/split x -> xp: zero-haloed copy of x, every element already scaled and split into an fp16 (hi, lo) pair packed
@@ -25,14 +25,13 @@
 //   combine   out[a][b] = sum_net relu(b2 + sum_(ta,tb) P_(ta,tb)[a + (ta-1, tb-1)][b])  (fixed summation order:
 //             deterministic), fused with the row/column maxima of the MutualMatching that follows.
 //
-// Precision: fp16 hi/lo operand pairs, three products per term (lo*hi + hi*lo + hi*hi, fp32 accumulate in TMEM, each
+// Precision: fp16 hi/lo operand pairs, three products per term (lo*hi + hi*lo + hi*hi, fp32 accumulate in registers, each
 // product kind in its own accumulator so the chains are short and independent): products good to ~2^-22, i.e.
 // fp32-grade.  Activations are scaled by powers of two derived ON THE DEVICE from max|x| (and from a weight-norm bound
 // for the hidden tensor), so any input range is safe in fp16.
 //
-// Warp-specialised persistent kernels (loader thread, MMA issuer, TMEM allocator, 4 epilogue warps = TMEM lane
-// quadrants, producer warps in layer 1), mbarrier rings, two TMEM accumulator slots so that the epilogue of tile i
-// overlaps the MMAs of tile i+1.
+// Warp-specialised persistent kernels (loader thread, two consumer warpgroups that issue the MMAs and run the epilogue
+// on the accumulator fragments, producer warps in layer 1) with mbarrier rings.
 #include <math.h>
 
 #include <type_traits>
@@ -45,7 +44,6 @@
 namespace p2p {
 
 constexpr int kNcAtom = 128 * 128;   // bytes of one [128 rows x 64 fp16] swizzled operand atom
-constexpr int kNcSlots = 4;          // TMEM accumulator slots per CTA: MMAs of up to 3 tiles run ahead of the epilogue
 
 struct NcParams {
   int hA, wA, hB, wB, nA, nB;
@@ -80,19 +78,6 @@ __device__ __forceinline__ void nc_scales(const NcParams& p, float& sx, float& s
   if (!(hb > 0.f) || !isfinite(hb)) hb = 1.f;
   frexpf(hb, &e);
   sh = ldexpf(1.f, min(12 - e, 60));
-}
-
-// operands that are bounded by construction (|v| < 4096): no saturation needed
-__device__ __forceinline__ void split8_bounded(const float* v, uint4& hi, uint4& lo) {
-  __half2 h[4], l[4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    h[i] = __floats2half2_rn(v[2 * i], v[2 * i + 1]);
-    const float2 f = __half22float2(h[i]);
-    l[i] = __floats2half2_rn(v[2 * i] - f.x, v[2 * i + 1] - f.y);
-  }
-  hi = *reinterpret_cast<uint4*>(h);
-  lo = *reinterpret_cast<uint4*>(l);
 }
 
 // exact n / d for 0 <= n < 2^22 with inv = 1.f / d (the quotient of n + 0.5 is at least 0.5 / d away from an integer)
@@ -136,14 +121,15 @@ __global__ void __launch_bounds__(256) nc_pad_split_kernel(const __grid_constant
 // ------------------------------------------------------------------------------------------------
 // layer 1.  Tile = (A cell a, 128 consecutive B cells).  The B rows of the 9 A-neighbours the tile touches are staged
 // from xp with 9 bulk copies by one thread (double-buffered: tile i+1 is in flight while tile i is built), so a tap is
-// a plain `ld.shared [row base + tk*pitch + tl]` with no validity logic.  Sixteen producer warps (four threads per
-// tile row, each a quarter of the 11 tap chunks) pack the (hi, lo) words into the swizzled operand chunks.
-// The three products of the hi/lo split (lo*hi, hi*lo, hi*hi) accumulate in three SEPARATE TMEM blocks -- three
-// independent MMA chains instead of one 18-deep dependent chain of tiny (N = 32) MMAs -- and are summed by the epilogue.
-// 768 threads (warp 1 MMA, 2 TMEM, 3 loader, 4..7 epilogue, 8..23 producers), 1 CTA per SM, 4 x 32 KB operand stages.
+// a plain `ld.shared [row base + tk*pitch + tl]` with no validity logic.  Eight producer warps (two threads per tile
+// row, each half of the 11 tap chunks) pack the (hi, lo) words into the swizzled operand chunks.
+// Two consumer warpgroups (tile rows 0..63 and 64..127) run the MMAs: the three products of the hi/lo split (lo*hi,
+// hi*lo, hi*hi) accumulate in SEPARATE register accumulators -- a_hi x [w_hi | w_lo] (N = 64) gives hi*hi and hi*lo,
+// a_lo x w_hi (N = 32) gives lo*hi -- and are summed by the epilogue, which works on the accumulator fragments directly.
+// 640 threads (warp 3 loader, warps 4..11 MMA + epilogue, 12..19 producers), 1 CTA per SM, 4 x 32 KB operand stages.
 // ------------------------------------------------------------------------------------------------
 constexpr int kL1Stages = 4;
-constexpr int kL1Threads = 768, kL1ProducerWarps = 16;
+constexpr int kL1Threads = 640, kL1ProducerWarps = 8;
 
 __host__ __device__ inline int nc_l1_rows(int wB) { return 127 / wB + 4; }      // padded B rows a tile can touch
 
@@ -151,7 +137,6 @@ __global__ void __launch_bounds__(kL1Threads, 1) nc_l1_umma_kernel(const __grid_
                                                                   const __grid_constant__ CUtensorMap hstore) {
   constexpr int STAGE_BYTES = 2 * kNcAtom;         // A_hi + A_lo of one atom
   constexpr int WATOM = 64 * 128;                  // weight image of one atom: rows 0..31 w_hi, 32..63 w_lo
-  constexpr uint32_t IDESC64 = make_idesc_f16(128, 64), IDESC32 = make_idesc_f16(128, 32);
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* wsm = smem + kL1Stages * STAGE_BYTES;                          // [atom][hi|lo] weight images, 16 KB
@@ -159,11 +144,8 @@ __global__ void __launch_bounds__(kL1Threads, 1) nc_l1_umma_kernel(const __grid_
   uint8_t* xs = hst + 2 * kNcAtom;                                        // [bufs][9][rows][pitch] words
   __shared__ __align__(8) uint64_t full_bar[kL1Stages];
   __shared__ __align__(8) uint64_t empty_bar[kL1Stages];
-  __shared__ __align__(8) uint64_t tfull_bar[kNcSlots];
-  __shared__ __align__(8) uint64_t tempty_bar[kNcSlots];
   __shared__ __align__(8) uint64_t xfull_bar[2];
   __shared__ __align__(8) uint64_t xempty_bar[2];
-  __shared__ uint32_t tmem_base_smem;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles = p.tiles;
@@ -179,11 +161,7 @@ __global__ void __launch_bounds__(kL1Threads, 1) nc_l1_umma_kernel(const __grid_
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < kL1Stages; ++i) {
       mbar_init(&full_bar[i], kL1ProducerWarps);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < kNcSlots; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], 4);
+      mbar_init(&empty_bar[i], 2);
     }
     for (int i = 0; i < 2; ++i) {
       mbar_init(&xfull_bar[i], 1);
@@ -191,45 +169,89 @@ __global__ void __launch_bounds__(kL1Threads, 1) nc_l1_umma_kernel(const __grid_
     }
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(&tmem_base_smem, 512);
   fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
 
-  if (warp == 1) {
-    // ===================== MMA issuer: the whole warp runs the loop (uniform), one elected lane issues =====================
-    int it = 0, tl = 0;
+  if (warp >= 4 && warp < 12) {
+    // ===================== MMA + epilogue: warpgroup wg owns tile rows 64 wg .. 64 wg + 63 =====================
+    const int wg = (warp >> 2) - 1, wl = warp & 3;
+    const int t = lane & 3;
+    const int r0 = wg * 64 + 16 * wl + (lane >> 2);          // fragment rows r0 and r0 + 8
+    float sx, sh;
+    nc_scales(p, sx, sh);
+    const float inv = p.inv_sw1 / sx;
     const uint32_t sbase = smem_u32(smem), wbase = smem_u32(wsm);
+    int it = 0, tl = 0;
     for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++tl) {
-      const int slot = tl % kNcSlots;
-      mbar_wait(&tempty_bar[slot], ((uint32_t)(tl / kNcSlots) & 1u) ^ 1u);
-      tc_fence_after();
-      const uint32_t d0 = tmem_base + (uint32_t)(slot * 96);            // [0,32) hi*hi, [32,64) hi*lo, [64,96) lo*hi
+      float d64[32], d32[16];                                // [0,32) hi*hi | [32,64) hi*lo ; lo*hi
+      int st[2];
 #pragma unroll
       for (int atom = 0; atom < 2; ++atom, ++it) {
         const int s = it % kL1Stages;
+        st[atom] = s;
         mbar_wait(&full_bar[s], (uint32_t)(it / kL1Stages) & 1u);
-        tc_fence_after();
-        const uint32_t sa = sbase + (uint32_t)(s * STAGE_BYTES);
+        const uint32_t sa = sbase + (uint32_t)(s * STAGE_BYTES) + (uint32_t)(wg * 8192);
         const uint64_t a_hi = make_sw128_desc(sa), a_lo = make_sw128_desc(sa + kNcAtom);
         const uint64_t w = make_sw128_desc(wbase + (uint32_t)(atom * WATOM));     // rows 0..31 w_hi, 32..63 w_lo
         constexpr int nk0 = 4, nk1 = 2;             // taps 64..80 live in the first two K16 slices of atom 1
-        if (elect_one()) {
+        wgmma_fence();
 #pragma unroll
-          for (int kk = 0; kk < nk0; ++kk) {
-            if (atom == 1 && kk >= nk1) break;
-            const uint32_t acc = (atom > 0 || kk > 0) ? 1u : 0u;
-            umma_f16(d0, a_hi + 2 * kk, w + 2 * kk, IDESC64, acc);          // hi*hi | hi*lo
-            umma_f16(d0 + 64, a_lo + 2 * kk, w + 2 * kk, IDESC32, acc);     // lo*hi
-          }
-          umma_commit(&empty_bar[s]);
-          if (atom == 1) umma_commit(&tfull_bar[slot]);
+        for (int kk = 0; kk < nk0; ++kk) {
+          if (atom == 1 && kk >= nk1) break;
+          const uint32_t acc = (atom > 0 || kk > 0) ? 1u : 0u;
+          wgmma_f16<64>(d64, a_hi + 2 * kk, w + 2 * kk, acc);      // hi*hi | hi*lo
+          wgmma_f16<32>(d32, a_lo + 2 * kk, w + 2 * kk, acc);      // lo*hi
         }
-        __syncwarp();
+        wgmma_commit();
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs<32>(d64);
+      wgmma_fence_regs<16>(d32);
+      if (threadIdx.x % 128 == 0) {
+        mbar_arrive(&empty_bar[st[0]]);
+        mbar_arrive(&empty_bar[st[1]]);
+      }
+      const int a = fast_div(tile, inv_tb), b0 = (tile - a * TB) << 7;
+      // The tile's 128 hidden lines are contiguous in global memory.  They go through a swizzled shared staging
+      // buffer and leave with ONE tensor-map store per tile.  Rows past the end of the B grid are clipped by the
+      // tensor map.
+      uint8_t* sb = hst + (size_t)(tl & 1) * kNcAtom;
+      if (threadIdx.x == 128) bulk_wait_group_read<1>();        // the store of tile tl-2 has finished reading this buffer
+      asm volatile("bar.sync 2, 256;" ::: "memory");
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = r0 + 8 * h;
+        if (b0 + row < p.nB) {
+          const uint32_t so = smem_u32(sb) + (uint32_t)(row * 128);
+          const uint32_t sw = (uint32_t)(row & 7);
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const int c = 8 * j + 2 * t;                           // channels c, c + 1: net c / 16
+            float hv[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int i = 4 * j + 2 * h + e;
+              const float acc = (d32[i] + d64[16 + i]) + d64[i];   // (lo*hi + hi*lo) + hi*hi
+              hv[e] = fmaxf(fmaf(acc, inv, __ldg(p.b1p + c + e)), 0.f) * sh;
+            }
+            const __half2 hi = __floats2half2_rn(hv[0], hv[1]);
+            const float2 hf = __half22float2(hi);
+            const __half2 lo = __floats2half2_rn(hv[0] - hf.x, hv[1] - hf.y);
+            const int idx = (c >> 4) * 32 + (c & 15);                 // [net][hi 16 | lo 16]
+            const uint32_t chi = (uint32_t)(idx >> 3), clo = chi + 2, wi = (uint32_t)((idx & 7) * 2);
+            asm volatile("st.shared.b32 [%0], %1;" ::"r"(so + ((chi ^ sw) << 4) + wi), "r"(*reinterpret_cast<const uint32_t*>(&hi)) : "memory");
+            asm volatile("st.shared.b32 [%0], %1;" ::"r"(so + ((clo ^ sw) << 4) + wi), "r"(*reinterpret_cast<const uint32_t*>(&lo)) : "memory");
+          }
+        }
+      }
+      fence_proxy_async();
+      asm volatile("bar.sync 2, 256;" ::: "memory");
+      if (threadIdx.x == 128) {
+        tma_store_3d(&hstore, sb, 0, b0, a);
+        bulk_commit_group();
       }
     }
+    if (threadIdx.x == 128) bulk_wait_group_read<0>();
   } else if (warp == 3) {
     // ===================== loader: 9 bulk copies per tile =====================
     if (lane == 0) {
@@ -249,11 +271,11 @@ __global__ void __launch_bounds__(kL1Threads, 1) nc_l1_umma_kernel(const __grid_
         }
       }
     }
-  } else if (warp >= 8) {
-    // ===================== producers: 512 threads = 128 tile rows x 4 chunk quarters =====================
-    const int ptid = threadIdx.x - 256;
+  } else if (warp >= 12) {
+    // ===================== producers: 256 threads = 128 tile rows x 2 chunk halves =====================
+    const int ptid = threadIdx.x - 384;
     const int r = ptid & 127;
-    const int qt = ptid >> 7;          // warp-uniform: chunks qt and qt + 4 of atom 0, chunk qt of atom 1 (qt < 3)
+    const int qh = ptid >> 7;          // warp-uniform: quarters 2 qh and 2 qh + 1 (chunks Q, Q + 4 of atom 0, Q of atom 1)
     const uint32_t sw = (uint32_t)(r & 7);
     const uint32_t otk = (uint32_t)(p.WP * 4);
     int it = 0, tl = 0;
@@ -286,15 +308,17 @@ __global__ void __launch_bounds__(kL1Threads, 1) nc_l1_umma_kernel(const __grid_
         sts_v4(o + kNcAtom, __byte_perm(w[0], w[1], 0x7632), __byte_perm(w[2], w[3], 0x7632),
                __byte_perm(w[4], w[5], 0x7632), __byte_perm(w[6], w[7], 0x7632));
       };
-      auto build = [&](auto QT) {
-        constexpr int Q = decltype(QT)::value;
-        {   // atom 0: chunks Q and Q + 4
+      auto build = [&](auto QH) {
+        constexpr int Q0 = 2 * decltype(QH)::value, Q1 = Q0 + 1;
+        {   // atom 0: chunks Q, Q + 4 of both quarters
           const int s = it % kL1Stages;
           mbar_wait(&empty_bar[s], ((uint32_t)(it / kL1Stages) & 1u) ^ 1u);
           const uint32_t st = smem_u32(smem) + (uint32_t)(s * STAGE_BYTES + r * 128);
           if (rv) {
-            chunk(std::integral_constant<int, 0>{}, std::integral_constant<int, Q>{}, st);
-            chunk(std::integral_constant<int, 0>{}, std::integral_constant<int, Q + 4>{}, st);
+            chunk(std::integral_constant<int, 0>{}, std::integral_constant<int, Q0>{}, st);
+            chunk(std::integral_constant<int, 0>{}, std::integral_constant<int, Q0 + 4>{}, st);
+            chunk(std::integral_constant<int, 0>{}, std::integral_constant<int, Q1>{}, st);
+            chunk(std::integral_constant<int, 0>{}, std::integral_constant<int, Q1 + 4>{}, st);
           }
           fence_proxy_async();
           __syncwarp();
@@ -304,122 +328,53 @@ __global__ void __launch_bounds__(kL1Threads, 1) nc_l1_umma_kernel(const __grid_
         {   // atom 1: chunk Q (taps 64 + 8Q ..; Q = 3 has nothing to write, chunks 3..7 stay zero)
           const int s = it % kL1Stages;
           mbar_wait(&empty_bar[s], ((uint32_t)(it / kL1Stages) & 1u) ^ 1u);
-          if (Q < 3) {
-            const uint32_t st = smem_u32(smem) + (uint32_t)(s * STAGE_BYTES + r * 128);
-            if (rv) chunk(std::integral_constant<int, 1>{}, std::integral_constant<int, (Q < 3 ? Q : 0)>{}, st);
-            fence_proxy_async();
+          const uint32_t st = smem_u32(smem) + (uint32_t)(s * STAGE_BYTES + r * 128);
+          if (rv) {
+            chunk(std::integral_constant<int, 1>{}, std::integral_constant<int, Q0>{}, st);
+            if (Q1 < 3) chunk(std::integral_constant<int, 1>{}, std::integral_constant<int, (Q1 < 3 ? Q1 : 0)>{}, st);
           }
+          fence_proxy_async();
           __syncwarp();
           if (lane == 0) mbar_arrive(&full_bar[s]);
           ++it;
         }
       };
-      if (qt == 0) build(std::integral_constant<int, 0>{});
-      else if (qt == 1) build(std::integral_constant<int, 1>{});
-      else if (qt == 2) build(std::integral_constant<int, 2>{});
-      else build(std::integral_constant<int, 3>{});
+      if (qh == 0) build(std::integral_constant<int, 0>{});
+      else build(std::integral_constant<int, 1>{});
       __syncwarp();
       if (lane == 0) mbar_arrive(&xempty_bar[buf]);            // this warp's reads of the staging buffer are done
     }
-  } else if (warp >= 4) {
-    // ===================== epilogue =====================
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    float sx, sh;
-    nc_scales(p, sx, sh);
-    const float inv = p.inv_sw1 / sx;
-    int tl = 0;
-    for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++tl) {
-      const int slot = tl % kNcSlots;
-      mbar_wait(&tfull_bar[slot], (uint32_t)(tl / kNcSlots) & 1u);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(slot * 96);
-      float acc[32], t1[32];
-      tmem_ld32(taddr + 64, acc);                  // lo*hi
-      tmem_ld32(taddr + 32, t1);                   // hi*lo
-#pragma unroll
-      for (int c = 0; c < 32; ++c) acc[c] += t1[c];
-      tmem_ld32(taddr, t1);                        // hi*hi
-#pragma unroll
-      for (int c = 0; c < 32; ++c) acc[c] += t1[c];
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[slot]);     // accumulators are in registers: the slot can be refilled
-      const int a = fast_div(tile, inv_tb), b0 = (tile - a * TB) << 7;
-      // The tile's 128 hidden lines are contiguous in global memory.  They go through a swizzled shared staging
-      // buffer (conflict-free 16-byte stores) and leave with ONE tensor-map store per tile: a per-thread
-      // st.global.v4 of its own 128-byte line costs 32 LSU wavefronts per warp instruction and made the epilogue the
-      // largest consumer of the LSU data pipe.  Rows past the end of the B grid are clipped by the tensor map.
-      uint8_t* sb = hst + (size_t)(tl & 1) * kNcAtom;
-      if (threadIdx.x == 128) bulk_wait_group_read<1>();        // the store of tile tl-2 has finished reading this buffer
-      asm volatile("bar.sync 2, 128;" ::: "memory");
-      if (b0 + row < p.nB) {
-        const uint32_t so = smem_u32(sb) + (uint32_t)(row * 128);
-        const uint32_t sw = (uint32_t)(row & 7);
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {                    // 8 channels at a time: net 0 ch 0-7, 8-15, net 1 ch 0-7, 8-15
-          float hval[8];
-#pragma unroll
-          for (int c = 0; c < 8; ++c) hval[c] = fmaxf(fmaf(acc[g * 8 + c], inv, __ldg(p.b1p + g * 8 + c)), 0.f) * sh;
-          uint4 hi, lo;
-          split8_bounded(hval, hi, lo);
-          const uint32_t chi = (uint32_t)((g >> 1) * 4 + (g & 1)), clo = chi + 2;        // [net][hi0 hi1 lo0 lo1]
-          sts_v4(so + ((chi ^ sw) << 4), hi.x, hi.y, hi.z, hi.w);
-          sts_v4(so + ((clo ^ sw) << 4), lo.x, lo.y, lo.z, lo.w);
-        }
-      }
-      fence_proxy_async();
-      asm volatile("bar.sync 2, 128;" ::: "memory");
-      if (threadIdx.x == 128) {
-        tma_store_3d(&hstore, sb, 0, b0, a);
-        bulk_commit_group();
-      }
-    }
-    if (threadIdx.x == 128) bulk_wait_group_read<0>();
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
   }
 }
 
 // ------------------------------------------------------------------------------------------------
 // layer 2.  Tile = R rows x TW columns of the B grid of one hidden cell a', both nets, enumerated as MMA rows
 // m = kk * P + ll (pitch P lines).  A tensor-map load brings the tile's block of 128-byte hidden lines -- rows
-// k0-1 .. k0+R, zero-filled outside the grid -- into shared memory in the 128B-swizzled layout tcgen05 reads, and the
+// k0-1 .. k0+R, zero-filled outside the grid -- into shared memory in the 128B-swizzled layout wgmma reads, and the
 // A operand of B-tap (tk, tl) is simply that block starting (tk * P + tl) lines further on:
 //   copies = 1   the block carries its column halo (box TW + 2 wide, P = TW + 2): one load per tile; the two MMA rows
 //                per tile row that fall on the halo are junk and skipped by the epilogue.
 //   copies = 3   one block per column tap tl, loaded with the column origin shifted by tl - 1 (P = TW): no junk rows,
 //                3 loads per tile (wins when TW + 2 would waste too many of the 128 MMA rows, e.g. wB = 64).
-// Tap starts are 128-byte granular, not 1024-byte aligned.  The 128B swizzle -- of TMA writes and of tcgen05 operand
-// reads alike -- is a pure function of the shared-memory ADDRESS bits (chunk ^= address bits 7..9), so a descriptor
-// that starts mid-pattern reads consistently with its "base offset" field left 0 (measured: with the field set to the
-// start's phase the results are wrong, with 0 they are exact for every shift; tools/nc_debug.py).
+// Tap starts are 128-byte granular, not 1024-byte aligned.  The 128B swizzle -- of TMA writes and of tensor-core
+// operand reads alike -- is a pure function of the shared-memory ADDRESS bits (chunk ^= address bits 7..9), so a
+// descriptor that starts mid-pattern reads consistently with its "base offset" field left 0.
 // Per tap and net: a_hi x [w_hi | w_lo] (one N = 32 MMA gives hi*hi and hi*lo) and a_lo x w_hi (N = 16): four
 // independent accumulator chains per tile, summed by the epilogue.
-// 256 threads (warp 1 MMA, 2 TMEM, 3 loader, 4..7 epilogue); ring of block buffers; two CTAs per SM when the ring fits
-// twice (each with two of the TMEM accumulator slots): the kernel is bound by the tensor cores' shared-memory operand
-// fetch of its many tiny MMAs, which two interleaved streams keep busier than one (105 -> 92 us).
+// 384 threads (warp 3 loader, warps 4..11 = two consumer warpgroups, MMA + epilogue); ring of block buffers; two CTAs
+// per SM when the ring fits twice, so that one CTA's epilogue overlaps the other's MMAs.
 // ------------------------------------------------------------------------------------------------
 constexpr int kL2MaxRing = 8;
 constexpr int kL2WTap = 32 * 128;     // weight image per B-tap: rows 0..15 w_hi (9 used), 16..31 w_lo; K16 slice = net
 
 template <int COPIES, int CTAS>
-__global__ void __launch_bounds__(256, CTAS) nc_l2_umma_kernel(const __grid_constant__ NcParams p,
+__global__ void __launch_bounds__(384, CTAS) nc_l2_umma_kernel(const __grid_constant__ NcParams p,
                                                             const __grid_constant__ CUtensorMap hmap) {
-  constexpr uint32_t IDESC32 = make_idesc_f16(128, 32), IDESC16 = make_idesc_f16(128, 16);
-  constexpr int SLOTS = CTAS == 1 ? kNcSlots : 2;      // two CTAs per SM share the 512 TMEM columns
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* wsm = smem + (size_t)p.ring * p.unit_bytes;      // [9 taps][32 rows][64] weight images, 36 KB
   __shared__ __align__(8) uint64_t full_bar[kL2MaxRing];
   __shared__ __align__(8) uint64_t empty_bar[kL2MaxRing];
-  __shared__ __align__(8) uint64_t tfull_bar[SLOTS];
-  __shared__ __align__(8) uint64_t tempty_bar[SLOTS];
-  __shared__ uint32_t tmem_base_smem;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles = p.tiles, ring = p.ring;
@@ -427,27 +382,19 @@ __global__ void __launch_bounds__(256, CTAS) nc_l2_umma_kernel(const __grid_cons
   const int per_a = p.KB * p.LB;
   const float inv_pa = 1.f / (float)per_a, inv_lb = 1.f / (float)p.LB;
 
-  for (int i = threadIdx.x; i < ring * p.unit_bytes / 16; i += 256) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
-  for (int i = threadIdx.x; i < 9 * kL2WTap / 16; i += 256)
+  for (int i = threadIdx.x; i < ring * p.unit_bytes / 16; i += 384) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
+  for (int i = threadIdx.x; i < 9 * kL2WTap / 16; i += 384)
     reinterpret_cast<uint4*>(wsm)[i] = __ldg(reinterpret_cast<const uint4*>(p.wimg) + i);
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < kL2MaxRing; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < SLOTS; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], 4);
+      mbar_init(&empty_bar[i], 2);
     }
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(&tmem_base_smem, SLOTS * 128);
   if (warp == 3 && lane == 0) tma_prefetch_desc(&hmap);
   fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
 
   if (warp == 3) {
     // ===================== loader =====================
@@ -466,88 +413,70 @@ __global__ void __launch_bounds__(256, CTAS) nc_l2_umma_kernel(const __grid_cons
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer: the whole warp runs the loop (uniform), one elected lane issues =====================
-    int u = 0, tl = 0;
+  } else if (warp >= 4) {
+    // ===================== MMA + epilogue: warpgroup wg owns MMA rows 64 wg .. 64 wg + 63 =====================
+    const int wg = (warp >> 2) - 1, wl = warp & 3;
+    const int t = lane & 3;
+    const int m0 = wg * 64 + 16 * wl + (lane >> 2);          // fragment rows m0 and m0 + 8
+    float sx, sh;
+    nc_scales(p, sx, sh);
+    const float inv = p.inv_sw2 / sh;
     const uint32_t wbase = smem_u32(wsm), sbase = smem_u32(smem);
     const uint32_t tk_stride = (uint32_t)(p.P * 128);
-    for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++tl) {
-      const int slot = tl % SLOTS;
-      mbar_wait(&tempty_bar[slot], ((uint32_t)(tl / SLOTS) & 1u) ^ 1u);
-      tc_fence_after();
-      const uint32_t d_slot = tmem_base + (uint32_t)(slot * 128);   // [0,64) hi products of net 0 | 1, [64,96) lo*hi
+    int u = 0;
+    for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+      float da[2][16], db[2][8];       // per net: [0,8) hi*hi, [8,16) hi*lo fragments ; lo*hi
 #pragma unroll
       for (int c = 0; c < COPIES; ++c, ++u) {
         const int s = u % ring;
         mbar_wait(&full_bar[s], (uint32_t)(u / ring) & 1u);
-        tc_fence_after();
-        const uint32_t blk = sbase + (uint32_t)(s * p.unit_bytes);
-        if (elect_one()) {
+        const uint32_t blk = sbase + (uint32_t)(s * p.unit_bytes) + (uint32_t)(wg * 64 * 128);
+        wgmma_fence();
 #pragma unroll
-          for (int j = 0; j < (COPIES == 1 ? 3 : 1); ++j) {        // taps in (tl outer, tk inner) order for either layout
-            const int tlx = COPIES == 1 ? j : c;
+        for (int j = 0; j < (COPIES == 1 ? 3 : 1); ++j) {        // taps in (tl outer, tk inner) order for either layout
+          const int tlx = COPIES == 1 ? j : c;
 #pragma unroll
-            for (int tk = 0; tk < 3; ++tk) {
-              // 128-byte granular start, base offset 0 (see above)
-              const uint64_t adesc = make_sw128_desc(blk + (uint32_t)tk * tk_stride + (COPIES == 1 ? (uint32_t)(tlx * 128) : 0u));
-              const uint64_t wdesc = make_sw128_desc(wbase + (uint32_t)((tk * 3 + tlx) * kL2WTap));
-              const uint32_t acc = (tlx > 0 || tk > 0) ? 1u : 0u;
+          for (int tk = 0; tk < 3; ++tk) {
+            // 128-byte granular start, base offset 0 (see above)
+            const uint64_t adesc = make_sw128_desc(blk + (uint32_t)tk * tk_stride + (COPIES == 1 ? (uint32_t)(tlx * 128) : 0u));
+            const uint64_t wdesc = make_sw128_desc(wbase + (uint32_t)((tk * 3 + tlx) * kL2WTap));
+            const uint32_t acc = (tlx > 0 || tk > 0) ? 1u : 0u;
 #pragma unroll
-              for (int net = 0; net < 2; ++net) {
-                umma_f16(d_slot + (uint32_t)(net * 32), adesc + 2 * (net * 2), wdesc + 2 * net, IDESC32, acc);           // hi*hi | hi*lo
-                umma_f16(d_slot + (uint32_t)(64 + net * 16), adesc + 2 * (net * 2 + 1), wdesc + 2 * net, IDESC16, acc);  // lo*hi
-              }
+            for (int net = 0; net < 2; ++net) {
+              wgmma_f16<32>(da[net], adesc + 2 * (net * 2), wdesc + 2 * net, acc);       // hi*hi | hi*lo
+              wgmma_f16<16>(db[net], adesc + 2 * (net * 2 + 1), wdesc + 2 * net, acc);   // lo*hi
             }
           }
-          umma_commit(&empty_bar[s]);
-          if (c == COPIES - 1) umma_commit(&tfull_bar[slot]);
         }
-        __syncwarp();
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs<16>(da[0]);
+        wgmma_fence_regs<16>(da[1]);
+        wgmma_fence_regs<8>(db[0]);
+        wgmma_fence_regs<8>(db[1]);
+        if (threadIdx.x % 128 == 0) mbar_arrive(&empty_bar[s]);
       }
-    }
-  } else if (warp >= 4) {
-    // ===================== epilogue =====================
-    const int q = warp & 3;
-    const int m = q * 32 + lane;
-    const int kk = m / p.P, ll = m - kk * p.P;
-    float sx, sh;
-    nc_scales(p, sx, sh);
-    const float inv = p.inv_sw2 / sh;
-    int tl = 0;
-    for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++tl) {
-      const int slot = tl % SLOTS;
-      mbar_wait(&tfull_bar[slot], (uint32_t)(tl / SLOTS) & 1u);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(slot * 128);
-      float acc[2][9];
-#pragma unroll
-      for (int net = 0; net < 2; ++net) {
-        float da[32], db[16];
-        tmem_ld32(taddr + net * 32, da);                     // [0,16) hi*hi, [16,32) hi*lo
-        tmem_ld16(taddr + 64 + net * 16, db);                // lo*hi
-#pragma unroll
-        for (int d = 0; d < 9; ++d) acc[net][d] = (db[d] + da[16 + d]) + da[d];
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[slot]);
       const int a = fast_div(tile, inv_pa), rem = tile - a * per_a;
       const int kb = fast_div(rem, inv_lb), lb = rem - kb * p.LB;
-      const int k = kb * p.R + kk, l = lb * p.TW + ll;
-      if (kk < p.R && ll < p.TW && k < p.hB && l < p.wB) {
-        const size_t v = (size_t)a * p.nB + (size_t)k * p.wB + l;
 #pragma unroll
-        for (int net = 0; net < 2; ++net)
+      for (int h = 0; h < 2; ++h) {
+        const int m = m0 + 8 * h;
+        const int kk = m / p.P, ll = m - kk * p.P;
+        const int k = kb * p.R + kk, l = lb * p.TW + ll;
+        if (kk < p.R && ll < p.TW && k < p.hB && l < p.wB) {
+          const size_t v = (size_t)a * p.nB + (size_t)k * p.wB + l;
 #pragma unroll
-          for (int d = 0; d < 9; ++d) p.partial[(size_t)(net * 9 + d) * p.V + v] = acc[net][d] * inv;
+          for (int net = 0; net < 2; ++net)
+#pragma unroll
+            for (int j = 0; j < 2; ++j)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const int d = 8 * j + 2 * t + e, i = 4 * j + 2 * h + e;
+                if (d < 9) p.partial[(size_t)(net * 9 + d) * p.V + v] = ((db[net][i] + da[net][8 + i]) + da[net][i]) * inv;
+              }
+        }
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, SLOTS * 128);
   }
 }
 
@@ -783,7 +712,7 @@ static void nc_l2_geometry(int hB, int wB, int mode, int ctas, NcParams& p) {
 // x [hA*wA][hB*wB] -> out (NeighConsensus output); rowmax / colmax (optional) receive the maxima MutualMatching needs.
 // xmax: device word holding the float bits of max |x| (launch_absmax or the fused mutual_apply pass).
 // xp: scratch of nc_umma_xp_bytes().  l2_mode: 0 auto, 1 one haloed block per tile, 2 one block per column tap; + 8: one
-// layer-2 CTA per SM with four TMEM slots instead of two CTAs with two slots each (105 vs 92 us at 640x480).
+// layer-2 CTA per SM instead of two.
 int launch_neigh_consensus_umma(const float* x, int hA, int wA, int hB, int wB, const NcUmmaWeights& W, const float* b1p,
                                 float b2, const unsigned int* xmax, uint32_t* xp, __half* hidden, float* partial,
                                 float* out, float* rowmax, unsigned int* colmax, int l2_mode, int num_sms, cudaStream_t st) {
@@ -839,7 +768,7 @@ int launch_neigh_consensus_umma(const float* x, int hA, int wA, int hB, int wB, 
   {                                               \
     auto k = nc_l2_umma_kernel<C, T>;             \
     P2P_ENSURE_SMEM(k, smem);                     \
-    k<<<grid, 256, smem, st>>>(p, hmap);          \
+    k<<<grid, 384, smem, st>>>(p, hmap);          \
   }
     if (p.copies == 1 && p.l2_ctas == 1) P2P_NC_L2_LAUNCH(1, 1)
     else if (p.copies == 1) P2P_NC_L2_LAUNCH(1, 2)

@@ -1,24 +1,17 @@
-// tcgen05 implicit-GEMM kernel for sm_100a: TMA-staged fp16 operand tiles in shared memory
-// (128B swizzle, K-major), tcgen05.mma (kind::f16, fp32 accumulate) into TMEM, tcgen05.ld epilogue.
+// wgmma implicit-GEMM kernel for sm_90a: TMA-staged fp16 operand tiles in shared memory (128B swizzle,
+// K-major), wgmma.mma_async (f16 inputs, fp32 accumulate in registers), shared-memory-staged epilogue.
 //
-// One kernel serves three contractions of the Patch2Pix hot path (reference file:line):
+// One kernel serves four contractions of the Patch2Pix hot path (reference file:line):
 //   conv1 of FeatRegressNet  (Conv2d 518->512 k3 s2 p1 + BN)       networks/modules.py:76-87,103-105
 //   conv2 of FeatRegressNet  (Conv2d 512->512 k3 s1 p1 + BN, ReLU, MaxPool 8)   same
+//   the two big Linear layers of the regressor head (+ BN1d, ReLU)
 //   FeatCorrelation + maxpool4d (C x n1 x n2 contraction + 2^4 max)  networks/modules.py:11-53
 //
 // Precision: operands are fp16 "hi" (+ optional fp16 "lo" residual) pairs of scaled fp32 values.
 //   PASSES = 1:  hi*hi                      (fp16-grade inputs, fp32 accumulate)
 //   PASSES = 3:  lo*hi + hi*lo + hi*hi      (~2^-22 relative products, i.e. fp32-grade)
-// SEGMENTED accumulation: the tensor core accumulates only `seg_len` k-steps at a time in TMEM;
-// the epilogue warps drain each partial sum and add it to fp32 register totals with
-// round-to-nearest, which bounds the accumulator-rounding drift of long K chains.
-//
-// CTA = 384 threads: warp 0 TMA producer, warp 1 MMA issuer, warp 2 TMEM allocator, warp 3 idle,
-// warps 4..11 epilogue (TMEM lane quadrant = warp % 4, column half = (warp-4)/4).
-// Tile = 128 rows x 256 columns, K chunk 64 (one 128-byte swizzle row); two TMEM accumulator
-// slots (2 x 256 columns) so the drain of one segment/tile overlaps the MMAs of the next.
-// PAIR variants (default for the conv launches): clusters of two CTAs issue tcgen05.mma.cta_group::2
-// (M = 256 over the two SMs of a TPC, B split between their shared memories); see the kernel comment.
+// SEGMENTED accumulation: the tensor core accumulates only `seg_len` k-steps at a time; each partial sum is
+// added to fp32 register totals with round-to-nearest, which bounds the accumulator-rounding drift of long K chains.
 #include <cuda.h>
 
 #include <vector>
@@ -138,7 +131,18 @@ __device__ __forceinline__ void epilogue_piece(const UmmaEpilogue& e, int n_patc
 // the kernel
 // ------------------------------------------------------------------------------------------------
 constexpr int kATile = 128 * 128;   // 128 rows x 64 fp16
-constexpr int kBTile = 256 * 128;   // 256 rows x 64 fp16
+constexpr int kBTile = 128 * 128;   // 128 output columns x 64 fp16
+constexpr int kEpiPitch = 65;       // floats per staged accumulator row: row-wise reads hit 32 distinct banks
+constexpr int kEpiBytes = 64 * kEpiPitch * 4;
+
+template <int PASSES, int AMODE>
+struct GemmCfg {
+  static constexpr int NOP = PASSES == 3 ? 2 : 1;
+  static constexpr int STAGE_BYTES = NOP * (kATile + kBTile);
+  static constexpr int STAGES = PASSES == 3 ? 3 : (AMODE == AMODE_TMA ? 6 : 4);
+  static constexpr int THREADS = AMODE == AMODE_TMA ? 384 : 512;
+  static constexpr int SMEM = STAGES * STAGE_BYTES + 2 * kEpiBytes + 1024;
+};
 
 __device__ __forceinline__ int fg_clamp(int v, int ds, int full) {   // ((x+dx)//ds).clamp(0, full//ds-1)
   if (v < 0) return 0;
@@ -146,30 +150,38 @@ __device__ __forceinline__ int fg_clamp(int v, int ds, int full) {   // ((x+dx)/
   return q < m ? q : m;
 }
 
-// FUSED (conv1, 1-pass): warps 12..15 are A-operand producers that gather, normalise and convert the
-// patch windows straight into the swizzled shared-memory tile (select_local_patch_feats + patch
-// L2Normalize, networks/utils.py:4-36, networks/patch2pix.py:173-178); TMA then only streams the weights.
-// PAIR: two CTAs of a cluster (one TPC) share every tile step through tcgen05.mma.cta_group::2 -- an M=256
-// (2 x 128 rows) x N=256 instruction whose B operand is split between the two CTAs' shared memories, so each
-// SM ingests 16 KB A + 16 KB B per k-step instead of 16 + 32 and the ring holds 6 (3 for 3-pass) stages.
-template <int PASSES, bool SEGMENTED, int EPI, bool FUSED, bool PAIR>
-__global__ void __launch_bounds__(FUSED ? 512 : 384, 1) umma_gemm_kernel(const __grid_constant__ UmmaGemmParams p) {
-  static_assert(!FUSED || (PASSES == 1 && !SEGMENTED && EPI == EPI_CONV1), "fused gather: conv1, 1-pass only");
-  static_assert(!(FUSED && PAIR), "the fused-gather variant is single-CTA");
-  constexpr int BT = PAIR ? kBTile / 2 : kBTile;      // B rows held by this CTA: 128 of the 256 when paired
-  constexpr int STAGES = PAIR ? ((PASSES == 3) ? 3 : 6) : ((PASSES == 3) ? 2 : 4);
-  constexpr int NOP = (PASSES == 3) ? 2 : 1;
-  constexpr int STAGE_BYTES = NOP * (kATile + BT);
-  constexpr uint32_t IDESC = make_idesc_f16(PAIR ? 256 : 128, 256);
+__device__ __forceinline__ void named_bar(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+
+// Tile = 128 rows x 128 columns; K chunk 64 (one 128-byte swizzle row) per pipeline stage.
+// Warpgroup 0: warp 0 is the TMA producer.  Warpgroups 1 and 2: wgmma consumers, rows 0..63 and 64..127, fp32
+// accumulators in registers; their epilogue stages the accumulators through shared memory so that every epilogue
+// thread owns one tile row (32 consecutive columns per piece), the layout epilogue_piece expects.
+// Warpgroup 3 (conv1 1-pass only) builds the A operand:
+//   AMODE_GATHER  gathers, normalises and converts the patch windows straight into the swizzled stage
+//                 (select_local_patch_feats + patch L2Normalize, networks/utils.py:4-36, networks/patch2pix.py:173-178);
+//   AMODE_WINDOW  the A boxes come by TMA from the per-image window maps (one strided box {64 ch, 8 px stride 2, 8 px
+//                 stride 2} per patch and tap); these warps restore the conv's zero padding -- window pixel -1 must
+//                 contribute 0, but the box holds the neighbouring image pixel there -- by zeroing the affected rows,
+//                 and build the rgb k-step (54 real K values) as an im2col of the normalised rgb map.
+// Both A modes produce bit-identical operands and the same MMA sequence per output element.
+// PASSES = 3: lo*hi + hi*lo + hi*hi into one accumulator.  SEGMENTED: the accumulator restarts every `seg_len`
+// k-steps and each partial sum is added to fp32 register totals with round-to-nearest, which bounds the
+// accumulator-rounding drift of long K chains.
+template <int PASSES, bool SEGMENTED, int EPI, int AMODE>
+__global__ void __launch_bounds__(GemmCfg<PASSES, AMODE>::THREADS, 1) umma_gemm_kernel(const __grid_constant__ UmmaGemmParams p) {
+  static_assert(AMODE == AMODE_TMA || (PASSES == 1 && !SEGMENTED && EPI == EPI_CONV1), "fused A operand: conv1, 1-pass only");
+  using Cfg = GemmCfg<PASSES, AMODE>;
+  constexpr int STAGES = Cfg::STAGES, NOP = Cfg::NOP, STAGE_BYTES = Cfg::STAGE_BYTES;
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  __shared__ __align__(8) uint64_t full_bar[STAGES];
-  __shared__ __align__(8) uint64_t empty_bar[STAGES];
-  __shared__ __align__(8) uint64_t tfull_bar[2];
-  __shared__ __align__(8) uint64_t tempty_bar[2];
-  __shared__ uint32_t tmem_base_smem;
-  constexpr int FG = FUSED ? 16 : 1;
+  float* epi_smem = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);
+  __shared__ __align__(8) uint64_t full_bar[STAGES];    // TMA bytes landed (+ gather warps in AMODE_GATHER)
+  __shared__ __align__(8) uint64_t ready_bar[STAGES];   // AMODE_WINDOW: the aux warps have fixed the stage up
+  __shared__ __align__(8) uint64_t empty_bar[STAGES];   // both consumer warpgroups are done reading the stage
+  constexpr int FG = AMODE == AMODE_GATHER ? 16 : 1;
   __shared__ float fg_dinv[2][2][FG][FG];               // act_scale / patch norm per (patch, image, window pixel)
   __shared__ int fg_org[2][4];                          // window origins (x1,y1,x2,y2) - 8
 
@@ -180,18 +192,18 @@ __global__ void __launch_bounds__(FUSED ? 512 : 384, 1) umma_gemm_kernel(const _
     n_units = __ldg(p.d_units);
     m_tiles = (n_units + p.a_units_per_tile - 1) / p.a_units_per_tile;
   }
-  // paired: a "tile" is two consecutive 128-row m-tiles (one per CTA of the cluster) x one 256-column n-tile
-  const int rank = PAIR ? (int)cluster_ctarank() : 0;
-  const int cta0 = PAIR ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int ctas = PAIR ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-  const int total_tiles = (PAIR ? (m_tiles + 1) / 2 : m_tiles) * p.n_tiles;
+  const int n_halves = 2 * p.n_tiles;                    // 128-column tiles
+  const int total_tiles = m_tiles * n_halves;
   const int nsteps = p.nsteps;
   const int seg_len = SEGMENTED ? p.seg_len : nsteps;
-  const int nseg = (nsteps + seg_len - 1) / seg_len;
 
   if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&p.a_main_hi);
     tma_prefetch_desc(&p.b_hi);
+    if (AMODE == AMODE_TMA) tma_prefetch_desc(&p.a_main_hi);
+    if (AMODE == AMODE_WINDOW) {
+      tma_prefetch_desc(&p.wm.map[0]);
+      tma_prefetch_desc(&p.wm.map[1]);
+    }
     if (PASSES == 3) {
       tma_prefetch_desc(&p.a_main_lo);
       tma_prefetch_desc(&p.b_lo);
@@ -199,140 +211,165 @@ __global__ void __launch_bounds__(FUSED ? 512 : 384, 1) umma_gemm_kernel(const _
   }
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&full_bar[i], FUSED ? 257 : 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], FUSED ? 4 : (PAIR ? 16 : 8));   // paired: the epilogue warps of both CTAs
+      mbar_init(&full_bar[i], AMODE == AMODE_GATHER ? 5 : 1);
+      mbar_init(&ready_bar[i], 4);
+      mbar_init(&empty_bar[i], 2);
     }
     fence_barrier_init();
   }
-  if (warp == 2) {
-    if (PAIR) tmem_alloc_pair(&tmem_base_smem, 512);
-    else tmem_alloc(&tmem_base_smem, 512);
-  }
-  tc_fence_before();
-  if (PAIR) cluster_sync_all();      // the peer's barriers must exist before any remote arrive / TMA completion
-  else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
+  __syncthreads();
 
-  if (warp < 4) {
-    if (SEGMENTED) asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
+  // AMODE_WINDOW: window origin of patch n in padded map coordinates: window pixel (wy, wx) lives at (oy + wy, ox + wx).
+  // Truncation = `.long()` (networks/utils.py:19); clamping the origin to [-7, W + 8] leaves every clamped window
+  // pixel unchanged (beyond that all of them sit on the border pixel) and keeps the boxes inside the padded map.
+  auto origin = [&](int n, int j) -> int {
+    if (n >= n_units) n = 0;      // past the end (odd patch counts): any valid patch, the epilogue discards the rows
+    int v;
+    if (p.wm.is_float) v = (int)reinterpret_cast<const float*>(p.wm.matches)[(size_t)n * 4 + j];
+    else v = (int)reinterpret_cast<const long long*>(p.wm.matches)[(size_t)n * 4 + j];
+    const int lim = (j & 1) ? p.wm.H[j >> 1] : p.wm.W[j >> 1];
+    v = v < -7 ? -7 : (v > lim + 8 ? lim + 8 : v);
+    return v - 8 + kMapPad;
+  };
+
   if (warp == 0) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       int it = 0;
-      for (int tile = cta0; tile < total_tiles; tile += ctas) {
-        const int mt = tile / p.n_tiles, n_tile = tile - mt * p.n_tiles;
-        const int m_tile = PAIR ? mt * 2 + rank : mt;     // past the last m-tile (odd count): TMA zero-fills
+      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+        const int m_tile = tile / n_halves, brow = (tile - m_tile * n_halves) * 128;
+        const int a4 = m_tile * p.a_units_per_tile;
+        int o[2][4];
+        if (AMODE == AMODE_WINDOW) {
+#pragma unroll
+          for (int pp = 0; pp < 2; ++pp)
+#pragma unroll
+            for (int j = 0; j < 4; ++j) o[pp][j] = origin(m_tile * 2 + pp, j);
+        }
         for (int ks = 0; ks < nsteps; ++ks, ++it) {
           const int s = it % STAGES;
-          const uint32_t ph = (uint32_t)(it / STAGES) & 1u;
-          mbar_wait(&empty_bar[s], ph ^ 1u);
+          mbar_wait(&empty_bar[s], ((uint32_t)(it / STAGES) & 1u) ^ 1u);
           const KStep k = p.steps[ks];  // param space (constant bank)
           uint8_t* st = smem + (size_t)s * STAGE_BYTES;
-          if (FUSED) {
+          if (AMODE == AMODE_GATHER) {
             mbar_expect_tx(&full_bar[s], kBTile);
-            tma_load_2d(&p.b_hi, &full_bar[s], st + kATile, k.bk, n_tile * 256);
-            continue;
-          }
-          const int a4 = m_tile * p.a_units_per_tile;
-          if (PAIR) {
-            // both CTAs' bytes complete on the leader's barrier; its single arrival carries the whole count
-            if (rank == 0) mbar_expect_tx(&full_bar[s], 2 * STAGE_BYTES);
-            const int brow = n_tile * 256 + rank * 128;
+            tma_load_2d(&p.b_hi, &full_bar[s], st + kATile, k.bk, brow);
+          } else if (AMODE == AMODE_WINDOW) {
+            mbar_expect_tx(&full_bar[s], k.kind == 0 ? kATile + kBTile : kBTile);
+            tma_load_2d(&p.b_hi, &full_bar[s], st + kATile, k.bk, brow);
             if (k.kind == 0) {
-              tma_load_5d_pair(&p.a_main_hi, &full_bar[s], st, k.c0, k.x, k.y, k.plane, a4);
-              if (PASSES == 3) tma_load_5d_pair(&p.a_main_lo, &full_bar[s], st + kATile, k.c0, k.x, k.y, k.plane, a4);
-            } else {
-              tma_load_5d_pair(&p.a_rgb_hi, &full_bar[s], st, 0, 0, 0, 0, a4);
-              if (PASSES == 3) tma_load_5d_pair(&p.a_rgb_lo, &full_bar[s], st + kATile, 0, 0, 0, 0, a4);
+              const int ty = (k.plane & 2) ? 1 : (k.y < 0 ? 0 : 2), tx = (k.plane & 1) ? 1 : (k.x < 0 ? 0 : 2);
+              const int chunk = k.c0 >> 6, si = chunk >> 2, c0 = (chunk & 3) * 64;
+#pragma unroll
+              for (int pp = 0; pp < 2; ++pp)
+                tma_load_3d(&p.wm.map[si], &full_bar[s], st + pp * 8192, c0, o[pp][2 * si] - 1 + tx, o[pp][2 * si + 1] - 1 + ty);
             }
-            tma_load_2d_pair(&p.b_hi, &full_bar[s], st + NOP * kATile, k.bk, brow);
-            if (PASSES == 3) tma_load_2d_pair(&p.b_lo, &full_bar[s], st + NOP * kATile + BT, k.bk, brow);
-            continue;
-          }
-          mbar_expect_tx(&full_bar[s], STAGE_BYTES);
-          if (k.kind == 0) {
-            tma_load_5d(&p.a_main_hi, &full_bar[s], st, k.c0, k.x, k.y, k.plane, a4);
-            if (PASSES == 3) tma_load_5d(&p.a_main_lo, &full_bar[s], st + kATile, k.c0, k.x, k.y, k.plane, a4);
           } else {
-            tma_load_5d(&p.a_rgb_hi, &full_bar[s], st, 0, 0, 0, 0, a4);
-            if (PASSES == 3) tma_load_5d(&p.a_rgb_lo, &full_bar[s], st + kATile, 0, 0, 0, 0, a4);
+            mbar_expect_tx(&full_bar[s], STAGE_BYTES);
+            if (k.kind == 0) {
+              tma_load_5d(&p.a_main_hi, &full_bar[s], st, k.c0, k.x, k.y, k.plane, a4);
+              if (PASSES == 3) tma_load_5d(&p.a_main_lo, &full_bar[s], st + kATile, k.c0, k.x, k.y, k.plane, a4);
+            } else {
+              tma_load_5d(&p.a_rgb_hi, &full_bar[s], st, 0, 0, 0, 0, a4);
+              if (PASSES == 3) tma_load_5d(&p.a_rgb_lo, &full_bar[s], st + kATile, 0, 0, 0, 0, a4);
+            }
+            tma_load_2d(&p.b_hi, &full_bar[s], st + NOP * kATile, k.bk, brow);
+            if (PASSES == 3) tma_load_2d(&p.b_lo, &full_bar[s], st + NOP * kATile + kBTile, k.bk, brow);
           }
-          tma_load_2d(&p.b_hi, &full_bar[s], st + NOP * kATile, k.bk, n_tile * 256);
-          if (PASSES == 3) tma_load_2d(&p.b_lo, &full_bar[s], st + NOP * kATile + kBTile, k.bk, n_tile * 256);
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (paired: the leader CTA issues for both) =====================
-    if (lane == 0 && rank == 0) {
-      int it = 0, seg = 0;
-      for (int tile = cta0; tile < total_tiles; tile += ctas) {
-        uint32_t d_tmem = 0;
-        for (int ks = 0; ks < nsteps; ++ks, ++it) {
-          const bool seg_start = (ks % seg_len) == 0;
-          if (seg_start) {
-            const int slot = seg & 1;
-            const uint32_t sph = (uint32_t)(seg >> 1) & 1u;
-            mbar_wait(&tempty_bar[slot], sph ^ 1u);
-            tc_fence_after();
-            d_tmem = tmem_base + (uint32_t)slot * 256u;
-          }
-          const int s = it % STAGES;
-          const uint32_t ph = (uint32_t)(it / STAGES) & 1u;
-          mbar_wait(&full_bar[s], ph);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + (size_t)s * STAGE_BYTES);
-          const uint64_t a_hi = make_sw128_desc(sa);
-          const uint64_t b_hi = make_sw128_desc(sa + NOP * kATile);
-          uint32_t acc = seg_start ? 0u : 1u;
-          auto mma = [&](uint64_t a, uint64_t b, uint32_t accum) {
-            if (PAIR) umma_f16_pair(d_tmem, a, b, IDESC, accum);
-            else umma_f16(d_tmem, a, b, IDESC, accum);
-          };
-          if (PASSES == 3) {
-            const uint64_t a_lo = make_sw128_desc(sa + kATile);
-            const uint64_t b_lo = make_sw128_desc(sa + NOP * kATile + BT);
+  } else if (warp >= 4 && warp < 12) {
+    // ===================== wgmma consumers + epilogue (warpgroups 1 and 2) =====================
+    const int wg = (warp >> 2) - 1, wl = warp & 3;
+    uint64_t* ready = AMODE == AMODE_WINDOW ? ready_bar : full_bar;
+    float* stg = epi_smem + wg * (64 * kEpiPitch);
+    float acc[64];
+    float tot[SEGMENTED ? 64 : 1];
+    int it = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      const int m_tile = tile / n_halves, col0 = (tile - m_tile * n_halves) * 128;
+      if (SEGMENTED) {
 #pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {
-              mma(a_lo + 2 * kk, b_hi + 2 * kk, acc);
-              acc = 1u;
-            }
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) mma(a_hi + 2 * kk, b_lo + 2 * kk, 1u);
-          }
+        for (int i = 0; i < 64; ++i) tot[i] = 0.f;
+      }
+      int prev_s = -1;
+      for (int ks = 0; ks < nsteps; ++ks, ++it) {
+        const int s = it % STAGES;
+        mbar_wait(&ready[s], (uint32_t)(it / STAGES) & 1u);
+        const uint32_t sa = smem_u32(smem + (size_t)s * STAGE_BYTES);
+        const uint64_t a_hi = make_sw128_desc(sa + wg * 8192);
+        const uint64_t b_hi = make_sw128_desc(sa + NOP * kATile);
+        uint32_t accf = (ks % seg_len) == 0 ? 0u : 1u;
+        wgmma_fence();
+        if (PASSES == 3) {
+          const uint64_t a_lo = make_sw128_desc(sa + kATile + wg * 8192);
+          const uint64_t b_lo = make_sw128_desc(sa + NOP * kATile + kBTile);
 #pragma unroll
           for (int kk = 0; kk < 4; ++kk) {
-            mma(a_hi + 2 * kk, b_hi + 2 * kk, acc);
-            acc = 1u;
+            wgmma_f16<128>(acc, a_lo + 2 * kk, b_hi + 2 * kk, accf);
+            accf = 1u;
           }
-          if (PAIR) umma_commit_pair(&empty_bar[s]);
-          else umma_commit(&empty_bar[s]);
-          const bool seg_end = ((ks + 1) % seg_len) == 0 || (ks + 1) == nsteps;
-          if (seg_end) {
-            if (PAIR) umma_commit_pair(&tfull_bar[seg & 1]);
-            else umma_commit(&tfull_bar[seg & 1]);
-            ++seg;
+#pragma unroll
+          for (int kk = 0; kk < 4; ++kk) wgmma_f16<128>(acc, a_hi + 2 * kk, b_lo + 2 * kk, 1u);
+        }
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+          wgmma_f16<128>(acc, a_hi + 2 * kk, b_hi + 2 * kk, accf);
+          accf = 1u;
+        }
+        wgmma_commit();
+        const bool seg_end = ((ks + 1) % seg_len) == 0 || (ks + 1) == nsteps;
+        if (seg_end) {
+          wgmma_wait<0>();
+          wgmma_fence_regs<64>(acc);
+          if (prev_s >= 0 && threadIdx.x % 128 == 0) mbar_arrive(&empty_bar[prev_s]);
+          if (threadIdx.x % 128 == 0) mbar_arrive(&empty_bar[s]);
+          prev_s = -1;
+          if (SEGMENTED) {
+#pragma unroll
+            for (int i = 0; i < 64; ++i) tot[i] += acc[i];
           }
+        } else {
+          wgmma_wait<1>();          // the previous k-step's MMAs are done: its stage can be refilled
+          if (prev_s >= 0 && threadIdx.x % 128 == 0) mbar_arrive(&empty_bar[prev_s]);
+          prev_s = s;
         }
       }
+      const float* res = SEGMENTED ? tot : acc;
+      // fragment -> row-major staging, 64 columns at a time; then one row per thread
+      const int fr = 16 * wl + (lane >> 2), fc = 2 * (lane & 3);
+      const int er = (wl & 1) * 32 + lane, ec = (wl >> 1) * 32;
+#pragma unroll
+      for (int half = 0; half < 2; ++half) {
+        named_bar(1 + wg, 128);                 // the previous piece has been read
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float* d = res + 4 * (half * 8 + j);
+          float* o = stg + fr * kEpiPitch + 8 * j + fc;
+          o[0] = d[0];
+          o[1] = d[1];
+          o[8 * kEpiPitch] = d[2];
+          o[8 * kEpiPitch + 1] = d[3];
+        }
+        named_bar(1 + wg, 128);
+        float v[32];
+#pragma unroll
+        for (int i = 0; i < 32; ++i) v[i] = stg[er * kEpiPitch + ec + i];
+        epilogue_piece<EPI>(p.epi, n_units, m_tile, wg * 64 + er, col0 + half * 64 + ec, v);
+      }
     }
-  }
-  } else if (FUSED && warp >= 8) {
-    // ===================== fused A-operand producers (8 warps, 256 threads) =====================
-    // 8 lanes per tile row (8 channels = 16 B each), 32 rows per pass, 4 passes per k-step.  Warps
-    // drift across pipeline stages independently, which hides the L2 latency of the gathers.
-    const int ptid = threadIdx.x - 256;
-    const int l8 = ptid & 7, r32 = ptid >> 3;
+  } else if (AMODE == AMODE_GATHER && warp >= 12) {
+    // ===================== fused A-operand producers (warpgroup 3) =====================
+    // 8 lanes per tile row (8 channels = 16 B each), 16 rows per pass, 8 passes per k-step.  Warps drift across
+    // pipeline stages independently, which hides the L2 latency of the gathers.
+    const int ptid = threadIdx.x - 384;
+    const int l8 = ptid & 7, r16 = ptid >> 3;
     const FusedGather& g = p.fg;
     int it = 0;
-    for (int tile = cta0; tile < total_tiles; tile += ctas) {
-      const int m_tile = tile / p.n_tiles;
-      asm volatile("bar.sync 1, 256;" ::: "memory");   // nobody still reads the previous tile's tables
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      const int m_tile = tile / n_halves;
+      named_bar(3, 128);   // nobody still reads the previous tile's tables
       if (ptid < 8) {
         const int pp = ptid >> 2, j = ptid & 3;
         const int n = m_tile * 2 + pp;
@@ -345,8 +382,8 @@ __global__ void __launch_bounds__(FUSED ? 512 : 384, 1) umma_gemm_kernel(const _
         }
         fg_org[pp][j] = v - 8;
       }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      for (int i = ptid; i < 1024; i += 256) {
+      named_bar(3, 128);
+      for (int i = ptid; i < 1024; i += 128) {
         const int pp = i >> 9, si = (i >> 8) & 1, wy = (i >> 4) & 15, wx = i & 15;
         const int X = fg_org[pp][2 * si] + wx, Y = fg_org[pp][2 * si + 1] + wy;
         float t = 0.f;
@@ -358,7 +395,7 @@ __global__ void __launch_bounds__(FUSED ? 512 : 384, 1) umma_gemm_kernel(const _
         }
         fg_dinv[pp][si][wy][wx] = (m_tile * 2 + pp < n_units) ? __fdiv_rn(kActScale, sqrtf(t + 1e-6f)) : 0.f;
       }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
+      named_bar(3, 128);
       for (int ks = 0; ks < nsteps; ++ks, ++it) {
         const int s = it % STAGES;
         const uint32_t ph = (uint32_t)(it / STAGES) & 1u;
@@ -373,31 +410,29 @@ __global__ void __launch_bounds__(FUSED ? 512 : 384, 1) umma_gemm_kernel(const _
           const __half* fmap = g.nhwc16[si][lvl];
           const float* nsq = g.nsq[si][lvl + 1];
           const int wl = g.W[si] >> sh, hl = g.H[si] >> sh;
-          const int ox0 = fg_org[0][2 * si], oy0 = fg_org[0][2 * si + 1];
-          const int ox1 = fg_org[1][2 * si], oy1 = fg_org[1][2 * si + 1];
-          uint4 vals[4];
-          float nq[4], dv[4];
+          uint4 vals[8];
+          float sc[8];
 #pragma unroll
-          for (int ps = 0; ps < 4; ++ps) {               // phase 1: every load in flight before any use
-            const int row = ps * 32 + r32;
+          for (int ps = 0; ps < 8; ++ps) {               // phase 1: every load in flight before any use
+            const int row = ps * 16 + r16;
             const int pp = row >> 6, wy = 2 * ((row >> 3) & 7) - 1 + ty, wx = 2 * (row & 7) - 1 + tx;
-            const int X = (pp ? ox1 : ox0) + wx, Y = (pp ? oy1 : oy0) + wy;
+            const int X = fg_org[pp][2 * si] + wx, Y = fg_org[pp][2 * si + 1] + wy;
             const int xi = X < 0 ? 0 : min(X >> sh, wl - 1), yi = Y < 0 ? 0 : min(Y >> sh, hl - 1);
             const int px = yi * wl + xi;
             vals[ps] = __ldg(reinterpret_cast<const uint4*>(fmap + (size_t)px * C + coff));
-            nq[ps] = __ldg(nsq + px);
-            dv[ps] = (wy >= 0 && wx >= 0) ? fg_dinv[pp][si][wy & 15][wx & 15] : 0.f;   // -1 = conv zero padding
+            // undo the per-level normalisation; window pixel -1 = conv zero padding
+            const float dv = (wy >= 0 && wx >= 0) ? fg_dinv[pp][si][wy & 15][wx & 15] : 0.f;
+            sc[ps] = dv * sqrtf(__ldg(nsq + px) + 1e-30f);
           }
           mbar_wait(&empty_bar[s], ph ^ 1u);
 #pragma unroll
-          for (int ps = 0; ps < 4; ++ps) {               // phase 2: scale, convert, swizzled store
-            const int row = ps * 32 + r32;
-            const float sc = dv[ps] * sqrtf(nq[ps] + 1e-30f);   // undo the per-level normalisation
+          for (int ps = 0; ps < 8; ++ps) {               // phase 2: scale, convert, swizzled store
+            const int row = ps * 16 + r16;
             __half2* h2 = reinterpret_cast<__half2*>(&vals[ps]);
 #pragma unroll
             for (int q = 0; q < 4; ++q) {
               const float2 f = __half22float2(h2[q]);
-              h2[q] = __floats2half2_rn(f.x * sc, f.y * sc);
+              h2[q] = __floats2half2_rn(f.x * sc[ps], f.y * sc[ps]);
             }
             *reinterpret_cast<uint4*>(at + row * 128 + ((l8 ^ (row & 7)) << 4)) = vals[ps];
           }
@@ -405,8 +440,8 @@ __global__ void __launch_bounds__(FUSED ? 512 : 384, 1) umma_gemm_kernel(const _
           // rgb im2col chunk: k = tap*6 + img*3 + ch (54 used)
           mbar_wait(&empty_bar[s], ph ^ 1u);
 #pragma unroll 1
-          for (int ps = 0; ps < 4; ++ps) {
-            const int row = ps * 32 + r32;
+          for (int ps = 0; ps < 8; ++ps) {
+            const int row = ps * 16 + r16;
             const int pp = row >> 6, oy = (row >> 3) & 7, ox = row & 7;
             __align__(16) __half hv[8];
 #pragma unroll
@@ -429,538 +464,51 @@ __global__ void __launch_bounds__(FUSED ? 512 : 384, 1) umma_gemm_kernel(const _
           }
         }
         fence_proxy_async();            // generic-proxy stores -> visible to the tensor core (async proxy)
-        mbar_arrive(&full_bar[s]);
-      }
-    }
-  } else if (warp >= 4 && warp < (FUSED ? 8 : 12)) {
-    // ===================== epilogue (8 warps; 4 warps covering both column halves when FUSED) =====================
-    if (SEGMENTED) asm volatile("setmaxnreg.inc.sync.aligned.u32 216;");
-    const int q = warp & 3, hf = (warp - 4) >> 2;
-    const int row = q * 32 + lane;
-    int seg = 0;
-    auto release_slot = [&](int slot) {
-      if (PAIR) mbar_arrive_leader(&tempty_bar[slot]);
-      else mbar_arrive(&tempty_bar[slot]);
-    };
-    for (int tile = cta0; tile < total_tiles; tile += ctas) {
-      const int mt = tile / p.n_tiles, n_tile = tile - mt * p.n_tiles;
-      const int m_tile = PAIR ? mt * 2 + rank : mt;
-      const int colbase = n_tile * 256 + hf * 128;
-      if (SEGMENTED) {
-        float tot[128];
-#pragma unroll
-        for (int i = 0; i < 128; ++i) tot[i] = 0.f;
-        for (int sg = 0; sg < nseg; ++sg, ++seg) {
-          const int slot = seg & 1;
-          const uint32_t sph = (uint32_t)(seg >> 1) & 1u;
-          mbar_wait(&tfull_bar[slot], sph);
-          tc_fence_after();
-          const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(slot * 256 + hf * 128);
-#pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            float v[32];
-            tmem_ld32(taddr + c * 32, v);
-#pragma unroll
-            for (int i = 0; i < 32; ++i) tot[c * 32 + i] += v[i];
-          }
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) release_slot(slot);
-        }
-#pragma unroll
-        for (int c = 0; c < 4; ++c) epilogue_piece<EPI>(p.epi, n_units, m_tile, row, colbase + c * 32, tot + c * 32);
-      } else {
-        const int slot = seg & 1;
-        const uint32_t sph = (uint32_t)(seg >> 1) & 1u;
-        mbar_wait(&tfull_bar[slot], sph);
-        tc_fence_after();
-        constexpr int NH = FUSED ? 2 : 1;              // column halves handled by this warp
-#pragma unroll 1
-        for (int hh = 0; hh < NH; ++hh) {
-          const int hcol = FUSED ? hh : hf;
-          const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(slot * 256 + hcol * 128);
-#pragma unroll 1
-          for (int c = 0; c < 4; ++c) {
-            float v[32];
-            tmem_ld32(taddr + c * 32, v);
-            epilogue_piece<EPI>(p.epi, n_units, m_tile, row, n_tile * 256 + hcol * 128 + c * 32, v);
-          }
-        }
-        tc_fence_before();
         __syncwarp();
-        if (lane == 0) release_slot(slot);
-        ++seg;
+        if (lane == 0) mbar_arrive(&full_bar[s]);
       }
     }
-  }
-  tc_fence_before();
-  if (PAIR) cluster_sync_all();      // neither CTA may free TMEM / exit while the pair's MMAs can still touch it
-  else __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    if (PAIR) tmem_dealloc_pair(tmem_base, 512);
-    else tmem_dealloc(tmem_base, 512);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// conv1 (1-pass) with the patch gather fused in, second generation: one CTA owns a 128 x 512 tile
-// (all output channels of 2 patches), so every gathered A tile is built once and feeds 8 MMAs
-// (N = 2 x 256); per-tile lookup tables (pixel offset and scale per image / level / window pixel)
-// in shared memory reduce the per-row producer work to two LDS, one LDG and the fp16 re-scaling.
-// 512 threads: warp 0 TMA (weights), 1 MMA, 2 TMEM alloc, 3 idle, 4..7 epilogue, 8..15 A producers.
-// smem: 2 stages x (16 KB A + 64 KB B) + 24 KB tables.
-// ------------------------------------------------------------------------------------------------
-// PAIR: a cluster of two CTAs owns 256 rows (4 patches) x 512 columns through cta_group::2 MMAs; each CTA
-// gathers its own 128 A rows and streams only half of the weights (2 x 16 KB per k-step), which makes room
-// for kF2PairStages stages.  Producer warps of both CTAs arrive (once per warp) on the leader's full barrier.
-constexpr int kF2Stages = 2;
-constexpr int kF2PairStages = 3;
-constexpr int kF2StageBytes = kATile + 2 * kBTile;
-constexpr int kF2PairStageBytes = kATile + kBTile;
-
-template <bool PAIR>
-__global__ void __launch_bounds__(512, 1) umma_conv1_fused_kernel(const __grid_constant__ UmmaGemmParams p) {
-  constexpr uint32_t IDESC = make_idesc_f16(PAIR ? 256 : 128, 256);
-  constexpr int kF2Stages = PAIR ? p2p::kF2PairStages : p2p::kF2Stages;
-  constexpr int kF2StageBytes = PAIR ? p2p::kF2PairStageBytes : p2p::kF2StageBytes;
-  constexpr int BH = PAIR ? kBTile / 2 : kBTile;      // bytes of one 256-column weight half held by this CTA
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  int* tab_px = reinterpret_cast<int*>(smem + kF2Stages * kF2StageBytes);        // [2 patches][2 img][3 lvl][256]
-  float* tab_sc = reinterpret_cast<float*>(tab_px + 3072);                       // same shape
-  __shared__ __align__(8) uint64_t full_bar[kF2Stages];
-  __shared__ __align__(8) uint64_t empty_bar[kF2Stages];
-  __shared__ __align__(8) uint64_t tfull_bar[2];     // per accumulator half
-  __shared__ __align__(8) uint64_t tempty_bar[2];
-  __shared__ uint32_t tmem_base_smem;
-  __shared__ float fg_dinv[2][2][16][16];
-  __shared__ int fg_org[2][4];
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n_units = p.epi.n_patches;
-  const int rank = PAIR ? (int)cluster_ctarank() : 0;
-  const int cta0 = PAIR ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int ctas = PAIR ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-  const int total_tiles = PAIR ? (p.m_tiles + 1) / 2 : p.m_tiles;     // cluster tiles when paired
-  const int nsteps = p.nsteps;
-
-  if (warp == 0 && lane == 0) tma_prefetch_desc(&p.b_hi);
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < kF2Stages; ++i) {
-      mbar_init(&full_bar[i], PAIR ? 17 : 257);     // TMA expect_tx + producers (per thread; per warp x 2 CTAs)
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], PAIR ? 8 : 4);
-    }
-    fence_barrier_init();
-  }
-  if (warp == 2) {
-    if (PAIR) tmem_alloc_pair(&tmem_base_smem, 512);
-    else tmem_alloc(&tmem_base_smem, 512);
-  }
-  tc_fence_before();
-  if (PAIR) cluster_sync_all();
-  else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      int it = 0;
-      for (int tile = cta0; tile < total_tiles; tile += ctas) {
-        for (int ks = 0; ks < nsteps; ++ks, ++it) {
-          const int s = it % kF2Stages;
-          const uint32_t ph = (uint32_t)(it / kF2Stages) & 1u;
-          mbar_wait(&empty_bar[s], ph ^ 1u);
-          const KStep k = p.steps[ks];
-          uint8_t* st = smem + (size_t)s * kF2StageBytes;
-          if (PAIR) {
-            if (rank == 0) mbar_expect_tx(&full_bar[s], 2 * kBTile);     // 2 CTAs x 2 halves x 16 KB
-            tma_load_2d_pair(&p.b_hi, &full_bar[s], st + kATile, k.bk, rank * 128);
-            tma_load_2d_pair(&p.b_hi, &full_bar[s], st + kATile + BH, k.bk, 256 + rank * 128);
-          } else {
-            mbar_expect_tx(&full_bar[s], 2 * kBTile);
-            tma_load_2d(&p.b_hi, &full_bar[s], st + kATile, k.bk, 0);
-            tma_load_2d(&p.b_hi, &full_bar[s], st + kATile + kBTile, k.bk, 256);
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0 && rank == 0) {
-      int it = 0, t = 0;
-      for (int tile = cta0; tile < total_tiles; tile += ctas, ++t) {
-        const uint32_t tph = (uint32_t)t & 1u;
-        for (int ks = 0; ks < nsteps; ++ks, ++it) {
-          const int s = it % kF2Stages;
-          const uint32_t ph = (uint32_t)(it / kF2Stages) & 1u;
-          mbar_wait(&full_bar[s], ph);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + (size_t)s * kF2StageBytes);
-          const uint64_t a = make_sw128_desc(sa);
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            if (ks == 0) {
-              mbar_wait(&tempty_bar[h], tph ^ 1u);     // the epilogue has drained this half of the previous tile
-              tc_fence_after();
-            }
-            const uint64_t b = make_sw128_desc(sa + kATile + h * BH);
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {
-              if (PAIR)
-                umma_f16_pair(tmem_base + (uint32_t)h * 256u, a + 2 * kk, b + 2 * kk, IDESC, (ks > 0 || kk > 0) ? 1u : 0u);
-              else
-                umma_f16(tmem_base + (uint32_t)h * 256u, a + 2 * kk, b + 2 * kk, IDESC, (ks > 0 || kk > 0) ? 1u : 0u);
-            }
-          }
-          if (PAIR) umma_commit_pair(&empty_bar[s]);
-          else umma_commit(&empty_bar[s]);
-          if (ks + 1 == nsteps) {
-            if (PAIR) {
-              umma_commit_pair(&tfull_bar[0]);
-              umma_commit_pair(&tfull_bar[1]);
-            } else {
-              umma_commit(&tfull_bar[0]);
-              umma_commit(&tfull_bar[1]);
-            }
-          }
-        }
-      }
-    }
-  } else if (warp >= 8) {
-    // ===================== A producers =====================
-    const int ptid = threadIdx.x - 256;
-    const int l8 = ptid & 7, r32 = ptid >> 3;
-    const FusedGather& g = p.fg;
+  } else if (AMODE == AMODE_WINDOW && warp >= 12) {
+    // ===================== aux warps (warpgroup 3): zero-padding fix-up and the rgb im2col k-step =====================
+    const int row = threadIdx.x - 384;               // 0..127: the tile row this thread owns
     int it = 0;
-    for (int ctile = cta0; ctile < total_tiles; ctile += ctas) {
-      const int tile = PAIR ? ctile * 2 + rank : ctile;       // this CTA's 128-row tile (2 patches); may be past the end
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      if (ptid < 8) {
-        const int pp = ptid >> 2, j = ptid & 3;
-        const int n = tile * 2 + pp;
-        int v = 0;
-        if (n < n_units) {
-          if (g.is_float)
-            v = (int)reinterpret_cast<const float*>(g.matches)[(size_t)n * 4 + j];
-          else
-            v = (int)reinterpret_cast<const long long*>(g.matches)[(size_t)n * 4 + j];
-        }
-        fg_org[pp][j] = v - 8;
-      }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      for (int i = ptid; i < 1024; i += 256) {
-        const int pp = i >> 9, si = (i >> 8) & 1, wy = (i >> 4) & 15, wx = i & 15;
-        const int X = fg_org[pp][2 * si] + wx, Y = fg_org[pp][2 * si + 1] + wy;
-        float t = 0.f;
-#pragma unroll
-        for (int l = 0; l < 4; ++l) {
-          const int xi = X < 0 ? 0 : min(X >> l, (g.W[si] >> l) - 1), yi = Y < 0 ? 0 : min(Y >> l, (g.H[si] >> l) - 1);
-          t += __ldg(g.nsq[si][l] + (size_t)yi * (g.W[si] >> l) + xi);
-        }
-        fg_dinv[pp][si][wy][wx] = (tile * 2 + pp < n_units) ? __fdiv_rn(kActScale, sqrtf(t + 1e-6f)) : 0.f;
-      }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      for (int i = ptid; i < 3072; i += 256) {           // [pp][si][lvl][wy][wx]
-        const int wx = i & 15, wy = (i >> 4) & 15, r = i >> 8;
-        const int lvl = r % 3, si = (r / 3) & 1, pp = r / 6;
-        const int sh = lvl + 1;
-        const int X = fg_org[pp][2 * si] + wx, Y = fg_org[pp][2 * si + 1] + wy;
-        const int wl = g.W[si] >> sh, hl = g.H[si] >> sh;
-        const int xi = X < 0 ? 0 : min(X >> sh, wl - 1), yi = Y < 0 ? 0 : min(Y >> sh, hl - 1);
-        const int px = yi * wl + xi;
-        tab_px[i] = px;
-        tab_sc[i] = fg_dinv[pp][si][wy][wx] * sqrtf(__ldg(g.nsq[si][lvl + 1] + px) + 1e-30f);
-      }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      const int m_tile = tile / n_halves;
       for (int ks = 0; ks < nsteps; ++ks, ++it) {
-        const int s = it % kF2Stages;
-        const uint32_t ph = (uint32_t)(it / kF2Stages) & 1u;
+        const int s = it % STAGES;
+        const uint32_t ph = (uint32_t)(it / STAGES) & 1u;
         const KStep k = p.steps[ks];
-        uint8_t* at = smem + (size_t)s * kF2StageBytes;
-        if (k.kind == 0) {
-          const int ty = (k.plane & 2) ? 1 : (k.y < 0 ? 0 : 2), tx = (k.plane & 1) ? 1 : (k.x < 0 ? 0 : 2);
-          const int chunk = k.c0 >> 6, si = chunk >> 2, jj = chunk & 3;
-          const int lvl = jj == 0 ? 0 : (jj == 1 ? 1 : 2);
-          const int C = lvl == 2 ? 128 : 64;
-          const int coff = (jj == 3 ? 64 : 0) + l8 * 8;
-          const __half* fmap = g.nhwc16[si][lvl] + coff;
-          uint4 vals[4];
-          float sc[4];
-#pragma unroll
-          for (int ps = 0; ps < 4; ++ps) {
-            const int row = ps * 32 + r32;
-            const int pp = row >> 6, wy = 2 * ((row >> 3) & 7) - 1 + ty, wx = 2 * (row & 7) - 1 + tx;
-            const int ti = ((pp * 2 + si) * 3 + lvl) * 256 + ((wy & 15) << 4) + (wx & 15);
-            const int px = tab_px[ti];
-            sc[ps] = (wy >= 0 && wx >= 0) ? tab_sc[ti] : 0.f;      // -1 = conv zero padding
-            vals[ps] = __ldg(reinterpret_cast<const uint4*>(fmap + (size_t)px * C));
-          }
-          mbar_wait(&empty_bar[s], ph ^ 1u);
-#pragma unroll
-          for (int ps = 0; ps < 4; ++ps) {
-            const int row = ps * 32 + r32;
-            __half2* h2 = reinterpret_cast<__half2*>(&vals[ps]);
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const float2 f = __half22float2(h2[q]);
-              h2[q] = __floats2half2_rn(f.x * sc[ps], f.y * sc[ps]);
-            }
-            *reinterpret_cast<uint4*>(at + row * 128 + ((l8 ^ (row & 7)) << 4)) = vals[ps];
-          }
-        } else {
-          mbar_wait(&empty_bar[s], ph ^ 1u);
-#pragma unroll 1
-          for (int ps = 0; ps < 4; ++ps) {
-            const int row = ps * 32 + r32;
-            const int pp = row >> 6, oy = (row >> 3) & 7, ox = row & 7;
-            __align__(16) __half hv[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const int kk = l8 * 8 + i;
-              float v = 0.f;
-              if (kk < 54) {
-                const int tap = kk / 6, r = kk - tap * 6;
-                const int si = r / 3, ch = r - si * 3;
-                const int wx = 2 * ox - 1 + tap % 3, wy = 2 * oy - 1 + tap / 3;
-                if (wx >= 0 && wy >= 0) {
-                  const int xi = fg_clamp(fg_org[pp][2 * si] + wx, 1, g.W[si]);
-                  const int yi = fg_clamp(fg_org[pp][2 * si + 1] + wy, 1, g.H[si]);
-                  v = __ldg(g.img[si] + ((size_t)ch * g.H[si] + yi) * g.W[si] + xi) * fg_dinv[pp][si][wy][wx];
-                }
-              }
-              hv[i] = __float2half_rn(v);
-            }
-            *reinterpret_cast<uint4*>(at + row * 128 + ((l8 ^ (row & 7)) << 4)) = *reinterpret_cast<const uint4*>(hv);
-          }
-        }
-        fence_proxy_async();
-        if (PAIR) {
-          __syncwarp();
-          if (lane == 0) mbar_arrive_leader(&full_bar[s]);
-        } else {
-          mbar_arrive(&full_bar[s]);
-        }
-      }
-    }
-  } else if (warp >= 4) {
-    // ===================== epilogue: 4 warps, one TMEM lane quadrant each, 512 columns =====================
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    int t = 0;
-    for (int ctile = cta0; ctile < total_tiles; ctile += ctas, ++t) {
-      const int tile = PAIR ? ctile * 2 + rank : ctile;
-      const uint32_t tph = (uint32_t)t & 1u;
-#pragma unroll 1
-      for (int h = 0; h < 2; ++h) {
-        mbar_wait(&tfull_bar[h], tph);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(h * 256);
-#pragma unroll 1
-        for (int c = 0; c < 8; ++c) {
-          float v[32];
-          tmem_ld32(taddr + c * 32, v);
-          epilogue_piece<EPI_CONV1>(p.epi, n_units, tile, row, h * 256 + c * 32, v);
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) {
-          if (PAIR) mbar_arrive_leader(&tempty_bar[h]);
-          else mbar_arrive(&tempty_bar[h]);
-        }
-      }
-    }
-  }
-  tc_fence_before();
-  if (PAIR) cluster_sync_all();
-  else __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    if (PAIR) tmem_dealloc_pair(tmem_base, 512);
-    else tmem_dealloc(tmem_base, 512);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// conv1 (1-pass) fed by strided TMA boxes of the per-image window maps (fuse_gather = 3).
-// The patch-normalised 256-channel vector of every image pixel is computed once per pair (window_map_kernel), so a
-// conv tap of one patch is ONE cp.async.bulk.tensor box {64 ch, 8 px stride 2, 8 px stride 2} of the replicate-padded
-// map: no producer warps, no lookup tables, no per-k-step gather latency.  Only two things are left for the four
-// "aux" warps: (a) the conv's zero padding -- window pixel -1 must contribute 0, but the box holds the neighbouring
-// image pixel there -- is restored by zeroing the <= 15 affected rows per patch after the box has landed (taps with
-// tx = 0 or ty = 0); (b) the rgb k-step (54 real K values) is an im2col of the normalised rgb map built with plain
-// loads.  Cluster of two CTAs = 4 patches x 512 channels (tcgen05.mma.cta_group::2, M = 256); every CTA loads its own
-// 2 patches and its own half of the weights to its own shared memory / its own TMA barrier; its aux warps then
-// (fix up and) arrive on the LEADER's operand barrier, which the MMA issuer waits on.
-// 384 threads: warp 0 TMA, 1 MMA, 2 TMEM alloc, 4..7 epilogue, 8..11 aux.  4 stages x (16 KB A + 2 x 16 KB weights).
-// Same MMA sequence per output element as umma_conv1_fused_kernel on a bit-identical A operand -> bit-identical y1.
-// ------------------------------------------------------------------------------------------------
-constexpr int kC1Stages = 4;
-constexpr int kC1StageBytes = kATile + kBTile;
-
-__global__ void __launch_bounds__(384, 1) umma_conv1_tma_kernel(const __grid_constant__ Conv1TmaParams p) {
-  constexpr uint32_t IDESC = make_idesc_f16(256, 256);
-  constexpr int BH = kBTile / 2;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  __shared__ __align__(8) uint64_t full_tma[kC1Stages];    // local: this CTA's A boxes + weight halves have landed
-  __shared__ __align__(8) uint64_t full_mma[kC1Stages];    // leader's: both CTAs' operands are ready (8 arrivals)
-  __shared__ __align__(8) uint64_t empty_bar[kC1Stages];
-  __shared__ __align__(8) uint64_t tfull_bar[2];
-  __shared__ __align__(8) uint64_t tempty_bar[2];
-  __shared__ uint32_t tmem_base_smem;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n_units = p.epi.n_patches;
-  const int rank = (int)cluster_ctarank();
-  const int cta0 = (int)(blockIdx.x >> 1), ctas = (int)(gridDim.x >> 1);
-  const int total_tiles = (p.m_tiles + 1) / 2;
-  const int nsteps = p.nsteps;
-  const WindowMaps& wm = p.wm;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&p.b_hi);
-    tma_prefetch_desc(&wm.map[0]);
-    tma_prefetch_desc(&wm.map[1]);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < kC1Stages; ++i) {
-      mbar_init(&full_tma[i], 1);
-      mbar_init(&full_mma[i], 8);      // 4 aux warps x 2 CTAs
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], 8);
-    }
-    fence_barrier_init();
-  }
-  if (warp == 2) tmem_alloc_pair(&tmem_base_smem, 512);
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
-
-  // window origin of patch n in padded map coordinates: window pixel (wy, wx) lives at (oy + wy, ox + wx).
-  // Truncation = `.long()` (networks/utils.py:19); clamping the origin to [-7, W + 8] leaves every clamped window
-  // pixel unchanged (beyond that all of them sit on the border pixel) and keeps the boxes inside the padded map.
-  auto origin = [&](int n, int j) -> int {
-    if (n >= n_units) n = 0;      // past the end (odd tile counts): any valid patch, the epilogue discards the rows
-    int v;
-    if (wm.is_float) v = (int)reinterpret_cast<const float*>(wm.matches)[(size_t)n * 4 + j];
-    else v = (int)reinterpret_cast<const long long*>(wm.matches)[(size_t)n * 4 + j];
-    const int lim = (j & 1) ? wm.H[j >> 1] : wm.W[j >> 1];
-    v = v < -7 ? -7 : (v > lim + 8 ? lim + 8 : v);
-    return v - 8 + kMapPad;
-  };
-
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
-      int it = 0;
-      for (int ctile = cta0; ctile < total_tiles; ctile += ctas) {
-        const int tile = ctile * 2 + rank;
-        int o[2][4];
-#pragma unroll
-        for (int pp = 0; pp < 2; ++pp)
-#pragma unroll
-          for (int j = 0; j < 4; ++j) o[pp][j] = origin(tile * 2 + pp, j);
-        for (int ks = 0; ks < nsteps; ++ks, ++it) {
-          const int s = it % kC1Stages;
-          mbar_wait(&empty_bar[s], ((uint32_t)(it / kC1Stages) & 1u) ^ 1u);
-          const KStep k = p.steps[ks];
-          uint8_t* st = smem + (size_t)s * kC1StageBytes;
-          mbar_expect_tx(&full_tma[s], k.kind == 0 ? kATile + kBTile : kBTile);
-          tma_load_2d(&p.b_hi, &full_tma[s], st + kATile, k.bk, rank * 128);
-          tma_load_2d(&p.b_hi, &full_tma[s], st + kATile + BH, k.bk, 256 + rank * 128);
-          if (k.kind == 0) {
-            const int ty = (k.plane & 2) ? 1 : (k.y < 0 ? 0 : 2), tx = (k.plane & 1) ? 1 : (k.x < 0 ? 0 : 2);
-            const int chunk = k.c0 >> 6, si = chunk >> 2, c0 = (chunk & 3) * 64;
-#pragma unroll
-            for (int pp = 0; pp < 2; ++pp)
-              tma_load_3d(&wm.map[si], &full_tma[s], st + pp * 8192, c0, o[pp][2 * si] - 1 + tx, o[pp][2 * si + 1] - 1 + ty);
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader CTA) =====================
-    if (lane == 0 && rank == 0) {
-      int it = 0, t = 0;
-      for (int ctile = cta0; ctile < total_tiles; ctile += ctas, ++t) {
-        const uint32_t tph = (uint32_t)t & 1u;
-        for (int ks = 0; ks < nsteps; ++ks, ++it) {
-          const int s = it % kC1Stages;
-          mbar_wait(&full_mma[s], (uint32_t)(it / kC1Stages) & 1u);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + (size_t)s * kC1StageBytes);
-          const uint64_t a = make_sw128_desc(sa);
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            if (ks == 0) {
-              mbar_wait(&tempty_bar[h], tph ^ 1u);
-              tc_fence_after();
-            }
-            const uint64_t b = make_sw128_desc(sa + kATile + h * BH);
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk)
-              umma_f16_pair(tmem_base + (uint32_t)h * 256u, a + 2 * kk, b + 2 * kk, IDESC, (ks > 0 || kk > 0) ? 1u : 0u);
-          }
-          umma_commit_pair(&empty_bar[s]);
-          if (ks + 1 == nsteps) {
-            umma_commit_pair(&tfull_bar[0]);
-            umma_commit_pair(&tfull_bar[1]);
-          }
-        }
-      }
-    }
-  } else if (warp >= 8) {
-    // ===================== aux warps: zero-padding fix-up (warp 8) and the rgb im2col k-step (all four) =====================
-    const int row = threadIdx.x - 256;               // 0..127: tile row owned in the rgb step
-    int it = 0;
-    for (int ctile = cta0; ctile < total_tiles; ctile += ctas) {
-      const int tile = ctile * 2 + rank;
-      for (int ks = 0; ks < nsteps; ++ks, ++it) {
-        const int s = it % kC1Stages;
-        const uint32_t ph = (uint32_t)(it / kC1Stages) & 1u;
-        const KStep k = p.steps[ks];
-        uint8_t* st = smem + (size_t)s * kC1StageBytes;
+        uint8_t* st = smem + (size_t)s * STAGE_BYTES;
         if (k.kind == 0) {
           // every aux warp follows every stage (wait + arrive): parity waits are only valid within one ring
           // revolution, so no warp may run ahead of -- or fall behind -- the pipeline
-          mbar_wait(&full_tma[s], ph);
+          mbar_wait(&full_bar[s], ph);
           const bool zx = !(k.plane & 1) && k.x < 0, zy = !(k.plane & 2) && k.y < 0;      // tap tx = 0 / ty = 0
           if (zx || zy) {
-            const int r = threadIdx.x - 256;          // one tile row per aux thread
-            if ((zx && (r & 7) == 0) || (zy && ((r >> 3) & 7) == 0)) {
-              uint4* d = reinterpret_cast<uint4*>(st + r * 128);
+            if ((zx && (row & 7) == 0) || (zy && ((row >> 3) & 7) == 0)) {
+              uint4* d = reinterpret_cast<uint4*>(st + row * 128);
 #pragma unroll
               for (int c = 0; c < 8; ++c) d[c] = make_uint4(0, 0, 0, 0);
             }
             fence_proxy_async();
           }
-          __syncwarp();
-          if (lane == 0) mbar_arrive_leader(&full_mma[s]);
         } else {
           // rgb im2col row: k = tap*6 + img*3 + ch (54 used, rest zero); window pixel -1 = conv zero padding
           mbar_wait(&empty_bar[s], ph ^ 1u);
           const int pp = row >> 6, oy = (row >> 3) & 7, ox = row & 7;
-          const int n = tile * 2 + pp;
+          const int n = m_tile * 2 + pp;
           __align__(16) __half hv[64];
 #pragma unroll
           for (int i = 0; i < 64; ++i) hv[i] = __float2half_rn(0.f);
 #pragma unroll
           for (int si = 0; si < 2; ++si) {
             const int bx = origin(n, 2 * si), by = origin(n, 2 * si + 1);
-            const int Wp = wm.W[si] + 2 * kMapPad;
+            const int Wp = p.wm.W[si] + 2 * kMapPad;
 #pragma unroll
             for (int tap = 0; tap < 9; ++tap) {
               const int wx = 2 * ox - 1 + tap % 3, wy = 2 * oy - 1 + tap / 3;
               if (wx >= 0 && wy >= 0 && n < n_units) {
-                const uint2 q = __ldg(reinterpret_cast<const uint2*>(wm.rgbn[si] + ((size_t)(by + wy) * Wp + bx + wx) * 4));
+                const uint2 q = __ldg(reinterpret_cast<const uint2*>(p.wm.rgbn[si] + ((size_t)(by + wy) * Wp + bx + wx) * 4));
                 const __half* hq = reinterpret_cast<const __half*>(&q);
                 hv[tap * 6 + si * 3 + 0] = hq[0];
                 hv[tap * 6 + si * 3 + 1] = hq[1];
@@ -972,44 +520,15 @@ __global__ void __launch_bounds__(384, 1) umma_conv1_tma_kernel(const __grid_con
           for (int c = 0; c < 8; ++c)
             *reinterpret_cast<uint4*>(st + row * 128 + ((c ^ (row & 7)) << 4)) = reinterpret_cast<const uint4*>(hv)[c];
           fence_proxy_async();
-          mbar_wait(&full_tma[s], ph);            // this CTA's weight halves
-          __syncwarp();
-          if (lane == 0) mbar_arrive_leader(&full_mma[s]);
+          mbar_wait(&full_bar[s], ph);            // the weight tile
         }
-      }
-    }
-  } else if (warp >= 4) {
-    // ===================== epilogue: 4 warps, one TMEM lane quadrant each, 512 columns =====================
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    int t = 0;
-    for (int ctile = cta0; ctile < total_tiles; ctile += ctas, ++t) {
-      const int tile = ctile * 2 + rank;
-      const uint32_t tph = (uint32_t)t & 1u;
-#pragma unroll 1
-      for (int h = 0; h < 2; ++h) {
-        mbar_wait(&tfull_bar[h], tph);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(h * 256);
-#pragma unroll 1
-        for (int c = 0; c < 8; ++c) {
-          float v[32];
-          tmem_ld32(taddr + c * 32, v);
-          epilogue_piece<EPI_CONV1>(p.epi, n_units, tile, row, h * 256 + c * 32, v);
-        }
-        tc_fence_before();
         __syncwarp();
-        if (lane == 0) mbar_arrive_leader(&tempty_bar[h]);
+        if (lane == 0) mbar_arrive(&ready_bar[s]);
       }
     }
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc_pair(tmem_base, 512);
   }
 }
+
 
 // ------------------------------------------------------------------------------------------------
 // host side
@@ -1094,92 +613,33 @@ int make_tmap_fp16(CUtensorMap* out, const void* base, int rank, const uint64_t*
   return 0;
 }
 
-template <int PASSES, bool SEGMENTED, int EPI, bool FUSED = false, bool PAIR = false>
+template <int PASSES, bool SEGMENTED, int EPI, int AMODE = AMODE_TMA>
 static int launch_one(const UmmaGemmParams& p, int grid, cudaStream_t st) {
-  constexpr int STAGES = PAIR ? ((PASSES == 3) ? 3 : 6) : ((PASSES == 3) ? 2 : 4);
-  constexpr int NOP = (PASSES == 3) ? 2 : 1;
-  const int smem = STAGES * NOP * (kATile + (PAIR ? kBTile / 2 : kBTile)) + 1024;
-  auto kern = umma_gemm_kernel<PASSES, SEGMENTED, EPI, FUSED, PAIR>;
-  P2P_ENSURE_SMEM(kern, smem);
-  if (PAIR) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)grid);
-    cfg.blockDim = dim3(384);
-    cfg.dynamicSmemBytes = (size_t)smem;
-    cfg.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = 2;
-    at[0].val.clusterDim.y = 1;
-    at[0].val.clusterDim.z = 1;
-    cfg.attrs = at;
-    cfg.numAttrs = 1;
-    P2P_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, p));
-  } else {
-    kern<<<grid, FUSED ? 512 : 384, smem, st>>>(p);
-  }
+  using Cfg = GemmCfg<PASSES, AMODE>;
+  auto kern = umma_gemm_kernel<PASSES, SEGMENTED, EPI, AMODE>;
+  P2P_ENSURE_SMEM(kern, Cfg::SMEM);
+  kern<<<grid, Cfg::THREADS, Cfg::SMEM, st>>>(p);
   P2P_LAUNCH_OK();
   return 0;
 }
 
 template <int EPI>
 static int launch_epi(const UmmaGemmParams& p, int passes, bool seg, int grid, cudaStream_t st) {
-  if (p.pair) {
-    if (passes == 3)
-      return seg ? launch_one<3, true, EPI, false, true>(p, grid, st) : launch_one<3, false, EPI, false, true>(p, grid, st);
-    return seg ? launch_one<1, true, EPI, false, true>(p, grid, st) : launch_one<1, false, EPI, false, true>(p, grid, st);
-  }
   if (passes == 3) return seg ? launch_one<3, true, EPI>(p, grid, st) : launch_one<3, false, EPI>(p, grid, st);
   return seg ? launch_one<1, true, EPI>(p, grid, st) : launch_one<1, false, EPI>(p, grid, st);
 }
 
-int launch_umma_gemm(const UmmaGemmParams& p, int epi, int passes, int num_sms, cudaStream_t st, bool fused) {
+int launch_umma_gemm(const UmmaGemmParams& p, int epi, int passes, int num_sms, cudaStream_t st, int amode) {
   P2P_REQUIRE(passes == 1 || passes == 3, "umma gemm: passes must be 1 or 3");
   P2P_REQUIRE(p.nsteps > 0 && p.m_tiles > 0 && p.n_tiles > 0, "umma gemm: empty problem");
   const bool seg = p.seg_len > 0 && p.seg_len < p.nsteps;
-  const int total = p.m_tiles * p.n_tiles;
-  int grid = total < num_sms ? total : num_sms;
-  if (p.pair) {      // clusters of 2 CTAs; a pair tile = two m-tiles x one n-tile
-    P2P_REQUIRE(!fused || p.fg.generation == 2, "the first-generation fused-gather kernel is single-CTA");
-    const int pair_tiles = ((p.m_tiles + 1) / 2) * p.n_tiles;
-    const int max_clusters = num_sms >= 2 ? num_sms / 2 : 1;
-    const int clusters = pair_tiles < max_clusters ? pair_tiles : max_clusters;
-    grid = 2 * clusters;
-  }
-  if (fused) {
-    P2P_REQUIRE(epi == EPI_CONV1 && passes == 1 && !seg, "fused gather is available for 1-pass conv1 only");
-    if (p.fg.generation == 1)     // first version (128 x 256 tiles, no tables), kept for comparison: fuse_gather = 2
-      return launch_one<1, false, EPI_CONV1, true>(p, grid, st);
-    if (p.pair) {
-      const int smem = kF2PairStages * kF2PairStageBytes + 3072 * 8 + 1024;
-      auto kern = umma_conv1_fused_kernel<true>;
-      P2P_ENSURE_SMEM(kern, smem);
-      const int ptiles = (p.m_tiles + 1) / 2;
-      const int max_clusters = num_sms >= 2 ? num_sms / 2 : 1;
-      const int clusters = ptiles < max_clusters ? ptiles : max_clusters;
-      cudaLaunchConfig_t cfg = {};
-      cfg.gridDim = dim3((unsigned)(2 * clusters));
-      cfg.blockDim = dim3(512);
-      cfg.dynamicSmemBytes = (size_t)smem;
-      cfg.stream = st;
-      cudaLaunchAttribute at[1];
-      at[0].id = cudaLaunchAttributeClusterDimension;
-      at[0].val.clusterDim.x = 2;
-      at[0].val.clusterDim.y = 1;
-      at[0].val.clusterDim.z = 1;
-      cfg.attrs = at;
-      cfg.numAttrs = 1;
-      P2P_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, p));
-      P2P_LAUNCH_OK();
-      return 0;
-    }
-    const int smem = kF2Stages * kF2StageBytes + 3072 * 8 + 1024;
-    auto kern = umma_conv1_fused_kernel<false>;
-    P2P_ENSURE_SMEM(kern, smem);
-    const int g2 = p.m_tiles < num_sms ? p.m_tiles : num_sms;
-    kern<<<g2, 512, smem, st>>>(p);
-    P2P_LAUNCH_OK();
-    return 0;
+  const int total = p.m_tiles * p.n_tiles * 2;
+  const int grid = total < num_sms ? total : num_sms;
+  if (amode != AMODE_TMA) {
+    P2P_REQUIRE(epi == EPI_CONV1 && passes == 1 && !seg, "the fused A operand is available for 1-pass conv1 only");
+    if (amode == AMODE_GATHER) return launch_one<1, false, EPI_CONV1, AMODE_GATHER>(p, grid, st);
+    P2P_REQUIRE(amode == AMODE_WINDOW, "umma gemm: unknown A mode");
+    return launch_one<1, false, EPI_CONV1, AMODE_WINDOW>(p, grid, st);
   }
   switch (epi) {
     case EPI_PLAIN: return launch_epi<EPI_PLAIN>(p, passes, seg, grid, st);
@@ -1190,31 +650,6 @@ int launch_umma_gemm(const UmmaGemmParams& p, int epi, int passes, int num_sms, 
   }
   set_last_error("umma gemm: unknown epilogue");
   return -1;
-}
-
-int launch_conv1_tma(const Conv1TmaParams& p, int num_sms, cudaStream_t st) {
-  P2P_REQUIRE(p.nsteps > 0 && p.m_tiles > 0, "conv1 (window-map TMA): empty problem");
-  const int smem = kC1Stages * kC1StageBytes + 1024;
-  auto kern = umma_conv1_tma_kernel;
-  P2P_ENSURE_SMEM(kern, smem);
-  const int ptiles = (p.m_tiles + 1) / 2;
-  const int max_clusters = num_sms >= 2 ? num_sms / 2 : 1;
-  const int clusters = ptiles < max_clusters ? ptiles : max_clusters;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(2 * clusters));
-  cfg.blockDim = dim3(384);
-  cfg.dynamicSmemBytes = (size_t)smem;
-  cfg.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeClusterDimension;
-  at[0].val.clusterDim.x = 2;
-  at[0].val.clusterDim.y = 1;
-  at[0].val.clusterDim.z = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = 1;
-  P2P_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, p));
-  P2P_LAUNCH_OK();
-  return 0;
 }
 
 }  // namespace p2p

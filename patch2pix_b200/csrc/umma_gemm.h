@@ -1,4 +1,4 @@
-// Parameters of the tcgen05 implicit-GEMM kernel (umma_gemm.cu).
+// Parameters of the wgmma implicit-GEMM kernel (umma_gemm.cu).
 #pragma once
 #include <cuda.h>
 
@@ -7,6 +7,9 @@
 namespace p2p {
 
 enum { EPI_PLAIN = 0, EPI_CONV1 = 1, EPI_CONV2 = 2, EPI_CORR = 3, EPI_FC = 4 };
+// where the A operand of a k-step comes from: TMA of a materialised tensor, gathered by producer warps (conv1), or TMA of
+// the per-image window maps (conv1)
+enum { AMODE_TMA = 0, AMODE_GATHER = 1, AMODE_WINDOW = 2 };
 constexpr int kMaxKSteps = 96;
 
 struct UmmaEpilogue {
@@ -27,7 +30,7 @@ struct UmmaEpilogue {
   int n_patches;
 };
 
-// conv1 with the patch gather fused into producer warps (1-pass launches): the A tile of every k-step
+// conv1 with the patch gather fused into producer warps (AMODE_GATHER): the A tile of every k-step
 // is built in shared memory straight from the channels-last fp16 pyramid copies.
 struct FusedGather {
   const float* img[2];            // [3][H][W]
@@ -36,10 +39,9 @@ struct FusedGather {
   int H[2], W[2];
   const void* matches;            // [n][4] int64 or fp32
   int is_float;
-  int generation;                 // 2: 128x512 tiles + lookup tables (default); 1: first version (128x256 tiles)
 };
 
-// conv1 fed by strided TMA boxes of the per-image window maps (fuse_gather = 3)
+// conv1 fed by strided TMA boxes of the per-image window maps (AMODE_WINDOW)
 struct WindowMaps {
   CUtensorMap map[2];             // [H + 2 pad][W + 2 pad][256] fp16 per image; box = 64 ch x 8 (stride 2) x 8 (stride 2)
   const __half* rgbn[2];          // [H + 2 pad][W + 2 pad][4]
@@ -53,28 +55,18 @@ struct UmmaGemmParams {
   KStep steps[kMaxKSteps];
   int nsteps;
   int m_tiles;           // 128-row tiles
-  int n_tiles;           // 256-column tiles
+  int n_tiles;           // 256-column blocks of B, each computed as two 128-column tiles (B tensor maps: 128-row boxes)
   int a_units_per_tile;  // step of the outermost A coordinate per m-tile (2 patches, or 128 rows)
-  int seg_len;           // k-steps accumulated in TMEM before a drain (0 / >= nsteps: whole K)
-  int pair;              // 1: CTA-pair kernel (cta_group::2); the B tensor maps must then use 128-row boxes
+  int seg_len;           // k-steps accumulated by the tensor core before a drain (0 / >= nsteps: whole K)
   const int* d_units;    // optional device count of A units (patches): m_tiles = ceil(*d_units / a_units_per_tile)
   UmmaEpilogue epi;
-  FusedGather fg;
+  FusedGather fg;        // AMODE_GATHER
+  WindowMaps wm;         // AMODE_WINDOW
 };
-
-struct Conv1TmaParams {
-  CUtensorMap b_hi;               // weights [512][73*64], 128-row boxes
-  WindowMaps wm;
-  KStep steps[kMaxKSteps];
-  int nsteps;
-  int m_tiles;                    // 128-row tiles (2 patches)
-  UmmaEpilogue epi;
-};
-int launch_conv1_tma(const Conv1TmaParams& p, int num_sms, cudaStream_t st);
 
 // estrides (optional): traversal strides; with stride s the box must be N * s to load N elements.
 int make_tmap_fp16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                    const uint32_t* box, const uint32_t* estrides = nullptr);
-int launch_umma_gemm(const UmmaGemmParams& p, int epi, int passes, int num_sms, cudaStream_t st, bool fused = false);
+int launch_umma_gemm(const UmmaGemmParams& p, int epi, int passes, int num_sms, cudaStream_t st, int amode = AMODE_TMA);
 
 }  // namespace p2p

@@ -2,7 +2,7 @@
 
 Same constructor config, same method names, same argument meaning and return shapes as
 `networks/patch2pix.py` (reference file:line cited per method), with the computation done by
-libp2p_b200.so (hand-written sm_100a kernels) instead of eager PyTorch:
+libp2p_b200.so (hand-written sm_90a kernels) instead of eager PyTorch:
 
     forward_coarse_match   networks/patch2pix.py:120-136
     cal_coarse_matches     networks/patch2pix.py:340-375
@@ -346,7 +346,7 @@ class Patch2PixB200(nn.Module):
             raise RuntimeError('Patch2PixB200 implements the inference path only (config.training must be False)')
         self.device = torch.device(config.device)
         if self.device.type != 'cuda':
-            raise RuntimeError('Patch2PixB200 needs a CUDA (sm_100a) device; there is no CPU fallback')
+            raise RuntimeError('Patch2PixB200 needs a CUDA (sm_90a) device; there is no CPU fallback')
         if config.backbone != 'ResNet34':
             raise RuntimeError('only the ResNet34 backbone of the released model is supported')
         self.backbone = config.backbone

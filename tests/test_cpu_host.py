@@ -180,10 +180,9 @@ def test_preprocess_oracle_is_pinned_against_pillow():
         assert cal_rescale_size(s, w, h, 2, 1 / 16) == PO.cal_rescale_size(s, w, h, 2, 1 / 16)
 
 
-def test_shipped_library_is_blackwell_native_sass():
-    """The hot kernels of the built library contain the sm_100a tensor-core / TMA mnemonics (tcgen05.mma = UTC*MMA incl.
-    the cta_group::2 form, cp.async.bulk.tensor = UTMALDG / UTMASTG, cp.async.bulk = UBLKCP, tcgen05.ld = LDTM) and no
-    legacy mma.sync (HMMA); profiles/r02_sass_summary.md is generated by the same scan (tools/sass_summary.py)."""
+def test_shipped_library_is_hopper_native_sass():
+    """The hot kernels of the built library contain the sm_90a tensor-core / TMA mnemonics (wgmma = HGMMA,
+    cp.async.bulk.tensor = UTMALDG / UTMASTG, cp.async.bulk = UBLKCP) and no legacy mma.sync (HMMA)."""
     import shutil
     if shutil.which('cuobjdump') is None:
         pytest.skip('cuobjdump not on PATH')
@@ -204,11 +203,9 @@ def test_shipped_library_is_blackwell_native_sass():
         hits = [v for k, v in per.items() if tag in k]
         assert hits, tag
         return '\n'.join(hits)
-    assert re.search(r'(?<![A-Z])HMMA', sass) is None          # UTCHMMA is tcgen05; a bare HMMA would be mma.sync
+    assert re.search(r'(?<![A-Z])HMMA', sass) is None          # HGMMA is wgmma; a bare HMMA would be mma.sync
     l1, l2 = body('nc_l1_umma_kernel'), body('nc_l2_umma_kernel')
-    assert l1.count('UTCHMMA') == 12 and 'UBLKCP' in l1 and 'UTMASTG' in l1 and 'LDTM' in l1
-    assert l2.count('UTCHMMA') >= 36 and 'UTMALDG' in l2 and 'LDTM' in l2
-    c1 = body('umma_conv1_tma_kernel')
-    assert 'UTCHMMA.2CTA' in c1 and 'UTMALDG' in c1
+    assert l1.count('HGMMA') == 12 and 'UBLKCP' in l1 and 'UTMASTG' in l1
+    assert l2.count('HGMMA') >= 36 and 'UTMALDG' in l2
     gemm = body('umma_gemm_kernel')
-    assert 'UTCHMMA.2CTA' in gemm and 'UTMALDG' in gemm and 'UTCBAR' in gemm
+    assert 'HGMMA.64x128x16.F32' in gemm and 'UTMALDG' in gemm
