@@ -172,9 +172,11 @@ __global__ void __launch_bounds__(kL1Threads, 1) nc_l1_umma_kernel(const __grid_
   fence_proxy_async();
   __syncthreads();
 
-  if (warp >= 4 && warp < 12) {
+  const int wgi = warpgroup_index();
+  if (wgi == 1 || wgi == 2) {
     // ===================== MMA + epilogue: warpgroup wg owns tile rows 64 wg .. 64 wg + 63 =====================
-    const int wg = (warp >> 2) - 1, wl = warp & 3;
+    const int wg = wgi - 1, wl = warp & 3;
+    const bool leader = threadIdx.x % 128 == 0;
     const int t = lane & 3;
     const int r0 = wg * 64 + 16 * wl + (lane >> 2);          // fragment rows r0 and r0 + 8
     float sx, sh;
@@ -207,10 +209,8 @@ __global__ void __launch_bounds__(kL1Threads, 1) nc_l1_umma_kernel(const __grid_
       wgmma_wait<0>();
       wgmma_fence_regs<32>(d64);
       wgmma_fence_regs<16>(d32);
-      if (threadIdx.x % 128 == 0) {
-        mbar_arrive(&empty_bar[st[0]]);
-        mbar_arrive(&empty_bar[st[1]]);
-      }
+      mbar_arrive_if(&empty_bar[st[0]], leader);
+      mbar_arrive_if(&empty_bar[st[1]], leader);
       const int a = fast_div(tile, inv_tb), b0 = (tile - a * TB) << 7;
       // The tile's 128 hidden lines are contiguous in global memory.  They go through a swizzled shared staging
       // buffer and leave with ONE tensor-map store per tile.  Rows past the end of the B grid are clipped by the
@@ -396,6 +396,7 @@ __global__ void __launch_bounds__(384, CTAS) nc_l2_umma_kernel(const __grid_cons
   fence_proxy_async();
   __syncthreads();
 
+  const int wgi = warpgroup_index();
   if (warp == 3) {
     // ===================== loader =====================
     if (lane == 0) {
@@ -413,9 +414,10 @@ __global__ void __launch_bounds__(384, CTAS) nc_l2_umma_kernel(const __grid_cons
         }
       }
     }
-  } else if (warp >= 4) {
+  } else if (wgi >= 1) {
     // ===================== MMA + epilogue: warpgroup wg owns MMA rows 64 wg .. 64 wg + 63 =====================
-    const int wg = (warp >> 2) - 1, wl = warp & 3;
+    const int wg = wgi - 1, wl = warp & 3;
+    const bool leader = threadIdx.x % 128 == 0;
     const int t = lane & 3;
     const int m0 = wg * 64 + 16 * wl + (lane >> 2);          // fragment rows m0 and m0 + 8
     float sx, sh;
@@ -454,7 +456,7 @@ __global__ void __launch_bounds__(384, CTAS) nc_l2_umma_kernel(const __grid_cons
         wgmma_fence_regs<16>(da[1]);
         wgmma_fence_regs<8>(db[0]);
         wgmma_fence_regs<8>(db[1]);
-        if (threadIdx.x % 128 == 0) mbar_arrive(&empty_bar[s]);
+        mbar_arrive_if(&empty_bar[s], leader);
       }
       const int a = fast_div(tile, inv_pa), rem = tile - a * per_a;
       const int kb = fast_div(rem, inv_lb), lb = rem - kb * p.LB;

@@ -142,6 +142,15 @@ struct GemmCfg {
   static constexpr int STAGES = PASSES == 3 ? 3 : (AMODE == AMODE_TMA ? 6 : 4);
   static constexpr int THREADS = AMODE == AMODE_TMA ? 384 : 512;
   static constexpr int SMEM = STAGES * STAGE_BYTES + 2 * kEpiBytes + 1024;
+  // Per-thread registers after setmaxnreg.  The kernel starts with 65536 / THREADS (rounded down to 8) everywhere;
+  // the producer warpgroup gives most of its share to the two consumer warpgroups (64 accumulators, plus 64 totals
+  // when SEGMENTED); the conv1 A-operand warpgroup (512 threads) keeps what it needs.
+  static constexpr int LAUNCH_REGS = (65536 / THREADS) & ~7;
+  static constexpr int PRODUCER_REGS = THREADS == 512 ? 24 : 40;
+  static constexpr int AUX_REGS = THREADS == 512 ? 128 : 0;
+  static constexpr int CONSUMER_REGS = THREADS == 512 ? 176 : 232;
+  static_assert(128 * (PRODUCER_REGS + 2 * CONSUMER_REGS + AUX_REGS) <= 65536, "register file overcommitted");
+  static_assert(PRODUCER_REGS <= LAUNCH_REGS && CONSUMER_REGS >= LAUNCH_REGS && AUX_REGS <= LAUNCH_REGS, "setmaxnreg direction");
 };
 
 __device__ __forceinline__ int fg_clamp(int v, int ds, int full) {   // ((x+dx)//ds).clamp(0, full//ds-1)
@@ -232,9 +241,11 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, AMODE>::THREADS, 1) umma_gemm_
     return v - 8 + kMapPad;
   };
 
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
+  const int wgi = warpgroup_index();
+  if (wgi == 0) {
+    // ===================== TMA producer (warp 0, one thread) =====================
+    setmaxnreg_dec<Cfg::PRODUCER_REGS>();
+    if (warp == 0 && lane == 0) {
       int it = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         const int m_tile = tile / n_halves, brow = (tile - m_tile * n_halves) * 128;
@@ -279,9 +290,11 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, AMODE>::THREADS, 1) umma_gemm_
         }
       }
     }
-  } else if (warp >= 4 && warp < 12) {
+  } else if (wgi < 3) {
     // ===================== wgmma consumers + epilogue (warpgroups 1 and 2) =====================
-    const int wg = (warp >> 2) - 1, wl = warp & 3;
+    setmaxnreg_inc<Cfg::CONSUMER_REGS>();
+    const int wg = wgi - 1, wl = warp & 3;
+    const bool leader = threadIdx.x % 128 == 0;    // arrives on empty_bar for the warpgroup
     uint64_t* ready = AMODE == AMODE_WINDOW ? ready_bar : full_bar;
     float* stg = epi_smem + wg * (64 * kEpiPitch);
     float acc[64];
@@ -293,7 +306,9 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, AMODE>::THREADS, 1) umma_gemm_
 #pragma unroll
         for (int i = 0; i < 64; ++i) tot[i] = 0.f;
       }
-      int prev_s = -1;
+      // Each k-step's MMAs are one wgmma group.  wait_group 1 after issuing step ks retires step ks - 1, whose stage
+      // is then released, so the tensor core always has the next group queued.  An interior segment end drains the
+      // pipe (wait_group 0) to add the partial sum and releases both stages; the tile's last step drains after the loop.
       for (int ks = 0; ks < nsteps; ++ks, ++it) {
         const int s = it % STAGES;
         mbar_wait(&ready[s], (uint32_t)(it / STAGES) & 1u);
@@ -319,22 +334,26 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, AMODE>::THREADS, 1) umma_gemm_
           accf = 1u;
         }
         wgmma_commit();
-        const bool seg_end = ((ks + 1) % seg_len) == 0 || (ks + 1) == nsteps;
+        // both conditions depend on the k-step counter and kernel parameters only: uniform across the warpgroup
+        const bool seg_end = SEGMENTED && ((ks + 1) % seg_len) == 0 && (ks + 1) < nsteps;
+        const bool prev_pending = SEGMENTED ? (ks % seg_len) != 0 : ks != 0;   // step ks - 1 is not yet released
         if (seg_end) {
           wgmma_wait<0>();
           wgmma_fence_regs<64>(acc);
-          if (prev_s >= 0 && threadIdx.x % 128 == 0) mbar_arrive(&empty_bar[prev_s]);
-          if (threadIdx.x % 128 == 0) mbar_arrive(&empty_bar[s]);
-          prev_s = -1;
-          if (SEGMENTED) {
 #pragma unroll
-            for (int i = 0; i < 64; ++i) tot[i] += acc[i];
-          }
+          for (int i = 0; i < 64; ++i) tot[i] += acc[i];
         } else {
-          wgmma_wait<1>();          // the previous k-step's MMAs are done: its stage can be refilled
-          if (prev_s >= 0 && threadIdx.x % 128 == 0) mbar_arrive(&empty_bar[prev_s]);
-          prev_s = s;
+          wgmma_wait<1>();
         }
+        mbar_arrive_if(&empty_bar[(s + STAGES - 1) % STAGES], leader && prev_pending);
+        mbar_arrive_if(&empty_bar[s], leader && seg_end);
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs<64>(acc);
+      mbar_arrive_if(&empty_bar[(it + STAGES - 1) % STAGES], leader);   // the tile's last k-step
+      if (SEGMENTED) {
+#pragma unroll
+        for (int i = 0; i < 64; ++i) tot[i] += acc[i];
       }
       const float* res = SEGMENTED ? tot : acc;
       // fragment -> row-major staging, 64 columns at a time; then one row per thread
@@ -359,8 +378,9 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, AMODE>::THREADS, 1) umma_gemm_
         epilogue_piece<EPI>(p.epi, n_units, m_tile, wg * 64 + er, col0 + half * 64 + ec, v);
       }
     }
-  } else if (AMODE == AMODE_GATHER && warp >= 12) {
+  } else if (AMODE == AMODE_GATHER) {
     // ===================== fused A-operand producers (warpgroup 3) =====================
+    if constexpr (Cfg::AUX_REGS < Cfg::LAUNCH_REGS) setmaxnreg_dec<Cfg::AUX_REGS>();
     // 8 lanes per tile row (8 channels = 16 B each), 16 rows per pass, 8 passes per k-step.  Warps drift across
     // pipeline stages independently, which hides the L2 latency of the gathers.
     const int ptid = threadIdx.x - 384;
@@ -468,8 +488,9 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, AMODE>::THREADS, 1) umma_gemm_
         if (lane == 0) mbar_arrive(&full_bar[s]);
       }
     }
-  } else if (AMODE == AMODE_WINDOW && warp >= 12) {
+  } else if (AMODE == AMODE_WINDOW) {
     // ===================== aux warps (warpgroup 3): zero-padding fix-up and the rgb im2col k-step =====================
+    if constexpr (Cfg::AUX_REGS < Cfg::LAUNCH_REGS) setmaxnreg_dec<Cfg::AUX_REGS>();
     const int row = threadIdx.x - 384;               // 0..127: the tile row this thread owns
     int it = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {

@@ -20,34 +20,46 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
+// arrive only where `pred` holds (one elected thread): a predicated instruction, not a branch, so it may sit between
+// wgmma issue and wgmma.wait_group without making ptxas serialise the MMAs
+__device__ __forceinline__ void mbar_arrive_if(uint64_t* bar, bool pred) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-      "selp.u32 %0, 1, 0, p;\n"
-      "}\n"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
+      "setp.ne.b32 p, %1, 0;\n"
+      "@p mbarrier.arrive.shared::cta.b64 _, [%0];\n"
+      "}\n" ::"r"(smem_u32(bar)), "r"((uint32_t)pred)
       : "memory");
-  return ok != 0;
 }
 // Bounded spin: a protocol bug traps (launch error) instead of hanging the GPU.  The clock is read once per 4096
-// failed probes only (an if-converted clock read in the probe loop costs issue slots the producer warps need).
+// failed probes only (a clock read in the probe loop costs issue slots the producer warps need).  The whole loop is
+// one asm block: a function call (printf) or a C++-level loop around the probe inside the consumers' wgmma region
+// makes ptxas serialise every MMA of the kernel.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  if (mbar_try_wait(bar, parity)) return;
-  const long long t0 = clock64();
-  for (;;) {
-#pragma unroll 1
-    for (int i = 0; i < 4096; ++i)
-      if (mbar_try_wait(bar, parity)) return;
-    if (clock64() - t0 > 6000000000ll) {           // ~3-4 s
-      printf("mbar_wait timeout: block %d thread %d barrier 0x%x parity %u\n", (int)blockIdx.x, (int)threadIdx.x,
-             smem_u32(bar), parity);
-      __trap();
-    }
-  }
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      ".reg .u32 n;\n"
+      ".reg .s64 t0, t1;\n"
+      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
+      "@p bra DONE;\n"
+      "mov.u64 t0, %%clock64;\n"
+      "ROUND:\n"
+      "mov.u32 n, 4096;\n"
+      "PROBE:\n"
+      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
+      "@p bra DONE;\n"
+      "sub.u32 n, n, 1;\n"
+      "setp.ne.u32 p, n, 0;\n"
+      "@p bra PROBE;\n"
+      "mov.u64 t1, %%clock64;\n"
+      "sub.s64 t1, t1, t0;\n"
+      "setp.lt.s64 p, t1, 6000000000;\n"           // ~3-4 s
+      "@p bra ROUND;\n"
+      "trap;\n"
+      "DONE:\n"
+      "}\n" ::"r"(smem_u32(bar)), "r"(parity)
+      : "memory");
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 // generic-proxy shared-memory stores -> visible to TMA and the tensor core (async proxy)
@@ -111,6 +123,16 @@ template <int N>
 __device__ __forceinline__ void wgmma_wait() {     // at most N committed groups still in flight
   asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
+// Register reallocation between warpgroups: every thread of the warpgroup executes it, with a multiple of 8 in
+// [24, 256].  dec hands registers back to the CTA's pool, inc blocks until the pool has them.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+// threadIdx.x / 128 as a value ptxas knows to be warp-uniform: role branches on it are not divergent, which wgmma
+// pipelining needs
+__device__ __forceinline__ int warpgroup_index() { return __shfl_sync(0xffffffffu, (int)threadIdx.x / 128, 0); }
+
 // keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
 template <int R>
 __device__ __forceinline__ void wgmma_fence_regs(float* d) {
