@@ -131,25 +131,43 @@ __device__ __forceinline__ void epilogue_piece(const UmmaEpilogue& e, int n_patc
 // the kernel
 // ------------------------------------------------------------------------------------------------
 constexpr int kATile = 128 * 128;   // 128 rows x 64 fp16
-constexpr int kBTile = 128 * 128;   // 128 output columns x 64 fp16
+constexpr int kBTile = 128 * 128;   // one TMA box of B: 128 output columns x 64 fp16
 constexpr int kEpiPitch = 65;       // floats per staged accumulator row: row-wise reads hit 32 distinct banks
 constexpr int kEpiBytes = 64 * kEpiPitch * 4;
+constexpr int kMaxSmemPerBlock = 232448;   // sm_90 opt-in limit, static + dynamic
 
-template <int PASSES, int AMODE>
+template <int PASSES, bool SEGMENTED, int AMODE>
 struct GemmCfg {
   static constexpr int NOP = PASSES == 3 ? 2 : 1;
-  static constexpr int STAGE_BYTES = NOP * (kATile + kBTile);
-  static constexpr int STAGES = PASSES == 3 ? 3 : (AMODE == AMODE_TMA ? 6 : 4);
   static constexpr int THREADS = AMODE == AMODE_TMA ? 384 : 512;
+  // Output columns per tile.  The 1-pass unsegmented 384-thread kernels use 128x256 tiles (m64n256k16, 128
+  // accumulators per consumer thread): half the shared-memory operand reads per MAC, half the A re-streaming and half
+  // the epilogues of 128x128.  Everything else stays at 128:
+  //   3-pass and segmented kernels: their fp32 totals do not fit beside 128 accumulators;
+  //   512-thread conv1 kernels (AMODE_GATHER / AMODE_WINDOW): ptxas needs each instruction's operands to fit the
+  //   kernel-wide register target, 65536 / 512 = 128, whatever setmaxnreg grants, so m64n256k16 does not compile
+  //   there; two m64n128k16 per k16 slice do, but the epilogue beside 128 accumulators then spills at every
+  //   producer / A-operand / consumer split that fits their 4 x 128 registers per thread slot.
+  static constexpr int BN = PASSES == 1 && !SEGMENTED && THREADS == 384 ? 256 : 128;
+  static constexpr int B_BYTES = BN * 128;                 // BN rows x 64 fp16, BN / 128 TMA boxes back to back
+  static constexpr int STAGE_BYTES = NOP * (kATile + B_BYTES);
+  // 48 KB 256-wide stages: 4 fit beside the epilogue staging (6 of the 32 KB 1-pass 128-wide ones)
+  static constexpr int STAGES = PASSES == 3 ? 3 : (THREADS == 512 ? 4 : (BN == 256 ? 4 : 6));
   static constexpr int SMEM = STAGES * STAGE_BYTES + 2 * kEpiBytes + 1024;
+  static constexpr int FG = AMODE == AMODE_GATHER ? 16 : 1;
+  static constexpr int STATIC_SMEM = 3 * STAGES * 8 + 2 * 2 * FG * FG * 4 + 2 * 4 * 4;   // barriers, fg_dinv, fg_org
+  static_assert(SMEM + STATIC_SMEM <= kMaxSmemPerBlock, "shared memory over the per-block limit");
   // Per-thread registers after setmaxnreg.  The kernel starts with 65536 / THREADS (rounded down to 8) everywhere;
-  // the producer warpgroup gives most of its share to the two consumer warpgroups (64 accumulators, plus 64 totals
-  // when SEGMENTED); the conv1 A-operand warpgroup (512 threads) keeps what it needs.
+  // the producer warpgroup gives most of its share to the two consumer warpgroups (BN / 2 accumulators, plus 64
+  // totals when SEGMENTED); the conv1 A-operand warpgroup (512 threads) keeps what it needs.
   static constexpr int LAUNCH_REGS = (65536 / THREADS) & ~7;
-  static constexpr int PRODUCER_REGS = THREADS == 512 ? 24 : 40;
+  // 256-wide: 240 per consumer (the 1-pass correlation epilogue spills at 232 beside 128 accumulators).
+  static constexpr int PRODUCER_REGS = THREADS == 512 || BN == 256 ? 24 : 40;
   static constexpr int AUX_REGS = THREADS == 512 ? 128 : 0;
-  static constexpr int CONSUMER_REGS = THREADS == 512 ? 176 : 232;
-  static_assert(128 * (PRODUCER_REGS + 2 * CONSUMER_REGS + AUX_REGS) <= 65536, "register file overcommitted");
+  static constexpr int CONSUMER_REGS = THREADS == 512 ? 176 : (BN == 256 ? 240 : 232);
+  // setmaxnreg.inc only gets what other warpgroups of the CTA released from its launch allocation (LAUNCH_REGS per
+  // thread), not the rest of the register file: a larger sum leaves the consumers blocked in setmaxnreg forever
+  static_assert(PRODUCER_REGS + 2 * CONSUMER_REGS + AUX_REGS <= THREADS / 128 * LAUNCH_REGS, "register budget overcommitted");
   static_assert(PRODUCER_REGS <= LAUNCH_REGS && CONSUMER_REGS >= LAUNCH_REGS && AUX_REGS <= LAUNCH_REGS, "setmaxnreg direction");
 };
 
@@ -163,7 +181,8 @@ __device__ __forceinline__ void named_bar(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
-// Tile = 128 rows x 128 columns; K chunk 64 (one 128-byte swizzle row) per pipeline stage.
+// Tile = 128 rows x BN columns (see GemmCfg); K chunk 64 (one 128-byte swizzle row)
+// per pipeline stage.
 // Warpgroup 0: warp 0 is the TMA producer.  Warpgroups 1 and 2: wgmma consumers, rows 0..63 and 64..127, fp32
 // accumulators in registers; their epilogue stages the accumulators through shared memory so that every epilogue
 // thread owns one tile row (32 consecutive columns per piece), the layout epilogue_piece expects.
@@ -179,10 +198,11 @@ __device__ __forceinline__ void named_bar(int id, int threads) {
 // k-steps and each partial sum is added to fp32 register totals with round-to-nearest, which bounds the
 // accumulator-rounding drift of long K chains.
 template <int PASSES, bool SEGMENTED, int EPI, int AMODE>
-__global__ void __launch_bounds__(GemmCfg<PASSES, AMODE>::THREADS, 1) umma_gemm_kernel(const __grid_constant__ UmmaGemmParams p) {
+__global__ void __launch_bounds__(GemmCfg<PASSES, SEGMENTED, AMODE>::THREADS, 1) umma_gemm_kernel(const __grid_constant__ UmmaGemmParams p) {
   static_assert(AMODE == AMODE_TMA || (PASSES == 1 && !SEGMENTED && EPI == EPI_CONV1), "fused A operand: conv1, 1-pass only");
-  using Cfg = GemmCfg<PASSES, AMODE>;
+  using Cfg = GemmCfg<PASSES, SEGMENTED, AMODE>;
   constexpr int STAGES = Cfg::STAGES, NOP = Cfg::NOP, STAGE_BYTES = Cfg::STAGE_BYTES;
+  constexpr int BN = Cfg::BN, B_BYTES = Cfg::B_BYTES, NACC = BN / 2;
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -190,7 +210,7 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, AMODE>::THREADS, 1) umma_gemm_
   __shared__ __align__(8) uint64_t full_bar[STAGES];    // TMA bytes landed (+ gather warps in AMODE_GATHER)
   __shared__ __align__(8) uint64_t ready_bar[STAGES];   // AMODE_WINDOW: the aux warps have fixed the stage up
   __shared__ __align__(8) uint64_t empty_bar[STAGES];   // both consumer warpgroups are done reading the stage
-  constexpr int FG = AMODE == AMODE_GATHER ? 16 : 1;
+  constexpr int FG = Cfg::FG;
   __shared__ float fg_dinv[2][2][FG][FG];               // act_scale / patch norm per (patch, image, window pixel)
   __shared__ int fg_org[2][4];                          // window origins (x1,y1,x2,y2) - 8
 
@@ -201,8 +221,8 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, AMODE>::THREADS, 1) umma_gemm_
     n_units = __ldg(p.d_units);
     m_tiles = (n_units + p.a_units_per_tile - 1) / p.a_units_per_tile;
   }
-  const int n_halves = 2 * p.n_tiles;                    // 128-column tiles
-  const int total_tiles = m_tiles * n_halves;
+  const int n_col_tiles = p.n_tiles * (256 / BN);          // BN-column tiles
+  const int total_tiles = m_tiles * n_col_tiles;
   const int nsteps = p.nsteps;
   const int seg_len = SEGMENTED ? p.seg_len : nsteps;
 
@@ -247,8 +267,13 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, AMODE>::THREADS, 1) umma_gemm_
     setmaxnreg_dec<Cfg::PRODUCER_REGS>();
     if (warp == 0 && lane == 0) {
       int it = 0;
+      // B tile of a stage: BN / 128 boxes of 128 rows into consecutive 16 KB, one descriptor spans them
+      auto load_b = [&](const CUtensorMap* map, uint64_t* bar, uint8_t* dst, int bk, int brow) {
+#pragma unroll
+        for (int h = 0; h < BN / 128; ++h) tma_load_2d(map, bar, dst + h * kBTile, bk, brow + h * 128);
+      };
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const int m_tile = tile / n_halves, brow = (tile - m_tile * n_halves) * 128;
+        const int m_tile = tile / n_col_tiles, brow = (tile - m_tile * n_col_tiles) * BN;
         const int a4 = m_tile * p.a_units_per_tile;
         int o[2][4];
         if (AMODE == AMODE_WINDOW) {
@@ -263,11 +288,11 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, AMODE>::THREADS, 1) umma_gemm_
           const KStep k = p.steps[ks];  // param space (constant bank)
           uint8_t* st = smem + (size_t)s * STAGE_BYTES;
           if (AMODE == AMODE_GATHER) {
-            mbar_expect_tx(&full_bar[s], kBTile);
-            tma_load_2d(&p.b_hi, &full_bar[s], st + kATile, k.bk, brow);
+            mbar_expect_tx(&full_bar[s], B_BYTES);
+            load_b(&p.b_hi, &full_bar[s], st + kATile, k.bk, brow);
           } else if (AMODE == AMODE_WINDOW) {
-            mbar_expect_tx(&full_bar[s], k.kind == 0 ? kATile + kBTile : kBTile);
-            tma_load_2d(&p.b_hi, &full_bar[s], st + kATile, k.bk, brow);
+            mbar_expect_tx(&full_bar[s], k.kind == 0 ? kATile + B_BYTES : B_BYTES);
+            load_b(&p.b_hi, &full_bar[s], st + kATile, k.bk, brow);
             if (k.kind == 0) {
               const int ty = (k.plane & 2) ? 1 : (k.y < 0 ? 0 : 2), tx = (k.plane & 1) ? 1 : (k.x < 0 ? 0 : 2);
               const int chunk = k.c0 >> 6, si = chunk >> 2, c0 = (chunk & 3) * 64;
@@ -284,8 +309,8 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, AMODE>::THREADS, 1) umma_gemm_
               tma_load_5d(&p.a_rgb_hi, &full_bar[s], st, 0, 0, 0, 0, a4);
               if (PASSES == 3) tma_load_5d(&p.a_rgb_lo, &full_bar[s], st + kATile, 0, 0, 0, 0, a4);
             }
-            tma_load_2d(&p.b_hi, &full_bar[s], st + NOP * kATile, k.bk, brow);
-            if (PASSES == 3) tma_load_2d(&p.b_lo, &full_bar[s], st + NOP * kATile + kBTile, k.bk, brow);
+            load_b(&p.b_hi, &full_bar[s], st + NOP * kATile, k.bk, brow);
+            if (PASSES == 3) load_b(&p.b_lo, &full_bar[s], st + NOP * kATile + B_BYTES, k.bk, brow);
           }
         }
       }
@@ -297,14 +322,14 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, AMODE>::THREADS, 1) umma_gemm_
     const bool leader = threadIdx.x % 128 == 0;    // arrives on empty_bar for the warpgroup
     uint64_t* ready = AMODE == AMODE_WINDOW ? ready_bar : full_bar;
     float* stg = epi_smem + wg * (64 * kEpiPitch);
-    float acc[64];
-    float tot[SEGMENTED ? 64 : 1];
+    float acc[NACC];
+    float tot[SEGMENTED ? NACC : 1];
     int it = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      const int m_tile = tile / n_halves, col0 = (tile - m_tile * n_halves) * 128;
+      const int m_tile = tile / n_col_tiles, col0 = (tile - m_tile * n_col_tiles) * BN;
       if (SEGMENTED) {
 #pragma unroll
-        for (int i = 0; i < 64; ++i) tot[i] = 0.f;
+        for (int i = 0; i < NACC; ++i) tot[i] = 0.f;
       }
       // Each k-step's MMAs are one wgmma group.  wait_group 1 after issuing step ks retires step ks - 1, whose stage
       // is then released, so the tensor core always has the next group queued.  An interior segment end drains the
@@ -319,18 +344,18 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, AMODE>::THREADS, 1) umma_gemm_
         wgmma_fence();
         if (PASSES == 3) {
           const uint64_t a_lo = make_sw128_desc(sa + kATile + wg * 8192);
-          const uint64_t b_lo = make_sw128_desc(sa + NOP * kATile + kBTile);
+          const uint64_t b_lo = make_sw128_desc(sa + NOP * kATile + B_BYTES);
 #pragma unroll
           for (int kk = 0; kk < 4; ++kk) {
-            wgmma_f16<128>(acc, a_lo + 2 * kk, b_hi + 2 * kk, accf);
+            wgmma_f16<BN>(acc, a_lo + 2 * kk, b_hi + 2 * kk, accf);
             accf = 1u;
           }
 #pragma unroll
-          for (int kk = 0; kk < 4; ++kk) wgmma_f16<128>(acc, a_hi + 2 * kk, b_lo + 2 * kk, 1u);
+          for (int kk = 0; kk < 4; ++kk) wgmma_f16<BN>(acc, a_hi + 2 * kk, b_lo + 2 * kk, 1u);
         }
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk) {
-          wgmma_f16<128>(acc, a_hi + 2 * kk, b_hi + 2 * kk, accf);
+          wgmma_f16<BN>(acc, a_hi + 2 * kk, b_hi + 2 * kk, accf);
           accf = 1u;
         }
         wgmma_commit();
@@ -339,9 +364,9 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, AMODE>::THREADS, 1) umma_gemm_
         const bool prev_pending = SEGMENTED ? (ks % seg_len) != 0 : ks != 0;   // step ks - 1 is not yet released
         if (seg_end) {
           wgmma_wait<0>();
-          wgmma_fence_regs<64>(acc);
+          wgmma_fence_regs<NACC>(acc);
 #pragma unroll
-          for (int i = 0; i < 64; ++i) tot[i] += acc[i];
+          for (int i = 0; i < NACC; ++i) tot[i] += acc[i];
         } else {
           wgmma_wait<1>();
         }
@@ -349,22 +374,22 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, AMODE>::THREADS, 1) umma_gemm_
         mbar_arrive_if(&empty_bar[s], leader && seg_end);
       }
       wgmma_wait<0>();
-      wgmma_fence_regs<64>(acc);
+      wgmma_fence_regs<NACC>(acc);
       mbar_arrive_if(&empty_bar[(it + STAGES - 1) % STAGES], leader);   // the tile's last k-step
       if (SEGMENTED) {
 #pragma unroll
-        for (int i = 0; i < 64; ++i) tot[i] += acc[i];
+        for (int i = 0; i < NACC; ++i) tot[i] += acc[i];
       }
       const float* res = SEGMENTED ? tot : acc;
       // fragment -> row-major staging, 64 columns at a time; then one row per thread
       const int fr = 16 * wl + (lane >> 2), fc = 2 * (lane & 3);
       const int er = (wl & 1) * 32 + lane, ec = (wl >> 1) * 32;
 #pragma unroll
-      for (int half = 0; half < 2; ++half) {
+      for (int c64 = 0; c64 < BN / 64; ++c64) {
         named_bar(1 + wg, 128);                 // the previous piece has been read
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
-          const float* d = res + 4 * (half * 8 + j);
+          const float* d = res + 4 * (c64 * 8 + j);
           float* o = stg + fr * kEpiPitch + 8 * j + fc;
           o[0] = d[0];
           o[1] = d[1];
@@ -375,7 +400,7 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, AMODE>::THREADS, 1) umma_gemm_
         float v[32];
 #pragma unroll
         for (int i = 0; i < 32; ++i) v[i] = stg[er * kEpiPitch + ec + i];
-        epilogue_piece<EPI>(p.epi, n_units, m_tile, wg * 64 + er, col0 + half * 64 + ec, v);
+        epilogue_piece<EPI>(p.epi, n_units, m_tile, wg * 64 + er, col0 + c64 * 64 + ec, v);
       }
     }
   } else if (AMODE == AMODE_GATHER) {
@@ -388,7 +413,7 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, AMODE>::THREADS, 1) umma_gemm_
     const FusedGather& g = p.fg;
     int it = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      const int m_tile = tile / n_halves;
+      const int m_tile = tile / n_col_tiles;
       named_bar(3, 128);   // nobody still reads the previous tile's tables
       if (ptid < 8) {
         const int pp = ptid >> 2, j = ptid & 3;
@@ -494,7 +519,7 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, AMODE>::THREADS, 1) umma_gemm_
     const int row = threadIdx.x - 384;               // 0..127: the tile row this thread owns
     int it = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      const int m_tile = tile / n_halves;
+      const int m_tile = tile / n_col_tiles;
       for (int ks = 0; ks < nsteps; ++ks, ++it) {
         const int s = it % STAGES;
         const uint32_t ph = (uint32_t)(it / STAGES) & 1u;
@@ -635,9 +660,11 @@ int make_tmap_fp16(CUtensorMap* out, const void* base, int rank, const uint64_t*
 }
 
 template <int PASSES, bool SEGMENTED, int EPI, int AMODE = AMODE_TMA>
-static int launch_one(const UmmaGemmParams& p, int grid, cudaStream_t st) {
-  using Cfg = GemmCfg<PASSES, AMODE>;
+static int launch_one(const UmmaGemmParams& p, int num_sms, cudaStream_t st) {
+  using Cfg = GemmCfg<PASSES, SEGMENTED, AMODE>;
   auto kern = umma_gemm_kernel<PASSES, SEGMENTED, EPI, AMODE>;
+  const int total = p.m_tiles * p.n_tiles * (256 / Cfg::BN);
+  const int grid = total < num_sms ? total : num_sms;
   P2P_ENSURE_SMEM(kern, Cfg::SMEM);
   kern<<<grid, Cfg::THREADS, Cfg::SMEM, st>>>(p);
   P2P_LAUNCH_OK();
@@ -645,29 +672,27 @@ static int launch_one(const UmmaGemmParams& p, int grid, cudaStream_t st) {
 }
 
 template <int EPI>
-static int launch_epi(const UmmaGemmParams& p, int passes, bool seg, int grid, cudaStream_t st) {
-  if (passes == 3) return seg ? launch_one<3, true, EPI>(p, grid, st) : launch_one<3, false, EPI>(p, grid, st);
-  return seg ? launch_one<1, true, EPI>(p, grid, st) : launch_one<1, false, EPI>(p, grid, st);
+static int launch_epi(const UmmaGemmParams& p, int passes, bool seg, int num_sms, cudaStream_t st) {
+  if (passes == 3) return seg ? launch_one<3, true, EPI>(p, num_sms, st) : launch_one<3, false, EPI>(p, num_sms, st);
+  return seg ? launch_one<1, true, EPI>(p, num_sms, st) : launch_one<1, false, EPI>(p, num_sms, st);
 }
 
 int launch_umma_gemm(const UmmaGemmParams& p, int epi, int passes, int num_sms, cudaStream_t st, int amode) {
   P2P_REQUIRE(passes == 1 || passes == 3, "umma gemm: passes must be 1 or 3");
   P2P_REQUIRE(p.nsteps > 0 && p.m_tiles > 0 && p.n_tiles > 0, "umma gemm: empty problem");
   const bool seg = p.seg_len > 0 && p.seg_len < p.nsteps;
-  const int total = p.m_tiles * p.n_tiles * 2;
-  const int grid = total < num_sms ? total : num_sms;
   if (amode != AMODE_TMA) {
     P2P_REQUIRE(epi == EPI_CONV1 && passes == 1 && !seg, "the fused A operand is available for 1-pass conv1 only");
-    if (amode == AMODE_GATHER) return launch_one<1, false, EPI_CONV1, AMODE_GATHER>(p, grid, st);
+    if (amode == AMODE_GATHER) return launch_one<1, false, EPI_CONV1, AMODE_GATHER>(p, num_sms, st);
     P2P_REQUIRE(amode == AMODE_WINDOW, "umma gemm: unknown A mode");
-    return launch_one<1, false, EPI_CONV1, AMODE_WINDOW>(p, grid, st);
+    return launch_one<1, false, EPI_CONV1, AMODE_WINDOW>(p, num_sms, st);
   }
   switch (epi) {
-    case EPI_PLAIN: return launch_epi<EPI_PLAIN>(p, passes, seg, grid, st);
-    case EPI_CONV1: return launch_epi<EPI_CONV1>(p, passes, seg, grid, st);
-    case EPI_CONV2: return launch_epi<EPI_CONV2>(p, passes, seg, grid, st);
-    case EPI_CORR: return launch_epi<EPI_CORR>(p, passes, seg, grid, st);
-    case EPI_FC: return launch_epi<EPI_FC>(p, passes, seg, grid, st);
+    case EPI_PLAIN: return launch_epi<EPI_PLAIN>(p, passes, seg, num_sms, st);
+    case EPI_CONV1: return launch_epi<EPI_CONV1>(p, passes, seg, num_sms, st);
+    case EPI_CONV2: return launch_epi<EPI_CONV2>(p, passes, seg, num_sms, st);
+    case EPI_CORR: return launch_epi<EPI_CORR>(p, passes, seg, num_sms, st);
+    case EPI_FC: return launch_epi<EPI_FC>(p, passes, seg, num_sms, st);
   }
   set_last_error("umma gemm: unknown epilogue");
   return -1;

@@ -55,7 +55,8 @@ struct UmmaGemmParams {
   KStep steps[kMaxKSteps];
   int nsteps;
   int m_tiles;           // 128-row tiles
-  int n_tiles;           // 256-column blocks of B, each computed as two 128-column tiles (B tensor maps: 128-row boxes)
+  int n_tiles;           // 256-column blocks of B: one 256-column tile (1-pass unsegmented) or two 128-column tiles;
+                         // B tensor maps have 128-row boxes
   int a_units_per_tile;  // step of the outermost A coordinate per m-tile (2 patches, or 128 rows)
   int seg_len;           // k-steps accumulated by the tensor core before a drain (0 / >= nsteps: whole K)
   const int* d_units;    // optional device count of A units (patches): m_tiles = ceil(*d_units / a_units_per_tile)
