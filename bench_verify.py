@@ -1,0 +1,121 @@
+"""Time match verification: p2p_find_model on the GPU against OpenCV on the host, on the same rows.
+
+    python bench_verify.py [--calls 200] [--cpu-reps 20]
+
+Two workloads of 3200 rows each, for F and for H:
+  * `fine`: the fine matches of one pair of bench.py's workload (640x480 synthetic_pair_shifted, consensus NC weights,
+    ptmax 400, panc 8).  The seeded regressor is untrained, so these rows carry little consistent geometry and RANSAC
+    tends to run to max_iters.
+  * `scene`: synthetic_two_view with 50 % outliers and 0.5 px noise (planar for H), where the stopping bound ends
+    RANSAC early.
+Threshold 1 px for F and 2 px for H as in the reference's notebook, conf 0.999, at most 10000 iterations, seed 0.
+GPU time: CUDA events around `--calls` back-to-back calls.  CPU time: host clock around `--cpu-reps` calls of
+cv2.findFundamentalMat (USAC_ACCURATE) / cv2.findHomography (RANSAC), or null without cv2.  Prints one JSON line and
+writes nothing.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+import torch
+
+ROOT = os.path.dirname(os.path.abspath(__file__))
+sys.path.insert(0, ROOT)
+
+TH = {'F': 1.0, 'H': 2.0}
+
+
+def fine_matches(dev):
+    from argparse import Namespace
+    from patch2pix_b200.model import Patch2PixB200
+    from patch2pix_b200.synth import make_seeded_state_dict, synthetic_pair_shifted
+    rc = Namespace(conv_dims=[512, 512], conv_kers=[3, 3], conv_strs=[2, 1], fc_dims=[512, 256], feat_comb='pre',
+                   psize=[16, 16], pshift=8, panc=8, shared=False)
+    cfg = Namespace(training=False, device=dev, regr_batch=1200, backbone='ResNet34', feat_idx=[0, 1, 2, 3],
+                    weights_dict=make_seeded_state_dict(0, nc_init='consensus'), change_stride=True, regressor_config=rc)
+    net = Patch2PixB200(cfg)
+    im1, im2 = synthetic_pair_shifted(0, 480, 640)
+    with torch.no_grad():
+        f1 = net.extract.forward_all(im1.to(dev), [], True)
+        f2 = net.extract.forward_all(im2.to(dev), [], True)
+        np.random.seed(0)
+        fine, _, _ = net.match_from_feats(f1, f2, 2, ptmax=400)
+    return fine[0].reshape(-1, 4).double().contiguous()
+
+
+def scene_rows(kind, n, dev):
+    from patch2pix_b200.synth import synthetic_two_view
+    sc = synthetic_two_view(0, n, 0.5, 0.5, planar=kind == 'H')
+    return torch.from_numpy(np.concatenate([sc['pts1'], sc['pts2']], 1)).to(dev)
+
+
+def time_one(kind, rows, calls, cpu_reps):
+    from patch2pix_b200 import _lib
+    from patch2pix_b200 import verify as V
+    th, n = TH[kind], int(rows.shape[0])
+    h = _lib.default_handle(rows.device)
+    out = torch.empty(V.out_size(n), dtype=torch.float64, device=rows.device)
+    model = V.MODEL_F if kind == 'F' else V.MODEL_H
+    for _ in range(5):
+        V.find_model_into(h, model, rows, 4, n, None, th, 0.999, 10000, 0, out)
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    torch.cuda.synchronize()
+    e0.record()
+    for _ in range(calls):
+        V.find_model_into(h, model, rows, 4, n, None, th, 0.999, 10000, 0, out)
+    e1.record()
+    torch.cuda.synchronize()
+    _, mask = V.parse_host(out.cpu().numpy(), n)
+    res = {'rows': n, 'ms_gpu': e0.elapsed_time(e1) / calls, 'inliers_gpu': int(mask.sum()), 'ms_cpu': None,
+           'inliers_cpu': None}
+    try:
+        import cv2
+    except ImportError:
+        return res
+    pts = rows.cpu().numpy()
+    p1, p2 = pts[:, :2].copy(), pts[:, 2:].copy()
+    if kind == 'F':
+        run = lambda: cv2.findFundamentalMat(p1, p2, cv2.USAC_ACCURATE, th, 0.999, 10000)
+    else:
+        run = lambda: cv2.findHomography(p1, p2, cv2.RANSAC, th, maxIters=10000, confidence=0.999)
+    _, cm = run()
+    t0 = time.perf_counter()
+    for _ in range(cpu_reps):
+        run()
+    res.update(ms_cpu=(time.perf_counter() - t0) * 1e3 / cpu_reps, inliers_cpu=None if cm is None else int(cm.sum()))
+    return res
+
+
+def card():
+    try:
+        q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'],
+                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
+        return q[torch.cuda.current_device()] if q else None
+    except (OSError, subprocess.SubprocessError):
+        return None
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument('--calls', type=int, default=200)
+    ap.add_argument('--cpu-reps', type=int, default=20)
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise RuntimeError('bench_verify.py needs a CUDA device: there is no CPU fallback')
+    dev = torch.device('cuda', torch.cuda.current_device())
+    fine = fine_matches(dev)
+    line = {'metric': 'ms per verification call', 'card': card(), 'cpu_cores': os.cpu_count(),
+            'config': {'th_px': TH, 'conf': 0.999, 'max_iters': 10000, 'seed': 0, 'calls': args.calls,
+                       'cpu_reps': args.cpu_reps, 'cpu': 'cv2.findFundamentalMat USAC_ACCURATE / cv2.findHomography RANSAC'}}
+    for kind in ('F', 'H'):
+        line[kind] = {'fine': time_one(kind, fine, args.calls, args.cpu_reps),
+                      'scene': time_one(kind, scene_rows(kind, fine.shape[0], dev), args.calls, args.cpu_reps)}
+    print(json.dumps(line), flush=True)
+
+
+if __name__ == '__main__':
+    main()

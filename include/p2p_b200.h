@@ -190,6 +190,32 @@ P2P_API int p2p_finalize_matches(p2p_handle_t h, const float* fine, const float*
 P2P_API int p2p_preprocess_image(p2p_handle_t h, const uint8_t* rgb_hwc, int ho, int wo, int ht, int wt, float* out_chw,
                          uint8_t* resized_hwc_out, void* stream);
 
+/* ---- match verification: what every consumer of the match list does next in the reference -- pydegensac's
+ * findFundamentalMatrix / findHomography in examples/visualize_matches.ipynb (first cell), the F / pose RANSAC of
+ * utils/train/eval_epoch_immatch.py:51-80 and utils/eval/geometry.py:32-71 -- as RANSAC on the device.
+ * rows: fp64 (x1, y1, x2, y2) in pixels, row r at rows + r * row_stride (row_stride >= 4; 9 consumes the packed_out of
+ * p2p_finalize_matches in place); n_dev (nullable, DEVICE double): use min(n, *n_dev) rows, e.g. packed_out + n * 9.
+ * model 0 = fundamental matrix, x2^T F x1 = 0 (7-point minimal solver, inlier iff the Sampson error
+ * dd^2 / (l1x^2 + l1y^2 + l2x^2 + l2y^2) < px_th^2); model 1 = homography x2 ~ H x1 (4-point DLT, inlier iff the
+ * one-sided transfer error |pi(H x1) - x2|^2 < px_th^2 with (H x1)_z > 0).  Hartley-normalised minimal samples from a
+ * counter-based generator of (seed, hypothesis, draw); rounds of 1024 hypotheses stop, on the device, once
+ * log(1 - conf) / log(1 - w^s) hypotheses have been drawn (w the best inlier ratio) or at max_iters; the winner (most
+ * inliers, ties to the lowest (hypothesis, root) index) is refitted on its inliers (F: 8-point + rank 2; H: DLT) while
+ * the count grows.  Bit-reproducible.  model_out DEVICE double [9] row-major (F: unit Frobenius norm, H: H[2][2] = 1),
+ * mask_out DEVICE uint8 [n], n_inliers_out DEVICE int32: 0 = no model (fewer rows than a sample or every sample
+ * degenerate; model and mask zeroed), -1 = a coordinate is not finite (model NaN, mask zeroed). */
+P2P_API int p2p_find_model(p2p_handle_t h, int model, const double* rows, int row_stride, int n, const double* n_dev,
+                   double px_th, double conf, int max_iters, unsigned long long seed, double* model_out, uint8_t* mask_out,
+                   int32_t* n_inliers_out, void* stream);
+/* The reference's sampson_distance (utils/eval/measure.py:18-40, eps = 1e-8) in fp64: dist_out[r] =
+ * (x2^T F x1)^2 / (eps + l1x^2 + l1y^2 + l2x^2 + l2y^2).  F DEVICE double [9], dist_out DEVICE double [n]. */
+P2P_API int p2p_sampson_distance(p2p_handle_t h, const double* rows, int row_stride, int n, const double* F,
+                         double* dist_out, void* stream);
+/* Test hook: hypotheses 0 .. count-1 of p2p_find_model without selection.  models_out DEVICE double [count*slots][9]
+ * (slots 3 for F, 1 for H; zero where a slot has no model), counts_out DEVICE int32 [count*slots] (-1: no model). */
+P2P_API int p2p_test_hypotheses(p2p_handle_t h, int model, const double* rows, int row_stride, int n, double px_th,
+                        unsigned long long seed, int count, double* models_out, int32_t* counts_out, void* stream);
+
 /* ---- bring-up / accuracy probe: C[M,N] = alpha * A[M,K] B[N,K]^T on the wgmma path with the
  * same operand format as the hot path (fp32 inputs are split to fp16 hi/lo on the device).
  * a, b, c are DEVICE fp32; K % 64 == 0. */

@@ -52,6 +52,9 @@ _SIGNATURES = {
     'p2p_preprocess_image': (_I, [_P, _P, _I, _I, _I, _I, _P, _P, _P]),
     'p2p_profile_read': (_I, [_P, C.POINTER(C.c_float), C.POINTER(_I), _I]),
     'p2p_test_gemm': (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _F, _P]),
+    'p2p_find_model': (_I, [_P, _I, _P, _I, _I, _P, C.c_double, C.c_double, _I, C.c_ulonglong, _P, _P, _P, _P]),
+    'p2p_sampson_distance': (_I, [_P, _P, _I, _I, _P, _P, _P]),
+    'p2p_test_hypotheses': (_I, [_P, _I, _P, _I, _I, C.c_double, C.c_ulonglong, _I, _P, _P, _P]),
 }
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
 PROF_KINDS = ('l2norm', 'corr', 'mutual', 'nc', 'proposals', 'prep', 'gather_mid', 'conv1_mid', 'conv2_mid', 'fc_mid',

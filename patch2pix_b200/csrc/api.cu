@@ -103,7 +103,7 @@ struct p2p_handle_s {
   int opt_nc_l2_mode = 0;       // NC layer 2 block layout: 0 auto, 1 one haloed block per tile, 2 one block per column tap
   int opt_nc_impl = 1;          // 1: NeighConsensus on the tensor cores (nc_umma.cu); 0: fp32 CUDA-core kernels (shape-capped)
   Regressor reg[2];
-  Arena coarse, refine, feat, misc, uniq, pre;
+  Arena coarse, refine, feat, misc, uniq, pre, verify;
   std::vector<PreprocessCoefs> pre_coefs;   // cached resampling tables, one per image geometry
   PairFeatures pf[2];
   bool prepared = false;
@@ -416,6 +416,7 @@ int p2p_destroy(p2p_handle_t h) {
   h->misc.release();
   h->uniq.release();
   h->pre.release();
+  h->verify.release();
   for (auto& c : h->pre_coefs)
     if (c.d) cudaFree(c.d);
   for (auto& e : h->prof) { cudaEventDestroy(e.a); cudaEventDestroy(e.b); }
@@ -1144,6 +1145,44 @@ int p2p_preprocess_image(p2p_handle_t h, const uint8_t* rgb_hwc, int ho, int wo,
   P2P_REQUIRE(tmp != nullptr, "scratch carve failed");
   const float mean[3] = {0.485f, 0.456f, 0.406f}, stdv[3] = {0.229f, 0.224f, 0.225f};   // ImageNet, preprocess.py:93
   return launch_preprocess(rgb_hwc, *C, mean, stdv, out_chw, resized_hwc_out, tmp, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int p2p_find_model(p2p_handle_t h, int model, const double* rows, int row_stride, int n, const double* n_dev, double px_th,
+                   double conf, int max_iters, unsigned long long seed, double* model_out, uint8_t* mask_out,
+                   int32_t* n_inliers_out, void* stream) {
+  P2P_ENTER(h);
+  P2P_REQUIRE(model == 0 || model == 1, "model must be 0 (F) or 1 (H)");
+  P2P_REQUIRE(model_out && mask_out && n_inliers_out && (rows || n == 0), "null tensor pointer");
+  P2P_REQUIRE(n >= 0 && n <= (1 << 26) && row_stride >= 4, "bad row count or stride");
+  P2P_REQUIRE(px_th > 0.0 && isfinite(px_th), "px_th must be positive");
+  P2P_REQUIRE(conf > 0.0 && conf < 1.0, "conf must lie in (0, 1)");
+  P2P_REQUIRE(max_iters > 0 && max_iters <= (1 << 24), "max_iters must lie in [1, 2^24]");
+  int rc = h->verify.reserve(verify_scratch_bytes(n, true) + 4096);
+  if (rc) return rc;
+  void* scratch = h->verify.take(verify_scratch_bytes(n, true));
+  return launch_find_model(model, rows, row_stride, n, n_dev, px_th, conf, max_iters, seed, scratch, model_out, mask_out,
+                           n_inliers_out, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int p2p_sampson_distance(p2p_handle_t h, const double* rows, int row_stride, int n, const double* F, double* dist_out,
+                         void* stream) {
+  P2P_ENTER(h);
+  P2P_REQUIRE(F && dist_out && (rows || n == 0), "null tensor pointer");
+  P2P_REQUIRE(n >= 0 && row_stride >= 4, "bad row count or stride");
+  return launch_sampson_distance(rows, row_stride, n, F, dist_out, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int p2p_test_hypotheses(p2p_handle_t h, int model, const double* rows, int row_stride, int n, double px_th,
+                        unsigned long long seed, int count, double* models_out, int32_t* counts_out, void* stream) {
+  P2P_ENTER(h);
+  P2P_REQUIRE(model == 0 || model == 1, "model must be 0 (F) or 1 (H)");
+  P2P_REQUIRE(rows && models_out && counts_out && count > 0 && row_stride >= 4, "bad argument");
+  P2P_REQUIRE(n >= (model == 0 ? 7 : 4) && n <= (1 << 26), "fewer rows than a minimal sample");
+  int rc = h->verify.reserve(verify_scratch_bytes(n, false) + 4096);
+  if (rc) return rc;
+  void* scratch = h->verify.take(verify_scratch_bytes(n, false));
+  return launch_test_hypotheses(model, rows, row_stride, n, px_th, seed, count, scratch, models_out, counts_out,
+                                reinterpret_cast<cudaStream_t>(stream));
 }
 
 int p2p_test_gemm(p2p_handle_t h, const float* a, const float* b, float* c, int M, int N, int K, int passes,

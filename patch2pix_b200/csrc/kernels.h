@@ -105,6 +105,17 @@ int launch_fc_parse(const float* pooled, const FcWeights& fc, const void* matche
 int launch_finalize_matches(const float* fine, const float* scores, const long long* coarse, int N, float io_thres,
                             const double up[4], double* packed, cudaStream_t st);
 
+// ---- verify.cu: RANSAC for F (model 0, 7-point) / H (model 1, 4-point DLT) and the Sampson distance ----------------
+// rows: fp64 (x1, y1, x2, y2) at `stride` doubles apart; n_dev (optional, device): effective row count min(n, *n_dev).
+size_t verify_scratch_bytes(int n, bool rounds);
+int launch_find_model(int model, const double* rows, int stride, int n, const double* n_dev, double px_th, double conf,
+                      int max_iters, unsigned long long seed, void* scratch, double* model_out, uint8_t* mask_out,
+                      int* count_out, cudaStream_t st);
+// Hypotheses 0 .. count-1 without selection: models_out [count*slots][9], counts_out [count*slots] (-1: no model).
+int launch_test_hypotheses(int model, const double* rows, int stride, int n, double px_th, unsigned long long seed,
+                           int count, void* scratch, double* models_out, int* counts_out, cudaStream_t st);
+int launch_sampson_distance(const double* rows, int stride, int n, const double* F, double* out, cudaStream_t st);
+
 // Tensor-core FC path helpers: pooled fp32 -> fp16 hi/lo A operand; final Linear(256,5) + parse_regressor_out.
 constexpr float kFcActScale = 16.f;
 int launch_pooled_split(const float* pooled, int n, __half* hi, __half* lo, const int* d_count, cudaStream_t st);

@@ -54,14 +54,22 @@ def load_checkpoint(ckpt_path, device='cuda:0', method='patch2pix', lprint=print
     raise ValueError('Wrong method name.')
 
 
-def _finalize(net, fine, scores, coarse, io_thres, upscale):
-    """One launch + ONE device->host copy for the tail of estimate_matches (model_helper.py:97-109)."""
+def _finalize(net, fine, scores, coarse, io_thres, upscale, verify=None):
+    """One launch (+ the RANSAC launches with `verify`) and ONE device->host copy for the tail of estimate_matches
+    (model_helper.py:97-109)."""
     import ctypes as C
     from . import _lib
     h = net._handle
     n = int(scores.shape[0])
     dev = scores.device
-    packed = torch.empty(n * 9 + 1, dtype=torch.float64, device=dev)
+    extra = 0
+    if verify is not None:
+        from . import verify as V
+        kind, px_th = verify
+        if kind not in ('F', 'H'):
+            raise ValueError("verify must be None, ('F', px_th) or ('H', px_th)")
+        extra = V.out_size(n)
+    packed = torch.empty(n * 9 + 1 + extra, dtype=torch.float64, device=dev)
     up = (C.c_double * 4)(*[float(v) for v in upscale])
     fine_c = fine.reshape(-1, 4).contiguous() if fine is not None else None
     scores_c = scores.reshape(-1).contiguous()
@@ -69,37 +77,50 @@ def _finalize(net, fine, scores, coarse, io_thres, upscale):
     with torch.cuda.device(dev):
         _lib.check(h.lib.p2p_finalize_matches(h.h, _lib.ptr(fine_c), _lib.ptr(scores_c), _lib.ptr(coarse_c), n, float(io_thres),
                                               up, _lib.ptr(packed), h.stream()))
+    if verify is not None:        # RANSAC on the kept, rescaled rows (refined columns 0..3), in place, count read on the device
+        V.find_model_into(h, V.MODEL_F if kind == 'F' else V.MODEL_H, packed, 9, n,
+                          C.c_void_p(packed.data_ptr() + n * 9 * 8), px_th, 0.999, 10000, 0, packed[n * 9 + 1:])
     host = packed.cpu().numpy()                      # the single synchronising copy
-    m = int(host[-1])
-    rows = host[:-1].reshape(n, 9)[:m]
-    return rows[:, 0:4].copy(), rows[:, 4].astype(np.float32), rows[:, 5:9].copy()
+    m = int(host[n * 9])
+    rows = host[:n * 9].reshape(n, 9)[:m]
+    out = (rows[:, 0:4].copy(), rows[:, 4].astype(np.float32), rows[:, 5:9].copy())
+    if verify is None:
+        return out
+    model, mask = V.parse_host(host[n * 9 + 1:], n)
+    return out + (mask[:m], model)
 
 
 def estimate_matches(net, im1, im2, scale1=(1.0, 1.0), scale2=(1.0, 1.0), ksize=2, ncn_thres=0.0, mutual=True,
-                     io_thres=0.25, eval_type='fine'):
+                     io_thres=0.25, eval_type='fine', verify=None):
     """utils/eval/model_helper.py:64-109 on image tensors -> (matches, scores, coarse_matches) numpy arrays
     (float64 matches in original-image pixels, float32 scores), with the inlier filter and the rescaling on the device
-    and a single device->host copy (the reference does three `.cpu()` round trips)."""
+    and a single device->host copy (the reference does three `.cpu()` round trips).
+
+    verify=('F', px_th) or ('H', px_th) also runs RANSAC (patch2pix_b200.verify, conf 0.999, 10000 iterations, seed 0)
+    on the device on those matches, px_th in original-image pixels, still before the single copy, and returns
+    (matches, scores, coarse_matches, inliers, model): a bool mask over the matches and the 3x3 float64 F or H
+    (None when no model was found)."""
     upscale = tuple(scale1) + tuple(scale2)
     im1 = im1.to(net.device)
     im2 = im2.to(net.device)
     with torch.no_grad():
         if eval_type == 'coarse':
             coarse_matches, scores = net.predict_coarse(im1, im2, ksize=ksize, ncn_thres=ncn_thres, mutual=mutual)
-            m, s, _ = _finalize(net, None, scores[0], coarse_matches[0], float('-inf'), upscale)
-            return m, s, m
+            res = _finalize(net, None, scores[0], coarse_matches[0], float('-inf'), upscale, verify)
+            return (res[0], res[1], res[0]) + res[3:]
         if eval_type != 'fine':
             raise ValueError("eval_type must be 'coarse' or 'fine'")
         fine_matches, fine_scores, coarse_matches = net.predict_fine(im1, im2, ksize=ksize, ncn_thres=ncn_thres,
                                                                     mutual=mutual)
-    return _finalize(net, fine_matches[0], fine_scores[0], coarse_matches[0], io_thres, upscale)
+    return _finalize(net, fine_matches[0], fine_scores[0], coarse_matches[0], io_thres, upscale, verify)
 
 
 def estimate_matches_from_files(net, im1_path, im2_path, ksize=2, ncn_thres=0.0, mutual=True, io_thres=0.25,
-                                eval_type='fine', imsize=None):
+                                eval_type='fine', imsize=None, verify=None):
     """utils/eval/model_helper.py:64-72 + the above: image files in, numpy matches out.  Only the file decode runs on
     the host; resize / ToTensor / Normalize are GPU kernels (patch2pix_b200.preprocess)."""
     from .preprocess import load_im_flexible
     im1, sc1 = load_im_flexible(im1_path, ksize, net.upsample, imsize=imsize, device=net.device, handle=net._handle)
     im2, sc2 = load_im_flexible(im2_path, ksize, net.upsample, imsize=imsize, device=net.device, handle=net._handle)
-    return estimate_matches(net, im1.unsqueeze(0), im2.unsqueeze(0), sc1, sc2, ksize, ncn_thres, mutual, io_thres, eval_type)
+    return estimate_matches(net, im1.unsqueeze(0), im2.unsqueeze(0), sc1, sc2, ksize, ncn_thres, mutual, io_thres, eval_type,
+                            verify)

@@ -12,6 +12,7 @@ stay O(1) through the regressor, like a trained network's.
 """
 import math
 
+import numpy as np
 import torch
 import torch.nn.functional as F
 
@@ -119,6 +120,66 @@ def shifted_pair_offset(pair_idx):
     if dx == 0 and dy == 0:
         dx = 16
     return dx, dy
+
+
+def _skew(t):
+    return np.array([[0.0, -t[2], t[1]], [t[2], 0.0, -t[0]], [-t[1], t[0], 0.0]])
+
+
+def _rotation(axis_angle):
+    th = float(np.linalg.norm(axis_angle))
+    if th == 0:
+        return np.eye(3)
+    K = _skew(axis_angle / th)
+    return np.eye(3) + math.sin(th) * K + (1 - math.cos(th)) * K @ K
+
+
+def synthetic_two_view(seed, n, outlier_ratio, noise_px, planar=False, width=640, height=480):
+    """Seeded two-view scene for match verification: a random camera pair (focal 500 px, principal point at the
+    image centre, camera 2 rotated up to ~0.15 rad and translated by ~1 unit at 4-8 units of depth), round(n * (1 -
+    outlier_ratio)) true correspondences visible in both images with N(0, noise_px^2) noise on every coordinate, and
+    uniformly random outlier pairs, shuffled.  With `planar` the 3-D points lie on one plane.
+    Returns dict(pts1 [n, 2], pts2 [n, 2] float64, F (x2^T F x1 = 0, unit norm), H (x2 ~ H x1 with H[2][2] = 1, or
+    None unless planar), inlier [n] bool)."""
+    rng = np.random.default_rng(int(seed))
+    Kc = np.array([[500.0, 0, width / 2], [0, 500.0, height / 2], [0, 0, 1]])
+    R = _rotation(rng.uniform(-0.09, 0.09, 3))
+    t = np.array([rng.uniform(0.6, 1.0) * rng.choice([-1, 1]), rng.uniform(-0.3, 0.3), rng.uniform(-0.2, 0.2)])
+    normal = np.array([rng.uniform(-0.3, 0.3), rng.uniform(-0.3, 0.3), 1.0])
+    normal /= np.linalg.norm(normal)
+    d = rng.uniform(5.0, 7.0)                                   # plane normal^T X = d (camera-1 frame)
+    n_in = int(round(n * (1.0 - outlier_ratio)))
+    p1, p2 = np.zeros((0, 2)), np.zeros((0, 2))
+    while p1.shape[0] < n_in:
+        m = 4 * n_in + 16
+        uv = rng.uniform([0, 0], [width, height], (m, 2))
+        ray = np.linalg.solve(Kc, np.concatenate([uv, np.ones((m, 1))], 1).T).T
+        depth = d / (ray @ normal) if planar else rng.uniform(4.0, 8.0, m)
+        X = ray * depth[:, None]
+        X2 = X @ R.T + t
+        q = X2 @ Kc.T
+        ok = (X[:, 2] > 0) & (X2[:, 2] > 0.5)
+        q = q[ok, :2] / q[ok, 2:3]
+        inside = (q[:, 0] >= 0) & (q[:, 0] < width) & (q[:, 1] >= 0) & (q[:, 1] < height)
+        p1 = np.concatenate([p1, uv[ok][inside]])
+        p2 = np.concatenate([p2, q[inside]])
+    p1 = p1[:n_in] + rng.normal(0, noise_px, (n_in, 2))
+    p2 = p2[:n_in] + rng.normal(0, noise_px, (n_in, 2))
+    n_out = n - n_in
+    o1 = rng.uniform([0, 0], [width, height], (n_out, 2))
+    o2 = rng.uniform([0, 0], [width, height], (n_out, 2))
+    perm = rng.permutation(n)
+    pts1 = np.concatenate([p1, o1])[perm]
+    pts2 = np.concatenate([p2, o2])[perm]
+    inlier = np.concatenate([np.ones(n_in, bool), np.zeros(n_out, bool)])[perm]
+    Ki = np.linalg.inv(Kc)
+    F = Ki.T @ _skew(t) @ R @ Ki
+    F /= np.linalg.norm(F)
+    H = None
+    if planar:
+        H = Kc @ (R + np.outer(t, normal) / d) @ Ki
+        H /= H[2, 2]
+    return dict(pts1=pts1, pts2=pts2, F=F, H=H, inlier=inlier)
 
 
 def synthetic_pair_shifted(pair_idx, height, width, noise=0.6):
