@@ -10,8 +10,11 @@ Two workloads of 3200 rows each, for F and for H:
     RANSAC early.
 Threshold 1 px for F and 2 px for H as in the reference's notebook, conf 0.999, at most 10000 iterations, seed 0.
 GPU time: CUDA events around `--calls` back-to-back calls.  CPU time: host clock around `--cpu-reps` calls of
-cv2.findFundamentalMat (USAC_ACCURATE) / cv2.findHomography (RANSAC), or null without cv2.  Prints one JSON line and
-writes nothing.
+cv2.findFundamentalMat (USAC_ACCURATE) / cv2.findHomography (RANSAC), or null without cv2.
+E (relative pose, the reference's matches2relapose_cv) runs on the same two workloads (the `scene` one non-planar)
+with K at focal 500 px and the principal point at the image centre, 1 px, conf 0.999, at most 1000 iterations
+(cv2's defaults): p2p_find_essential + p2p_recover_pose on its inliers against cv2.findEssentialMat (RANSAC) +
+cv2.recoverPose.  Prints one JSON line and writes nothing.
 """
 import argparse
 import json
@@ -90,6 +93,52 @@ def time_one(kind, rows, calls, cpu_reps):
     return res
 
 
+def time_pose(rows, calls, cpu_reps):
+    from patch2pix_b200 import _lib
+    from patch2pix_b200 import pose as P
+    n = int(rows.shape[0])
+    K = np.array([[500.0, 0, 320.0], [0, 500.0, 240.0], [0, 0, 1]])
+    intr = P.intrinsics(K, K)
+    h = _lib.default_handle(rows.device)
+    out = torch.zeros(P.out_size(n), dtype=torch.float64, device=rows.device)
+
+    def run_gpu():
+        P.find_essential_into(h, rows, 4, n, None, intr, 1.0, 0.999, 1000, 0, out)
+        P.recover_pose_into(h, rows, 4, n, None, intr, out.data_ptr(), out.data_ptr() + 184, out)
+    for _ in range(5):
+        run_gpu()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    torch.cuda.synchronize()
+    e0.record()
+    for _ in range(calls):
+        run_gpu()
+    e1.record()
+    torch.cuda.synchronize()
+    _, emask, n_good, _, _, _ = P.parse_host(out.cpu().numpy(), n)
+    res = {'rows': n, 'ms_gpu': e0.elapsed_time(e1) / calls, 'inliers_gpu': int(emask.sum()), 'good_gpu': n_good,
+           'ms_cpu': None, 'inliers_cpu': None, 'good_cpu': None}
+    try:
+        import cv2
+    except ImportError:
+        return res
+    pts = rows.cpu().numpy()
+    p1, p2 = pts[:, :2].copy(), pts[:, 2:].copy()
+
+    def run_cpu():
+        E, m = cv2.findEssentialMat(p1, p2, K, cv2.RANSAC, 0.999, 1.0, maxIters=1000)
+        if E is None or E.shape[0] != 3:
+            return m, 0
+        inl = np.where(m.ravel() > 0)[0]
+        return m, cv2.recoverPose(E, p1[inl], p2[inl], K)[0]
+    cm, good = run_cpu()
+    t0 = time.perf_counter()
+    for _ in range(cpu_reps):
+        run_cpu()
+    res.update(ms_cpu=(time.perf_counter() - t0) * 1e3 / cpu_reps, inliers_cpu=None if cm is None else int(cm.sum()),
+               good_cpu=int(good))
+    return res
+
+
 def card():
     try:
         q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'],
@@ -110,10 +159,14 @@ def main():
     fine = fine_matches(dev)
     line = {'metric': 'ms per verification call', 'card': card(), 'cpu_cores': os.cpu_count(),
             'config': {'th_px': TH, 'conf': 0.999, 'max_iters': 10000, 'seed': 0, 'calls': args.calls,
-                       'cpu_reps': args.cpu_reps, 'cpu': 'cv2.findFundamentalMat USAC_ACCURATE / cv2.findHomography RANSAC'}}
+                       'cpu_reps': args.cpu_reps, 'cpu': 'cv2.findFundamentalMat USAC_ACCURATE / cv2.findHomography RANSAC',
+                       'E': {'th_px': 1.0, 'max_iters': 1000, 'K': 'focal 500 px, principal point (320, 240)',
+                             'cpu': 'cv2.findEssentialMat RANSAC + cv2.recoverPose'}}}
     for kind in ('F', 'H'):
         line[kind] = {'fine': time_one(kind, fine, args.calls, args.cpu_reps),
                       'scene': time_one(kind, scene_rows(kind, fine.shape[0], dev), args.calls, args.cpu_reps)}
+    line['E'] = {'fine': time_pose(fine, args.calls, args.cpu_reps),
+                 'scene': time_pose(scene_rows('E', fine.shape[0], dev), args.calls, args.cpu_reps)}
     print(json.dumps(line), flush=True)
 
 

@@ -216,6 +216,35 @@ P2P_API int p2p_sampson_distance(p2p_handle_t h, const double* rows, int row_str
 P2P_API int p2p_test_hypotheses(p2p_handle_t h, int model, const double* rows, int row_stride, int n, double px_th,
                         unsigned long long seed, int count, double* models_out, int32_t* counts_out, void* stream);
 
+/* Relative pose -- the reference's matches2relapose_cv (utils/eval/geometry.py:32-48): cv2.findEssentialMat(RANSAC) and
+ * cv2.recoverPose, on the device.  rows / row_stride / n / n_dev as p2p_find_model; intr HOST double[8] = (fx1, fy1,
+ * cx1, cy1, fx2, fy2, cx2, cy2), focal lengths positive.  Points map to camera coordinates ((x - cx) / fx, (y - cy) / fy).
+ *
+ * p2p_find_essential: RANSAC for E (x2^T E x1 = 0 in camera coordinates) with the 5-point minimal solver (null space of
+ * the 5 x 9 epipolar system, 10 cubic constraints, Gauss-Jordan, Nister's degree-10 polynomial, Sturm bisection; up to
+ * 10 models per sample).  Inlier iff the Sampson error in camera coordinates is below th^2, th = px_th / ((fx2 + fy2)
+ * / 2) (OpenCV's rule).  Same generator, rounds, stopping bound (s = 5), tie rule and reproducibility as
+ * p2p_find_model; the winner is refitted (8-point, projected onto singular values (1, 1, 0)) while the count grows.
+ * E_out DEVICE double [9] row-major at unit Frobenius norm, mask_out DEVICE uint8 [n], n_inliers_out DEVICE int32:
+ * 0 = no model (E and mask zeroed), -1 = a coordinate is not finite (E NaN, mask zeroed). */
+P2P_API int p2p_find_essential(p2p_handle_t h, const double* rows, int row_stride, int n, const double* n_dev,
+                               const double* intr, double px_th, double conf, int max_iters, unsigned long long seed,
+                               double* E_out, uint8_t* mask_out, int32_t* n_inliers_out, void* stream);
+/* p2p_recover_pose: decomposes E (DEVICE double [9]) as cv2.decomposeEssentialMat into [R1|t], [R2|t], [R1|-t],
+ * [R2|-t], triangulates every row under mask_in (DEVICE uint8 [n], nullable = all rows) against [I|0] and each
+ * candidate, and keeps the candidate with the most points with Q2 Q3 > 0, depth in camera 1 below dist_th and depth in
+ * camera 2 in (0, dist_th) (ties to the first).  Rt_out DEVICE double [12]: R row-major then t (unit norm,
+ * x2 = R x1 + t); mask_out DEVICE uint8 [n]: the good points; n_good_out DEVICE int32.  A zero or non-finite E gives
+ * zero R, t, count and mask. */
+P2P_API int p2p_recover_pose(p2p_handle_t h, const double* rows, int row_stride, int n, const double* n_dev,
+                             const double* intr, const double* E, const uint8_t* mask_in, double dist_th,
+                             double* Rt_out, uint8_t* mask_out, int32_t* n_good_out, void* stream);
+/* Test hook: hypotheses 0 .. count-1 of p2p_find_essential without selection.  models_out DEVICE double [count*10][9]
+ * (camera coordinates, zero where a slot has no model), counts_out DEVICE int32 [count*10] (-1: no model). */
+P2P_API int p2p_test_essential_hypotheses(p2p_handle_t h, const double* rows, int row_stride, int n, const double* intr,
+                                          double px_th, unsigned long long seed, int count, double* models_out,
+                                          int32_t* counts_out, void* stream);
+
 /* ---- bring-up / accuracy probe: C[M,N] = alpha * A[M,K] B[N,K]^T on the wgmma path with the
  * same operand format as the hot path (fp32 inputs are split to fp16 hi/lo on the device).
  * a, b, c are DEVICE fp32; K % 64 == 0. */

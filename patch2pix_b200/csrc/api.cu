@@ -1185,6 +1185,64 @@ int p2p_test_hypotheses(p2p_handle_t h, int model, const double* rows, int row_s
                                 reinterpret_cast<cudaStream_t>(stream));
 }
 
+static bool intrinsics_ok(const double* intr, Intrinsics& K) {
+  if (intr == nullptr) return false;
+  for (int i = 0; i < 8; ++i)
+    if (!isfinite(intr[i])) return false;
+  K = Intrinsics{intr[0], intr[1], intr[2], intr[3], intr[4], intr[5], intr[6], intr[7]};
+  return K.fx1 > 0.0 && K.fy1 > 0.0 && K.fx2 > 0.0 && K.fy2 > 0.0;
+}
+
+int p2p_find_essential(p2p_handle_t h, const double* rows, int row_stride, int n, const double* n_dev, const double* intr,
+                       double px_th, double conf, int max_iters, unsigned long long seed, double* E_out, uint8_t* mask_out,
+                       int32_t* n_inliers_out, void* stream) {
+  P2P_ENTER(h);
+  P2P_REQUIRE(E_out && mask_out && n_inliers_out && (rows || n == 0), "null tensor pointer");
+  P2P_REQUIRE(n >= 0 && n <= (1 << 26) && row_stride >= 4, "bad row count or stride");
+  Intrinsics K;
+  P2P_REQUIRE(intrinsics_ok(intr, K), "intr must be 8 finite values with positive focal lengths");
+  P2P_REQUIRE(px_th > 0.0 && isfinite(px_th), "px_th must be positive");
+  P2P_REQUIRE(conf > 0.0 && conf < 1.0, "conf must lie in (0, 1)");
+  P2P_REQUIRE(max_iters > 0 && max_iters <= (1 << 24), "max_iters must lie in [1, 2^24]");
+  int rc = h->verify.reserve(essential_scratch_bytes(n, true) + 4096);
+  if (rc) return rc;
+  void* scratch = h->verify.take(essential_scratch_bytes(n, true));
+  return launch_find_essential(rows, row_stride, n, n_dev, K, px_th, conf, max_iters, seed, scratch, E_out, mask_out,
+                               n_inliers_out, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int p2p_recover_pose(p2p_handle_t h, const double* rows, int row_stride, int n, const double* n_dev, const double* intr,
+                     const double* E, const uint8_t* mask_in, double dist_th, double* Rt_out, uint8_t* mask_out,
+                     int32_t* n_good_out, void* stream) {
+  P2P_ENTER(h);
+  P2P_REQUIRE(E && Rt_out && mask_out && n_good_out && (rows || n == 0), "null tensor pointer");
+  P2P_REQUIRE(n >= 0 && n <= (1 << 26) && row_stride >= 4, "bad row count or stride");
+  Intrinsics K;
+  P2P_REQUIRE(intrinsics_ok(intr, K), "intr must be 8 finite values with positive focal lengths");
+  P2P_REQUIRE(dist_th > 0.0 && isfinite(dist_th), "dist_th must be positive");
+  int rc = h->verify.reserve(pose_scratch_bytes(n) + 4096);
+  if (rc) return rc;
+  void* scratch = h->verify.take(pose_scratch_bytes(n));
+  return launch_recover_pose(rows, row_stride, n, n_dev, K, E, mask_in, dist_th, scratch, Rt_out, mask_out, n_good_out,
+                             reinterpret_cast<cudaStream_t>(stream));
+}
+
+int p2p_test_essential_hypotheses(p2p_handle_t h, const double* rows, int row_stride, int n, const double* intr,
+                                  double px_th, unsigned long long seed, int count, double* models_out,
+                                  int32_t* counts_out, void* stream) {
+  P2P_ENTER(h);
+  P2P_REQUIRE(rows && models_out && counts_out && count > 0 && row_stride >= 4, "bad argument");
+  P2P_REQUIRE(n >= 5 && n <= (1 << 26), "fewer rows than a minimal sample");
+  Intrinsics K;
+  P2P_REQUIRE(intrinsics_ok(intr, K), "intr must be 8 finite values with positive focal lengths");
+  P2P_REQUIRE(px_th > 0.0 && isfinite(px_th), "px_th must be positive");
+  int rc = h->verify.reserve(essential_scratch_bytes(n, false) + 4096);
+  if (rc) return rc;
+  void* scratch = h->verify.take(essential_scratch_bytes(n, false));
+  return launch_test_essential_hypotheses(rows, row_stride, n, K, px_th, seed, count, scratch, models_out, counts_out,
+                                          reinterpret_cast<cudaStream_t>(stream));
+}
+
 int p2p_test_gemm(p2p_handle_t h, const float* a, const float* b, float* c, int M, int N, int K, int passes,
                   int seg_len, float in_scale, void* stream) {
   P2P_ENTER(h);

@@ -116,6 +116,21 @@ int launch_test_hypotheses(int model, const double* rows, int stride, int n, dou
                            int count, void* scratch, double* models_out, int* counts_out, cudaStream_t st);
 int launch_sampson_distance(const double* rows, int stride, int n, const double* F, double* out, cudaStream_t st);
 
+// ---- pose.cu: essential-matrix RANSAC (5-point) and pose recovery ------------------------------------------------
+struct Intrinsics { double fx1, fy1, cx1, cy1, fx2, fy2, cx2, cy2; };   // pixels -> camera coordinates of both views
+size_t essential_scratch_bytes(int n, bool rounds);
+size_t pose_scratch_bytes(int n);
+int launch_find_essential(const double* rows, int stride, int n, const double* n_dev, const Intrinsics& K, double px_th,
+                          double conf, int max_iters, unsigned long long seed, void* scratch, double* E_out,
+                          uint8_t* mask_out, int* count_out, cudaStream_t st);
+// Hypotheses 0 .. count-1 without selection: models_out [count*10][9], counts_out [count*10] (-1: no model).
+int launch_test_essential_hypotheses(const double* rows, int stride, int n, const Intrinsics& K, double px_th,
+                                     unsigned long long seed, int count, void* scratch, double* models_out,
+                                     int* counts_out, cudaStream_t st);
+int launch_recover_pose(const double* rows, int stride, int n, const double* n_dev, const Intrinsics& K, const double* E,
+                        const uint8_t* mask_in, double dist_th, void* scratch, double* Rt_out, uint8_t* mask_out,
+                        int* count_out, cudaStream_t st);
+
 // Tensor-core FC path helpers: pooled fp32 -> fp16 hi/lo A operand; final Linear(256,5) + parse_regressor_out.
 constexpr float kFcActScale = 16.f;
 int launch_pooled_split(const float* pooled, int n, __half* hi, __half* lo, const int* d_count, cudaStream_t st);

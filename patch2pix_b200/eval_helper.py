@@ -64,11 +64,13 @@ def _finalize(net, fine, scores, coarse, io_thres, upscale, verify=None):
     dev = scores.device
     extra = 0
     if verify is not None:
+        from . import pose as P
         from . import verify as V
-        kind, px_th = verify
-        if kind not in ('F', 'H'):
-            raise ValueError("verify must be None, ('F', px_th) or ('H', px_th)")
-        extra = V.out_size(n)
+        kind = verify[0] if isinstance(verify, (tuple, list)) and len(verify) > 0 else None
+        if not (kind in ('F', 'H') and len(verify) == 2 or kind == 'E' and len(verify) == 4):
+            raise ValueError("verify must be None, ('F', px_th), ('H', px_th) or ('E', px_th, K1, K2)")
+        px_th = verify[1]
+        extra = P.out_size(n) if kind == 'E' else V.out_size(n)
     packed = torch.empty(n * 9 + 1 + extra, dtype=torch.float64, device=dev)
     up = (C.c_double * 4)(*[float(v) for v in upscale])
     fine_c = fine.reshape(-1, 4).contiguous() if fine is not None else None
@@ -77,15 +79,24 @@ def _finalize(net, fine, scores, coarse, io_thres, upscale, verify=None):
     with torch.cuda.device(dev):
         _lib.check(h.lib.p2p_finalize_matches(h.h, _lib.ptr(fine_c), _lib.ptr(scores_c), _lib.ptr(coarse_c), n, float(io_thres),
                                               up, _lib.ptr(packed), h.stream()))
-    if verify is not None:        # RANSAC on the kept, rescaled rows (refined columns 0..3), in place, count read on the device
-        V.find_model_into(h, V.MODEL_F if kind == 'F' else V.MODEL_H, packed, 9, n,
-                          C.c_void_p(packed.data_ptr() + n * 9 * 8), px_th, 0.999, 10000, 0, packed[n * 9 + 1:])
+    n_dev = C.c_void_p(packed.data_ptr() + n * 9 * 8)
+    if verify is not None and kind == 'E':   # E RANSAC + pose on the kept, rescaled rows, in place (cv2's defaults)
+        out = packed[n * 9 + 1:]
+        intr = P.reference_intrinsics(verify[2], verify[3])
+        P.find_essential_into(h, packed, 9, n, n_dev, intr, px_th, 0.999, 1000, 0, out)
+        P.recover_pose_into(h, packed, 9, n, n_dev, intr, out.data_ptr(), out.data_ptr() + 184, out)
+    elif verify is not None:      # RANSAC on the kept, rescaled rows (refined columns 0..3), in place, count read on the device
+        V.find_model_into(h, V.MODEL_F if kind == 'F' else V.MODEL_H, packed, 9, n, n_dev, px_th, 0.999, 10000, 0,
+                          packed[n * 9 + 1:])
     host = packed.cpu().numpy()                      # the single synchronising copy
     m = int(host[n * 9])
     rows = host[:n * 9].reshape(n, 9)[:m]
     out = (rows[:, 0:4].copy(), rows[:, 4].astype(np.float32), rows[:, 5:9].copy())
     if verify is None:
         return out
+    if kind == 'E':
+        E, mask, _, R, t, _ = P.parse_host(host[n * 9 + 1:], n)
+        return out + (mask[:m], E, R, t)
     model, mask = V.parse_host(host[n * 9 + 1:], n)
     return out + (mask[:m], model)
 
@@ -99,7 +110,12 @@ def estimate_matches(net, im1, im2, scale1=(1.0, 1.0), scale2=(1.0, 1.0), ksize=
     verify=('F', px_th) or ('H', px_th) also runs RANSAC (patch2pix_b200.verify, conf 0.999, 10000 iterations, seed 0)
     on the device on those matches, px_th in original-image pixels, still before the single copy, and returns
     (matches, scores, coarse_matches, inliers, model): a bool mask over the matches and the 3x3 float64 F or H
-    (None when no model was found)."""
+    (None when no model was found).
+
+    verify=('E', px_th, K1, K2), with K1, K2 the 3x3 intrinsics in original-image pixels, runs the reference's
+    matches2relapose_cv instead (patch2pix_b200.pose: E RANSAC at conf 0.999 and 1000 iterations, then pose recovery on
+    its inliers) and returns (matches, scores, coarse_matches, inliers, E, R, t): the E-RANSAC mask, E (None when no
+    model was found), R and t [3, 1] (x2 = R x1 + t)."""
     upscale = tuple(scale1) + tuple(scale2)
     im1 = im1.to(net.device)
     im2 = im2.to(net.device)

@@ -134,15 +134,17 @@ def _rotation(axis_angle):
     return np.eye(3) + math.sin(th) * K + (1 - math.cos(th)) * K @ K
 
 
-def synthetic_two_view(seed, n, outlier_ratio, noise_px, planar=False, width=640, height=480):
+def synthetic_two_view(seed, n, outlier_ratio, noise_px, planar=False, width=640, height=480, focal2=None):
     """Seeded two-view scene for match verification: a random camera pair (focal 500 px, principal point at the
     image centre, camera 2 rotated up to ~0.15 rad and translated by ~1 unit at 4-8 units of depth), round(n * (1 -
     outlier_ratio)) true correspondences visible in both images with N(0, noise_px^2) noise on every coordinate, and
     uniformly random outlier pairs, shuffled.  With `planar` the 3-D points lie on one plane.
+    `focal2` (default: 500) is the focal length of camera 2, in px.
     Returns dict(pts1 [n, 2], pts2 [n, 2] float64, F (x2^T F x1 = 0, unit norm), H (x2 ~ H x1 with H[2][2] = 1, or
-    None unless planar), inlier [n] bool)."""
+    None unless planar), inlier [n] bool, K1, K2 (3x3 intrinsics), R, t (camera 2 from camera 1: X2 = R X1 + t))."""
     rng = np.random.default_rng(int(seed))
     Kc = np.array([[500.0, 0, width / 2], [0, 500.0, height / 2], [0, 0, 1]])
+    K2 = Kc if focal2 is None else np.array([[float(focal2), 0, width / 2], [0, float(focal2), height / 2], [0, 0, 1]])
     R = _rotation(rng.uniform(-0.09, 0.09, 3))
     t = np.array([rng.uniform(0.6, 1.0) * rng.choice([-1, 1]), rng.uniform(-0.3, 0.3), rng.uniform(-0.2, 0.2)])
     normal = np.array([rng.uniform(-0.3, 0.3), rng.uniform(-0.3, 0.3), 1.0])
@@ -157,7 +159,7 @@ def synthetic_two_view(seed, n, outlier_ratio, noise_px, planar=False, width=640
         depth = d / (ray @ normal) if planar else rng.uniform(4.0, 8.0, m)
         X = ray * depth[:, None]
         X2 = X @ R.T + t
-        q = X2 @ Kc.T
+        q = X2 @ K2.T
         ok = (X[:, 2] > 0) & (X2[:, 2] > 0.5)
         q = q[ok, :2] / q[ok, 2:3]
         inside = (q[:, 0] >= 0) & (q[:, 0] < width) & (q[:, 1] >= 0) & (q[:, 1] < height)
@@ -173,13 +175,14 @@ def synthetic_two_view(seed, n, outlier_ratio, noise_px, planar=False, width=640
     pts2 = np.concatenate([p2, o2])[perm]
     inlier = np.concatenate([np.ones(n_in, bool), np.zeros(n_out, bool)])[perm]
     Ki = np.linalg.inv(Kc)
-    F = Ki.T @ _skew(t) @ R @ Ki
+    K2i = Ki if focal2 is None else np.linalg.inv(K2)
+    F = K2i.T @ _skew(t) @ R @ Ki
     F /= np.linalg.norm(F)
     H = None
     if planar:
-        H = Kc @ (R + np.outer(t, normal) / d) @ Ki
+        H = K2 @ (R + np.outer(t, normal) / d) @ Ki
         H /= H[2, 2]
-    return dict(pts1=pts1, pts2=pts2, F=F, H=H, inlier=inlier)
+    return dict(pts1=pts1, pts2=pts2, F=F, H=H, inlier=inlier, K1=Kc.copy(), K2=K2.copy(), R=R, t=t)
 
 
 def synthetic_pair_shifted(pair_idx, height, width, noise=0.6):
