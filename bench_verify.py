@@ -14,7 +14,11 @@ cv2.findFundamentalMat (USAC_ACCURATE) / cv2.findHomography (RANSAC), or null wi
 E (relative pose, the reference's matches2relapose_cv) runs on the same two workloads (the `scene` one non-planar)
 with K at focal 500 px and the principal point at the image centre, 1 px, conf 0.999, at most 1000 iterations
 (cv2's defaults): p2p_find_essential + p2p_recover_pose on its inliers against cv2.findEssentialMat (RANSAC) +
-cv2.recoverPose.  Prints one JSON line and writes nothing.
+cv2.recoverPose.
+DEGENSAC (F with the plane-degeneracy check, model 2 of p2p_find_model) runs on the `fine` workload and on `plane`, a
+3200-row synthetic_dominant_plane scene (30 % outliers, 8 % of the inliers off the dominant plane, 0.5 px noise), at 1 px
+against cv2.findFundamentalMat (USAC_ACCURATE); for `plane` it also reports the recall of the off-plane inliers.
+Prints one JSON line and writes nothing.
 """
 import argparse
 import json
@@ -29,7 +33,8 @@ import torch
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-TH = {'F': 1.0, 'H': 2.0}
+TH = {'F': 1.0, 'H': 2.0, 'DEGENSAC': 1.0}
+MODEL = {'F': 0, 'H': 1, 'DEGENSAC': 2}
 
 
 def fine_matches(dev):
@@ -56,13 +61,19 @@ def scene_rows(kind, n, dev):
     return torch.from_numpy(np.concatenate([sc['pts1'], sc['pts2']], 1)).to(dev)
 
 
-def time_one(kind, rows, calls, cpu_reps):
+def plane_rows(n, dev):
+    from patch2pix_b200.synth import OFF_PLANE, synthetic_dominant_plane
+    sc = synthetic_dominant_plane(0, n, 0.3, 0.08, 0.5)
+    return torch.from_numpy(np.concatenate([sc['pts1'], sc['pts2']], 1)).to(dev), sc['label'] == OFF_PLANE
+
+
+def time_one(kind, rows, calls, cpu_reps, off=None):
     from patch2pix_b200 import _lib
     from patch2pix_b200 import verify as V
     th, n = TH[kind], int(rows.shape[0])
     h = _lib.default_handle(rows.device)
     out = torch.empty(V.out_size(n), dtype=torch.float64, device=rows.device)
-    model = V.MODEL_F if kind == 'F' else V.MODEL_H
+    model = MODEL[kind]
     for _ in range(5):
         V.find_model_into(h, model, rows, 4, n, None, th, 0.999, 10000, 0, out)
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -75,13 +86,15 @@ def time_one(kind, rows, calls, cpu_reps):
     _, mask = V.parse_host(out.cpu().numpy(), n)
     res = {'rows': n, 'ms_gpu': e0.elapsed_time(e1) / calls, 'inliers_gpu': int(mask.sum()), 'ms_cpu': None,
            'inliers_cpu': None}
+    if off is not None:
+        res['off_plane_recall_gpu'] = float(mask[off].mean())
     try:
         import cv2
     except ImportError:
         return res
     pts = rows.cpu().numpy()
     p1, p2 = pts[:, :2].copy(), pts[:, 2:].copy()
-    if kind == 'F':
+    if kind in ('F', 'DEGENSAC'):
         run = lambda: cv2.findFundamentalMat(p1, p2, cv2.USAC_ACCURATE, th, 0.999, 10000)
     else:
         run = lambda: cv2.findHomography(p1, p2, cv2.RANSAC, th, maxIters=10000, confidence=0.999)
@@ -90,6 +103,8 @@ def time_one(kind, rows, calls, cpu_reps):
     for _ in range(cpu_reps):
         run()
     res.update(ms_cpu=(time.perf_counter() - t0) * 1e3 / cpu_reps, inliers_cpu=None if cm is None else int(cm.sum()))
+    if off is not None and cm is not None:
+        res['off_plane_recall_cpu'] = float(cm.ravel()[off].astype(bool).mean())
     return res
 
 
@@ -159,12 +174,15 @@ def main():
     fine = fine_matches(dev)
     line = {'metric': 'ms per verification call', 'card': card(), 'cpu_cores': os.cpu_count(),
             'config': {'th_px': TH, 'conf': 0.999, 'max_iters': 10000, 'seed': 0, 'calls': args.calls,
-                       'cpu_reps': args.cpu_reps, 'cpu': 'cv2.findFundamentalMat USAC_ACCURATE / cv2.findHomography RANSAC',
+                       'cpu_reps': args.cpu_reps, 'cpu': 'cv2.findFundamentalMat USAC_ACCURATE (F, DEGENSAC) / cv2.findHomography RANSAC',
                        'E': {'th_px': 1.0, 'max_iters': 1000, 'K': 'focal 500 px, principal point (320, 240)',
                              'cpu': 'cv2.findEssentialMat RANSAC + cv2.recoverPose'}}}
     for kind in ('F', 'H'):
         line[kind] = {'fine': time_one(kind, fine, args.calls, args.cpu_reps),
                       'scene': time_one(kind, scene_rows(kind, fine.shape[0], dev), args.calls, args.cpu_reps)}
+    prow, off = plane_rows(fine.shape[0], dev)
+    line['DEGENSAC'] = {'fine': time_one('DEGENSAC', fine, args.calls, args.cpu_reps),
+                        'plane': time_one('DEGENSAC', prow, args.calls, args.cpu_reps, off)}
     line['E'] = {'fine': time_pose(fine, args.calls, args.cpu_reps),
                  'scene': time_pose(scene_rows('E', fine.shape[0], dev), args.calls, args.cpu_reps)}
     print(json.dumps(line), flush=True)

@@ -203,7 +203,22 @@ P2P_API int p2p_preprocess_image(p2p_handle_t h, const uint8_t* rgb_hwc, int ho,
  * inliers, ties to the lowest (hypothesis, root) index) is refitted on its inliers (F: 8-point + rank 2; H: DLT) while
  * the count grows.  Bit-reproducible.  model_out DEVICE double [9] row-major (F: unit Frobenius norm, H: H[2][2] = 1),
  * mask_out DEVICE uint8 [n], n_inliers_out DEVICE int32: 0 = no model (fewer rows than a sample or every sample
- * degenerate; model and mask zeroed), -1 = a coordinate is not finite (model NaN, mask zeroed). */
+ * degenerate; model and mask zeroed), -1 = a coordinate is not finite (model NaN, mask zeroed).
+ * model 2 = F with the DEGENSAC plane-degeneracy check (Chum, Werner & Matas, CVPR 2005), pydegensac's
+ * findFundamentalMatrix: model 0's rounds, scoring, select, stopping bound, LO and outputs, plus, in each round, an
+ * H-degeneracy test of the round's records (every slot whose count beats the best so far and all earlier slots of the
+ * round: the models a sequential RANSAC would adopt, the round's winner among them), in slot order.  For each triplet
+ * {0,1,2}, {3,4,5}, {0,1,6}, {3,4,6}, {2,5,6} of the record's 7-point sample (hypothesis first + slot / 3) the
+ * homography induced by F and the three points (Hartley & Zisserman, result 13.6: H = A - e' (M^-1 b)^T with
+ * A = [e']x F, M the rows x_i^T, b_i = (x'_i x A x_i)^T (x'_i x e') / |x'_i x e'|^2) is built in fp64 in the Hartley-
+ * normalised coordinates; the sample is degenerate when at least 5 of its 7 points have a one-sided transfer error
+ * below h_th = 2 px_th (the notebook's 2 px H threshold beside its 1 px F threshold); a vanishing e', a point at the
+ * epipole or collinear x_i give no H.  The first degenerate record starts a plane-and-parallax round: its H is refitted
+ * on the rows within h_th (DLT while the count grows, fp64 tests), then 1024 two-row samples from a second stream of
+ * the generator (seed ^ 0x5851F42D4C957F2D, hypotheses first .. first + 1023; a draw within h_th of H is re-drawn,
+ * at most 64 draws) give e' = (H x_a x x'_a) x (H x_b x x'_b) and F = [e']x H, scored as F and adopted only with
+ * strictly more inliers.  One such round finds a pair of off-plane inliers among the H outliers (fraction w) with
+ * probability 1 - (1 - w^2)^1024, 0.998 at w = 8 %. */
 P2P_API int p2p_find_model(p2p_handle_t h, int model, const double* rows, int row_stride, int n, const double* n_dev,
                    double px_th, double conf, int max_iters, unsigned long long seed, double* model_out, uint8_t* mask_out,
                    int32_t* n_inliers_out, void* stream);
@@ -215,6 +230,12 @@ P2P_API int p2p_sampson_distance(p2p_handle_t h, const double* rows, int row_str
  * (slots 3 for F, 1 for H; zero where a slot has no model), counts_out DEVICE int32 [count*slots] (-1: no model). */
 P2P_API int p2p_test_hypotheses(p2p_handle_t h, int model, const double* rows, int row_stride, int n, double px_th,
                         unsigned long long seed, int count, double* models_out, int32_t* counts_out, void* stream);
+/* Test hook: model 2's degeneracy test on every root of F hypotheses 0 .. count-1 (count <= 2^20), slot layout as
+ * p2p_test_hypotheses.  triplet_out DEVICE int32 [count*3]: -2 = no model in the slot, -1 = not degenerate, else the
+ * index (0..4) of the first degenerate triplet; H_out DEVICE double [count*3][9]: that triplet's induced H in pixel
+ * coordinates at H[2][2] = 1 (zeros unless degenerate). */
+P2P_API int p2p_test_degeneracy(p2p_handle_t h, const double* rows, int row_stride, int n, double px_th,
+                                unsigned long long seed, int count, int32_t* triplet_out, double* H_out, void* stream);
 
 /* Relative pose -- the reference's matches2relapose_cv (utils/eval/geometry.py:32-48): cv2.findEssentialMat(RANSAC) and
  * cv2.recoverPose, on the device.  rows / row_stride / n / n_dev as p2p_find_model; intr HOST double[8] = (fx1, fy1,

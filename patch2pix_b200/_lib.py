@@ -55,6 +55,7 @@ _SIGNATURES = {
     'p2p_find_model': (_I, [_P, _I, _P, _I, _I, _P, C.c_double, C.c_double, _I, C.c_ulonglong, _P, _P, _P, _P]),
     'p2p_sampson_distance': (_I, [_P, _P, _I, _I, _P, _P, _P]),
     'p2p_test_hypotheses': (_I, [_P, _I, _P, _I, _I, C.c_double, C.c_ulonglong, _I, _P, _P, _P]),
+    'p2p_test_degeneracy': (_I, [_P, _P, _I, _I, C.c_double, C.c_ulonglong, _I, _P, _P, _P]),
     'p2p_find_essential': (_I, [_P, _P, _I, _I, _P, _P, C.c_double, C.c_double, _I, C.c_ulonglong, _P, _P, _P, _P]),
     'p2p_recover_pose': (_I, [_P, _P, _I, _I, _P, _P, _P, _P, C.c_double, _P, _P, _P, _P]),
     'p2p_test_essential_hypotheses': (_I, [_P, _P, _I, _I, _P, C.c_double, C.c_ulonglong, _I, _P, _P, _P]),

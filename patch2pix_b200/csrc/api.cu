@@ -1151,7 +1151,7 @@ int p2p_find_model(p2p_handle_t h, int model, const double* rows, int row_stride
                    double conf, int max_iters, unsigned long long seed, double* model_out, uint8_t* mask_out,
                    int32_t* n_inliers_out, void* stream) {
   P2P_ENTER(h);
-  P2P_REQUIRE(model == 0 || model == 1, "model must be 0 (F) or 1 (H)");
+  P2P_REQUIRE(model >= 0 && model <= 2, "model must be 0 (F), 1 (H) or 2 (F with the DEGENSAC degeneracy check)");
   P2P_REQUIRE(model_out && mask_out && n_inliers_out && (rows || n == 0), "null tensor pointer");
   P2P_REQUIRE(n >= 0 && n <= (1 << 26) && row_stride >= 4, "bad row count or stride");
   P2P_REQUIRE(px_th > 0.0 && isfinite(px_th), "px_th must be positive");
@@ -1182,6 +1182,19 @@ int p2p_test_hypotheses(p2p_handle_t h, int model, const double* rows, int row_s
   if (rc) return rc;
   void* scratch = h->verify.take(verify_scratch_bytes(n, false));
   return launch_test_hypotheses(model, rows, row_stride, n, px_th, seed, count, scratch, models_out, counts_out,
+                                reinterpret_cast<cudaStream_t>(stream));
+}
+
+int p2p_test_degeneracy(p2p_handle_t h, const double* rows, int row_stride, int n, double px_th, unsigned long long seed,
+                        int count, int32_t* triplet_out, double* H_out, void* stream) {
+  P2P_ENTER(h);
+  P2P_REQUIRE(rows && triplet_out && H_out && count > 0 && count <= (1 << 20) && row_stride >= 4, "bad argument");
+  P2P_REQUIRE(n >= 7 && n <= (1 << 26), "fewer rows than a minimal sample");
+  P2P_REQUIRE(px_th > 0.0 && isfinite(px_th), "px_th must be positive");
+  int rc = h->verify.reserve(verify_degeneracy_scratch_bytes(n, count) + 4096);
+  if (rc) return rc;
+  void* scratch = h->verify.take(verify_degeneracy_scratch_bytes(n, count));
+  return launch_test_degeneracy(rows, row_stride, n, px_th, seed, count, scratch, triplet_out, H_out,
                                 reinterpret_cast<cudaStream_t>(stream));
 }
 

@@ -105,7 +105,8 @@ int launch_fc_parse(const float* pooled, const FcWeights& fc, const void* matche
 int launch_finalize_matches(const float* fine, const float* scores, const long long* coarse, int N, float io_thres,
                             const double up[4], double* packed, cudaStream_t st);
 
-// ---- verify.cu: RANSAC for F (model 0, 7-point) / H (model 1, 4-point DLT) and the Sampson distance ----------------
+// ---- verify.cu: RANSAC for F (model 0, 7-point) / H (model 1, 4-point DLT) / F with DEGENSAC (model 2) and the
+// Sampson distance ----------------------------------------------------------------------------------------------------
 // rows: fp64 (x1, y1, x2, y2) at `stride` doubles apart; n_dev (optional, device): effective row count min(n, *n_dev).
 size_t verify_scratch_bytes(int n, bool rounds);
 int launch_find_model(int model, const double* rows, int stride, int n, const double* n_dev, double px_th, double conf,
@@ -115,6 +116,15 @@ int launch_find_model(int model, const double* rows, int stride, int n, const do
 int launch_test_hypotheses(int model, const double* rows, int stride, int n, double px_th, unsigned long long seed,
                            int count, void* scratch, double* models_out, int* counts_out, cudaStream_t st);
 int launch_sampson_distance(const double* rows, int stride, int n, const double* F, double* out, cudaStream_t st);
+// ---- degensac.cu: model 2 of launch_find_model (same scratch) and its test hook
+int launch_find_model_degensac(const double* rows, int stride, int n, const double* n_dev, double px_th, double conf,
+                               int max_iters, unsigned long long seed, void* scratch, double* model_out, uint8_t* mask_out,
+                               int* count_out, cudaStream_t st);
+// DEGENSAC's degeneracy test of every slot of F hypotheses 0 .. count-1: tri_out [count*3] (-2: no model, -1: not
+// degenerate, else the first degenerate triplet), H_out [count*3][9] (its induced H in pixels, zeros otherwise).
+size_t verify_degeneracy_scratch_bytes(int n, int count);
+int launch_test_degeneracy(const double* rows, int stride, int n, double px_th, unsigned long long seed, int count,
+                           void* scratch, int* tri_out, double* H_out, cudaStream_t st);
 
 // ---- pose.cu: essential-matrix RANSAC (5-point) and pose recovery ------------------------------------------------
 struct Intrinsics { double fx1, fy1, cx1, cy1, fx2, fy2, cx2, cy2; };   // pixels -> camera coordinates of both views

@@ -151,12 +151,13 @@ __device__ __forceinline__ double block_sum_1024(double v, double* red) {   // f
 // ---- per-round selection (one block of 1024 threads) --------------------------------------------------------------
 // Best of this round's nm models -> state if strictly better than the best so far (most inliers, ties to the lowest
 // (hypothesis, root) index); then the stopping bound log(1-conf) / log(1-w^s).  State has best[9], n, stop, best_count.
+// `past_stop` selects even when an earlier select of the same round has set stop (extra candidates of that round).
 template <typename State>
 __device__ __forceinline__ void select_round(State* __restrict__ st, const double* __restrict__ models,
                                              const int* __restrict__ counts, int nm, int done, int sample, double conf,
-                                             int max_iters) {
+                                             int max_iters, bool past_stop = false) {
   __shared__ unsigned long long red[32];
-  if (st->stop) return;
+  if (st->stop && !past_stop) return;
   const int tid = threadIdx.x;
   unsigned long long key = 0;     // (count, lowest index first)
   for (int m = tid; m < nm; m += 1024) {

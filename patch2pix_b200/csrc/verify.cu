@@ -1,5 +1,6 @@
 // Robust two-view model estimation on the device: RANSAC for a fundamental matrix (7-point minimal solver) or a homography
-// (4-point DLT), with local optimisation, plus the reference's Sampson distance (utils/eval/measure.py:18-40).
+// (4-point DLT), with local optimisation; F with the DEGENSAC plane-degeneracy check (Chum, Werner & Matas, CVPR 2005);
+// and the reference's Sampson distance (utils/eval/measure.py:18-40).
 //
 // One call enqueues, with no host sync:
 //   verify_prep_kernel     (1 block)  effective row count, finiteness, Hartley normalisation, fp32 copy of the rows
@@ -8,442 +9,15 @@
 //   verify_select_kernel   (x rounds) best model so far (most inliers, ties to the lowest (hypothesis, root) index) and
 //                                     the stopping bound log(1-conf) / log(1-w^s); later rounds return at once past it
 //   verify_lo_kernel       (1 block)  non-minimal refit on the winner's inliers while the count grows, final mask
+// (verify_common.cuh; model 2, F with the DEGENSAC check, adds its launches in degensac.cu)
 // Every reduction runs in a fixed order and no grid size depends on the device, so results are bit-reproducible.
 #include <math.h>
 
 #include "kernels.h"
-#include "ransac_common.cuh"
+#include "verify_common.cuh"
 
 namespace p2p {
 namespace {
-
-constexpr int kRound = 1024;        // hypotheses per round
-constexpr int kHypPerBlock = 8;     // hypotheses solved (one thread each) and scored per block
-constexpr int kScoreThreads = 256;  // 8 warps
-constexpr int kTile = 2048;         // rows staged in shared memory per pass (32 KB)
-constexpr int kLoIters = 4;         // local-optimisation refits
-constexpr int kLoThreads = 256;
-
-struct VerifyState {
-  double cx[2], cy[2], s[2];        // Hartley normalisation x' = s (x - c) of image 1 and image 2
-  double best[9];                   // best model so far, pixel coordinates
-  int n;                            // effective row count
-  int bad;                          // a coordinate is not finite
-  int stop;                         // no further rounds are needed
-  int best_count;                   // 0: no model yet
-};
-
-template <int KIND> struct Kind;
-template <> struct Kind<0> { static constexpr int kSample = 7, kSlots = 3, kLoMin = 8; };   // F: up to 3 roots
-template <> struct Kind<1> { static constexpr int kSample = 4, kSlots = 1, kLoMin = 4; };   // H
-
-// ---- fp64 linear algebra (one thread) ----------------------------------------------------------------------------
-
-__device__ __forceinline__ double det3(const double* m) {
-  return m[0] * (m[4] * m[8] - m[5] * m[7]) - m[1] * (m[3] * m[8] - m[5] * m[6]) + m[2] * (m[3] * m[7] - m[4] * m[6]);
-}
-
-// Real roots of a3 l^3 + a2 l^2 + a1 l + a0 (trigonometric form for three real roots, Cardano for one).
-__device__ int cubic_roots(double a3, double a2, double a1, double a0, double (&r)[3]) {
-  const double m = fmax(fmax(fabs(a3), fabs(a2)), fmax(fabs(a1), fabs(a0)));
-  if (!(m > 0.0)) return 0;
-  if (fabs(a3) <= 1e-12 * m) {                        // degree drop: one root went to infinity
-    if (fabs(a2) <= 1e-12 * m) {
-      if (fabs(a1) <= 1e-12 * m) return 0;
-      r[0] = -a0 / a1;
-      return 1;
-    }
-    const double disc = a1 * a1 - 4.0 * a2 * a0;
-    if (disc < 0.0) return 0;
-    const double qq = -0.5 * (a1 + copysign(sqrt(disc), a1));
-    r[0] = qq / a2;
-    if (qq == 0.0) return 1;
-    r[1] = a0 / qq;
-    return 2;
-  }
-  const double b = a2 / a3, c = a1 / a3, d = a0 / a3;
-  const double p = c - b * b / 3.0, q = 2.0 * b * b * b / 27.0 - b * c / 3.0 + d, shift = -b / 3.0;
-  const double disc = q * q / 4.0 + p * p * p / 27.0;
-  if (disc > 0.0) {
-    const double sq = sqrt(disc);
-    r[0] = cbrt(-q / 2.0 + sq) + cbrt(-q / 2.0 - sq) + shift;
-    return 1;
-  }
-  if (p >= 0.0) {
-    r[0] = shift;
-    return 1;
-  }
-  const double rr = 2.0 * sqrt(-p / 3.0);
-  const double phi = acos(fmin(1.0, fmax(-1.0, 1.5 * q / p * sqrt(-3.0 / p)))) / 3.0;
-  for (int k = 0; k < 3; ++k) r[k] = rr * cos(phi - 2.0943951023931957 * k) + shift;
-  return 3;
-}
-
-__device__ __forceinline__ void mat3_mul(const double* a, const double* b, double* c) {
-  for (int i = 0; i < 3; ++i)
-    for (int j = 0; j < 3; ++j) c[i * 3 + j] = a[i * 3] * b[j] + a[i * 3 + 1] * b[3 + j] + a[i * 3 + 2] * b[6 + j];
-}
-
-// Normalised-coordinate model -> pixel coordinates.  F = T2^T Fn T1 scaled to unit Frobenius norm;
-// H = T2^-1 Hn T1 scaled to H[2][2] = 1.  False when the scale is degenerate.
-template <int KIND>
-__device__ bool denormalise(const VerifyState& S, const double* mn, double* out) {
-  const double T1[9] = {S.s[0], 0.0, -S.s[0] * S.cx[0], 0.0, S.s[0], -S.s[0] * S.cy[0], 0.0, 0.0, 1.0};
-  double tmp[9];
-  mat3_mul(mn, T1, tmp);
-  if (KIND == 0) {
-    const double T2t[9] = {S.s[1], 0.0, 0.0, 0.0, S.s[1], 0.0, -S.s[1] * S.cx[1], -S.s[1] * S.cy[1], 1.0};
-    mat3_mul(T2t, tmp, out);
-    double nrm = 0.0;
-    for (int j = 0; j < 9; ++j) nrm += out[j] * out[j];
-    if (!(nrm > 0.0)) return false;
-    nrm = 1.0 / sqrt(nrm);
-    for (int j = 0; j < 9; ++j) out[j] *= nrm;
-    return true;
-  }
-  const double T2i[9] = {1.0 / S.s[1], 0.0, S.cx[1], 0.0, 1.0 / S.s[1], S.cy[1], 0.0, 0.0, 1.0};
-  mat3_mul(T2i, tmp, out);
-  double amax = 0.0;
-  for (int j = 0; j < 9; ++j) amax = fmax(amax, fabs(out[j]));
-  if (!(fabs(out[8]) > 1e-12 * amax)) return false;
-  const double inv = 1.0 / out[8];
-  for (int j = 0; j < 9; ++j) out[j] *= inv;
-  out[8] = 1.0;
-  return true;
-}
-
-// 7-point solver on normalised rows (x1, y1, x2, y2): up to 3 models x2^T F x1 = 0 in normalised coordinates,
-// ordered by ascending lambda of det(lambda F1 + (1 - lambda) F2) = 0.
-__device__ int solve_f7(const double (&p)[7][4], double (&out)[3][9]) {
-  double A[7][9], N[2][9];
-  for (int i = 0; i < 7; ++i) {
-    const double x1 = p[i][0], y1 = p[i][1], x2 = p[i][2], y2 = p[i][3];
-    const double row[9] = {x2 * x1, x2 * y1, x2, y2 * x1, y2 * y1, y2, x1, y1, 1.0};
-    for (int j = 0; j < 9; ++j) A[i][j] = row[j];
-  }
-  if (!null_space<7>(A, N)) return 0;
-  double D[9], M[9], v[4];
-  for (int j = 0; j < 9; ++j) D[j] = N[0][j] - N[1][j];
-  const double ls[4] = {0.0, 1.0, -1.0, 2.0};        // the cubic from its values at lambda = 0, 1, -1, 2
-  for (int t = 0; t < 4; ++t) {
-    for (int j = 0; j < 9; ++j) M[j] = N[1][j] + ls[t] * D[j];
-    v[t] = det3(M);
-  }
-  const double a0 = v[0], a2 = 0.5 * (v[1] + v[2]) - v[0], odd = 0.5 * (v[1] - v[2]);
-  const double a3 = (v[3] - v[0] - 4.0 * a2 - 2.0 * odd) / 6.0, a1 = odd - a3;
-  double r[3];
-  const int nr = cubic_roots(a3, a2, a1, a0, r);
-  for (int k = 0; k < nr; ++k)
-    for (int it = 0; it < 2; ++it) {                    // Newton polish
-      const double l = r[k];
-      const double f = ((a3 * l + a2) * l + a1) * l + a0, df = (3.0 * a3 * l + 2.0 * a2) * l + a1;
-      if (df != 0.0) r[k] = l - f / df;
-    }
-  for (int i = 1; i < nr; ++i)
-    for (int k = i; k > 0 && r[k] < r[k - 1]; --k) { const double t = r[k]; r[k] = r[k - 1]; r[k - 1] = t; }
-  for (int k = 0; k < nr; ++k)
-    for (int j = 0; j < 9; ++j) out[k][j] = N[1][j] + r[k] * D[j];
-  return nr;
-}
-
-__device__ __forceinline__ double orient(double ax, double ay, double bx, double by, double cx, double cy) {
-  return (bx - ax) * (cy - ay) - (by - ay) * (cx - ax);
-}
-
-// 4-point DLT on normalised rows.  Rejects a sample with 3 (near-)collinear points in either image, or whose
-// triangle orientations do not agree between the images in the same way for all four triples.
-__device__ int solve_h4(const double (&p)[4][4], double (&out)[1][9]) {
-  const int tri[4][3] = {{0, 1, 2}, {0, 1, 3}, {0, 2, 3}, {1, 2, 3}};
-  int sgn = 0;
-  for (int t = 0; t < 4; ++t) {
-    const int a = tri[t][0], b = tri[t][1], c = tri[t][2];
-    const double o1 = orient(p[a][0], p[a][1], p[b][0], p[b][1], p[c][0], p[c][1]);
-    const double o2 = orient(p[a][2], p[a][3], p[b][2], p[b][3], p[c][2], p[c][3]);
-    if (!(fabs(o1) > 1e-6) || !(fabs(o2) > 1e-6)) return 0;
-    const int s = (o1 > 0.0) == (o2 > 0.0) ? 1 : -1;
-    if (t == 0) sgn = s;
-    else if (s != sgn) return 0;
-  }
-  double A[8][9], N[1][9];
-  for (int i = 0; i < 4; ++i) {
-    const double x = p[i][0], y = p[i][1], u = p[i][2], v = p[i][3];
-    const double r0[9] = {-x, -y, -1.0, 0.0, 0.0, 0.0, u * x, u * y, u};
-    const double r1[9] = {0.0, 0.0, 0.0, -x, -y, -1.0, v * x, v * y, v};
-    for (int j = 0; j < 9; ++j) { A[2 * i][j] = r0[j]; A[2 * i + 1][j] = r1[j]; }
-  }
-  if (!null_space<8>(A, N)) return 0;
-  for (int j = 0; j < 9; ++j) out[0][j] = N[0][j];
-  return 1;
-}
-
-// ---- scoring ------------------------------------------------------------------------------------------------------
-// F: dd^2 / den < th^2.  H: |pi(H x1) - x2|^2 < th^2, never with a non-positive or vanishing third coordinate.
-template <int KIND>
-__device__ __forceinline__ bool is_inlier(const float* m, float4 r, float th2) {
-  if (KIND == 0) {
-    float dd, den;
-    sampson_terms<float>(m, r.x, r.y, r.z, r.w, dd, den);
-    return dd * dd < th2 * den;
-  }
-  const float w = m[6] * r.x + m[7] * r.y + m[8];
-  const float u = m[0] * r.x + m[1] * r.y + m[2] - r.z * w, v = m[3] * r.x + m[4] * r.y + m[5] - r.w * w;
-  return w > 1e-8f && u * u + v * v < th2 * w * w;
-}
-
-// ---- kernels ------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(1024) verify_prep_kernel(const double* __restrict__ rows, int stride, int n,
-                                                           const double* __restrict__ n_dev, int min_rows,
-                                                           float4* __restrict__ rows32, VerifyState* __restrict__ st) {
-  __shared__ double red[33];
-  __shared__ int s_n, s_bad;
-  const int tid = threadIdx.x;
-  if (tid == 0) {
-    int m = n;
-    if (n_dev != nullptr) {
-      const double v = *n_dev;
-      if (v >= 0.0 && v < (double)n) m = (int)v;
-    }
-    s_n = m;
-    s_bad = 0;
-  }
-  __syncthreads();
-  const int m = s_n;
-  double sx[4] = {0.0, 0.0, 0.0, 0.0};
-  int bad = 0;
-  for (int r = tid; r < m; r += 1024) {
-    const double* p = rows + (size_t)r * stride;
-    const double a = p[0], b = p[1], c = p[2], d = p[3];
-    bad |= !(isfinite(a) && isfinite(b) && isfinite(c) && isfinite(d));
-    sx[0] += a; sx[1] += b; sx[2] += c; sx[3] += d;
-    rows32[r] = make_float4((float)a, (float)b, (float)c, (float)d);
-  }
-  if (bad) s_bad = 1;
-  double mean[4];
-  for (int k = 0; k < 4; ++k) mean[k] = block_sum_1024(sx[k], red) / (double)(m > 0 ? m : 1);
-  double dist[2] = {0.0, 0.0};
-  if (!s_bad)
-    for (int r = tid; r < m; r += 1024) {
-      const double* p = rows + (size_t)r * stride;
-      dist[0] += sqrt((p[0] - mean[0]) * (p[0] - mean[0]) + (p[1] - mean[1]) * (p[1] - mean[1]));
-      dist[1] += sqrt((p[2] - mean[2]) * (p[2] - mean[2]) + (p[3] - mean[3]) * (p[3] - mean[3]));
-    }
-  for (int k = 0; k < 2; ++k) dist[k] = block_sum_1024(dist[k], red) / (double)(m > 0 ? m : 1);
-  if (tid == 0) {
-    for (int k = 0; k < 2; ++k) {
-      st->cx[k] = mean[2 * k];
-      st->cy[k] = mean[2 * k + 1];
-      st->s[k] = dist[k] > 0.0 ? 1.4142135623730951 / dist[k] : 1.0;
-    }
-    for (int j = 0; j < 9; ++j) st->best[j] = 0.0;
-    st->n = m;
-    st->bad = s_bad;
-    st->stop = s_bad || m < min_rows;
-    st->best_count = 0;
-  }
-}
-
-// Hypotheses first .. first + count - 1.  models [count * slots][9] fp64 (pixel coordinates), counts [count * slots]
-// (-1: no model in that slot).
-template <int KIND>
-__global__ void __launch_bounds__(kScoreThreads, 1) verify_round_kernel(const VerifyState* __restrict__ st,
-                                                                     const float4* __restrict__ rows32,
-                                                                     const double* __restrict__ rows, int stride,
-                                                                     int first, int count, unsigned long long seed,
-                                                                     float th2, int ignore_stop, double* __restrict__ models,
-                                                                     int* __restrict__ counts) {
-  constexpr int S = Kind<KIND>::kSample, SL = Kind<KIND>::kSlots, NM = kHypPerBlock * SL;
-  __shared__ float4 s_rows[kTile];
-  __shared__ float s_model[NM][9];
-  __shared__ int s_valid[NM];
-  if (!ignore_stop && st->stop) return;
-  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  const int n = st->n;
-  if (tid < kHypPerBlock) {
-    const int local = blockIdx.x * kHypPerBlock + tid;
-    double out[SL][9];
-    int nm = 0;
-    if (local < count) {
-      int idx[S];
-      if (draw_sample<S>(seed, first + local, n, idx)) {
-        double p[S][4];
-#pragma unroll
-        for (int k = 0; k < S; ++k) {
-          const double* r = rows + (size_t)idx[k] * stride;
-          p[k][0] = (r[0] - st->cx[0]) * st->s[0];
-          p[k][1] = (r[1] - st->cy[0]) * st->s[0];
-          p[k][2] = (r[2] - st->cx[1]) * st->s[1];
-          p[k][3] = (r[3] - st->cy[1]) * st->s[1];
-        }
-        double mn[SL][9];
-        int raw;
-        if constexpr (KIND == 0) raw = solve_f7(p, mn);
-        else raw = solve_h4(p, mn);
-        for (int k = 0; k < raw; ++k)
-          if (denormalise<KIND>(*st, mn[k], out[nm])) ++nm;
-      }
-    }
-    for (int k = 0; k < SL; ++k) {
-      const int slot = tid * SL + k;
-      s_valid[slot] = k < nm;
-      for (int j = 0; j < 9; ++j) {
-        s_model[slot][j] = k < nm ? (float)out[k][j] : 0.f;
-        if (local < count) models[((size_t)local * SL + k) * 9 + j] = k < nm ? out[k][j] : 0.0;
-      }
-    }
-  }
-  int cnt[(NM + 7) / 8];
-#pragma unroll
-  for (int j = 0; j < (NM + 7) / 8; ++j) cnt[j] = 0;
-  for (int t0 = 0; t0 < n; t0 += kTile) {
-    const int tn = min(kTile, n - t0);
-    __syncthreads();
-    for (int r = tid; r < tn; r += kScoreThreads) s_rows[r] = rows32[t0 + r];
-    __syncthreads();
-#pragma unroll
-    for (int j = 0; j < (NM + 7) / 8; ++j) {
-      const int mi = wid + 8 * j;
-      if (mi >= NM || !s_valid[mi]) continue;
-      float m[9];
-#pragma unroll
-      for (int e = 0; e < 9; ++e) m[e] = s_model[mi][e];
-      for (int r0 = 0; r0 < tn; r0 += 32) {
-        const int r = r0 + lane;
-        const bool in = r < tn && is_inlier<KIND>(m, s_rows[r < tn ? r : 0], th2);
-        cnt[j] += __popc(__ballot_sync(0xffffffffu, in));
-      }
-    }
-  }
-  if (lane == 0) {
-#pragma unroll
-    for (int j = 0; j < (NM + 7) / 8; ++j) {
-      const int mi = wid + 8 * j;
-      const int local = blockIdx.x * kHypPerBlock + mi / SL;
-      if (mi < NM && local < count) counts[(size_t)blockIdx.x * NM + mi] = s_valid[mi] ? cnt[j] : -1;
-    }
-  }
-}
-
-// Best of this round's nm models -> state if strictly better than the best so far; then the stopping bound.
-__global__ void __launch_bounds__(1024) verify_select_kernel(VerifyState* __restrict__ st, const double* __restrict__ models,
-                                                             const int* __restrict__ counts, int nm, int done, int sample,
-                                                             double conf, int max_iters) {
-  select_round(st, models, counts, nm, done, sample, conf, max_iters);
-}
-
-// Local optimisation + outputs.  Refits on the inliers of the current model in normalised coordinates (F: 8-point with
-// rank-2 enforcement; H: DLT), keeps the refit while it has strictly more inliers, then writes model, mask and count.
-template <int KIND>
-__global__ void __launch_bounds__(kLoThreads, 1) verify_lo_kernel(const VerifyState* __restrict__ st,
-                                                               const float4* __restrict__ rows32,
-                                                               const double* __restrict__ rows, int stride, int n_all,
-                                                               float th2, double* __restrict__ model_out,
-                                                               uint8_t* __restrict__ mask_out, int* __restrict__ count_out) {
-  __shared__ double s_red[kLoThreads / 32][45];
-  __shared__ double s_cur[9], s_cand[9];
-  __shared__ float s_f32[9];
-  __shared__ int s_cnt[kLoThreads / 32], s_ok;
-  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  const int n = st->n, bad = st->bad;
-  int cur_count = bad ? 0 : st->best_count;
-  if (tid < 9) s_cur[tid] = st->best[tid];
-  __syncthreads();
-
-  auto count_inliers = [&](const double* m64) -> int {    // block-wide, fixed order
-    if (tid < 9) s_f32[tid] = (float)m64[tid];
-    __syncthreads();
-    float m[9];
-#pragma unroll
-    for (int e = 0; e < 9; ++e) m[e] = s_f32[e];
-    int c = 0;
-    for (int r = tid; r < n; r += kLoThreads) c += is_inlier<KIND>(m, rows32[r], th2);
-    for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
-    if (lane == 0) s_cnt[wid] = c;
-    __syncthreads();
-    int tot = 0;
-    for (int w = 0; w < kLoThreads / 32; ++w) tot += s_cnt[w];
-    __syncthreads();
-    return tot;
-  };
-
-  for (int it = 0; it < kLoIters && cur_count >= Kind<KIND>::kLoMin; ++it) {
-    if (tid < 9) s_f32[tid] = (float)s_cur[tid];
-    __syncthreads();
-    float m[9];
-#pragma unroll
-    for (int e = 0; e < 9; ++e) m[e] = s_f32[e];
-    double acc[45];
-#pragma unroll
-    for (int e = 0; e < 45; ++e) acc[e] = 0.0;
-    const double c1x = st->cx[0], c1y = st->cy[0], s1 = st->s[0], c2x = st->cx[1], c2y = st->cy[1], s2 = st->s[1];
-    for (int r = tid; r < n; r += kLoThreads) {
-      if (!is_inlier<KIND>(m, rows32[r], th2)) continue;
-      const double* p = rows + (size_t)r * stride;
-      const double x = (p[0] - c1x) * s1, y = (p[1] - c1y) * s1, u = (p[2] - c2x) * s2, v = (p[3] - c2y) * s2;
-      if (KIND == 0) {
-        const double a[9] = {u * x, u * y, u, v * x, v * y, v, x, y, 1.0};
-        int e = 0;
-#pragma unroll
-        for (int i = 0; i < 9; ++i)
-#pragma unroll
-          for (int j = i; j < 9; ++j) acc[e++] += a[i] * a[j];
-      } else {
-        const double a[9] = {-x, -y, -1.0, 0.0, 0.0, 0.0, u * x, u * y, u};
-        const double b[9] = {0.0, 0.0, 0.0, -x, -y, -1.0, v * x, v * y, v};
-        int e = 0;
-#pragma unroll
-        for (int i = 0; i < 9; ++i)
-#pragma unroll
-          for (int j = i; j < 9; ++j) acc[e++] += a[i] * a[j] + b[i] * b[j];
-      }
-    }
-#pragma unroll
-    for (int e = 0; e < 45; ++e) {
-      const double v = warp_sum_d(acc[e]);
-      if (lane == 0) s_red[wid][e] = v;
-    }
-    __syncthreads();
-    if (tid == 0) {
-      double M[9][9], h[9];
-      int e = 0;
-      for (int i = 0; i < 9; ++i)
-        for (int j = i; j < 9; ++j) {
-          double v = 0.0;
-          for (int w = 0; w < kLoThreads / 32; ++w) v += s_red[w][e];
-          M[i][j] = M[j][i] = v;
-          ++e;
-        }
-      jacobi_min_eigvec<9>(M, h);
-      if (KIND == 0) {                                     // rank 2: F <- F (I - e e^T), e the smallest right singular vector
-        double G[3][3], ev[3];
-        for (int i = 0; i < 3; ++i)
-          for (int j = 0; j < 3; ++j) G[i][j] = h[i] * h[j] + h[3 + i] * h[3 + j] + h[6 + i] * h[6 + j];
-        jacobi_min_eigvec<3>(G, ev);
-        for (int i = 0; i < 3; ++i) {
-          const double fe = h[3 * i] * ev[0] + h[3 * i + 1] * ev[1] + h[3 * i + 2] * ev[2];
-          for (int j = 0; j < 3; ++j) h[3 * i + j] -= fe * ev[j];
-        }
-      }
-      s_ok = denormalise<KIND>(*st, h, s_cand);
-    }
-    __syncthreads();
-    if (!s_ok) break;
-    const int c = count_inliers(s_cand);
-    if (c <= cur_count) break;
-    cur_count = c;
-    if (tid < 9) s_cur[tid] = s_cand[tid];
-    __syncthreads();
-  }
-
-  if (tid < 9) model_out[tid] = bad ? __longlong_as_double(0x7ff8000000000000ll) : (cur_count > 0 ? s_cur[tid] : 0.0);
-  if (tid == 0) *count_out = bad ? -1 : cur_count;
-  if (tid < 9) s_f32[tid] = (float)s_cur[tid];
-  __syncthreads();
-  float m[9];
-#pragma unroll
-  for (int e = 0; e < 9; ++e) m[e] = s_f32[e];
-  for (int r = tid; r < n_all; r += kLoThreads)
-    mask_out[r] = cur_count > 0 && r < n && is_inlier<KIND>(m, rows32[r], th2);
-}
 
 __global__ void sampson_kernel(const double* __restrict__ rows, int stride, int n, const double* __restrict__ F,
                                double* __restrict__ out) {
@@ -456,35 +30,6 @@ __global__ void sampson_kernel(const double* __restrict__ rows, int stride, int 
   double dd, den;
   sampson_terms<double>(m, p[0], p[1], p[2], p[3], dd, den);
   out[r] = dd * dd / (1e-8 + den);
-}
-
-struct Scratch {
-  VerifyState* st;
-  float4* rows32;
-  double* models;
-  int* counts;
-};
-
-Scratch carve(void* base, int n, int nhyp) {
-  char* p = (char*)base;
-  Scratch s;
-  s.st = (VerifyState*)p;
-  p += 1024;
-  s.rows32 = (float4*)p;
-  p += align_up((size_t)n * sizeof(float4) + 16, 1024);
-  s.models = (double*)p;
-  p += align_up((size_t)nhyp * 3 * 9 * sizeof(double), 1024);
-  s.counts = (int*)p;
-  return s;
-}
-
-template <int KIND>
-int enqueue_round(const Scratch& s, const double* rows, int stride, int first, int count, unsigned long long seed, float th2,
-                  int ignore_stop, cudaStream_t st) {
-  verify_round_kernel<KIND><<<cdiv(count, kHypPerBlock), kScoreThreads, 0, st>>>(s.st, s.rows32, rows, stride, first, count,
-                                                                                 seed, th2, ignore_stop, s.models, s.counts);
-  P2P_LAUNCH_OK();
-  return 0;
 }
 
 template <int KIND>
@@ -528,6 +73,9 @@ size_t verify_scratch_bytes(int n, bool rounds) {
 int launch_find_model(int model, const double* rows, int stride, int n, const double* n_dev, double px_th, double conf,
                       int max_iters, unsigned long long seed, void* scratch, double* model_out, uint8_t* mask_out,
                       int* count_out, cudaStream_t st) {
+  if (model == 2)
+    return launch_find_model_degensac(rows, stride, n, n_dev, px_th, conf, max_iters, seed, scratch, model_out, mask_out,
+                               count_out, st);
   return model == 0 ? find_model<0>(rows, stride, n, n_dev, px_th, conf, max_iters, seed, scratch, model_out, mask_out,
                                     count_out, st)
                     : find_model<1>(rows, stride, n, n_dev, px_th, conf, max_iters, seed, scratch, model_out, mask_out,

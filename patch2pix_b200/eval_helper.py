@@ -67,8 +67,9 @@ def _finalize(net, fine, scores, coarse, io_thres, upscale, verify=None):
         from . import pose as P
         from . import verify as V
         kind = verify[0] if isinstance(verify, (tuple, list)) and len(verify) > 0 else None
-        if not (kind in ('F', 'H') and len(verify) == 2 or kind == 'E' and len(verify) == 4):
-            raise ValueError("verify must be None, ('F', px_th), ('H', px_th) or ('E', px_th, K1, K2)")
+        if not (kind in ('F', 'H', 'DEGENSAC') and len(verify) == 2 or kind == 'E' and len(verify) == 4):
+            raise ValueError("verify must be None, ('F', px_th), ('H', px_th), ('DEGENSAC', px_th) or "
+                             "('E', px_th, K1, K2)")
         px_th = verify[1]
         extra = P.out_size(n) if kind == 'E' else V.out_size(n)
     packed = torch.empty(n * 9 + 1 + extra, dtype=torch.float64, device=dev)
@@ -86,8 +87,8 @@ def _finalize(net, fine, scores, coarse, io_thres, upscale, verify=None):
         P.find_essential_into(h, packed, 9, n, n_dev, intr, px_th, 0.999, 1000, 0, out)
         P.recover_pose_into(h, packed, 9, n, n_dev, intr, out.data_ptr(), out.data_ptr() + 184, out)
     elif verify is not None:      # RANSAC on the kept, rescaled rows (refined columns 0..3), in place, count read on the device
-        V.find_model_into(h, V.MODEL_F if kind == 'F' else V.MODEL_H, packed, 9, n, n_dev, px_th, 0.999, 10000, 0,
-                          packed[n * 9 + 1:])
+        model = {'F': V.MODEL_F, 'H': V.MODEL_H, 'DEGENSAC': V.MODEL_F_DEGENSAC}[kind]
+        V.find_model_into(h, model, packed, 9, n, n_dev, px_th, 0.999, 10000, 0, packed[n * 9 + 1:])
     host = packed.cpu().numpy()                      # the single synchronising copy
     m = int(host[n * 9])
     rows = host[:n * 9].reshape(n, 9)[:m]
@@ -110,7 +111,8 @@ def estimate_matches(net, im1, im2, scale1=(1.0, 1.0), scale2=(1.0, 1.0), ksize=
     verify=('F', px_th) or ('H', px_th) also runs RANSAC (patch2pix_b200.verify, conf 0.999, 10000 iterations, seed 0)
     on the device on those matches, px_th in original-image pixels, still before the single copy, and returns
     (matches, scores, coarse_matches, inliers, model): a bool mask over the matches and the 3x3 float64 F or H
-    (None when no model was found).
+    (None when no model was found).  verify=('DEGENSAC', px_th) runs F RANSAC with the DEGENSAC plane-degeneracy
+    check instead (the notebook's pydegensac.findFundamentalMatrix) and returns what ('F', px_th) returns.
 
     verify=('E', px_th, K1, K2), with K1, K2 the 3x3 intrinsics in original-image pixels, runs the reference's
     matches2relapose_cv instead (patch2pix_b200.pose: E RANSAC at conf 0.999 and 1000 iterations, then pose recovery on

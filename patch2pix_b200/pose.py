@@ -121,6 +121,34 @@ def reference_intrinsics(K1, K2):
     return (C.c_double * 8)(f1, f1, K1[0, 2], K1[1, 2], f2, f2, K2[0, 2], K2[1, 2])
 
 
+def matches2relapose_degensac(p1, p2, K1, K2, rthres=1):
+    """utils/eval/geometry.py:50-71 on the GPU -> (E, inls, R, t): the rows rescaled as the reference does (p1 ->
+    (p1 - pc1) * f2 / f1, p2 -> p2 - pc2, f = K[0, 0]), F RANSAC with the DEGENSAC check (model 2) at `rthres` px,
+    E = K^T F K with K = diag(f2, f2, 1), the indices of F's inliers and the pose recovered from those rows (t [3, 1]).
+    One device->host copy.  conf 0.999 and 10000 iterations are this project's F defaults; pydegensac's own defaults
+    were not checked.  E is None and R, t are zero when no model was found."""
+    from . import verify as V
+    rows, _ = _rows(p1, p2)
+    n = int(rows.shape[0])
+    K1 = np.asarray(K1, dtype=np.float64).reshape(3, 3)
+    K2 = np.asarray(K2, dtype=np.float64).reshape(3, 3)
+    f1, f2 = float(K1[0, 0]), float(K2[0, 0])
+    rows = torch.cat((((rows[:, 0:2] - torch.tensor(K1[:2, 2], device=rows.device)) * f2) / f1,
+                      rows[:, 2:4] - torch.tensor(K2[:2, 2], device=rows.device)), 1).contiguous()
+    h = _lib.default_handle(rows.device)
+    intr = (C.c_double * 8)(f2, f2, 0.0, 0.0, f2, f2, 0.0, 0.0)
+    buf = torch.zeros(out_size(n) + V.out_size(n), dtype=torch.float64, device=rows.device)
+    out, fbuf = buf[:out_size(n)], buf[out_size(n):]        # pose buffer with E in [0:9], then the F-RANSAC buffer
+    V.find_model_into(h, V.MODEL_F_DEGENSAC, rows, 4, n, None, rthres, 0.999, 10000, 0, fbuf)
+    k = torch.tensor([f2, f2, 1.0], dtype=torch.float64, device=rows.device)
+    out[:9] = ((fbuf[:9].view(3, 3) * k[:, None]) * k[None, :]).reshape(9)      # K^T F K, as fund2ess
+    recover_pose_into(h, rows, 4, n, None, intr, out.data_ptr(), fbuf.data_ptr() + 80, out)
+    host = buf.cpu().numpy()
+    F, fmask = V.parse_host(host[out_size(n):], n)
+    _, _, _, R, t, _ = parse_host(host[:out_size(n)], n)
+    return (host[:9].reshape(3, 3).copy() if F is not None else None), np.where(fmask)[0], R, t
+
+
 def matches2relapose(p1, p2, K1, K2, rthres=1):
     """utils/eval/geometry.py:32-48 on the GPU -> (E, inls, R, t): E-RANSAC (conf 0.999, 1000 iterations, as
     cv2.findEssentialMat's defaults) at `rthres` px, the indices of its inliers, and the pose recovered from those rows

@@ -185,6 +185,30 @@ def synthetic_two_view(seed, n, outlier_ratio, noise_px, planar=False, width=640
     return dict(pts1=pts1, pts2=pts2, F=F, H=H, inlier=inlier, K1=Kc.copy(), K2=K2.copy(), R=R, t=t)
 
 
+PLANE, OFF_PLANE, OUTLIER = 0, 1, 2
+
+
+def synthetic_dominant_plane(seed, n, outlier_ratio, off_plane_ratio, noise_px, focal2=None, width=640, height=480):
+    """Seeded two-view scene where most true correspondences lie on one plane, as on building facades and ground planes:
+    round(n * (1 - outlier_ratio)) inliers, a fraction `off_plane_ratio` of them at general depth and the rest on the
+    plane, plus uniformly random outlier pairs, shuffled.  Both inlier sets come from `synthetic_two_view(seed, ...)`
+    (planar and not), which share one camera pair per seed, so F, R and t hold for every inlier and H for the plane.
+    Returns the dict of synthetic_two_view (H of the plane) plus `label` [n] int8: PLANE, OFF_PLANE or OUTLIER."""
+    n_in = int(round(n * (1.0 - outlier_ratio)))
+    n_off = int(round(n_in * off_plane_ratio))
+    pl = synthetic_two_view(seed, n_in - n_off, 0.0, noise_px, planar=True, width=width, height=height, focal2=focal2)
+    gen = synthetic_two_view(seed, n_off, 0.0, noise_px, width=width, height=height, focal2=focal2)
+    rng = np.random.default_rng([int(seed), 1])           # own stream for the outliers and the order
+    n_out = n - n_in
+    o1 = rng.uniform([0, 0], [width, height], (n_out, 2))
+    o2 = rng.uniform([0, 0], [width, height], (n_out, 2))
+    label = np.concatenate([np.full(n_in - n_off, PLANE), np.full(n_off, OFF_PLANE), np.full(n_out, OUTLIER)])
+    perm = rng.permutation(n)
+    label = label.astype(np.int8)[perm]
+    return dict(pl, pts1=np.concatenate([pl['pts1'], gen['pts1'], o1])[perm],
+                pts2=np.concatenate([pl['pts2'], gen['pts2'], o2])[perm], inlier=label != OUTLIER, label=label)
+
+
 def synthetic_pair_shifted(pair_idx, height, width, noise=0.6):
     """Benchmark workload (round 2): two overlapping views of one texture whose offset is a multiple
     of 16 px (= one pooled correlation cell at ksize 2), so that coarse cells correspond one to one in

@@ -1,4 +1,5 @@
-"""Match verification on the GPU: RANSAC for a fundamental matrix or a homography, and the Sampson distance.
+"""Match verification on the GPU: RANSAC for a fundamental matrix (optionally with the DEGENSAC plane-degeneracy check)
+or a homography, and the Sampson distance.
 
 Drop-in for the reference's consumers of the match list -- ``pydegensac.findFundamentalMatrix(p1, p2, 1.0)`` and
 ``findHomography(p1, p2, 2.0)`` in examples/visualize_matches.ipynb, ``sampson_distance`` of utils/eval/measure.py:18-40
@@ -15,7 +16,7 @@ import torch
 
 from . import _lib
 
-MODEL_F, MODEL_H = 0, 1
+MODEL_F, MODEL_H, MODEL_F_DEGENSAC = 0, 1, 2
 
 
 def _rows(pts1, pts2):
@@ -73,10 +74,14 @@ def _find(model, pts1, pts2, px_th, conf, max_iters, seed):
     return out[:9].view(3, 3), mask
 
 
-def find_fundamental_matrix(pts1, pts2, px_th, conf=0.999, max_iters=10000, seed=0):
+def find_fundamental_matrix(pts1, pts2, px_th, conf=0.999, max_iters=10000, seed=0, degeneracy_check=False):
     """RANSAC fundamental matrix (x2^T F x1 = 0, unit Frobenius norm) from [n, 2] point lists -> (F, inlier mask).
-    A row is an inlier iff its Sampson error (measure.py:36-39 without eps) is below px_th^2."""
-    return _find(MODEL_F, pts1, pts2, px_th, conf, max_iters, seed)
+    A row is an inlier iff its Sampson error (measure.py:36-39 without eps) is below px_th^2.
+
+    degeneracy_check=True adds DEGENSAC's plane-degeneracy test (pydegensac.findFundamentalMatrix): when the samples
+    that win a round have 5 of their 7 points on one plane, a plane-and-parallax round recovers the off-plane
+    geometry that plain RANSAC loses on scenes dominated by one plane (include/p2p_b200.h, model 2)."""
+    return _find(MODEL_F_DEGENSAC if degeneracy_check else MODEL_F, pts1, pts2, px_th, conf, max_iters, seed)
 
 
 def find_homography(pts1, pts2, px_th, conf=0.999, max_iters=10000, seed=0):
@@ -111,3 +116,16 @@ def first_hypotheses(model, pts1, pts2, px_th, count, seed=0):
                                              int(seed) & (2 ** 64 - 1), count, _lib.ptr(models), _lib.ptr(counts),
                                              h.stream()))
     return models.cpu().numpy(), counts.cpu().numpy()
+
+
+def first_degeneracy(pts1, pts2, px_th, count, seed=0):
+    """Test hook: DEGENSAC's degeneracy test on every root of the first `count` F hypotheses -> (triplet [count*3]
+    int32: -2 no model, -1 not degenerate, else the first degenerate triplet; H [count*3, 9] float64 in pixels)."""
+    rows, _ = _rows(pts1, pts2)
+    tri = torch.empty(count * 3, dtype=torch.int32, device=rows.device)
+    H = torch.empty(count * 3, 9, dtype=torch.float64, device=rows.device)
+    h = _lib.default_handle(rows.device)
+    with torch.cuda.device(rows.device):
+        _lib.check(h.lib.p2p_test_degeneracy(h.h, _lib.ptr(rows), 4, int(rows.shape[0]), float(px_th),
+                                             int(seed) & (2 ** 64 - 1), count, _lib.ptr(tri), _lib.ptr(H), h.stream()))
+    return tri.cpu().numpy(), H.cpu().numpy()
