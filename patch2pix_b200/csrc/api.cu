@@ -964,7 +964,6 @@ int run_regressor(p2p_handle_s* h, Regressor& R, int which, int passes, const Re
         p.fg.matches = matches_in;
         p.fg.is_float = is_float;
       }
-      ProfScope ps(h, kb + 1, st);
       if (mapped) {
         for (int s2 = 0; s2 < 2; ++s2) {
           const uint64_t Wp = (uint64_t)h->pf[s2].W + 2 * kMapPad, Hp = (uint64_t)h->pf[s2].H + 2 * kMapPad;
@@ -979,7 +978,11 @@ int run_regressor(p2p_handle_s* h, Regressor& R, int which, int passes, const Re
         }
         p.wm.matches = matches_in;
         p.wm.is_float = is_float;
+        // the rgb k-step's A operand (r_hi, read through a_rgb_hi); the main k-steps read the window maps directly
+        ProfScope ps(h, kb, st);
+        if ((rc = launch_window_rgb(p.wm, n, B.npad, B.r_hi, st))) return rc;
       }
+      ProfScope ps(h, kb + 1, st);
       const int amode = mapped ? AMODE_WINDOW : (fused ? AMODE_GATHER : AMODE_TMA);
       if ((rc = launch_umma_gemm(p, EPI_CONV1, passes, sms(h), st, amode))) return rc;
     }

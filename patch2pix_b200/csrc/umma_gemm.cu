@@ -139,15 +139,15 @@ constexpr int kMaxSmemPerBlock = 232448;   // sm_90 opt-in limit, static + dynam
 template <int PASSES, bool SEGMENTED, int AMODE>
 struct GemmCfg {
   static constexpr int NOP = PASSES == 3 ? 2 : 1;
-  static constexpr int THREADS = AMODE == AMODE_TMA ? 384 : 512;
-  // Output columns per tile.  The 1-pass unsegmented 384-thread kernels use 128x256 tiles (m64n256k16, 128
-  // accumulators per consumer thread): half the shared-memory operand reads per MAC, half the A re-streaming and half
-  // the epilogues of 128x128.  Everything else stays at 128:
+  static constexpr int THREADS = AMODE == AMODE_GATHER ? 512 : 384;
+  // Output columns per tile.  The 1-pass unsegmented 384-thread kernels (the window-map conv1 among them) use 128x256
+  // tiles (m64n256k16, 128 accumulators per consumer thread): half the shared-memory operand reads per MAC, half the
+  // A re-streaming and half the epilogues of 128x128.  Everything else stays at 128:
   //   3-pass and segmented kernels: their fp32 totals do not fit beside 128 accumulators;
-  //   512-thread conv1 kernels (AMODE_GATHER / AMODE_WINDOW): ptxas needs each instruction's operands to fit the
-  //   kernel-wide register target, 65536 / 512 = 128, whatever setmaxnreg grants, so m64n256k16 does not compile
-  //   there; two m64n128k16 per k16 slice do, but the epilogue beside 128 accumulators then spills at every
-  //   producer / A-operand / consumer split that fits their 4 x 128 registers per thread slot.
+  //   the 512-thread gather conv1 (AMODE_GATHER): ptxas needs each instruction's operands to fit the kernel-wide
+  //   register target, 65536 / 512 = 128, whatever setmaxnreg grants, so m64n256k16 does not compile there; two
+  //   m64n128k16 per k16 slice do, but the epilogue beside 128 accumulators then spills at every producer /
+  //   A-operand / consumer split that fits their 4 x 128 registers per thread slot.
   static constexpr int BN = PASSES == 1 && !SEGMENTED && THREADS == 384 ? 256 : 128;
   static constexpr int B_BYTES = BN * 128;                 // BN rows x 64 fp16, BN / 128 TMA boxes back to back
   static constexpr int STAGE_BYTES = NOP * (kATile + B_BYTES);
@@ -159,7 +159,8 @@ struct GemmCfg {
   static_assert(SMEM + STATIC_SMEM <= kMaxSmemPerBlock, "shared memory over the per-block limit");
   // Per-thread registers after setmaxnreg.  The kernel starts with 65536 / THREADS (rounded down to 8) everywhere;
   // the producer warpgroup gives most of its share to the two consumer warpgroups (BN / 2 accumulators, plus 64
-  // totals when SEGMENTED); the conv1 A-operand warpgroup (512 threads) keeps what it needs.
+  // totals when SEGMENTED); the gather warpgroup (AMODE_GATHER, 512 threads) keeps what it needs.  The window-map
+  // fix-up warps (AMODE_WINDOW) are warps 1-3 of the producer warpgroup and run at the producer's 24.
   static constexpr int LAUNCH_REGS = (65536 / THREADS) & ~7;
   // 256-wide: 240 per consumer (the 1-pass correlation epilogue spills at 232 beside 128 accumulators).
   static constexpr int PRODUCER_REGS = THREADS == 512 || BN == 256 ? 24 : 40;
@@ -181,18 +182,32 @@ __device__ __forceinline__ void named_bar(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
+// AMODE_WINDOW: window origin of patch n in padded map coordinates: window pixel (wy, wx) lives at (oy + wy, ox + wx).
+// Truncation = `.long()` (networks/utils.py:19); clamping the origin to [-7, W + 8] leaves every clamped window
+// pixel unchanged (beyond that all of them sit on the border pixel) and keeps the boxes inside the padded map.
+__device__ __forceinline__ int window_origin(const WindowMaps& wm, int n, int n_units, int j) {
+  if (n >= n_units) n = 0;      // past the end (odd patch counts): any valid patch, the epilogue discards the rows
+  int v;
+  if (wm.is_float) v = (int)reinterpret_cast<const float*>(wm.matches)[(size_t)n * 4 + j];
+  else v = (int)reinterpret_cast<const long long*>(wm.matches)[(size_t)n * 4 + j];
+  const int lim = (j & 1) ? wm.H[j >> 1] : wm.W[j >> 1];
+  v = v < -7 ? -7 : (v > lim + 8 ? lim + 8 : v);
+  return v - 8 + kMapPad;
+}
+
 // Tile = 128 rows x BN columns (see GemmCfg); K chunk 64 (one 128-byte swizzle row)
 // per pipeline stage.
 // Warpgroup 0: warp 0 is the TMA producer.  Warpgroups 1 and 2: wgmma consumers, rows 0..63 and 64..127, fp32
 // accumulators in registers; their epilogue stages the accumulators through shared memory so that every epilogue
 // thread owns one tile row (32 consecutive columns per piece), the layout epilogue_piece expects.
-// Warpgroup 3 (conv1 1-pass only) builds the A operand:
-//   AMODE_GATHER  gathers, normalises and converts the patch windows straight into the swizzled stage
-//                 (select_local_patch_feats + patch L2Normalize, networks/utils.py:4-36, networks/patch2pix.py:173-178);
+// conv1 (1-pass only) can take its A operand from elsewhere than a materialised patch tensor:
+//   AMODE_GATHER  a fourth warpgroup gathers, normalises and converts the patch windows straight into the swizzled
+//                 stage (select_local_patch_feats + patch L2Normalize, networks/utils.py:4-36,
+//                 networks/patch2pix.py:173-178);
 //   AMODE_WINDOW  the A boxes come by TMA from the per-image window maps (one strided box {64 ch, 8 px stride 2, 8 px
-//                 stride 2} per patch and tap); these warps restore the conv's zero padding -- window pixel -1 must
-//                 contribute 0, but the box holds the neighbouring image pixel there -- by zeroing the affected rows,
-//                 and build the rgb k-step (54 real K values) as an im2col of the normalised rgb map.
+//                 stride 2} per patch and tap) and the rgb k-step from the im2col tensor window_rgb_kernel writes.
+//                 Warps 1-3 of the producer warpgroup restore the conv's zero padding -- window pixel -1 must
+//                 contribute 0, but the box holds the neighbouring image pixel there -- by zeroing the affected rows.
 // Both A modes produce bit-identical operands and the same MMA sequence per output element.
 // PASSES = 3: lo*hi + hi*lo + hi*hi into one accumulator.  SEGMENTED: the accumulator restarts every `seg_len`
 // k-steps and each partial sum is added to fp32 register totals with round-to-nearest, which bounds the
@@ -208,7 +223,7 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, SEGMENTED, AMODE>::THREADS, 1)
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   float* epi_smem = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);
   __shared__ __align__(8) uint64_t full_bar[STAGES];    // TMA bytes landed (+ gather warps in AMODE_GATHER)
-  __shared__ __align__(8) uint64_t ready_bar[STAGES];   // AMODE_WINDOW: the aux warps have fixed the stage up
+  __shared__ __align__(8) uint64_t ready_bar[STAGES];   // AMODE_WINDOW: the fix-up warps are done with the stage
   __shared__ __align__(8) uint64_t empty_bar[STAGES];   // both consumer warpgroups are done reading the stage
   constexpr int FG = Cfg::FG;
   __shared__ float fg_dinv[2][2][FG][FG];               // act_scale / patch norm per (patch, image, window pixel)
@@ -232,6 +247,7 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, SEGMENTED, AMODE>::THREADS, 1)
     if (AMODE == AMODE_WINDOW) {
       tma_prefetch_desc(&p.wm.map[0]);
       tma_prefetch_desc(&p.wm.map[1]);
+      tma_prefetch_desc(&p.a_rgb_hi);
     }
     if (PASSES == 3) {
       tma_prefetch_desc(&p.a_main_lo);
@@ -241,25 +257,12 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, SEGMENTED, AMODE>::THREADS, 1)
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], AMODE == AMODE_GATHER ? 5 : 1);
-      mbar_init(&ready_bar[i], 4);
+      mbar_init(&ready_bar[i], 3);
       mbar_init(&empty_bar[i], 2);
     }
     fence_barrier_init();
   }
   __syncthreads();
-
-  // AMODE_WINDOW: window origin of patch n in padded map coordinates: window pixel (wy, wx) lives at (oy + wy, ox + wx).
-  // Truncation = `.long()` (networks/utils.py:19); clamping the origin to [-7, W + 8] leaves every clamped window
-  // pixel unchanged (beyond that all of them sit on the border pixel) and keeps the boxes inside the padded map.
-  auto origin = [&](int n, int j) -> int {
-    if (n >= n_units) n = 0;      // past the end (odd patch counts): any valid patch, the epilogue discards the rows
-    int v;
-    if (p.wm.is_float) v = (int)reinterpret_cast<const float*>(p.wm.matches)[(size_t)n * 4 + j];
-    else v = (int)reinterpret_cast<const long long*>(p.wm.matches)[(size_t)n * 4 + j];
-    const int lim = (j & 1) ? p.wm.H[j >> 1] : p.wm.W[j >> 1];
-    v = v < -7 ? -7 : (v > lim + 8 ? lim + 8 : v);
-    return v - 8 + kMapPad;
-  };
 
   const int wgi = warpgroup_index();
   if (wgi == 0) {
@@ -280,7 +283,7 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, SEGMENTED, AMODE>::THREADS, 1)
 #pragma unroll
           for (int pp = 0; pp < 2; ++pp)
 #pragma unroll
-            for (int j = 0; j < 4; ++j) o[pp][j] = origin(m_tile * 2 + pp, j);
+            for (int j = 0; j < 4; ++j) o[pp][j] = window_origin(p.wm, m_tile * 2 + pp, n_units, j);
         }
         for (int ks = 0; ks < nsteps; ++ks, ++it) {
           const int s = it % STAGES;
@@ -291,7 +294,7 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, SEGMENTED, AMODE>::THREADS, 1)
             mbar_expect_tx(&full_bar[s], B_BYTES);
             load_b(&p.b_hi, &full_bar[s], st + kATile, k.bk, brow);
           } else if (AMODE == AMODE_WINDOW) {
-            mbar_expect_tx(&full_bar[s], k.kind == 0 ? kATile + B_BYTES : B_BYTES);
+            mbar_expect_tx(&full_bar[s], STAGE_BYTES);
             load_b(&p.b_hi, &full_bar[s], st + kATile, k.bk, brow);
             if (k.kind == 0) {
               const int ty = (k.plane & 2) ? 1 : (k.y < 0 ? 0 : 2), tx = (k.plane & 1) ? 1 : (k.x < 0 ? 0 : 2);
@@ -299,6 +302,8 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, SEGMENTED, AMODE>::THREADS, 1)
 #pragma unroll
               for (int pp = 0; pp < 2; ++pp)
                 tma_load_3d(&p.wm.map[si], &full_bar[s], st + pp * 8192, c0, o[pp][2 * si] - 1 + tx, o[pp][2 * si + 1] - 1 + ty);
+            } else {
+              tma_load_5d(&p.a_rgb_hi, &full_bar[s], st, 0, 0, 0, 0, a4);
             }
           } else {
             mbar_expect_tx(&full_bar[s], STAGE_BYTES);
@@ -312,6 +317,34 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, SEGMENTED, AMODE>::THREADS, 1)
             load_b(&p.b_hi, &full_bar[s], st + NOP * kATile, k.bk, brow);
             if (PASSES == 3) load_b(&p.b_lo, &full_bar[s], st + NOP * kATile + B_BYTES, k.bk, brow);
           }
+        }
+      }
+    } else if (AMODE == AMODE_WINDOW && warp > 0) {
+      // ===================== zero-padding fix-up (warps 1-3) =====================
+      // Taps with tx = 0 (ty = 0) read window column (row) -1 for output column ox = 0 (row oy = 0), which the conv
+      // pads with zeros: those 16 tile rows (8 per patch) are cleared after the TMA bytes land.  Work item i of the
+      // 2 x 16 candidate rows x 8 16-byte chunks: rows 0..15 are the ox = 0 rows, 16..31 the oy = 0 rows.
+      const int t = threadIdx.x - 32;                  // 0..95
+      int it = 0;
+      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+        for (int ks = 0; ks < nsteps; ++ks, ++it) {
+          const int s = it % STAGES;
+          // every fix-up warp follows every stage (wait + arrive): parity waits are only valid within one ring
+          // revolution, so no warp may run ahead of -- or fall behind -- the pipeline
+          mbar_wait(&full_bar[s], (uint32_t)(it / STAGES) & 1u);
+          const KStep k = p.steps[ks];
+          const bool zx = k.kind == 0 && !(k.plane & 1) && k.x < 0, zy = k.kind == 0 && !(k.plane & 2) && k.y < 0;
+          if (zx || zy) {
+            uint8_t* st = smem + (size_t)s * STAGE_BYTES;
+            for (int i = t; i < 256; i += 96) {
+              const int j = i >> 3, pp = (j >> 3) & 1, r8 = j & 7;
+              const int row = pp * 64 + (j < 16 ? r8 * 8 : r8);
+              if (j < 16 ? zx : zy) *reinterpret_cast<uint4*>(st + row * 128 + (i & 7) * 16) = make_uint4(0, 0, 0, 0);
+            }
+            fence_proxy_async();
+          }
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&ready_bar[s]);
         }
       }
     }
@@ -513,66 +546,49 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, SEGMENTED, AMODE>::THREADS, 1)
         if (lane == 0) mbar_arrive(&full_bar[s]);
       }
     }
-  } else if (AMODE == AMODE_WINDOW) {
-    // ===================== aux warps (warpgroup 3): zero-padding fix-up and the rgb im2col k-step =====================
-    if constexpr (Cfg::AUX_REGS < Cfg::LAUNCH_REGS) setmaxnreg_dec<Cfg::AUX_REGS>();
-    const int row = threadIdx.x - 384;               // 0..127: the tile row this thread owns
-    int it = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      const int m_tile = tile / n_col_tiles;
-      for (int ks = 0; ks < nsteps; ++ks, ++it) {
-        const int s = it % STAGES;
-        const uint32_t ph = (uint32_t)(it / STAGES) & 1u;
-        const KStep k = p.steps[ks];
-        uint8_t* st = smem + (size_t)s * STAGE_BYTES;
-        if (k.kind == 0) {
-          // every aux warp follows every stage (wait + arrive): parity waits are only valid within one ring
-          // revolution, so no warp may run ahead of -- or fall behind -- the pipeline
-          mbar_wait(&full_bar[s], ph);
-          const bool zx = !(k.plane & 1) && k.x < 0, zy = !(k.plane & 2) && k.y < 0;      // tap tx = 0 / ty = 0
-          if (zx || zy) {
-            if ((zx && (row & 7) == 0) || (zy && ((row >> 3) & 7) == 0)) {
-              uint4* d = reinterpret_cast<uint4*>(st + row * 128);
+  }
+}
+
+// AMODE_WINDOW's rgb k-step: the im2col rows of every patch, [npad][64 output px][64] fp16 with k = tap*6 + img*3 + ch
+// (54 used, rest zero), copied from the normalised rgb maps; window pixel -1 = conv zero padding, and the pad patch of
+// an odd count is all zero.  One thread per output pixel (row of 128 bytes).
+__global__ void __launch_bounds__(256) window_rgb_kernel(const __grid_constant__ WindowMaps wm, int n_units, int npad,
+                                                         __half* __restrict__ out) {
+  const int row = blockIdx.x * 256 + threadIdx.x;
+  if (row >= npad * 64) return;
+  const int n = row >> 6, oy = (row >> 3) & 7, ox = row & 7;
+  __align__(16) __half hv[64];
 #pragma unroll
-              for (int c = 0; c < 8; ++c) d[c] = make_uint4(0, 0, 0, 0);
-            }
-            fence_proxy_async();
-          }
-        } else {
-          // rgb im2col row: k = tap*6 + img*3 + ch (54 used, rest zero); window pixel -1 = conv zero padding
-          mbar_wait(&empty_bar[s], ph ^ 1u);
-          const int pp = row >> 6, oy = (row >> 3) & 7, ox = row & 7;
-          const int n = m_tile * 2 + pp;
-          __align__(16) __half hv[64];
+  for (int i = 0; i < 64; ++i) hv[i] = __float2half_rn(0.f);
+  if (n < n_units) {
 #pragma unroll
-          for (int i = 0; i < 64; ++i) hv[i] = __float2half_rn(0.f);
+    for (int si = 0; si < 2; ++si) {
+      const int bx = window_origin(wm, n, n_units, 2 * si), by = window_origin(wm, n, n_units, 2 * si + 1);
+      const int Wp = wm.W[si] + 2 * kMapPad;
 #pragma unroll
-          for (int si = 0; si < 2; ++si) {
-            const int bx = origin(n, 2 * si), by = origin(n, 2 * si + 1);
-            const int Wp = p.wm.W[si] + 2 * kMapPad;
-#pragma unroll
-            for (int tap = 0; tap < 9; ++tap) {
-              const int wx = 2 * ox - 1 + tap % 3, wy = 2 * oy - 1 + tap / 3;
-              if (wx >= 0 && wy >= 0 && n < n_units) {
-                const uint2 q = __ldg(reinterpret_cast<const uint2*>(p.wm.rgbn[si] + ((size_t)(by + wy) * Wp + bx + wx) * 4));
-                const __half* hq = reinterpret_cast<const __half*>(&q);
-                hv[tap * 6 + si * 3 + 0] = hq[0];
-                hv[tap * 6 + si * 3 + 1] = hq[1];
-                hv[tap * 6 + si * 3 + 2] = hq[2];
-              }
-            }
-          }
-#pragma unroll
-          for (int c = 0; c < 8; ++c)
-            *reinterpret_cast<uint4*>(st + row * 128 + ((c ^ (row & 7)) << 4)) = reinterpret_cast<const uint4*>(hv)[c];
-          fence_proxy_async();
-          mbar_wait(&full_bar[s], ph);            // the weight tile
+      for (int tap = 0; tap < 9; ++tap) {
+        const int wx = 2 * ox - 1 + tap % 3, wy = 2 * oy - 1 + tap / 3;
+        if (wx >= 0 && wy >= 0) {
+          const uint2 q = __ldg(reinterpret_cast<const uint2*>(wm.rgbn[si] + ((size_t)(by + wy) * Wp + bx + wx) * 4));
+          const __half* hq = reinterpret_cast<const __half*>(&q);
+          hv[tap * 6 + si * 3 + 0] = hq[0];
+          hv[tap * 6 + si * 3 + 1] = hq[1];
+          hv[tap * 6 + si * 3 + 2] = hq[2];
         }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&ready_bar[s]);
       }
     }
   }
+  uint4* dst = reinterpret_cast<uint4*>(out + (size_t)row * 64);
+#pragma unroll
+  for (int c = 0; c < 8; ++c) dst[c] = reinterpret_cast<const uint4*>(hv)[c];
+}
+
+int launch_window_rgb(const WindowMaps& wm, int n, int npad, __half* out, cudaStream_t st) {
+  P2P_REQUIRE(n >= 0 && npad >= n, "window rgb: bad patch count");
+  if (npad == 0) return 0;
+  window_rgb_kernel<<<(unsigned)cdiv(npad * 64, 256), 256, 0, st>>>(wm, n, npad, out);
+  P2P_LAUNCH_OK();
+  return 0;
 }
 
 

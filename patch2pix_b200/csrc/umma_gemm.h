@@ -41,7 +41,8 @@ struct FusedGather {
   int is_float;
 };
 
-// conv1 fed by strided TMA boxes of the per-image window maps (AMODE_WINDOW)
+// conv1 fed by strided TMA boxes of the per-image window maps (AMODE_WINDOW); the rgb k-step comes by TMA (a_rgb_hi)
+// from the im2col tensor launch_window_rgb builds out of rgbn
 struct WindowMaps {
   CUtensorMap map[2];             // [H + 2 pad][W + 2 pad][256] fp16 per image; box = 64 ch x 8 (stride 2) x 8 (stride 2)
   const __half* rgbn[2];          // [H + 2 pad][W + 2 pad][4]
@@ -69,5 +70,7 @@ struct UmmaGemmParams {
 int make_tmap_fp16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                    const uint32_t* box, const uint32_t* estrides = nullptr);
 int launch_umma_gemm(const UmmaGemmParams& p, int epi, int passes, int num_sms, cudaStream_t st, int amode = AMODE_TMA);
+// AMODE_WINDOW's rgb k-step operand: writes the [npad][64][64] fp16 im2col tensor of patches 0..n-1 (zeros beyond n)
+int launch_window_rgb(const WindowMaps& wm, int n, int npad, __half* out, cudaStream_t st);
 
 }  // namespace p2p
