@@ -226,6 +226,21 @@ P2P_API int p2p_find_model(p2p_handle_t h, int model, const double* rows, int ro
  * (x2^T F x1)^2 / (eps + l1x^2 + l1y^2 + l2x^2 + l2y^2).  F DEVICE double [9], dist_out DEVICE double [n]. */
 P2P_API int p2p_sampson_distance(p2p_handle_t h, const double* rows, int row_stride, int n, const double* F,
                          double* dist_out, void* stream);
+/* The three Sampson-distance histograms of the reference's validation loop (utils/train/eval_epoch_immatch.py:62-91:
+ * cdist, fdist, indist binned as check_inliers_distr does), in one launch and without a host sync.  rows / row_stride /
+ * n / n_dev as p2p_find_model: m = min(n, *n_dev) rows, refined (x1, y1, x2, y2) in columns 0..3, the coarse ones in
+ * columns coarse_col..coarse_col+3 (-1: no coarse histogram; row_stride 9 with coarse_col 5 reads the packed_out of
+ * p2p_finalize_matches in place).  The distance is bit-identical to p2p_sampson_distance.  F HOST double [9] and edges
+ * HOST double [n_edges] (2 <= n_edges <= 16, finite, strictly increasing; anything else returns -1) are passed by value
+ * to the kernel.  Binning as np.histogram(d, edges): bin i counts edges[i] <= d < edges[i+1], the last bin also
+ * d == edges[n_edges-1]; NaN, inf and values outside the edges are not counted.  counts_out DEVICE int32 [3][n_edges]:
+ * histogram 0 = coarse over the m rows (all zero when coarse_col = -1), 1 = refined over the m rows, 2 = refined over
+ * the rows with mask[r] != 0 (mask DEVICE uint8 [n], nullable: NULL zeroes histogram 2); entries 0 .. n_edges-2 of each
+ * are the bin counts and entry n_edges-1 the number of rows considered (the divisor of the reference's ratios, which
+ * includes the rows outside the bins).  Integer counts: identical across runs and num_sms settings. */
+P2P_API int p2p_epipolar_histograms(p2p_handle_t h, const double* rows, int row_stride, int n, const double* n_dev,
+                                    int coarse_col, const double* F, const uint8_t* mask, const double* edges,
+                                    int n_edges, int32_t* counts_out, void* stream);
 /* Test hook: hypotheses 0 .. count-1 of p2p_find_model without selection.  models_out DEVICE double [count*slots][9]
  * (slots 3 for F, 1 for H; zero where a slot has no model), counts_out DEVICE int32 [count*slots] (-1: no model). */
 P2P_API int p2p_test_hypotheses(p2p_handle_t h, int model, const double* rows, int row_stride, int n, double px_th,

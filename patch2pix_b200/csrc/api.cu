@@ -1175,6 +1175,26 @@ int p2p_sampson_distance(p2p_handle_t h, const double* rows, int row_stride, int
   return launch_sampson_distance(rows, row_stride, n, F, dist_out, reinterpret_cast<cudaStream_t>(stream));
 }
 
+int p2p_epipolar_histograms(p2p_handle_t h, const double* rows, int row_stride, int n, const double* n_dev,
+                            int coarse_col, const double* F, const uint8_t* mask, const double* edges, int n_edges,
+                            int32_t* counts_out, void* stream) {
+  P2P_ENTER(h);
+  P2P_REQUIRE(F && edges && counts_out && (rows || n == 0), "null pointer");
+  P2P_REQUIRE(n >= 0 && row_stride >= 4, "bad row count or stride");
+  P2P_REQUIRE(coarse_col == -1 || (coarse_col >= 0 && coarse_col + 4 <= row_stride),
+              "coarse_col must be -1 or a column with 4 columns of the row from it");
+  P2P_REQUIRE(n_edges >= 2 && n_edges <= kMaxHistEdges, "n_edges must be in 2..16");
+  EpiHistArgs a{};
+  for (int j = 0; j < 9; ++j) a.F[j] = F[j];
+  for (int i = 0; i < n_edges; ++i) {
+    P2P_REQUIRE(std::isfinite(edges[i]) && (i == 0 || edges[i] > edges[i - 1]), "edges must be finite and increasing");
+    a.edges[i] = edges[i];
+  }
+  a.n_edges = n_edges;
+  return launch_epipolar_histograms(rows, row_stride, n, n_dev, coarse_col, mask, a, counts_out,
+                                    reinterpret_cast<cudaStream_t>(stream));
+}
+
 int p2p_test_hypotheses(p2p_handle_t h, int model, const double* rows, int row_stride, int n, double px_th,
                         unsigned long long seed, int count, double* models_out, int32_t* counts_out, void* stream) {
   P2P_ENTER(h);

@@ -116,6 +116,18 @@ int launch_find_model(int model, const double* rows, int stride, int n, const do
 int launch_test_hypotheses(int model, const double* rows, int stride, int n, double px_th, unsigned long long seed,
                            int count, void* scratch, double* models_out, int* counts_out, cudaStream_t st);
 int launch_sampson_distance(const double* rows, int stride, int n, const double* F, double* out, cudaStream_t st);
+// ---- eval.cu: histograms of the Sampson distance against F (passed by value): coarse (columns coarse_col..,
+// skipped when < 0), refined (columns 0..3) and refined under mask (nullable); counts_out [3][n_edges], entry
+// n_edges-1 = rows considered.
+constexpr int kMaxHistEdges = 16;
+constexpr int kHistThreads = 1024;
+struct EpiHistArgs {
+  double F[9];
+  double edges[kMaxHistEdges];   // finite, strictly increasing
+  int n_edges;                   // 2 .. kMaxHistEdges
+};
+int launch_epipolar_histograms(const double* rows, int stride, int n, const double* n_dev, int coarse_col,
+                               const uint8_t* mask, const EpiHistArgs& a, int* counts_out, cudaStream_t st);
 // ---- degensac.cu: model 2 of launch_find_model (same scratch) and its test hook
 int launch_find_model_degensac(const double* rows, int stride, int n, const double* n_dev, double px_th, double conf,
                                int max_iters, unsigned long long seed, void* scratch, double* model_out, uint8_t* mask_out,

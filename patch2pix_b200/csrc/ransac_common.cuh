@@ -130,6 +130,14 @@ __device__ __forceinline__ void sampson_terms(const T* m, T x1, T y1, T x2, T y2
   den = l1x * l1x + l1y * l1y + l2x * l2x + l2y * l2y;
 }
 
+// The reference's sampson_distance of one row (measure.py:36-39, eps = 1e-8): the one expression of both
+// p2p_sampson_distance (verify.cu) and p2p_epipolar_histograms (eval.cu).
+__device__ __forceinline__ double sampson_distance(const double* m, const double* p) {
+  double dd, den;
+  sampson_terms<double>(m, p[0], p[1], p[2], p[3], dd, den);
+  return dd * dd / (1e-8 + den);
+}
+
 __device__ __forceinline__ double warp_sum_d(double v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

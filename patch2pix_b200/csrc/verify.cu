@@ -26,10 +26,7 @@ __global__ void sampson_kernel(const double* __restrict__ rows, int stride, int 
   double m[9];
 #pragma unroll
   for (int j = 0; j < 9; ++j) m[j] = F[j];
-  const double* p = rows + (size_t)r * stride;
-  double dd, den;
-  sampson_terms<double>(m, p[0], p[1], p[2], p[3], dd, den);
-  out[r] = dd * dd / (1e-8 + den);
+  out[r] = sampson_distance(m, rows + (size_t)r * stride);
 }
 
 template <int KIND>

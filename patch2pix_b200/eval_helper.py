@@ -54,9 +54,10 @@ def load_checkpoint(ckpt_path, device='cuda:0', method='patch2pix', lprint=print
     raise ValueError('Wrong method name.')
 
 
-def _finalize(net, fine, scores, coarse, io_thres, upscale, verify=None):
-    """One launch (+ the RANSAC launches with `verify`) and ONE device->host copy for the tail of estimate_matches
-    (model_helper.py:97-109)."""
+def _finalize_device(net, fine, scores, coarse, io_thres, upscale, verify=None):
+    """The device half of _finalize, enqueued without a host sync -> (packed, n, kind): packed holds the n rows of
+    p2p_finalize_matches (9 float64 each), the kept-row count at [n * 9] and, with `verify`, the RANSAC or pose buffer
+    from [n * 9 + 1] on; kind is verify[0] or None."""
     import ctypes as C
     from . import _lib
     h = net._handle
@@ -89,12 +90,24 @@ def _finalize(net, fine, scores, coarse, io_thres, upscale, verify=None):
     elif verify is not None:      # RANSAC on the kept, rescaled rows (refined columns 0..3), in place, count read on the device
         model = {'F': V.MODEL_F, 'H': V.MODEL_H, 'DEGENSAC': V.MODEL_F_DEGENSAC}[kind]
         V.find_model_into(h, model, packed, 9, n, n_dev, px_th, 0.999, 10000, 0, packed[n * 9 + 1:])
+    return packed, n, (kind if verify is not None else None)
+
+
+def _finalize(net, fine, scores, coarse, io_thres, upscale, verify=None):
+    """One launch (+ the RANSAC launches with `verify`) and ONE device->host copy for the tail of estimate_matches
+    (model_helper.py:97-109)."""
+    return _finalize_host(*_finalize_device(net, fine, scores, coarse, io_thres, upscale, verify))
+
+
+def _finalize_host(packed, n, kind):
     host = packed.cpu().numpy()                      # the single synchronising copy
     m = int(host[n * 9])
     rows = host[:n * 9].reshape(n, 9)[:m]
     out = (rows[:, 0:4].copy(), rows[:, 4].astype(np.float32), rows[:, 5:9].copy())
-    if verify is None:
+    if kind is None:
         return out
+    from . import pose as P
+    from . import verify as V
     if kind == 'E':
         E, mask, _, R, t, _ = P.parse_host(host[n * 9 + 1:], n)
         return out + (mask[:m], E, R, t)
@@ -118,19 +131,29 @@ def estimate_matches(net, im1, im2, scale1=(1.0, 1.0), scale2=(1.0, 1.0), ksize=
     matches2relapose_cv instead (patch2pix_b200.pose: E RANSAC at conf 0.999 and 1000 iterations, then pose recovery on
     its inliers) and returns (matches, scores, coarse_matches, inliers, E, R, t): the E-RANSAC mask, E (None when no
     model was found), R and t [3, 1] (x2 = R x1 + t)."""
+    res = _finalize_host(*match_device(net, im1, im2, scale1, scale2, ksize, ncn_thres, mutual, io_thres, eval_type,
+                                       verify))
+    if eval_type == 'coarse':
+        return (res[0], res[1], res[0]) + res[3:]
+    return res
+
+
+def match_device(net, im1, im2, scale1=(1.0, 1.0), scale2=(1.0, 1.0), ksize=2, ncn_thres=0.0, mutual=True,
+                 io_thres=0.25, eval_type='fine', verify=None):
+    """estimate_matches up to, not including, its device->host copy -> (packed, n, kind) as _finalize_device.  The
+    coarse matcher's rows repeat the coarse columns in the refined slots."""
     upscale = tuple(scale1) + tuple(scale2)
     im1 = im1.to(net.device)
     im2 = im2.to(net.device)
     with torch.no_grad():
         if eval_type == 'coarse':
             coarse_matches, scores = net.predict_coarse(im1, im2, ksize=ksize, ncn_thres=ncn_thres, mutual=mutual)
-            res = _finalize(net, None, scores[0], coarse_matches[0], float('-inf'), upscale, verify)
-            return (res[0], res[1], res[0]) + res[3:]
+            return _finalize_device(net, None, scores[0], coarse_matches[0], float('-inf'), upscale, verify)
         if eval_type != 'fine':
             raise ValueError("eval_type must be 'coarse' or 'fine'")
         fine_matches, fine_scores, coarse_matches = net.predict_fine(im1, im2, ksize=ksize, ncn_thres=ncn_thres,
                                                                     mutual=mutual)
-    return _finalize(net, fine_matches[0], fine_scores[0], coarse_matches[0], io_thres, upscale, verify)
+    return _finalize_device(net, fine_matches[0], fine_scores[0], coarse_matches[0], io_thres, upscale, verify)
 
 
 def estimate_matches_from_files(net, im1_path, im2_path, ksize=2, ncn_thres=0.0, mutual=True, io_thres=0.25,

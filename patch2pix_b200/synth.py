@@ -11,6 +11,7 @@ folding bugs) and the running variances are calibrated so that activations
 stay O(1) through the regressor, like a trained network's.
 """
 import math
+import os
 
 import numpy as np
 import torch
@@ -230,3 +231,50 @@ def synthetic_pair_shifted(pair_idx, height, width, noise=0.6):
     im2 = base[:, :, 48 + dy:48 + dy + height, 48 + dx:48 + dx + width].contiguous()
     im2 = im2 + noise * torch.randn(im2.shape, generator=g)
     return im1, im2
+
+
+def write_colmap_model(model_dir, cameras, images):
+    """COLMAP binary model (little-endian) with the given cameras [(id, model_id, width, height, params)] and images
+    [(id, qvec (w, x, y, z), tvec, camera_id, name)], without 2D points: cameras.bin and images.bin in model_dir."""
+    import struct
+    os.makedirs(model_dir, exist_ok=True)
+    with open(os.path.join(model_dir, 'cameras.bin'), 'wb') as f:
+        f.write(struct.pack('<Q', len(cameras)))
+        for cid, model_id, w, h, params in cameras:
+            f.write(struct.pack('<iiQQ', cid, model_id, w, h) + struct.pack(f'<{len(params)}d', *params))
+    with open(os.path.join(model_dir, 'images.bin'), 'wb') as f:
+        f.write(struct.pack('<Q', len(images)))
+        for iid, q, t, cid, name in images:
+            f.write(struct.pack('<i7di', iid, *q, *t, cid) + name.encode('utf-8') + b'\x00' + struct.pack('<Q', 0))
+
+
+def synthetic_val_scene(root, scene, seed, sizes, ext='.png', missing=(), min_overlap=0.3):
+    """One scene of a validation tree in the layout of the reference's PhotoTourism validation sets:
+    root/scene/dense/images/<names>, dense/sparse/{cameras,images}.bin and dense/sparse/ov_pairs.npy
+    ({min_overlap: pair names}).  Pair k is two views of one texture (synthetic_pair_shifted(seed * 1000 + k)) at
+    sizes[k] = (width, height) as 8-bit images, with a seeded SIMPLE_PINHOLE camera and pose per image (the poses do
+    not describe the textures: the matches are real, the pose errors are not meaningful).  Pair indices in `missing`
+    name a second image that is not written.  Returns the pair names."""
+    from PIL import Image
+    rng = np.random.default_rng([int(seed), 7])
+    im_dir = os.path.join(root, scene, 'dense', 'images')
+    os.makedirs(im_dir, exist_ok=True)
+    cameras, images, pairs = [], [], []
+    for k, (w, h) in enumerate(sizes):
+        views = synthetic_pair_shifted(int(seed) * 1000 + k, h, w)
+        names = []
+        for v, im in enumerate(views):
+            name = f'{scene}_{k:03d}_{v}{ext}'
+            if not (v == 1 and k in missing):
+                rgb = (im[0].permute(1, 2, 0).numpy() * 48.0 + 128.0).clip(0, 255).astype(np.uint8)
+                Image.fromarray(rgb).save(os.path.join(im_dir, name), **({'quality': 90} if ext == '.jpg' else {}))
+            iid = len(images) + 1
+            q = np.concatenate([[1.0], rng.uniform(-0.1, 0.1, 3)])
+            cameras.append((iid, 0, w, h, [0.9 * max(w, h), w / 2.0, h / 2.0]))
+            images.append((iid, q / np.linalg.norm(q), rng.normal(0.0, 1.0, 3), iid, name))
+            names.append(name)
+        pairs.append(tuple(names))
+    model_dir = os.path.join(root, scene, 'dense', 'sparse')
+    write_colmap_model(model_dir, cameras, images)
+    np.save(os.path.join(model_dir, 'ov_pairs.npy'), {min_overlap: pairs})
+    return pairs

@@ -103,6 +103,40 @@ def sampson_distance(pts1, pts2, F):
     return out.cpu().numpy() if is_np else out
 
 
+def epipolar_histograms_into(handle, rows, row_stride, n, n_dev, coarse_col, F, mask_ptr, edges, counts_ptr):
+    """Enqueue p2p_epipolar_histograms on `rows` (a float64 device tensor, row r at offset r * row_stride) with F and
+    the edges from the host; `n_dev`, `mask_ptr` and `counts_ptr` are device addresses (ctypes, None for the first
+    two) of the row count, the uint8 mask and the int32 [3][len(edges)] output."""
+    F = np.asarray(F, dtype=np.float64).reshape(9)
+    edges = np.asarray(edges, dtype=np.float64).reshape(-1)
+    with torch.cuda.device(rows.device):
+        _lib.check(handle.lib.p2p_epipolar_histograms(handle.h, C.c_void_p(rows.data_ptr()), row_stride, n, n_dev,
+                                                      int(coarse_col), (C.c_double * 9)(*F), mask_ptr,
+                                                      (C.c_double * len(edges))(*edges), len(edges), counts_ptr,
+                                                      handle.stream()))
+
+
+def epipolar_histograms(rows, F, edges, coarse_col=-1, mask=None, n_dev=None):
+    """Sampson-distance histograms of CUDA float64 rows [n, stride] against F (include/p2p_b200.h,
+    p2p_epipolar_histograms) -> int32 CUDA tensor [3, len(edges)]: coarse (columns coarse_col..+3, zeros with -1),
+    refined (columns 0..3), refined under `mask` (CUDA bool/uint8 [n], or None); each ends with its row count.
+    `n_dev`: optional CUDA float64 scalar, use min(n, n_dev) rows.  No host sync."""
+    if not (isinstance(rows, torch.Tensor) and rows.is_cuda and rows.dtype == torch.float64 and rows.dim() == 2):
+        raise ValueError('rows must be a CUDA float64 tensor [n, stride]')
+    rows = rows.contiguous()
+    n, stride = int(rows.shape[0]), int(rows.shape[1])
+    counts = torch.empty(3, len(edges), dtype=torch.int32, device=rows.device)
+    md = None
+    if mask is not None:
+        md = (mask.reshape(-1) != 0).to(torch.uint8).contiguous()
+        if md.shape[0] != n:
+            raise ValueError(f'mask has {md.shape[0]} entries for {n} rows')
+    epipolar_histograms_into(_lib.default_handle(rows.device), rows, stride, n,
+                             None if n_dev is None else C.c_void_p(n_dev.data_ptr()), coarse_col, F,
+                             None if md is None else C.c_void_p(md.data_ptr()), edges, C.c_void_p(counts.data_ptr()))
+    return counts
+
+
 def first_hypotheses(model, pts1, pts2, px_th, count, seed=0):
     """Test hook: the first `count` hypotheses of find_model without selection -> (models [count*slots, 9] float64,
     counts [count*slots] int32, -1 where a slot holds no model); slots = 3 for F, 1 for H."""
