@@ -241,6 +241,20 @@ P2P_API int p2p_sampson_distance(p2p_handle_t h, const double* rows, int row_str
 P2P_API int p2p_epipolar_histograms(p2p_handle_t h, const double* rows, int row_stride, int n, const double* n_dev,
                                     int coarse_col, const double* F, const uint8_t* mask, const double* edges,
                                     int n_edges, int32_t* counts_out, void* stream);
+/* The image-overlap matrix of the reference's validation-pair precompute (utils/colmap/data_loading.py:54-70,
+ * cal_overlap_scores), in two launches and without a host sync.  Image i's keypoints are point3D_ids[offsets[i] ..
+ * offsets[i+1]-1] (DEVICE int64; offsets DEVICE int64 [n_images+1], offsets_host the same values on the HOST, checked
+ * non-decreasing); A_i is the set of keypoint INDICES k whose point3D_id is > 0 (an id of 0 counts as missing, as -1).
+ * A pack kernel writes bits_out DEVICE uint32 [n_images][words] (bit k % 32 of word k / 32 set iff k is in A_i;
+ * words >= ceil(n2d / 32) of every image) and counts_out DEVICE int32 [n_images] = |A_i|.  A count kernel over 64 x 64
+ * image tiles of the upper triangle accumulates |A_i ∩ A_j| as int32 popcounts (exact) and writes EVERY entry of
+ * scores_out DEVICE double [n_images][n_images]: |A_i ∩ A_j| / max(|A_i|, |A_j|) (one IEEE division) for i < j, 1 on
+ * the diagonal, 0 below it.  Two images with empty sets give NaN where the reference raises ZeroDivisionError; the
+ * caller checks the counts.  Limits: n_images <= 2^20, n2d < 2^31 per image (words <= 2^26); anything beyond returns
+ * -1.  Integer counts: identical across runs. */
+P2P_API int p2p_overlap_scores(p2p_handle_t h, const int64_t* point3D_ids, const int64_t* offsets,
+                               const int64_t* offsets_host, int n_images, int words, uint32_t* bits_out,
+                               int32_t* counts_out, double* scores_out, void* stream);
 /* Test hook: hypotheses 0 .. count-1 of p2p_find_model without selection.  models_out DEVICE double [count*slots][9]
  * (slots 3 for F, 1 for H; zero where a slot has no model), counts_out DEVICE int32 [count*slots] (-1: no model). */
 P2P_API int p2p_test_hypotheses(p2p_handle_t h, int model, const double* rows, int row_stride, int n, double px_th,

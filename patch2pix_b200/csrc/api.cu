@@ -1195,6 +1195,29 @@ int p2p_epipolar_histograms(p2p_handle_t h, const double* rows, int row_stride, 
                                     reinterpret_cast<cudaStream_t>(stream));
 }
 
+int p2p_overlap_scores(p2p_handle_t h, const int64_t* point3D_ids, const int64_t* offsets,
+                       const int64_t* offsets_host, int n_images, int words, uint32_t* bits_out, int32_t* counts_out,
+                       double* scores_out, void* stream) {
+  P2P_ENTER(h);
+  P2P_REQUIRE(n_images >= 0 && n_images <= kMaxOverlapImages, "n_images must be in 0 .. 2^20");
+  P2P_REQUIRE(words >= 0 && words <= (int)((kMaxOverlapPoints + 31) / 32), "words must be in 0 .. 2^26");
+  P2P_REQUIRE(offsets_host != nullptr, "offsets_host is null");
+  if (n_images == 0) return 0;
+  P2P_REQUIRE(offsets && counts_out && scores_out && (bits_out || words == 0), "null pointer");
+  P2P_REQUIRE(offsets_host[0] >= 0, "offsets must be non-negative");
+  for (int i = 0; i < n_images; ++i) {
+    const int64_t len = offsets_host[i + 1] - offsets_host[i];
+    P2P_REQUIRE(len >= 0, "offsets must be non-decreasing");
+    P2P_REQUIRE(len <= kMaxOverlapPoints, "an image has 2^31 or more 2D points");
+    P2P_REQUIRE((len + 31) / 32 <= words, "words is smaller than ceil(n2d / 32) of an image");
+  }
+  P2P_REQUIRE(point3D_ids || offsets_host[n_images] == offsets_host[0], "point3D_ids is null");
+  return launch_overlap_scores(reinterpret_cast<const long long*>(point3D_ids),
+                               reinterpret_cast<const long long*>(offsets), n_images, words,
+                               reinterpret_cast<unsigned*>(bits_out), counts_out, scores_out,
+                               reinterpret_cast<cudaStream_t>(stream));
+}
+
 int p2p_test_hypotheses(p2p_handle_t h, int model, const double* rows, int row_stride, int n, double px_th,
                         unsigned long long seed, int count, double* models_out, int32_t* counts_out, void* stream) {
   P2P_ENTER(h);

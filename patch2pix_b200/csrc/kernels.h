@@ -128,6 +128,12 @@ struct EpiHistArgs {
 };
 int launch_epipolar_histograms(const double* rows, int stride, int n, const double* n_dev, int coarse_col,
                                const uint8_t* mask, const EpiHistArgs& a, int* counts_out, cudaStream_t st);
+// ---- overlap.cu: cal_overlap_scores' matrix.  ids: flat point3D_ids, image i at offsets[i] .. offsets[i+1]-1 (device);
+// bits [n][words] and counts [n] are written by the pack kernel, scores [n][n] (every entry) by the count kernel.
+constexpr int kMaxOverlapImages = 1 << 20;
+constexpr long long kMaxOverlapPoints = (1LL << 31) - 1;
+int launch_overlap_scores(const long long* ids, const long long* offsets, int n, int words, unsigned* bits,
+                          int* counts, double* scores, cudaStream_t st);
 // ---- degensac.cu: model 2 of launch_find_model (same scratch) and its test hook
 int launch_find_model_degensac(const double* rows, int stride, int n, const double* n_dev, double px_th, double conf,
                                int max_iters, unsigned long long seed, void* scratch, double* model_out, uint8_t* mask_out,

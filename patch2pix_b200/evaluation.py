@@ -8,6 +8,10 @@ histograms (``p2p_epipolar_histograms``) are enqueued on the device; the pair's 
 R|t, histograms) is copied, device to device, into a table that comes back in one copy at the end of the run.  The only
 other device->host copy per pair is the mutual-match count the matcher itself reads.  The two image decodes of the next
 pair run on a worker thread while the current pair is enqueued.
+
+The pair lists that loop reads (dense/sparse/ov_pairs.npy) come from `precompute_immatch_val_ovs` /
+`sav_model_multi_ov_pairs` (utils/colmap/data_loading.py:7-70): the image-overlap matrix is an integer Gram matrix of
+per-image keypoint bitsets (``p2p_overlap_scores``), and the pairs of every threshold come out of one torch.nonzero.
 """
 import ctypes as C
 import os
@@ -19,6 +23,7 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 import torch
 
+from . import _lib
 from . import pose as P
 from .verify import epipolar_histograms_into
 
@@ -74,18 +79,32 @@ def read_cameras_binary(path):
     return cameras
 
 
-def read_images_binary(path):
-    """images.bin -> {image_id: Namespace(id, qvec, tvec, camera_id, name)}, in file order.  The 2D points are
-    skipped."""
+_POINT2D = np.dtype([('xy', '<f8', (2,)), ('id', '<i8')])     # one 2D point of images.bin: x, y, point3D_id
+
+
+def _read_images(path, points2D, copy):
     r = _Reader(path)
     images = {}
     for _ in range(r.take('<Q')[0]):
         props = r.take('<i7di')
         name = r.cstring()
-        r.skip(24 * r.take('<Q')[0])            # n2d x (x: f64, y: f64, point3D_id: i64)
-        images[props[0]] = Namespace(id=props[0], qvec=np.array(props[1:5]), tvec=np.array(props[5:8]),
-                                     camera_id=props[8], name=name)
+        n2d = r.take('<Q')[0]
+        start = r.pos
+        r.skip(24 * n2d)
+        im = Namespace(id=props[0], qvec=np.array(props[1:5]), tvec=np.array(props[5:8]), camera_id=props[8], name=name)
+        if points2D:
+            pts = np.frombuffer(r.buf, _POINT2D, n2d, start)
+            im.xys = pts['xy'].copy() if copy else pts['xy']
+            im.point3D_ids = pts['id'].copy() if copy else pts['id']
+        images[props[0]] = im
     return images
+
+
+def read_images_binary(path, points2D=False):
+    """images.bin -> {image_id: Namespace(id, qvec, tvec, camera_id, name)}, in file order.  With points2D each image
+    also carries xys (float64 [n, 2]) and point3D_ids (int64 [n], -1 where the keypoint has no 3D point); otherwise
+    the 2D points are skipped."""
+    return _read_images(path, points2D, copy=True)
 
 
 def cam_params_to_matrix(params, model):
@@ -310,3 +329,126 @@ def eval_immatch_val_sets(net, data_root='data/immatch_benchmark/val_dense', ksi
     for line in lines:
         lprint_(line)
     return qt_err_mean, pass_rate
+
+
+# ---- validation pairs: the overlap precompute (utils/colmap/data_loading.py:7-70,
+# data_pairs/precompute_immatch_val_ovs.py) ---------------------------------------------------------------------------
+def overlap_scores_device(point3D_ids, device='cuda'):
+    """p2p_overlap_scores on one int64 array of point3D_ids per image -> (scores [N, N] float64, counts [N] int32), CUDA
+    tensors enqueued on the current stream: scores[i, j] = |A_i ∩ A_j| / max(|A_i|, |A_j|) for i < j, 1 on the
+    diagonal and 0 below, A_i the indices of image i's keypoints with an id > 0.  Raises ZeroDivisionError, as the
+    reference does, when two or more images have an empty A_i."""
+    ids = [np.asarray(a, dtype=np.int64).reshape(-1) for a in point3D_ids]
+    n = len(ids)
+    if sum(1 for a in ids if not np.any(a > 0)) >= 2:
+        raise ZeroDivisionError('division by zero')
+    offsets = np.zeros(n + 1, dtype=np.int64)
+    np.cumsum([len(a) for a in ids], out=offsets[1:])
+    h = _lib.default_handle(torch.device(device))
+    dev = h.device
+    words = int((np.diff(offsets).max(initial=0) + 31) // 32)
+    flat = torch.from_numpy(np.concatenate(ids) if n else np.zeros(0, dtype=np.int64)).to(dev)
+    off = torch.from_numpy(offsets).to(dev)
+    bits = torch.empty(n * words, dtype=torch.int32, device=dev)
+    counts = torch.empty(n, dtype=torch.int32, device=dev)
+    scores = torch.empty(n, n, dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(h.lib.p2p_overlap_scores(h.h, _lib.ptr(flat), _lib.ptr(off),
+                                            offsets.ctypes.data_as(C.POINTER(C.c_int64)), n, words, _lib.ptr(bits),
+                                            _lib.ptr(counts), _lib.ptr(scores), h.stream()))
+    return scores, counts
+
+
+def cal_overlap_scores(im_ids, images, device='cuda'):
+    """data_loading.py:54-70 -> (overlap_scores [N, N] float64, nums_3d [N] int64) as numpy, N = len(im_ids): the
+    overlap of images i < j is the number of keypoint indices both have with a point3D_id > 0 over the larger of the
+    two counts."""
+    if len(im_ids) == 0:
+        return np.eye(0), np.array([])          # the reference's empty result: a float64 nums_3d
+    scores, counts = overlap_scores_device([images[i].point3D_ids for i in im_ids], device)
+    return scores.cpu().numpy(), counts.cpu().numpy().astype(np.int64)
+
+
+def _model_scores(model_dir, device):
+    """(image names in images.bin order as an object array, the device overlap matrix) of a COLMAP model."""
+    images = list(_read_images(os.path.join(model_dir, 'images.bin'), True, copy=False).values())
+    names = np.empty(len(images), dtype=object)
+    names[:] = [im.name for im in images]
+    scores, _ = overlap_scores_device([im.point3D_ids for im in images], device)
+    return names, scores
+
+
+def _pairs_by_threshold(names, scores, thresholds):
+    """The pair names of np.where((scores >= t) & (scores < 1)) for each t, each pair (max name, min name) by Python
+    string order.  One mask [T, N, N] and one torch.nonzero, whose rows come grouped by threshold and row-major within
+    a group (np.where's order): one device->host copy for nonzero's count and one for its rows."""
+    if not thresholds:
+        return []
+    below = scores < 1
+    mask = torch.stack([(scores >= t) & below for t in thresholds])
+    idx = torch.nonzero(mask).to(torch.int32).cpu().numpy()
+    rank = np.empty(len(names), dtype=np.int64)
+    rank[sorted(range(len(names)), key=names.__getitem__)] = np.arange(len(names))
+    bounds = np.searchsorted(idx[:, 0], np.arange(len(thresholds) + 1))
+    out = []
+    for k in range(len(thresholds)):
+        i, j = idx[bounds[k]:bounds[k + 1], 1], idx[bounds[k]:bounds[k + 1], 2]
+        swap = rank[i] < rank[j]
+        out.append(list(zip(names[np.where(swap, j, i)].tolist(), names[np.where(swap, i, j)].tolist())))
+    return out
+
+
+def sav_model_multi_ov_pairs(model_dir, overlaps, device='cuda'):
+    """data_loading.py:7-38: {overlap: pair names} of a COLMAP model, cached in model_dir/ov_pairs.npy.  A file holding
+    every requested overlap is returned as it is; otherwise every requested overlap is recomputed (keys of the file that
+    were not requested are dropped) and the file rewritten.  Prints the reference's lines."""
+    sav_file_path = os.path.join(model_dir, 'ov_pairs.npy')
+    if os.path.exists(sav_file_path):
+        ov_pair_dict = np.load(sav_file_path, allow_pickle=True).item()
+        if all(k in ov_pair_dict for k in overlaps):
+            print('All overlaps have been computed.')
+            return ov_pair_dict
+    names, scores = _model_scores(model_dir, device)
+    first = {}                                  # the reference's dict membership, for its skip rule
+    for t in overlaps:
+        first.setdefault(t, len(first))
+    pairs = _pairs_by_threshold(names, scores, list(first))
+    ov_pair_dict = {}
+    for min_overlap in overlaps:
+        if min_overlap in ov_pair_dict:
+            print(f'ov>{min_overlap} exists, skip.')
+            continue
+        pair_names = pairs[first[min_overlap]]
+        print(f'ov>{min_overlap} pairs: {len(pair_names)}')
+        ov_pair_dict[min_overlap] = pair_names
+    np.save(sav_file_path, ov_pair_dict)
+    return ov_pair_dict
+
+
+def load_model_ov_pairs(model_dir, min_overlap=0.3, device='cuda'):
+    """data_loading.py:40-52: the pair names of one overlap threshold, computed from the model (no cache)."""
+    names, scores = _model_scores(model_dir, device)
+    pair_names = _pairs_by_threshold(names, scores, [min_overlap])[0]
+    print('Loaded ov>{} pairs: {}'.format(min_overlap, len(pair_names)))
+    return pair_names
+
+
+def precompute_immatch_val_ovs(data_root, overlaps=(0.1, 0.2, 0.3, 0.4, 0.5), device='cuda'):
+    """data_pairs/precompute_immatch_val_ovs.py: sav_model_multi_ov_pairs for every scene directory of data_root
+    (os.listdir order), writing each scene's dense/sparse/ov_pairs.npy, with the script's printed lines."""
+    overlaps = list(overlaps)
+    scenes = os.listdir(data_root)
+    print(f'Target scenes: {scenes}, ovs: {overlaps}\n')
+    for scene in scenes:
+        print(f'Start processing scene: {scene}')
+        model_dir = os.path.join(data_root, scene, 'dense/sparse')
+        t0 = time.time()
+        sav_model_multi_ov_pairs(model_dir, overlaps, device)
+        print(f'Finished, time {time.time() - t0}')
+
+
+if __name__ == '__main__':
+    import argparse
+    parser = argparse.ArgumentParser(description='Write dense/sparse/ov_pairs.npy for every scene of a validation set.')
+    parser.add_argument('--data_root', type=str, default='data/immatch_benchmark/val_as_train')
+    precompute_immatch_val_ovs(parser.parse_args().data_root)

@@ -235,7 +235,8 @@ def synthetic_pair_shifted(pair_idx, height, width, noise=0.6):
 
 def write_colmap_model(model_dir, cameras, images):
     """COLMAP binary model (little-endian) with the given cameras [(id, model_id, width, height, params)] and images
-    [(id, qvec (w, x, y, z), tvec, camera_id, name)], without 2D points: cameras.bin and images.bin in model_dir."""
+    [(id, qvec (w, x, y, z), tvec, camera_id, name)] or [(..., name, point3D_ids)]: cameras.bin and images.bin in
+    model_dir.  An image without point3D_ids has no 2D points; with them, 2D point k is (k, 0) with point3D_ids[k]."""
     import struct
     os.makedirs(model_dir, exist_ok=True)
     with open(os.path.join(model_dir, 'cameras.bin'), 'wb') as f:
@@ -244,8 +245,31 @@ def write_colmap_model(model_dir, cameras, images):
             f.write(struct.pack('<iiQQ', cid, model_id, w, h) + struct.pack(f'<{len(params)}d', *params))
     with open(os.path.join(model_dir, 'images.bin'), 'wb') as f:
         f.write(struct.pack('<Q', len(images)))
-        for iid, q, t, cid, name in images:
-            f.write(struct.pack('<i7di', iid, *q, *t, cid) + name.encode('utf-8') + b'\x00' + struct.pack('<Q', 0))
+        for iid, q, t, cid, name, *ids in images:
+            ids = np.asarray(ids[0] if ids else [], dtype='<i8').reshape(-1)
+            pts = np.zeros(len(ids), dtype=[('xy', '<f8', (2,)), ('id', '<i8')])
+            pts['xy'][:, 0] = np.arange(len(ids))
+            pts['id'] = ids
+            f.write(struct.pack('<i7di', iid, *q, *t, cid) + name.encode('utf-8') + b'\x00' +
+                    struct.pack('<Q', len(ids)) + pts.tobytes())
+
+
+def synthetic_overlap_images(seed, n_images, n2d=8000, frac=(0.2, 0.6), vary_n2d=False, identical=()):
+    """Images [(id, qvec, tvec, camera_id, name, point3D_ids)] for write_colmap_model, for the overlap precompute:
+    image i has n2d keypoints (uniform in 1 .. n2d with vary_n2d), each triangulated (a 3D point id > 0) with a
+    probability drawn per image from U(frac), else -1 or 0.  Each pair (a, b) in `identical` gives image b image a's
+    ids.  Names are a seeded permutation, so file order and name order differ."""
+    rng = np.random.default_rng([int(seed), 11])
+    perm = rng.permutation(n_images)
+    ids = []
+    for i in range(n_images):
+        n = int(rng.integers(1, n2d + 1)) if vary_n2d else n2d
+        p = rng.uniform(*frac)
+        ids.append(np.where(rng.uniform(size=n) < p, rng.integers(1, 2 ** 40, n), rng.choice([-1, 0], n)))
+    for a, b in identical:
+        ids[b] = ids[a].copy()
+    q = [1.0, 0.0, 0.0, 0.0]
+    return [(i + 1, q, [0.0, 0.0, float(i)], 1, f'im_{perm[i]:05d}.jpg', ids[i]) for i in range(n_images)]
 
 
 def synthetic_val_scene(root, scene, seed, sizes, ext='.png', missing=(), min_overlap=0.3):
