@@ -1,6 +1,6 @@
 """Time match verification: p2p_find_model on the GPU against OpenCV on the host, on the same rows.
 
-    python bench_verify.py [--calls 200] [--cpu-reps 20]
+    python bench_verify.py [--calls 200] [--cpu-reps 20] [--batch-pairs 256] [--batch-calls 5]
 
 Two workloads of 3200 rows each, for F and for H:
   * `fine`: the fine matches of one pair of bench.py's workload (640x480 synthetic_pair_shifted, consensus NC weights,
@@ -18,6 +18,11 @@ cv2.recoverPose.
 DEGENSAC (F with the plane-degeneracy check, model 2 of p2p_find_model) runs on the `fine` workload and on `plane`, a
 3200-row synthetic_dominant_plane scene (30 % outliers, 8 % of the inliers off the dominant plane, 0.5 px noise), at 1 px
 against cv2.findFundamentalMat (USAC_ACCURATE); for `plane` it also reports the recall of the off-plane inliers.
+Batch workload (`batch` in the output): --batch-pairs seeded pairs with row counts drawn uniformly from 300..3200
+(synthetic_two_view, 40 % outliers, 0.5 px noise; planar for H; synthetic_dominant_plane for DEGENSAC), timed with CUDA
+events as the K back-to-back single-pair calls (`ms_single`) and as one batched call (`ms_batch`), each the mean of
+--batch-calls repetitions after a warm-up; for E both arms also run pose recovery on the inliers (`E+pose`).  The two
+arms' outputs are compared byte for byte (`identical`).  `ms_cpu`: one pass of OpenCV over the K pairs on the host.
 Prints one JSON line and writes nothing.
 """
 import argparse
@@ -154,6 +159,115 @@ def time_pose(rows, calls, cpu_reps):
     return res
 
 
+def batch_pairs(kind, count, seed=0):
+    from patch2pix_b200.synth import synthetic_dominant_plane, synthetic_two_view
+    sizes = np.random.default_rng(seed).integers(300, 3201, count)
+    out = []
+    for k, n in enumerate(sizes):
+        if kind == 'DEGENSAC':
+            sc = synthetic_dominant_plane(1000 + k, int(n), 0.3, 0.08, 0.5)
+        else:
+            sc = synthetic_two_view(1000 + k, int(n), 0.4, 0.5, planar=kind == 'H')
+        out.append(np.concatenate([sc['pts1'], sc['pts2']], 1))
+    return out
+
+
+def _events(fn, calls):
+    fn()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    torch.cuda.synchronize()
+    e0.record()
+    for _ in range(calls):
+        fn()
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / calls
+
+
+def time_batch(kind, count, calls, dev):
+    """The K back-to-back single-pair calls against one batched call on the same device rows."""
+    from patch2pix_b200 import _lib
+    from patch2pix_b200 import pose as P
+    from patch2pix_b200 import verify as V
+    pairs = batch_pairs('F' if kind in ('E', 'E+pose') else kind, count)
+    n = np.array([p.shape[0] for p in pairs])
+    offsets = np.concatenate(([0], np.cumsum(n))).astype(np.int64)
+    K, N = count, int(offsets[-1])
+    rows = torch.from_numpy(np.concatenate(pairs)).to(dev)
+    offs = torch.from_numpy(offsets).to(dev)
+    views = [rows[offsets[k]:offsets[k + 1]] for k in range(K)]
+    h = _lib.default_handle(dev)
+    res = {'pairs': K, 'rows_total': N}
+    if kind in ('F', 'H', 'DEGENSAC'):
+        model, th = MODEL[kind], TH[kind]
+        single = [torch.zeros(V.out_size(int(v)), dtype=torch.float64, device=dev) for v in n]
+        batch = torch.zeros(V.batch_out_size(K, N), dtype=torch.float64, device=dev)
+        b = batch.data_ptr()
+
+        def run_single():
+            for k in range(K):
+                V.find_model_into(h, model, views[k], 4, int(n[k]), None, th, 0.999, 10000, 0, single[k])
+
+        def run_batch():
+            V.find_model_batch_into(h, model, rows, 4, offs, offsets, None, th, 0.999, 10000, 0, b,
+                                    b + 8 * (9 * K + (K + 1) // 2), b + 72 * K)
+        res['ms_single'], res['ms_batch'] = _events(run_single, calls), _events(run_batch, calls)
+        got = V.parse_batch_host(batch.cpu().numpy(), offsets)
+        want = [V.parse_host(o.cpu().numpy(), int(v)) for o, v in zip(single, n)]
+        res['identical'] = all((g[0] is None) == (w[0] is None) and (g[0] is None or g[0].tobytes() == w[0].tobytes())
+                               and np.array_equal(g[1], w[1]) for g, w in zip(got, want))
+        res['inliers'] = int(sum(int(g[1].sum()) for g in got))
+    else:
+        pose = kind == 'E+pose'
+        Kc = np.array([[500.0, 0, 320.0], [0, 500.0, 240.0], [0, 0, 1]])
+        intr = P.intrinsics(Kc, Kc)
+        intr_d = torch.from_numpy(np.tile(np.asarray(intr), (K, 1))).to(dev)
+        single = [torch.zeros(P.out_size(int(v)), dtype=torch.float64, device=dev) for v in n]
+        batch = torch.zeros(P.batch_out_size(K, N), dtype=torch.float64, device=dev)
+        pp = P._batch_ptrs(batch, K, N)
+
+        def run_single():
+            for k in range(K):
+                P.find_essential_into(h, views[k], 4, int(n[k]), None, intr, 1.0, 0.999, 1000, 0, single[k])
+                if pose:
+                    o = single[k].data_ptr()
+                    P.recover_pose_into(h, views[k], 4, int(n[k]), None, intr, o, o + 184, single[k])
+
+        def run_batch():
+            P.find_essential_batch_into(h, rows, 4, offs, offsets, None, intr_d.data_ptr(), 1.0, 0.999, 1000, 0, pp['E'],
+                                        pp['emask'], pp['cnt'])
+            if pose:
+                P.recover_pose_batch_into(h, rows, 4, offs, offsets, None, intr_d.data_ptr(), pp['E'], pp['emask'],
+                                          pp['Rt'], pp['pmask'], pp['good'])
+        res['ms_single'], res['ms_batch'] = _events(run_single, calls), _events(run_batch, calls)
+        got = P._parse_batch(batch.cpu().numpy(), offsets, K, N)
+        want = [P.parse_host(o.cpu().numpy(), int(v)) for o, v in zip(single, n)]
+        keep = slice(0, 6) if pose else slice(0, 2)
+        res['identical'] = all(all(np.asarray(a).tobytes() == np.asarray(b_).tobytes() if a is not None else b_ is None
+                                   for a, b_ in zip(g[keep], w[keep])) for g, w in zip(got, want))
+        res['inliers'] = int(sum(int(g[1].sum()) for g in got))
+    res['speedup'] = res['ms_single'] / res['ms_batch']
+    res['ms_cpu'] = None
+    try:
+        import cv2
+    except ImportError:
+        return res
+    t0 = time.perf_counter()
+    for p in pairs:
+        p1, p2 = p[:, :2].copy(), p[:, 2:].copy()
+        if kind in ('F', 'DEGENSAC'):
+            cv2.findFundamentalMat(p1, p2, cv2.USAC_ACCURATE, TH[kind], 0.999, 10000)
+        elif kind == 'H':
+            cv2.findHomography(p1, p2, cv2.RANSAC, TH[kind], maxIters=10000, confidence=0.999)
+        else:
+            E, m = cv2.findEssentialMat(p1, p2, Kc, cv2.RANSAC, 0.999, 1.0, maxIters=1000)
+            if pose and E is not None and E.shape[0] == 3:
+                inl = np.where(m.ravel() > 0)[0]
+                cv2.recoverPose(E, p1[inl], p2[inl], Kc)
+    res['ms_cpu'] = (time.perf_counter() - t0) * 1e3
+    return res
+
+
 def card():
     try:
         q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'],
@@ -167,6 +281,8 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--calls', type=int, default=200)
     ap.add_argument('--cpu-reps', type=int, default=20)
+    ap.add_argument('--batch-pairs', type=int, default=256)
+    ap.add_argument('--batch-calls', type=int, default=5)
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise RuntimeError('bench_verify.py needs a CUDA device: there is no CPU fallback')
@@ -185,6 +301,9 @@ def main():
                         'plane': time_one('DEGENSAC', prow, args.calls, args.cpu_reps, off)}
     line['E'] = {'fine': time_pose(fine, args.calls, args.cpu_reps),
                  'scene': time_pose(scene_rows('E', fine.shape[0], dev), args.calls, args.cpu_reps)}
+    if args.batch_pairs > 0:
+        line['batch'] = {kind: time_batch(kind, args.batch_pairs, args.batch_calls, dev)
+                         for kind in ('F', 'H', 'DEGENSAC', 'E', 'E+pose')}
     print(json.dumps(line), flush=True)
 
 

@@ -295,6 +295,39 @@ P2P_API int p2p_test_essential_hypotheses(p2p_handle_t h, const double* rows, in
                                           double px_th, unsigned long long seed, int count, double* models_out,
                                           int32_t* counts_out, void* stream);
 
+/* ---- many pairs per call: p2p_find_model / p2p_find_essential / p2p_recover_pose over K pairs, each pair's result
+ * bit-identical to the single-pair call on its rows (the same kernels with the pair as one more grid dimension).
+ * rows: ONE fp64 row array with one row_stride; pair k owns rows offsets[k] .. offsets[k+1]-1 (offsets DEVICE int64
+ * [K+1]; offsets_host the same K+1 values on the HOST).  offsets_host is checked: non-decreasing, from 0 or more, at
+ * most 2^26 rows per pair and fewer than 2^31 rows in all (-1 otherwise).  That offsets holds the same values is the
+ * caller's contract, as the device-side counts are: it is not read back.  n_dev: DEVICE double [K] or NULL, pair k uses
+ * min(n_k, n_dev[k]) rows.  Masks are row-aligned: mask_out (and mask_in) DEVICE uint8 [offsets[K]], pair k's entries
+ * at offsets[k] ..; entries of rows before offsets[0] are not touched.  One px_th / conf / max_iters / seed / dist_th
+ * serves every pair, so pair k draws exactly the hypotheses of a single-pair call with that seed.  intr: DEVICE double
+ * [K][8] as p2p_find_essential's HOST intr; finite values with positive focal lengths are the caller's contract (not
+ * read back).  K = 0 enqueues nothing.  Pairs run in launches of at most p2p_batch_chunk_pairs pairs (about 256 MiB of
+ * per-pair scratch, and the grid's 65535 limit), one after another on `stream`; the split changes no result.  No host
+ * sync. */
+P2P_API int p2p_find_model_batch(p2p_handle_t h, int model, const double* rows, int row_stride, const int64_t* offsets,
+                                 const int64_t* offsets_host, int K, const double* n_dev, double px_th, double conf,
+                                 int max_iters, unsigned long long seed, double* models_out, uint8_t* mask_out,
+                                 int32_t* n_inliers_out, void* stream);
+/* models_out DEVICE double [K][9], n_inliers_out DEVICE int32 [K]: per pair as p2p_find_model. */
+P2P_API int p2p_find_essential_batch(p2p_handle_t h, const double* rows, int row_stride, const int64_t* offsets,
+                                     const int64_t* offsets_host, int K, const double* n_dev, const double* intr,
+                                     double px_th, double conf, int max_iters, unsigned long long seed, double* E_out,
+                                     uint8_t* mask_out, int32_t* n_inliers_out, void* stream);
+/* E_out DEVICE double [K][9], n_inliers_out DEVICE int32 [K]: per pair as p2p_find_essential. */
+P2P_API int p2p_recover_pose_batch(p2p_handle_t h, const double* rows, int row_stride, const int64_t* offsets,
+                                   const int64_t* offsets_host, int K, const double* n_dev, const double* intr,
+                                   const double* E, const uint8_t* mask_in, double dist_th, double* Rt_out,
+                                   uint8_t* mask_out, int32_t* n_good_out, void* stream);
+/* E DEVICE double [K][9], mask_in row-aligned or NULL (all rows), Rt_out DEVICE double [K][12], n_good_out DEVICE int32
+ * [K]: per pair as p2p_recover_pose. */
+/* Pairs per launch of the batched entry points: entry 0 = p2p_find_model_batch, 1 = p2p_find_essential_batch,
+ * 2 = p2p_recover_pose_batch. */
+P2P_API int p2p_batch_chunk_pairs(p2p_handle_t h, int entry, int* pairs_out);
+
 /* ---- bring-up / accuracy probe: C[M,N] = alpha * A[M,K] B[N,K]^T on the wgmma path with the
  * same operand format as the hot path (fp32 inputs are split to fp16 hi/lo on the device).
  * a, b, c are DEVICE fp32; K % 64 == 0. */

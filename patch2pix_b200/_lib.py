@@ -62,6 +62,13 @@ _SIGNATURES = {
     'p2p_find_essential': (_I, [_P, _P, _I, _I, _P, _P, C.c_double, C.c_double, _I, C.c_ulonglong, _P, _P, _P, _P]),
     'p2p_recover_pose': (_I, [_P, _P, _I, _I, _P, _P, _P, _P, C.c_double, _P, _P, _P, _P]),
     'p2p_test_essential_hypotheses': (_I, [_P, _P, _I, _I, _P, C.c_double, C.c_ulonglong, _I, _P, _P, _P]),
+    'p2p_find_model_batch': (_I, [_P, _I, _P, _I, _P, C.POINTER(C.c_int64), _I, _P, C.c_double, C.c_double, _I,
+                                  C.c_ulonglong, _P, _P, _P, _P]),
+    'p2p_find_essential_batch': (_I, [_P, _P, _I, _P, C.POINTER(C.c_int64), _I, _P, _P, C.c_double, C.c_double, _I,
+                                      C.c_ulonglong, _P, _P, _P, _P]),
+    'p2p_recover_pose_batch': (_I, [_P, _P, _I, _P, C.POINTER(C.c_int64), _I, _P, _P, _P, _P, C.c_double, _P, _P, _P,
+                                    _P]),
+    'p2p_batch_chunk_pairs': (_I, [_P, _I, C.POINTER(_I)]),
 }
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
 PROF_KINDS = ('l2norm', 'corr', 'mutual', 'nc', 'proposals', 'prep', 'gather_mid', 'conv1_mid', 'conv2_mid', 'fc_mid',

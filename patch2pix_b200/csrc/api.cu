@@ -2,6 +2,7 @@
 #include <math.h>
 #include <stdlib.h>
 
+#include <algorithm>
 #include <vector>
 
 #include "../../include/p2p_b200.h"
@@ -1160,11 +1161,80 @@ int p2p_find_model(p2p_handle_t h, int model, const double* rows, int row_stride
   P2P_REQUIRE(px_th > 0.0 && isfinite(px_th), "px_th must be positive");
   P2P_REQUIRE(conf > 0.0 && conf < 1.0, "conf must lie in (0, 1)");
   P2P_REQUIRE(max_iters > 0 && max_iters <= (1 << 24), "max_iters must lie in [1, 2^24]");
-  int rc = h->verify.reserve(verify_scratch_bytes(n, true) + 4096);
+  int rc = h->verify.reserve(verify_scratch_bytes(1, n, true) + 4096);
   if (rc) return rc;
-  void* scratch = h->verify.take(verify_scratch_bytes(n, true));
-  return launch_find_model(model, rows, row_stride, n, n_dev, px_th, conf, max_iters, seed, scratch, model_out, mask_out,
-                           n_inliers_out, reinterpret_cast<cudaStream_t>(stream));
+  void* scratch = h->verify.take(verify_scratch_bytes(1, n, true));
+  return launch_find_model(model, single_pair(rows, row_stride, n, n_dev), px_th, conf, max_iters, seed, scratch,
+                           model_out, mask_out, n_inliers_out, reinterpret_cast<cudaStream_t>(stream));
+}
+
+// ---- batches of pairs: validation of the host copy of the offsets and the split into launches ------------------------
+static int check_batch(const double* rows, int row_stride, const int64_t* offsets, const int64_t* offsets_host, int K) {
+  P2P_REQUIRE(K >= 0, "K must be non-negative");
+  P2P_REQUIRE(row_stride >= 4, "row_stride must be at least 4");
+  if (K == 0) return 0;
+  P2P_REQUIRE(offsets && offsets_host, "null offsets pointer");
+  P2P_REQUIRE(offsets_host[0] >= 0, "offsets must be non-negative");
+  for (int k = 0; k < K; ++k) {
+    const int64_t len = offsets_host[k + 1] - offsets_host[k];
+    P2P_REQUIRE(len >= 0, "offsets must be non-decreasing");
+    P2P_REQUIRE(len <= (1 << 26), "a pair has more than 2^26 rows");
+  }
+  P2P_REQUIRE(offsets_host[K] - offsets_host[0] < ((int64_t)1 << 31), "a batch must have fewer than 2^31 rows");
+  P2P_REQUIRE(rows || offsets_host[K] == offsets_host[0], "null rows pointer");
+  return 0;
+}
+
+// Pairs k0 .. k0 + pairs - 1 of a batch as one launch.
+static PairBatch batch_chunk(const double* rows, int row_stride, const int64_t* offsets, const int64_t* offsets_host,
+                             const double* n_dev, int k0, int pairs) {
+  return PairBatch{rows, row_stride, reinterpret_cast<const long long*>(offsets) + k0, 0,
+                   n_dev ? n_dev + k0 : nullptr, (long long)offsets_host[k0],
+                   (long long)(offsets_host[k0 + pairs] - offsets_host[k0]), pairs};
+}
+
+// Largest scratch of any launch of `chunk` pairs.
+static size_t batch_scratch(const int64_t* offsets_host, int K, int chunk, size_t (*bytes)(int, long long)) {
+  size_t need = 0;
+  for (int k0 = 0; k0 < K; k0 += chunk) {
+    const int pairs = std::min(chunk, K - k0);
+    need = std::max(need, bytes(pairs, (long long)(offsets_host[k0 + pairs] - offsets_host[k0])));
+  }
+  return need;
+}
+
+int p2p_batch_chunk_pairs(p2p_handle_t h, int entry, int* pairs_out) {
+  P2P_ENTER(h);
+  P2P_REQUIRE(pairs_out != nullptr, "null pointer");
+  P2P_REQUIRE(entry >= 0 && entry <= 2, "entry must be 0 (find_model), 1 (find_essential) or 2 (recover_pose)");
+  *pairs_out = entry == 0 ? verify_chunk_pairs() : entry == 1 ? essential_chunk_pairs() : pose_chunk_pairs();
+  return 0;
+}
+
+int p2p_find_model_batch(p2p_handle_t h, int model, const double* rows, int row_stride, const int64_t* offsets,
+                         const int64_t* offsets_host, int K, const double* n_dev, double px_th, double conf, int max_iters,
+                         unsigned long long seed, double* models_out, uint8_t* mask_out, int32_t* n_inliers_out,
+                         void* stream) {
+  P2P_ENTER(h);
+  P2P_REQUIRE(model >= 0 && model <= 2, "model must be 0 (F), 1 (H) or 2 (F with the DEGENSAC degeneracy check)");
+  int rc = check_batch(rows, row_stride, offsets, offsets_host, K);
+  if (rc) return rc;
+  P2P_REQUIRE(px_th > 0.0 && isfinite(px_th), "px_th must be positive");
+  P2P_REQUIRE(conf > 0.0 && conf < 1.0, "conf must lie in (0, 1)");
+  P2P_REQUIRE(max_iters > 0 && max_iters <= (1 << 24), "max_iters must lie in [1, 2^24]");
+  if (K == 0) return 0;
+  P2P_REQUIRE(models_out && mask_out && n_inliers_out, "null tensor pointer");
+  const int chunk = verify_chunk_pairs();
+  const size_t need = batch_scratch(offsets_host, K, chunk, [](int p, long long r) { return verify_scratch_bytes(p, r, true); });
+  if ((rc = h->verify.reserve(need + 4096))) return rc;
+  void* scratch = h->verify.take(need);
+  for (int k0 = 0; k0 < K; k0 += chunk) {
+    const PairBatch B = batch_chunk(rows, row_stride, offsets, offsets_host, n_dev, k0, std::min(chunk, K - k0));
+    if ((rc = launch_find_model(model, B, px_th, conf, max_iters, seed, scratch, models_out + 9 * (size_t)k0, mask_out,
+                                n_inliers_out + k0, reinterpret_cast<cudaStream_t>(stream))))
+      return rc;
+  }
+  return 0;
 }
 
 int p2p_sampson_distance(p2p_handle_t h, const double* rows, int row_stride, int n, const double* F, double* dist_out,
@@ -1224,9 +1294,9 @@ int p2p_test_hypotheses(p2p_handle_t h, int model, const double* rows, int row_s
   P2P_REQUIRE(model == 0 || model == 1, "model must be 0 (F) or 1 (H)");
   P2P_REQUIRE(rows && models_out && counts_out && count > 0 && row_stride >= 4, "bad argument");
   P2P_REQUIRE(n >= (model == 0 ? 7 : 4) && n <= (1 << 26), "fewer rows than a minimal sample");
-  int rc = h->verify.reserve(verify_scratch_bytes(n, false) + 4096);
+  int rc = h->verify.reserve(verify_scratch_bytes(1, n, false) + 4096);
   if (rc) return rc;
-  void* scratch = h->verify.take(verify_scratch_bytes(n, false));
+  void* scratch = h->verify.take(verify_scratch_bytes(1, n, false));
   return launch_test_hypotheses(model, rows, row_stride, n, px_th, seed, count, scratch, models_out, counts_out,
                                 reinterpret_cast<cudaStream_t>(stream));
 }
@@ -1263,11 +1333,38 @@ int p2p_find_essential(p2p_handle_t h, const double* rows, int row_stride, int n
   P2P_REQUIRE(px_th > 0.0 && isfinite(px_th), "px_th must be positive");
   P2P_REQUIRE(conf > 0.0 && conf < 1.0, "conf must lie in (0, 1)");
   P2P_REQUIRE(max_iters > 0 && max_iters <= (1 << 24), "max_iters must lie in [1, 2^24]");
-  int rc = h->verify.reserve(essential_scratch_bytes(n, true) + 4096);
+  int rc = h->verify.reserve(essential_scratch_bytes(1, n, true) + 4096);
   if (rc) return rc;
-  void* scratch = h->verify.take(essential_scratch_bytes(n, true));
-  return launch_find_essential(rows, row_stride, n, n_dev, K, px_th, conf, max_iters, seed, scratch, E_out, mask_out,
-                               n_inliers_out, reinterpret_cast<cudaStream_t>(stream));
+  void* scratch = h->verify.take(essential_scratch_bytes(1, n, true));
+  return launch_find_essential(single_pair(rows, row_stride, n, n_dev), nullptr, K, px_th, conf, max_iters, seed, scratch,
+                               E_out, mask_out, n_inliers_out, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int p2p_find_essential_batch(p2p_handle_t h, const double* rows, int row_stride, const int64_t* offsets,
+                             const int64_t* offsets_host, int K, const double* n_dev, const double* intr, double px_th,
+                             double conf, int max_iters, unsigned long long seed, double* E_out, uint8_t* mask_out,
+                             int32_t* n_inliers_out, void* stream) {
+  P2P_ENTER(h);
+  int rc = check_batch(rows, row_stride, offsets, offsets_host, K);
+  if (rc) return rc;
+  P2P_REQUIRE(px_th > 0.0 && isfinite(px_th), "px_th must be positive");
+  P2P_REQUIRE(conf > 0.0 && conf < 1.0, "conf must lie in (0, 1)");
+  P2P_REQUIRE(max_iters > 0 && max_iters <= (1 << 24), "max_iters must lie in [1, 2^24]");
+  if (K == 0) return 0;
+  P2P_REQUIRE(intr && E_out && mask_out && n_inliers_out, "null tensor pointer");
+  const int chunk = essential_chunk_pairs();
+  const size_t need =
+      batch_scratch(offsets_host, K, chunk, [](int p, long long r) { return essential_scratch_bytes(p, r, true); });
+  if ((rc = h->verify.reserve(need + 4096))) return rc;
+  void* scratch = h->verify.take(need);
+  for (int k0 = 0; k0 < K; k0 += chunk) {
+    const PairBatch B = batch_chunk(rows, row_stride, offsets, offsets_host, n_dev, k0, std::min(chunk, K - k0));
+    if ((rc = launch_find_essential(B, intr + 8 * (size_t)k0, Intrinsics{}, px_th, conf, max_iters, seed, scratch,
+                                    E_out + 9 * (size_t)k0, mask_out, n_inliers_out + k0,
+                                    reinterpret_cast<cudaStream_t>(stream))))
+      return rc;
+  }
+  return 0;
 }
 
 int p2p_recover_pose(p2p_handle_t h, const double* rows, int row_stride, int n, const double* n_dev, const double* intr,
@@ -1279,11 +1376,35 @@ int p2p_recover_pose(p2p_handle_t h, const double* rows, int row_stride, int n, 
   Intrinsics K;
   P2P_REQUIRE(intrinsics_ok(intr, K), "intr must be 8 finite values with positive focal lengths");
   P2P_REQUIRE(dist_th > 0.0 && isfinite(dist_th), "dist_th must be positive");
-  int rc = h->verify.reserve(pose_scratch_bytes(n) + 4096);
+  int rc = h->verify.reserve(pose_scratch_bytes(1, n) + 4096);
   if (rc) return rc;
-  void* scratch = h->verify.take(pose_scratch_bytes(n));
-  return launch_recover_pose(rows, row_stride, n, n_dev, K, E, mask_in, dist_th, scratch, Rt_out, mask_out, n_good_out,
-                             reinterpret_cast<cudaStream_t>(stream));
+  void* scratch = h->verify.take(pose_scratch_bytes(1, n));
+  return launch_recover_pose(single_pair(rows, row_stride, n, n_dev), nullptr, K, E, mask_in, dist_th, scratch, Rt_out,
+                             mask_out, n_good_out, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int p2p_recover_pose_batch(p2p_handle_t h, const double* rows, int row_stride, const int64_t* offsets,
+                           const int64_t* offsets_host, int K, const double* n_dev, const double* intr, const double* E,
+                           const uint8_t* mask_in, double dist_th, double* Rt_out, uint8_t* mask_out, int32_t* n_good_out,
+                           void* stream) {
+  P2P_ENTER(h);
+  int rc = check_batch(rows, row_stride, offsets, offsets_host, K);
+  if (rc) return rc;
+  P2P_REQUIRE(dist_th > 0.0 && isfinite(dist_th), "dist_th must be positive");
+  if (K == 0) return 0;
+  P2P_REQUIRE(intr && E && Rt_out && mask_out && n_good_out, "null tensor pointer");
+  const int chunk = pose_chunk_pairs();
+  const size_t need = batch_scratch(offsets_host, K, chunk, [](int p, long long r) { return pose_scratch_bytes(p, r); });
+  if ((rc = h->verify.reserve(need + 4096))) return rc;
+  void* scratch = h->verify.take(need);
+  for (int k0 = 0; k0 < K; k0 += chunk) {
+    const PairBatch B = batch_chunk(rows, row_stride, offsets, offsets_host, n_dev, k0, std::min(chunk, K - k0));
+    if ((rc = launch_recover_pose(B, intr + 8 * (size_t)k0, Intrinsics{}, E + 9 * (size_t)k0, mask_in, dist_th, scratch,
+                                  Rt_out + 12 * (size_t)k0, mask_out, n_good_out + k0,
+                                  reinterpret_cast<cudaStream_t>(stream))))
+      return rc;
+  }
+  return 0;
 }
 
 int p2p_test_essential_hypotheses(p2p_handle_t h, const double* rows, int row_stride, int n, const double* intr,
@@ -1295,9 +1416,9 @@ int p2p_test_essential_hypotheses(p2p_handle_t h, const double* rows, int row_st
   Intrinsics K;
   P2P_REQUIRE(intrinsics_ok(intr, K), "intr must be 8 finite values with positive focal lengths");
   P2P_REQUIRE(px_th > 0.0 && isfinite(px_th), "px_th must be positive");
-  int rc = h->verify.reserve(essential_scratch_bytes(n, false) + 4096);
+  int rc = h->verify.reserve(essential_scratch_bytes(1, n, false) + 4096);
   if (rc) return rc;
-  void* scratch = h->verify.take(essential_scratch_bytes(n, false));
+  void* scratch = h->verify.take(essential_scratch_bytes(1, n, false));
   return launch_test_essential_hypotheses(rows, row_stride, n, K, px_th, seed, count, scratch, models_out, counts_out,
                                           reinterpret_cast<cudaStream_t>(stream));
 }

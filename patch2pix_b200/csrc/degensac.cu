@@ -7,6 +7,7 @@
 //   verify_plane_kernel    (1 block)  DLT refit of that H on the rows within h_th while the count grows (fp64)
 //   verify_round_kernel<2> (x1 round) kRound plane-and-parallax models F = [e']x H, scored as F
 //   verify_parallax_select_kernel      adopts the best of them if it has strictly more inliers, clears `pending`
+// A batch of pairs adds grid dimension y to each launch, one block per pair (verify_common.cuh).
 // Testing every record rather than only the round's winner matters: a round of 1024 hypotheses often ends RANSAC on a
 // dominant-plane scene, and its winner is frequently a sample with 4 coplanar points, or with 5 whose induced H is
 // too noisy to pass the test, while an earlier record is degenerate.
@@ -99,14 +100,18 @@ __device__ int degeneracy_test(const VerifyState& S, const double* F, int hyp, c
 // earlier slot of the round, i.e. the models a sequential RANSAC would adopt -- are tested in slot order; the first
 // degenerate one sets `pending` and its induced H (st->plane).  Slots are scanned in contiguous chunks per thread with
 // a fixed-order exclusive max-scan, so the result does not depend on scheduling.
-__global__ void __launch_bounds__(kDegenThreads, 1) verify_degen_kernel(VerifyState* __restrict__ st,
-                                                                     const double* __restrict__ models,
-                                                                     const int* __restrict__ counts, int nm, int first,
-                                                                     const double* __restrict__ rows, int stride,
+__global__ void __launch_bounds__(kDegenThreads, 1) verify_degen_kernel(VerifyState* __restrict__ st_all,
+                                                                     const double* __restrict__ models_all,
+                                                                     const int* __restrict__ counts_all, int nm, int first,
+                                                                     const double* __restrict__ rows_all, int stride,
                                                                      unsigned long long seed, double h_th2) {
   constexpr int kChunk = kRound * 3 / kDegenThreads;
   __shared__ int s_max[kDegenThreads / 32], s_first[kDegenThreads / 32];
+  VerifyState* st = st_all + blockIdx.y;
   if (st->stop) return;
+  const double* models = models_all + blockIdx.y * kPairModels;
+  const int* counts = counts_all + blockIdx.y * kPairCounts;
+  const double* rows = rows_all + st->row0 * stride;
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, m0 = tid * kChunk;
   int mx = 0;
   for (int k = 0; k < kChunk && m0 + k < nm; ++k) mx = max(mx, counts[m0 + k]);
@@ -142,13 +147,15 @@ __global__ void __launch_bounds__(kDegenThreads, 1) verify_degen_kernel(VerifySt
 
 // DEGENSAC: the plane of a pending round -- DLT refit of st->plane on the rows within h_th (fp64 tests, normalised
 // coordinates), kept while the count grows, as the H path of verify_lo_kernel.
-__global__ void __launch_bounds__(kLoThreads, 1) verify_plane_kernel(VerifyState* __restrict__ st,
-                                                                  const double* __restrict__ rows, int stride,
+__global__ void __launch_bounds__(kLoThreads, 1) verify_plane_kernel(VerifyState* __restrict__ st_all,
+                                                                  const double* __restrict__ rows_all, int stride,
                                                                   double h_th2) {
   __shared__ double s_red[kLoThreads / 32][45];
   __shared__ double s_cur[9], s_cand[9];
   __shared__ int s_cnt[kLoThreads / 32], s_ok;
+  VerifyState* st = st_all + blockIdx.y;
   if (!st->pending) return;
+  const double* rows = rows_all + st->row0 * stride;
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   const int n = st->n;
   if (tid < 9) s_cur[tid] = st->plane[tid];
@@ -218,8 +225,10 @@ __global__ void __launch_bounds__(1024) verify_parallax_select_kernel(VerifyStat
                                                                       const double* __restrict__ models,
                                                                       const int* __restrict__ counts, int done,
                                                                       double conf, int max_iters) {
+  st += blockIdx.y;
   if (!st->pending) return;
-  select_round(st, models, counts, kRound, done, Kind<0>::kSample, conf, max_iters, true);
+  select_round(st, models + blockIdx.y * kPairModels, counts + blockIdx.y * kPairCounts, kRound, done, Kind<0>::kSample,
+               conf, max_iters, true);
   if (threadIdx.x == 0) st->pending = 0;
 }
 
@@ -239,30 +248,31 @@ __global__ void verify_degen_hook_kernel(const VerifyState* __restrict__ st, con
 
 // DEGENSAC (model 2): model 0's rounds, select and LO, plus the degeneracy test and plane-and-parallax launches of
 // every round; h_th = 2 px_th.
-int find_model_degensac(const double* rows, int stride, int n, const double* n_dev, double px_th, double conf,
-                        int max_iters, unsigned long long seed, void* scratch, double* model_out, uint8_t* mask_out,
-                        int* count_out, cudaStream_t st) {
-  const Scratch s = carve(scratch, n, kRound);
+int find_model_degensac(const PairBatch& B, double px_th, double conf, int max_iters, unsigned long long seed,
+                        void* scratch, double* model_out, uint8_t* mask_out, int* count_out, cudaStream_t st) {
+  const Scratch s = carve(scratch, B.pairs, B.total, kRound);
   const float th2 = (float)(px_th * px_th);
   const double h_th2 = (2.0 * px_th) * (2.0 * px_th);
-  verify_prep_kernel<<<1, 1024, 0, st>>>(rows, stride, n, n_dev, Kind<0>::kSample, s.rows32, s.st);
+  const dim3 one(1, B.pairs);
+  verify_prep_kernel<<<one, 1024, 0, st>>>(B, Kind<0>::kSample, s.rows32, s.st);
   P2P_LAUNCH_OK();
   for (int first = 0; first < max_iters; first += kRound) {
     const int count = min(kRound, max_iters - first);
-    int rc = enqueue_round<0>(s, rows, stride, first, count, seed, th2, 0, st);
+    int rc = enqueue_round<0>(s, B, first, count, seed, th2, 0, st);
     if (rc) return rc;
-    verify_degen_kernel<<<1, kDegenThreads, 0, st>>>(s.st, s.models, s.counts, count * 3, first, rows, stride, seed, h_th2);
+    verify_degen_kernel<<<one, kDegenThreads, 0, st>>>(s.st, s.models, s.counts, count * 3, first, B.rows, B.stride, seed,
+                                                       h_th2);
     P2P_LAUNCH_OK();
-    verify_select_kernel<<<1, 1024, 0, st>>>(s.st, s.models, s.counts, count * 3, first + count, Kind<0>::kSample, conf,
-                                             max_iters);
+    verify_select_kernel<<<one, 1024, 0, st>>>(s.st, s.models, s.counts, count * 3, first + count, Kind<0>::kSample, conf,
+                                               max_iters);
     P2P_LAUNCH_OK();
-    verify_plane_kernel<<<1, kLoThreads, 0, st>>>(s.st, rows, stride, h_th2);
+    verify_plane_kernel<<<one, kLoThreads, 0, st>>>(s.st, B.rows, B.stride, h_th2);
     P2P_LAUNCH_OK();
-    if ((rc = enqueue_round<2>(s, rows, stride, first, kRound, seed, th2, 0, st, h_th2))) return rc;
-    verify_parallax_select_kernel<<<1, 1024, 0, st>>>(s.st, s.models, s.counts, first + count, conf, max_iters);
+    if ((rc = enqueue_round<2>(s, B, first, kRound, seed, th2, 0, st, h_th2))) return rc;
+    verify_parallax_select_kernel<<<one, 1024, 0, st>>>(s.st, s.models, s.counts, first + count, conf, max_iters);
     P2P_LAUNCH_OK();
   }
-  verify_lo_kernel<0><<<1, kLoThreads, 0, st>>>(s.st, s.rows32, rows, stride, n, th2, model_out, mask_out, count_out);
+  verify_lo_kernel<0><<<one, kLoThreads, 0, st>>>(s.st, s.rows32, B.rows, B.stride, th2, model_out, mask_out, count_out);
   P2P_LAUNCH_OK();
   return 0;
 }
@@ -270,17 +280,18 @@ int find_model_degensac(const double* rows, int stride, int n, const double* n_d
 }  // namespace
 
 size_t verify_degeneracy_scratch_bytes(int n, int count) {
-  return verify_scratch_bytes(n, false) + align_up((size_t)count * 3 * 9 * sizeof(double), 1024) +
+  return verify_scratch_bytes(1, n, false) + align_up((size_t)count * 3 * 9 * sizeof(double), 1024) +
          (size_t)count * 3 * sizeof(int);
 }
 
 int launch_test_degeneracy(const double* rows, int stride, int n, double px_th, unsigned long long seed, int count,
                            void* scratch, int* tri_out, double* H_out, cudaStream_t st) {
-  Scratch s = carve(scratch, n, count);
+  const PairBatch B = single_pair(rows, stride, n, nullptr);
+  Scratch s = carve(scratch, 1, n, count);
   const double h_th2 = (2.0 * px_th) * (2.0 * px_th);
-  verify_prep_kernel<<<1, 1024, 0, st>>>(rows, stride, n, nullptr, Kind<0>::kSample, s.rows32, s.st);
+  verify_prep_kernel<<<1, 1024, 0, st>>>(B, Kind<0>::kSample, s.rows32, s.st);
   P2P_LAUNCH_OK();
-  int rc = enqueue_round<0>(s, rows, stride, 0, count, seed, (float)(px_th * px_th), 1, st);
+  int rc = enqueue_round<0>(s, B, 0, count, seed, (float)(px_th * px_th), 1, st);
   if (rc) return rc;
   verify_degen_hook_kernel<<<cdiv(count * 3, 128), 128, 0, st>>>(s.st, s.models, s.counts, count * 3, rows, stride, seed,
                                                                  h_th2, tri_out, H_out);
@@ -288,11 +299,9 @@ int launch_test_degeneracy(const double* rows, int stride, int n, double px_th, 
   return 0;
 }
 
-int launch_find_model_degensac(const double* rows, int stride, int n, const double* n_dev, double px_th, double conf,
-                               int max_iters, unsigned long long seed, void* scratch, double* model_out, uint8_t* mask_out,
-                               int* count_out, cudaStream_t st) {
-  return find_model_degensac(rows, stride, n, n_dev, px_th, conf, max_iters, seed, scratch, model_out, mask_out,
-                             count_out, st);
+int launch_find_model_degensac(const PairBatch& B, double px_th, double conf, int max_iters, unsigned long long seed,
+                               void* scratch, double* model_out, uint8_t* mask_out, int* count_out, cudaStream_t st) {
+  return find_model_degensac(B, px_th, conf, max_iters, seed, scratch, model_out, mask_out, count_out, st);
 }
 
 }  // namespace p2p

@@ -105,13 +105,35 @@ int launch_fc_parse(const float* pooled, const FcWeights& fc, const void* matche
 int launch_finalize_matches(const float* fine, const float* scores, const long long* coarse, int N, float io_thres,
                             const double up[4], double* packed, cudaStream_t st);
 
+// ---- batches of pairs (verify.cu, degensac.cu, pose.cu) -------------------------------------------------------------
+// Pair p of a launch reads rows offsets[p] .. offsets[p+1]-1 of `rows` (fp64 (x1, y1, x2, y2) at `stride` doubles
+// apart); offsets == nullptr: one pair of n1 rows.  n_dev (device, nullable): pair p uses min(n_p, n_dev[p]) rows.
+// Per-row scratch (fp32 rows, pose codes) of a launch is indexed by row - base, base = offsets[0].  Masks are indexed
+// by row.  pairs <= kMaxGridY; a batch beyond kBatchScratchBudget bytes of per-pair scratch runs in chunks.
+struct PairBatch {
+  const double* rows;
+  int stride;
+  const long long* offsets;
+  int n1;
+  const double* n_dev;
+  long long base;
+  long long total;                  // rows of the launch: offsets[pairs] - offsets[0], or n1
+  int pairs;
+};
+inline PairBatch single_pair(const double* rows, int stride, int n, const double* n_dev) {
+  return PairBatch{rows, stride, nullptr, n, n_dev, 0, n, 1};
+}
+constexpr int kMaxGridY = 65535;
+constexpr size_t kBatchScratchBudget = (size_t)256 << 20;
+
 // ---- verify.cu: RANSAC for F (model 0, 7-point) / H (model 1, 4-point DLT) / F with DEGENSAC (model 2) and the
 // Sampson distance ----------------------------------------------------------------------------------------------------
 // rows: fp64 (x1, y1, x2, y2) at `stride` doubles apart; n_dev (optional, device): effective row count min(n, *n_dev).
-size_t verify_scratch_bytes(int n, bool rounds);
-int launch_find_model(int model, const double* rows, int stride, int n, const double* n_dev, double px_th, double conf,
-                      int max_iters, unsigned long long seed, void* scratch, double* model_out, uint8_t* mask_out,
-                      int* count_out, cudaStream_t st);
+// Pair p writes model_out[9 p ..], count_out[p] and mask_out[row] for its rows.
+size_t verify_scratch_bytes(int pairs, long long rows, bool rounds);
+int verify_chunk_pairs();   // pairs per launch within kBatchScratchBudget
+int launch_find_model(int model, const PairBatch& B, double px_th, double conf, int max_iters, unsigned long long seed,
+                      void* scratch, double* model_out, uint8_t* mask_out, int* count_out, cudaStream_t st);
 // Hypotheses 0 .. count-1 without selection: models_out [count*slots][9], counts_out [count*slots] (-1: no model).
 int launch_test_hypotheses(int model, const double* rows, int stride, int n, double px_th, unsigned long long seed,
                            int count, void* scratch, double* models_out, int* counts_out, cudaStream_t st);
@@ -135,9 +157,8 @@ constexpr long long kMaxOverlapPoints = (1LL << 31) - 1;
 int launch_overlap_scores(const long long* ids, const long long* offsets, int n, int words, unsigned* bits,
                           int* counts, double* scores, cudaStream_t st);
 // ---- degensac.cu: model 2 of launch_find_model (same scratch) and its test hook
-int launch_find_model_degensac(const double* rows, int stride, int n, const double* n_dev, double px_th, double conf,
-                               int max_iters, unsigned long long seed, void* scratch, double* model_out, uint8_t* mask_out,
-                               int* count_out, cudaStream_t st);
+int launch_find_model_degensac(const PairBatch& B, double px_th, double conf, int max_iters, unsigned long long seed,
+                               void* scratch, double* model_out, uint8_t* mask_out, int* count_out, cudaStream_t st);
 // DEGENSAC's degeneracy test of every slot of F hypotheses 0 .. count-1: tri_out [count*3] (-2: no model, -1: not
 // degenerate, else the first degenerate triplet), H_out [count*3][9] (its induced H in pixels, zeros otherwise).
 size_t verify_degeneracy_scratch_bytes(int n, int count);
@@ -146,16 +167,21 @@ int launch_test_degeneracy(const double* rows, int stride, int n, double px_th, 
 
 // ---- pose.cu: essential-matrix RANSAC (5-point) and pose recovery ------------------------------------------------
 struct Intrinsics { double fx1, fy1, cx1, cy1, fx2, fy2, cx2, cy2; };   // pixels -> camera coordinates of both views
-size_t essential_scratch_bytes(int n, bool rounds);
-size_t pose_scratch_bytes(int n);
-int launch_find_essential(const double* rows, int stride, int n, const double* n_dev, const Intrinsics& K, double px_th,
-                          double conf, int max_iters, unsigned long long seed, void* scratch, double* E_out,
-                          uint8_t* mask_out, int* count_out, cudaStream_t st);
+// Batches as launch_find_model.  intr: DEVICE double [pairs][8] (fx1, fy1, cx1, cy1, fx2, fy2, cx2, cy2), or nullptr:
+// K1 for the single pair.
+size_t essential_scratch_bytes(int pairs, long long rows, bool rounds);
+size_t pose_scratch_bytes(int pairs, long long rows);
+int essential_chunk_pairs();
+int pose_chunk_pairs();
+int launch_find_essential(const PairBatch& B, const double* intr, const Intrinsics& K1, double px_th, double conf,
+                          int max_iters, unsigned long long seed, void* scratch, double* E_out, uint8_t* mask_out,
+                          int* count_out, cudaStream_t st);
 // Hypotheses 0 .. count-1 without selection: models_out [count*10][9], counts_out [count*10] (-1: no model).
 int launch_test_essential_hypotheses(const double* rows, int stride, int n, const Intrinsics& K, double px_th,
                                      unsigned long long seed, int count, void* scratch, double* models_out,
                                      int* counts_out, cudaStream_t st);
-int launch_recover_pose(const double* rows, int stride, int n, const double* n_dev, const Intrinsics& K, const double* E,
+// E [pairs][9], mask_in / mask_out indexed by row, Rt_out [pairs][12], count_out [pairs].
+int launch_recover_pose(const PairBatch& B, const double* intr, const Intrinsics& K1, const double* E,
                         const uint8_t* mask_in, double dist_th, void* scratch, double* Rt_out, uint8_t* mask_out,
                         int* count_out, cudaStream_t st);
 

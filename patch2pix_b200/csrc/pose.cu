@@ -13,7 +13,12 @@
 //   pose_count_kernel     (kPoseBlocks) linear triangulation of every masked row against each candidate, cheirality and
 //                                      distance test -> one 4-bit code per row and per-block integer counts
 //   pose_select_kernel    (1 block)   fixed-order sum of the counts, first best candidate, R, t, count, mask
+// A batch of pairs runs the same launches with the pair as grid dimension y: one block per pair for the one-block
+// kernels, cdiv(count, 8) x pairs for a round and kPoseBlocks x pairs for pose_count_kernel.  Pair p's intrinsics,
+// threshold and row range live in its state, so a pair's arithmetic does not depend on the other pairs.
 // No grid size depends on the device and every combine runs in a fixed order, so results are bit-reproducible.
+#include <algorithm>
+
 #include <math.h>
 
 #include "kernels.h"
@@ -39,17 +44,29 @@ constexpr int kPoseThreads = 256;
 
 struct EssState {
   double best[9];                   // best model so far, camera coordinates
+  Intrinsics K;                     // the pair's cameras
+  float th2;                        // squared inlier threshold in camera coordinates
   int n;                            // effective row count
   int bad;                          // a coordinate is not finite
   int stop;                         // no further rounds are needed
   int best_count;                   // 0: no model yet
+  int n_all;                        // rows of the pair (mask length)
+  long long row0;                   // first row of the pair in the row array and the mask
+  long long row32;                  // first row of the pair in rows32
 };
 
 struct PoseState {
   double R[2][9], t[3];             // R1, R2 row-major, t = U[:, 2]
+  Intrinsics K;                     // the pair's cameras
   int n;                            // effective row count
   int valid;                        // E was finite and non-zero
+  int n_all;                        // rows of the pair (mask length)
+  long long row0;                   // first row of the pair in the row array and the masks
+  long long row32;                  // first row of the pair in the codes
 };
+
+constexpr size_t kPairModels = (size_t)kRound * kSlots * 9;   // round-model doubles per pair
+constexpr size_t kPairCounts = (size_t)kRound * kSlots;       // round-count ints per pair
 
 // ---- 5-point solver (one thread; restated in oracle/pose_oracle.py) ------------------------------------------------
 // Monomials of degree <= 3 in (x, y, z): x^3 y^3 x^2y xy^2 x^2z x^2 y^2z y^2 xyz xy | xz^2 xz x yz^2 yz y z^3 z^2 z 1.
@@ -392,13 +409,32 @@ __device__ __forceinline__ int effective_rows(int n, const double* n_dev) {
   return m;
 }
 
+// Pair p's cameras: intr[8 p ..] (device), or K1 for a single pair (intr == nullptr).
+__device__ __forceinline__ Intrinsics pair_intrinsics(const double* intr, const Intrinsics& K1, int p) {
+  if (intr == nullptr) return K1;
+  const double* k = intr + 8 * (size_t)p;
+  return Intrinsics{k[0], k[1], k[2], k[3], k[4], k[5], k[6], k[7]};
+}
+
+// cv2.findEssentialMat's threshold in camera coordinates: px_th / ((fx + fy) / 2) of view 2, squared.
+__device__ __forceinline__ float ess_th2(double px_th, const Intrinsics& K) {
+  const double th = px_th / ((K.fx2 + K.fy2) / 2.0);
+  return (float)(th * th);
+}
+
 // ---- essential-matrix RANSAC kernels -------------------------------------------------------------------------------
-__global__ void __launch_bounds__(1024) ess_prep_kernel(const double* __restrict__ rows, int stride, int n,
-                                                        const double* __restrict__ n_dev, Intrinsics K,
-                                                        float4* __restrict__ rows32, EssState* __restrict__ st) {
+__global__ void __launch_bounds__(1024) ess_prep_kernel(PairBatch B, const double* __restrict__ intr, Intrinsics K1,
+                                                        double px_th, float4* __restrict__ rows32_all,
+                                                        EssState* __restrict__ st_all) {
   __shared__ int s_n;
-  const int tid = threadIdx.x;
-  if (tid == 0) s_n = effective_rows(n, n_dev);
+  const int tid = threadIdx.x, p = blockIdx.y;
+  EssState* st = st_all + p;
+  const PairRange pr = pair_range(B, p);
+  const int n = pr.n, stride = B.stride;
+  const double* rows = B.rows + pr.row0 * stride;
+  float4* rows32 = rows32_all + (pr.row0 - B.base);
+  const Intrinsics K = pair_intrinsics(intr, K1, p);
+  if (tid == 0) s_n = effective_rows(n, B.n_dev == nullptr ? nullptr : B.n_dev + p);
   __syncthreads();
   const int m = s_n;
   int bad = 0;
@@ -416,25 +452,37 @@ __global__ void __launch_bounds__(1024) ess_prep_kernel(const double* __restrict
     st->bad = bad;
     st->stop = bad || m < kSample;
     st->best_count = 0;
+    st->K = K;
+    st->th2 = ess_th2(px_th, K);
+    st->n_all = n;
+    st->row0 = pr.row0;
+    st->row32 = pr.row0 - B.base;
   }
 }
 
 // Hypotheses first .. first + count - 1.  models [count * kSlots][9] fp64 (camera coordinates), counts
 // [count * kSlots] (-1: no model in that slot).
-__global__ void __launch_bounds__(kScoreThreads, 1) ess_round_kernel(const EssState* __restrict__ st,
-                                                                  const float4* __restrict__ rows32,
-                                                                  const double* __restrict__ rows, int stride,
-                                                                  Intrinsics K, int first, int count,
-                                                                  unsigned long long seed, float th2, int ignore_stop,
-                                                                  double* __restrict__ models, int* __restrict__ counts) {
+__global__ void __launch_bounds__(kScoreThreads, 1) ess_round_kernel(const EssState* __restrict__ st_all,
+                                                                  const float4* __restrict__ rows32_all,
+                                                                  const double* __restrict__ rows_all, int stride,
+                                                                  int first, int count, unsigned long long seed,
+                                                                  int ignore_stop, double* __restrict__ models_all,
+                                                                  int* __restrict__ counts_all) {
   constexpr int NM = kHypPerBlock * kSlots, NJ = NM / 8;
   __shared__ float4 s_rows[kTile];
   __shared__ double s_M[kHypPerBlock][10][20];
   __shared__ float s_model[NM][9];
   __shared__ int s_valid[NM];
+  const EssState* st = st_all + blockIdx.y;
   if (!ignore_stop && st->stop) return;
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   const int n = st->n;
+  const Intrinsics K = st->K;
+  const float th2 = st->th2;
+  const double* rows = rows_all + st->row0 * stride;
+  const float4* rows32 = rows32_all + st->row32;
+  double* models = models_all + blockIdx.y * kPairModels;
+  int* counts = counts_all + blockIdx.y * kPairCounts;
   if (tid < kHypPerBlock) {
     const int local = blockIdx.x * kHypPerBlock + tid;
     double out[kSlots][9];
@@ -492,22 +540,31 @@ __global__ void __launch_bounds__(kScoreThreads, 1) ess_round_kernel(const EssSt
 __global__ void __launch_bounds__(1024) ess_select_kernel(EssState* __restrict__ st, const double* __restrict__ models,
                                                           const int* __restrict__ counts, int nm, int done, double conf,
                                                           int max_iters) {
-  select_round(st, models, counts, nm, done, kSample, conf, max_iters);
+  select_round(st + blockIdx.y, models + blockIdx.y * kPairModels, counts + blockIdx.y * kPairCounts, nm, done, kSample,
+               conf, max_iters);
 }
 
 // Local optimisation + outputs: 8-point refit on the inliers (fp64 normal matrix, Jacobi), projected onto the essential
 // manifold (singular values 1, 1, 0) at unit Frobenius norm, kept while it has strictly more inliers.
-__global__ void __launch_bounds__(kLoThreads, 1) ess_lo_kernel(const EssState* __restrict__ st,
-                                                            const float4* __restrict__ rows32,
-                                                            const double* __restrict__ rows, int stride, Intrinsics K,
-                                                            int n_all, float th2, double* __restrict__ E_out,
-                                                            uint8_t* __restrict__ mask_out, int* __restrict__ count_out) {
+__global__ void __launch_bounds__(kLoThreads, 1) ess_lo_kernel(const EssState* __restrict__ st_all,
+                                                            const float4* __restrict__ rows32_all,
+                                                            const double* __restrict__ rows_all, int stride,
+                                                            double* __restrict__ E_out, uint8_t* __restrict__ mask_out,
+                                                            int* __restrict__ count_out) {
   __shared__ double s_red[kLoThreads / 32][45];
   __shared__ double s_cur[9], s_cand[9];
   __shared__ float s_f32[9];
   __shared__ int s_cnt[kLoThreads / 32], s_ok;
+  const EssState* st = st_all + blockIdx.y;
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  const int n = st->n, bad = st->bad;
+  const int n = st->n, bad = st->bad, n_all = st->n_all;
+  const Intrinsics K = st->K;
+  const float th2 = st->th2;
+  const double* rows = rows_all + st->row0 * stride;
+  const float4* rows32 = rows32_all + st->row32;
+  E_out += 9 * blockIdx.y;
+  count_out += blockIdx.y;
+  mask_out += st->row0;
   int cur_count = bad ? 0 : st->best_count;
   if (tid < 9) s_cur[tid] = st->best[tid];
   __syncthreads();
@@ -602,10 +659,18 @@ __global__ void __launch_bounds__(kLoThreads, 1) ess_lo_kernel(const EssState* _
 
 // ---- pose recovery kernels ----------------------------------------------------------------------------------------
 // cv2.decomposeEssentialMat: E = U S V^T with det U, det V^T made positive; R1 = U W V^T, R2 = U W^T V^T, t = U[:, 2].
-__global__ void pose_decompose_kernel(const double* __restrict__ E, int n, const double* __restrict__ n_dev,
-                                      PoseState* __restrict__ ps) {
+__global__ void pose_decompose_kernel(PairBatch B, const double* __restrict__ intr, Intrinsics K1,
+                                      const double* __restrict__ E, PoseState* __restrict__ ps) {
   if (threadIdx.x != 0) return;
-  ps->n = effective_rows(n, n_dev);
+  const int p = blockIdx.y;
+  const PairRange pr = pair_range(B, p);
+  ps += p;
+  E += 9 * (size_t)p;
+  ps->K = pair_intrinsics(intr, K1, p);
+  ps->n_all = pr.n;
+  ps->row0 = pr.row0;
+  ps->row32 = pr.row0 - B.base;
+  ps->n = effective_rows(pr.n, B.n_dev == nullptr ? nullptr : B.n_dev + p);
   double e[9], amax = 0.0;
   bool fin = true;
   for (int j = 0; j < 9; ++j) {
@@ -652,12 +717,18 @@ __device__ bool good_point(const double* R, const double* t, double x1, double y
 
 __global__ void __launch_bounds__(kPoseThreads) pose_count_kernel(const PoseState* __restrict__ ps,
                                                                   const double* __restrict__ rows, int stride,
-                                                                  Intrinsics K, const uint8_t* __restrict__ mask_in,
-                                                                  double dist_th, uint8_t* __restrict__ codes,
+                                                                  const uint8_t* __restrict__ mask_in, double dist_th,
+                                                                  uint8_t* __restrict__ codes,
                                                                   int* __restrict__ partial) {
   __shared__ int s_cnt[kPoseThreads / 32][4];
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  ps += blockIdx.y;
   const int n = ps->valid ? ps->n : 0;
+  const Intrinsics K = ps->K;
+  rows += ps->row0 * stride;
+  if (mask_in != nullptr) mask_in += ps->row0;
+  codes += ps->row32;
+  partial += (size_t)blockIdx.y * kPoseBlocks * 4;
   int c[4] = {0, 0, 0, 0};
   for (int r = blockIdx.x * kPoseThreads + tid; r < n; r += kPoseBlocks * kPoseThreads) {
     int code = 0;
@@ -692,12 +763,18 @@ __global__ void __launch_bounds__(kPoseThreads) pose_count_kernel(const PoseStat
 // mask.  No valid E: zeros and an empty mask.
 __global__ void __launch_bounds__(1024) pose_select_kernel(const PoseState* __restrict__ ps,
                                                            const int* __restrict__ partial,
-                                                           const uint8_t* __restrict__ codes, int n_all,
+                                                           const uint8_t* __restrict__ codes,
                                                            double* __restrict__ Rt_out, uint8_t* __restrict__ mask_out,
                                                            int* __restrict__ count_out) {
   __shared__ int s_tot[4], s_best;
   const int tid = threadIdx.x;
-  const int valid = ps->valid, n = ps->n;
+  ps += blockIdx.y;
+  const int valid = ps->valid, n = ps->n, n_all = ps->n_all;
+  partial += (size_t)blockIdx.y * kPoseBlocks * 4;
+  codes += ps->row32;
+  Rt_out += 12 * blockIdx.y;
+  count_out += blockIdx.y;
+  mask_out += ps->row0;
   if (tid < 4) {
     int tot = 0;
     for (int b = 0; b < kPoseBlocks; ++b) tot += partial[b * 4 + tid];
@@ -727,50 +804,61 @@ struct EssScratch {
   int* counts;
 };
 
-EssScratch carve_ess(void* base, int n, int nhyp) {
+// `pairs` states, `rows` fp32 rows, then nhyp hypotheses' models and counts per pair (nhyp = kRound: pair strides
+// kPairModels / kPairCounts).
+EssScratch carve_ess(void* base, int pairs, long long rows, int nhyp) {
   char* p = (char*)base;
   EssScratch s;
   s.st = (EssState*)p;
-  p += 1024;
+  p += align_up((size_t)pairs * sizeof(EssState), 1024);
   s.rows32 = (float4*)p;
-  p += align_up((size_t)n * sizeof(float4) + 16, 1024);
+  p += align_up((size_t)rows * sizeof(float4) + 16, 1024);
   s.models = (double*)p;
-  p += align_up((size_t)nhyp * kSlots * 9 * sizeof(double), 1024);
+  p += align_up((size_t)pairs * nhyp * kSlots * 9 * sizeof(double), 1024);
   s.counts = (int*)p;
   return s;
 }
 
-float ess_th2(double px_th, const Intrinsics& K) {   // cv2.findEssentialMat: threshold / ((fx + fy) / 2)
-  const double th = px_th / ((K.fx2 + K.fy2) / 2.0);
-  return (float)(th * th);
-}
-
 }  // namespace
 
-size_t essential_scratch_bytes(int n, bool rounds) {
-  return 1024 + align_up((size_t)n * sizeof(float4) + 16, 1024) +
-         (rounds ? align_up((size_t)kRound * kSlots * 9 * sizeof(double), 1024) + (size_t)kRound * kSlots * sizeof(int)
+size_t essential_scratch_bytes(int pairs, long long rows, bool rounds) {
+  return align_up((size_t)pairs * sizeof(EssState), 1024) + align_up((size_t)rows * sizeof(float4) + 16, 1024) +
+         (rounds ? align_up((size_t)pairs * kPairModels * sizeof(double), 1024) + (size_t)pairs * kPairCounts * sizeof(int)
                  : 0);
 }
 
-size_t pose_scratch_bytes(int n) { return 1024 + align_up((size_t)kPoseBlocks * 4 * sizeof(int), 1024) + (size_t)n + 16; }
+// states, per-block partial counts of every pair, then one code byte per row
+size_t pose_scratch_bytes(int pairs, long long rows) {
+  return align_up((size_t)pairs * sizeof(PoseState), 1024) + align_up((size_t)pairs * kPoseBlocks * 4 * sizeof(int), 1024) +
+         (size_t)rows + 16;
+}
 
-int launch_find_essential(const double* rows, int stride, int n, const double* n_dev, const Intrinsics& K, double px_th,
-                          double conf, int max_iters, unsigned long long seed, void* scratch, double* E_out,
-                          uint8_t* mask_out, int* count_out, cudaStream_t st) {
-  const EssScratch s = carve_ess(scratch, n, kRound);
-  const float th2 = ess_th2(px_th, K);
-  ess_prep_kernel<<<1, 1024, 0, st>>>(rows, stride, n, n_dev, K, s.rows32, s.st);
+int essential_chunk_pairs() {
+  const size_t per_pair = sizeof(EssState) + kPairModels * sizeof(double) + kPairCounts * sizeof(int);
+  return (int)std::min<size_t>(kMaxGridY, std::max<size_t>(1, kBatchScratchBudget / per_pair));
+}
+
+int pose_chunk_pairs() {
+  const size_t per_pair = sizeof(PoseState) + kPoseBlocks * 4 * sizeof(int);
+  return (int)std::min<size_t>(kMaxGridY, std::max<size_t>(1, kBatchScratchBudget / per_pair));
+}
+
+int launch_find_essential(const PairBatch& B, const double* intr, const Intrinsics& K1, double px_th, double conf,
+                          int max_iters, unsigned long long seed, void* scratch, double* E_out, uint8_t* mask_out,
+                          int* count_out, cudaStream_t st) {
+  const EssScratch s = carve_ess(scratch, B.pairs, B.total, kRound);
+  const dim3 one(1, B.pairs);
+  ess_prep_kernel<<<one, 1024, 0, st>>>(B, intr, K1, px_th, s.rows32, s.st);
   P2P_LAUNCH_OK();
   for (int first = 0; first < max_iters; first += kRound) {
     const int count = min(kRound, max_iters - first);
-    ess_round_kernel<<<cdiv(count, kHypPerBlock), kScoreThreads, 0, st>>>(s.st, s.rows32, rows, stride, K, first, count,
-                                                                          seed, th2, 0, s.models, s.counts);
+    ess_round_kernel<<<dim3(cdiv(count, kHypPerBlock), B.pairs), kScoreThreads, 0, st>>>(
+        s.st, s.rows32, B.rows, B.stride, first, count, seed, 0, s.models, s.counts);
     P2P_LAUNCH_OK();
-    ess_select_kernel<<<1, 1024, 0, st>>>(s.st, s.models, s.counts, count * kSlots, first + count, conf, max_iters);
+    ess_select_kernel<<<one, 1024, 0, st>>>(s.st, s.models, s.counts, count * kSlots, first + count, conf, max_iters);
     P2P_LAUNCH_OK();
   }
-  ess_lo_kernel<<<1, kLoThreads, 0, st>>>(s.st, s.rows32, rows, stride, K, n, th2, E_out, mask_out, count_out);
+  ess_lo_kernel<<<one, kLoThreads, 0, st>>>(s.st, s.rows32, B.rows, B.stride, E_out, mask_out, count_out);
   P2P_LAUNCH_OK();
   return 0;
 }
@@ -778,29 +866,31 @@ int launch_find_essential(const double* rows, int stride, int n, const double* n
 int launch_test_essential_hypotheses(const double* rows, int stride, int n, const Intrinsics& K, double px_th,
                                      unsigned long long seed, int count, void* scratch, double* models_out,
                                      int* counts_out, cudaStream_t st) {
-  const EssScratch s = carve_ess(scratch, n, 0);
-  ess_prep_kernel<<<1, 1024, 0, st>>>(rows, stride, n, nullptr, K, s.rows32, s.st);
+  const PairBatch B = single_pair(rows, stride, n, nullptr);
+  const EssScratch s = carve_ess(scratch, 1, n, 0);
+  ess_prep_kernel<<<1, 1024, 0, st>>>(B, nullptr, K, px_th, s.rows32, s.st);
   P2P_LAUNCH_OK();
-  ess_round_kernel<<<cdiv(count, kHypPerBlock), kScoreThreads, 0, st>>>(s.st, s.rows32, rows, stride, K, 0, count, seed,
-                                                                        ess_th2(px_th, K), 1, models_out, counts_out);
+  ess_round_kernel<<<cdiv(count, kHypPerBlock), kScoreThreads, 0, st>>>(s.st, s.rows32, rows, stride, 0, count, seed, 1,
+                                                                        models_out, counts_out);
   P2P_LAUNCH_OK();
   return 0;
 }
 
-int launch_recover_pose(const double* rows, int stride, int n, const double* n_dev, const Intrinsics& K, const double* E,
+int launch_recover_pose(const PairBatch& B, const double* intr, const Intrinsics& K1, const double* E,
                         const uint8_t* mask_in, double dist_th, void* scratch, double* Rt_out, uint8_t* mask_out,
                         int* count_out, cudaStream_t st) {
   char* p = (char*)scratch;
   PoseState* ps = (PoseState*)p;
-  p += 1024;
+  p += align_up((size_t)B.pairs * sizeof(PoseState), 1024);
   int* partial = (int*)p;
-  p += align_up((size_t)kPoseBlocks * 4 * sizeof(int), 1024);
+  p += align_up((size_t)B.pairs * kPoseBlocks * 4 * sizeof(int), 1024);
   uint8_t* codes = (uint8_t*)p;
-  pose_decompose_kernel<<<1, 32, 0, st>>>(E, n, n_dev, ps);
+  pose_decompose_kernel<<<dim3(1, B.pairs), 32, 0, st>>>(B, intr, K1, E, ps);
   P2P_LAUNCH_OK();
-  pose_count_kernel<<<kPoseBlocks, kPoseThreads, 0, st>>>(ps, rows, stride, K, mask_in, dist_th, codes, partial);
+  pose_count_kernel<<<dim3(kPoseBlocks, B.pairs), kPoseThreads, 0, st>>>(ps, B.rows, B.stride, mask_in, dist_th, codes,
+                                                                          partial);
   P2P_LAUNCH_OK();
-  pose_select_kernel<<<1, 1024, 0, st>>>(ps, partial, codes, n, Rt_out, mask_out, count_out);
+  pose_select_kernel<<<dim3(1, B.pairs), 1024, 0, st>>>(ps, partial, codes, Rt_out, mask_out, count_out);
   P2P_LAUNCH_OK();
   return 0;
 }

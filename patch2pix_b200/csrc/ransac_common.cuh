@@ -4,10 +4,23 @@
 #pragma once
 #include <math.h>
 
+#include "kernels.h"
+
 namespace p2p {
 namespace {
 
 constexpr int kMaxDraws = 64;       // draws per sample before it counts as degenerate
+
+// Rows of pair p of a batch: rows offsets[p] .. offsets[p+1]-1 of the row array, or all n1 rows of a single pair.
+struct PairRange {
+  long long row0;
+  int n;
+};
+__device__ __forceinline__ PairRange pair_range(const PairBatch& B, int p) {
+  if (B.offsets == nullptr) return PairRange{0, B.n1};
+  const long long r0 = B.offsets[p];
+  return PairRange{r0, (int)(B.offsets[p + 1] - r0)};
+}
 
 // ---- stateless sample generator: index `draw` of hypothesis `hyp` (restated in oracle/verify_oracle.py) -------------
 __device__ __forceinline__ unsigned long long mix64(unsigned long long z) {   // splitmix64 finaliser

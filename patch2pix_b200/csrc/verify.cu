@@ -9,9 +9,13 @@
 //   verify_select_kernel   (x rounds) best model so far (most inliers, ties to the lowest (hypothesis, root) index) and
 //                                     the stopping bound log(1-conf) / log(1-w^s); later rounds return at once past it
 //   verify_lo_kernel       (1 block)  non-minimal refit on the winner's inliers while the count grows, final mask
-// (verify_common.cuh; model 2, F with the DEGENSAC check, adds its launches in degensac.cu)
+// (verify_common.cuh; model 2, F with the DEGENSAC check, adds its launches in degensac.cu).  A batch of pairs runs the
+// same launches with the pair as grid dimension y: one block per pair for prep / select / LO, cdiv(count, 8) blocks per
+// pair for a round; a pair past its stopping bound returns at once from later rounds.
 // Every reduction runs in a fixed order and no grid size depends on the device, so results are bit-reproducible.
 #include <math.h>
+
+#include <algorithm>
 
 #include "kernels.h"
 #include "verify_common.cuh"
@@ -30,21 +34,22 @@ __global__ void sampson_kernel(const double* __restrict__ rows, int stride, int 
 }
 
 template <int KIND>
-int find_model(const double* rows, int stride, int n, const double* n_dev, double px_th, double conf, int max_iters,
-               unsigned long long seed, void* scratch, double* model_out, uint8_t* mask_out, int* count_out, cudaStream_t st) {
-  const Scratch s = carve(scratch, n, kRound);
+int find_model(const PairBatch& B, double px_th, double conf, int max_iters, unsigned long long seed, void* scratch,
+               double* model_out, uint8_t* mask_out, int* count_out, cudaStream_t st) {
+  const Scratch s = carve(scratch, B.pairs, B.total, kRound);
   const float th2 = (float)(px_th * px_th);
-  verify_prep_kernel<<<1, 1024, 0, st>>>(rows, stride, n, n_dev, Kind<KIND>::kSample, s.rows32, s.st);
+  verify_prep_kernel<<<dim3(1, B.pairs), 1024, 0, st>>>(B, Kind<KIND>::kSample, s.rows32, s.st);
   P2P_LAUNCH_OK();
   for (int first = 0; first < max_iters; first += kRound) {
     const int count = min(kRound, max_iters - first);
-    int rc = enqueue_round<KIND>(s, rows, stride, first, count, seed, th2, 0, st);
+    int rc = enqueue_round<KIND>(s, B, first, count, seed, th2, 0, st);
     if (rc) return rc;
-    verify_select_kernel<<<1, 1024, 0, st>>>(s.st, s.models, s.counts, count * Kind<KIND>::kSlots, first + count,
-                                             Kind<KIND>::kSample, conf, max_iters);
+    verify_select_kernel<<<dim3(1, B.pairs), 1024, 0, st>>>(s.st, s.models, s.counts, count * Kind<KIND>::kSlots,
+                                                            first + count, Kind<KIND>::kSample, conf, max_iters);
     P2P_LAUNCH_OK();
   }
-  verify_lo_kernel<KIND><<<1, kLoThreads, 0, st>>>(s.st, s.rows32, rows, stride, n, th2, model_out, mask_out, count_out);
+  verify_lo_kernel<KIND><<<dim3(1, B.pairs), kLoThreads, 0, st>>>(s.st, s.rows32, B.rows, B.stride, th2, model_out,
+                                                                  mask_out, count_out);
   P2P_LAUNCH_OK();
   return 0;
 }
@@ -52,31 +57,34 @@ int find_model(const double* rows, int stride, int n, const double* n_dev, doubl
 template <int KIND>
 int test_hypotheses(const double* rows, int stride, int n, double px_th, unsigned long long seed, int count, void* scratch,
                     double* models_out, int* counts_out, cudaStream_t st) {
-  Scratch s = carve(scratch, n, 0);
+  const PairBatch B = single_pair(rows, stride, n, nullptr);
+  Scratch s = carve(scratch, 1, n, 0);
   s.models = models_out;
   s.counts = counts_out;
-  verify_prep_kernel<<<1, 1024, 0, st>>>(rows, stride, n, nullptr, Kind<KIND>::kSample, s.rows32, s.st);
+  verify_prep_kernel<<<1, 1024, 0, st>>>(B, Kind<KIND>::kSample, s.rows32, s.st);
   P2P_LAUNCH_OK();
-  return enqueue_round<KIND>(s, rows, stride, 0, count, seed, (float)(px_th * px_th), 1, st);
+  return enqueue_round<KIND>(s, B, 0, count, seed, (float)(px_th * px_th), 1, st);
 }
 
 }  // namespace
 
-size_t verify_scratch_bytes(int n, bool rounds) {
-  return 1024 + align_up((size_t)n * sizeof(float4) + 16, 1024) +
-         (rounds ? align_up((size_t)kRound * 3 * 9 * sizeof(double), 1024) + (size_t)kRound * 3 * sizeof(int) : 0);
+size_t verify_scratch_bytes(int pairs, long long rows, bool rounds) {
+  return align_up((size_t)pairs * sizeof(VerifyState), 1024) + align_up((size_t)rows * sizeof(float4) + 16, 1024) +
+         (rounds ? align_up((size_t)pairs * kPairModels * sizeof(double), 1024) + (size_t)pairs * kPairCounts * sizeof(int)
+                 : 0);
 }
 
-int launch_find_model(int model, const double* rows, int stride, int n, const double* n_dev, double px_th, double conf,
-                      int max_iters, unsigned long long seed, void* scratch, double* model_out, uint8_t* mask_out,
-                      int* count_out, cudaStream_t st) {
+int verify_chunk_pairs() {
+  const size_t per_pair = sizeof(VerifyState) + kPairModels * sizeof(double) + kPairCounts * sizeof(int);
+  return (int)std::min<size_t>(kMaxGridY, std::max<size_t>(1, kBatchScratchBudget / per_pair));
+}
+
+int launch_find_model(int model, const PairBatch& B, double px_th, double conf, int max_iters, unsigned long long seed,
+                      void* scratch, double* model_out, uint8_t* mask_out, int* count_out, cudaStream_t st) {
   if (model == 2)
-    return launch_find_model_degensac(rows, stride, n, n_dev, px_th, conf, max_iters, seed, scratch, model_out, mask_out,
-                               count_out, st);
-  return model == 0 ? find_model<0>(rows, stride, n, n_dev, px_th, conf, max_iters, seed, scratch, model_out, mask_out,
-                                    count_out, st)
-                    : find_model<1>(rows, stride, n, n_dev, px_th, conf, max_iters, seed, scratch, model_out, mask_out,
-                                    count_out, st);
+    return launch_find_model_degensac(B, px_th, conf, max_iters, seed, scratch, model_out, mask_out, count_out, st);
+  return model == 0 ? find_model<0>(B, px_th, conf, max_iters, seed, scratch, model_out, mask_out, count_out, st)
+                    : find_model<1>(B, px_th, conf, max_iters, seed, scratch, model_out, mask_out, count_out, st);
 }
 
 int launch_test_hypotheses(int model, const double* rows, int stride, int n, double px_th, unsigned long long seed,

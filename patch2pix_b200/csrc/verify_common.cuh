@@ -1,6 +1,10 @@
 // RANSAC machinery shared by verify.cu (F / H, models 0 and 1) and degensac.cu (F with the DEGENSAC check, model 2):
 // the state, minimal solvers, scoring, and the prep / round / select / local-optimisation kernels.  Each translation
 // unit instantiates the kernels it launches.  See verify.cu for the launch sequence.
+//
+// Every kernel serves a batch of pairs: pair p is blockIdx.y and owns VerifyState st[p], its rows of the concatenated
+// row array (st[p].row0 ..), its fp32 rows (rows32 + st[p].row32) and its round models / counts (kPairModels /
+// kPairCounts per pair).  A pair's arithmetic does not depend on the other pairs.
 #pragma once
 #include <math.h>
 
@@ -30,7 +34,13 @@ struct VerifyState {
   int stop;                         // no further rounds are needed
   int best_count;                   // 0: no model yet
   int pending;                      // DEGENSAC: this round's records hold an H-degenerate sample
+  int n_all;                        // rows of the pair (mask length)
+  long long row0;                   // first row of the pair in the row array and the mask
+  long long row32;                  // first row of the pair in rows32
 };
+
+constexpr size_t kPairModels = (size_t)kRound * 3 * 9;   // round-model doubles per pair (3 slots per hypothesis)
+constexpr size_t kPairCounts = (size_t)kRound * 3;       // round-count ints per pair
 
 // kScore: which inlier test scores the models.  Kind 2 is DEGENSAC's plane-and-parallax round: F from 2 rows and H.
 template <int KIND> struct Kind;
@@ -191,12 +201,16 @@ __device__ __forceinline__ bool is_inlier(const float* m, float4 r, float th2) {
   return w > 1e-8f && u * u + v * v < th2 * w * w;
 }
 
+// a x + b y + c with the rounding fixed as fma(a, x, b y) + c, so that the result does not depend on how the compiler
+// schedules the products of an expression it also computes elsewhere (DEGENSAC's H x1 in the tests and the models).
+__device__ __forceinline__ double affine2(double a, double b, double c, double x, double y) { return fma(a, x, b * y) + c; }
+
 // fp64 one-sided transfer error of row p under the pixel H below th2 (never with (H x1)_z <= 1e-8): DEGENSAC's plane
 // tests, in the form of the oracle's error so that both take the same decisions.
 __device__ __forceinline__ bool h_inlier64(const double* H, const double* p, double th2) {
-  const double w = H[6] * p[0] + H[7] * p[1] + H[8];
+  const double w = affine2(H[6], H[7], H[8], p[0], p[1]);
   if (!(w > 1e-8)) return false;
-  const double u = (H[0] * p[0] + H[1] * p[1] + H[2]) / w - p[2], v = (H[3] * p[0] + H[4] * p[1] + H[5]) / w - p[3];
+  const double u = affine2(H[0], H[1], H[2], p[0], p[1]) / w - p[2], v = affine2(H[3], H[4], H[5], p[0], p[1]) / w - p[3];
   return u * u + v * v < th2;
 }
 
@@ -235,8 +249,8 @@ __device__ bool parallax_model(const VerifyState& S, const double* rows, int str
   double l[2][3];
   for (int k = 0; k < 2; ++k) {
     const double* r = rows + (size_t)idx[k] * stride;
-    const double hx[3] = {H[0] * r[0] + H[1] * r[1] + H[2], H[3] * r[0] + H[4] * r[1] + H[5],
-                          H[6] * r[0] + H[7] * r[1] + H[8]};
+    const double hx[3] = {affine2(H[0], H[1], H[2], r[0], r[1]), affine2(H[3], H[4], H[5], r[0], r[1]),
+                          affine2(H[6], H[7], H[8], r[0], r[1])};
     const double x2[3] = {r[2], r[3], 1.0};
     cross3(hx, x2, l[k]);
   }
@@ -253,16 +267,20 @@ __device__ bool parallax_model(const VerifyState& S, const double* rows, int str
 }
 
 // ---- kernels ------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(1024) verify_prep_kernel(const double* __restrict__ rows, int stride, int n,
-                                                           const double* __restrict__ n_dev, int min_rows,
-                                                           float4* __restrict__ rows32, VerifyState* __restrict__ st) {
+__global__ void __launch_bounds__(1024) verify_prep_kernel(PairBatch B, int min_rows, float4* __restrict__ rows32_all,
+                                                           VerifyState* __restrict__ st_all) {
   __shared__ double red[33];
   __shared__ int s_n, s_bad;
   const int tid = threadIdx.x;
+  VerifyState* st = st_all + blockIdx.y;
+  const PairRange pr = pair_range(B, blockIdx.y);
+  const int n = pr.n, stride = B.stride;
+  const double* rows = B.rows + pr.row0 * stride;
+  float4* rows32 = rows32_all + (pr.row0 - B.base);
   if (tid == 0) {
     int m = n;
-    if (n_dev != nullptr) {
-      const double v = *n_dev;
+    if (B.n_dev != nullptr) {
+      const double v = B.n_dev[blockIdx.y];
       if (v >= 0.0 && v < (double)n) m = (int)v;
     }
     s_n = m;
@@ -302,25 +320,34 @@ __global__ void __launch_bounds__(1024) verify_prep_kernel(const double* __restr
     st->stop = s_bad || m < min_rows;
     st->best_count = 0;
     st->pending = 0;
+    st->n_all = n;
+    st->row0 = pr.row0;
+    st->row32 = pr.row0 - B.base;
   }
 }
 
 // Hypotheses first .. first + count - 1.  models [count * slots][9] fp64 (pixel coordinates), counts [count * slots]
 // (-1: no model in that slot).
 template <int KIND>
-__global__ void __launch_bounds__(kScoreThreads, 1) verify_round_kernel(const VerifyState* __restrict__ st,
-                                                                     const float4* __restrict__ rows32,
-                                                                     const double* __restrict__ rows, int stride,
+__global__ void __launch_bounds__(kScoreThreads, 1) verify_round_kernel(const VerifyState* __restrict__ st_all,
+                                                                     const float4* __restrict__ rows32_all,
+                                                                     const double* __restrict__ rows_all, int stride,
                                                                      int first, int count, unsigned long long seed,
                                                                      float th2, int ignore_stop, double h_th2,
-                                                                     double* __restrict__ models, int* __restrict__ counts) {
+                                                                     double* __restrict__ models_all,
+                                                                     int* __restrict__ counts_all) {
   constexpr int S = Kind<KIND>::kSample, SL = Kind<KIND>::kSlots, NM = kHypPerBlock * SL;
   __shared__ float4 s_rows[kTile];
   __shared__ float s_model[NM][9];
   __shared__ int s_valid[NM];
+  const VerifyState* st = st_all + blockIdx.y;
   if (KIND == 2 ? !st->pending : !ignore_stop && st->stop) return;
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   const int n = st->n;
+  const double* rows = rows_all + st->row0 * stride;
+  const float4* rows32 = rows32_all + st->row32;
+  double* models = models_all + blockIdx.y * kPairModels;
+  int* counts = counts_all + blockIdx.y * kPairCounts;
   if (tid < kHypPerBlock) {
     const int local = blockIdx.x * kHypPerBlock + tid;
     double out[SL][9];
@@ -393,23 +420,31 @@ __global__ void __launch_bounds__(kScoreThreads, 1) verify_round_kernel(const Ve
 __global__ void __launch_bounds__(1024) verify_select_kernel(VerifyState* __restrict__ st, const double* __restrict__ models,
                                                              const int* __restrict__ counts, int nm, int done, int sample,
                                                              double conf, int max_iters) {
-  select_round(st, models, counts, nm, done, sample, conf, max_iters);
+  select_round(st + blockIdx.y, models + blockIdx.y * kPairModels, counts + blockIdx.y * kPairCounts, nm, done, sample,
+               conf, max_iters);
 }
 
 // Local optimisation + outputs.  Refits on the inliers of the current model in normalised coordinates (F: 8-point with
 // rank-2 enforcement; H: DLT), keeps the refit while it has strictly more inliers, then writes model, mask and count.
+// Pair p writes model_out[9 p ..], count_out[p] and mask_out[row0 .. row0 + n_all).
 template <int KIND>
-__global__ void __launch_bounds__(kLoThreads, 1) verify_lo_kernel(const VerifyState* __restrict__ st,
-                                                               const float4* __restrict__ rows32,
-                                                               const double* __restrict__ rows, int stride, int n_all,
+__global__ void __launch_bounds__(kLoThreads, 1) verify_lo_kernel(const VerifyState* __restrict__ st_all,
+                                                               const float4* __restrict__ rows32_all,
+                                                               const double* __restrict__ rows_all, int stride,
                                                                float th2, double* __restrict__ model_out,
                                                                uint8_t* __restrict__ mask_out, int* __restrict__ count_out) {
   __shared__ double s_red[kLoThreads / 32][45];
   __shared__ double s_cur[9], s_cand[9];
   __shared__ float s_f32[9];
   __shared__ int s_cnt[kLoThreads / 32], s_ok;
+  const VerifyState* st = st_all + blockIdx.y;
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  const int n = st->n, bad = st->bad;
+  const int n = st->n, bad = st->bad, n_all = st->n_all;
+  const double* rows = rows_all + st->row0 * stride;
+  const float4* rows32 = rows32_all + st->row32;
+  model_out += 9 * blockIdx.y;
+  count_out += blockIdx.y;
+  mask_out += st->row0;
   int cur_count = bad ? 0 : st->best_count;
   if (tid < 9) s_cur[tid] = st->best[tid];
   __syncthreads();
@@ -518,25 +553,26 @@ struct Scratch {
   int* counts;
 };
 
-Scratch carve(void* base, int n, int nhyp) {
+// `pairs` states, `rows` fp32 rows, then nhyp hypotheses' models and counts per pair (nhyp = kRound: pair strides
+// kPairModels / kPairCounts).
+Scratch carve(void* base, int pairs, long long rows, int nhyp) {
   char* p = (char*)base;
   Scratch s;
   s.st = (VerifyState*)p;
-  p += 1024;
+  p += align_up((size_t)pairs * sizeof(VerifyState), 1024);
   s.rows32 = (float4*)p;
-  p += align_up((size_t)n * sizeof(float4) + 16, 1024);
+  p += align_up((size_t)rows * sizeof(float4) + 16, 1024);
   s.models = (double*)p;
-  p += align_up((size_t)nhyp * 3 * 9 * sizeof(double), 1024);
+  p += align_up((size_t)pairs * nhyp * 3 * 9 * sizeof(double), 1024);
   s.counts = (int*)p;
   return s;
 }
 
 template <int KIND>
-int enqueue_round(const Scratch& s, const double* rows, int stride, int first, int count, unsigned long long seed, float th2,
+int enqueue_round(const Scratch& s, const PairBatch& B, int first, int count, unsigned long long seed, float th2,
                   int ignore_stop, cudaStream_t st, double h_th2 = 0.0) {
-  verify_round_kernel<KIND><<<cdiv(count, kHypPerBlock), kScoreThreads, 0, st>>>(s.st, s.rows32, rows, stride, first, count,
-                                                                                 seed, th2, ignore_stop, h_th2, s.models,
-                                                                                 s.counts);
+  verify_round_kernel<KIND><<<dim3(cdiv(count, kHypPerBlock), B.pairs), kScoreThreads, 0, st>>>(
+      s.st, s.rows32, B.rows, B.stride, first, count, seed, th2, ignore_stop, h_th2, s.models, s.counts);
   P2P_LAUNCH_OK();
   return 0;
 }

@@ -255,3 +255,224 @@ def first_essential_hypotheses(pts1, pts2, K1, K2, px_th, count, seed=0):
                                                        float(px_th), int(seed) & (2 ** 64 - 1), count, _lib.ptr(models),
                                                        _lib.ptr(counts), h.stream()))
     return models.cpu().numpy(), counts.cpu().numpy()
+
+
+# ---- many pairs per call (p2p_find_essential_batch, p2p_recover_pose_batch) ------------------------------------------
+def _intr_rows(K1_list, K2_list, K, reference=False):
+    """Validated [K, 8] intrinsics (as intrinsics() / reference_intrinsics()) of K pairs, on the host."""
+    from .verify import _as_list
+    K1_list, K2_list = _as_list(K1_list, 'K1_list'), _as_list(K2_list, 'K2_list')
+    if len(K1_list) != K or len(K2_list) != K:
+        raise ValueError(f'K1_list and K2_list must have one matrix per pair ({K}), got {len(K1_list)} and '
+                         f'{len(K2_list)}')
+    out = np.empty((K, 8), dtype=np.float64)
+    for k in range(K):
+        try:
+            out[k] = (reference_intrinsics if reference else intrinsics)(K1_list[k], K2_list[k])
+        except ValueError as e:
+            raise ValueError(f'pair {k}: intrinsics must be 3x3: {e}') from None
+        if not (np.all(np.isfinite(out[k])) and out[k, [0, 1, 4, 5]].min() > 0):
+            raise ValueError(f'pair {k}: intrinsics must be finite with positive focal lengths')
+    return out
+
+
+def batch_out_size(K, N):
+    """float64 elements of a pose batch buffer: E [0:9K], R|t [9K:21K], int32 inlier and good counts [2K] from element
+    21K, then the row-aligned E-RANSAC mask and the row-aligned pose mask."""
+    return 22 * K + (2 * N + 7) // 8
+
+
+def _batch_ptrs(out, K, N):
+    base = out.data_ptr()
+    return dict(E=base, Rt=base + 72 * K, cnt=base + 168 * K, good=base + 172 * K, emask=base + 176 * K,
+                pmask=base + 176 * K + N)
+
+
+def find_essential_batch_into(handle, rows, row_stride, offsets, offsets_host, n_dev, intr_ptr, px_th, conf, max_iters,
+                              seed, E_ptr, mask_ptr, counts_ptr):
+    """Enqueue p2p_find_essential_batch (device addresses as verify.find_model_batch_into; intr_ptr: [K][8] doubles)."""
+    oh = np.ascontiguousarray(offsets_host, dtype=np.int64)
+    with torch.cuda.device(rows.device):
+        _lib.check(handle.lib.p2p_find_essential_batch(
+            handle.h, C.c_void_p(rows.data_ptr()), row_stride, C.c_void_p(offsets.data_ptr()),
+            oh.ctypes.data_as(C.POINTER(C.c_int64)), oh.size - 1, n_dev, C.c_void_p(intr_ptr), float(px_th), float(conf),
+            int(max_iters), int(seed) & (2 ** 64 - 1), C.c_void_p(E_ptr), C.c_void_p(mask_ptr), C.c_void_p(counts_ptr),
+            handle.stream()))
+
+
+def recover_pose_batch_into(handle, rows, row_stride, offsets, offsets_host, n_dev, intr_ptr, E_ptr, mask_in_ptr, Rt_ptr,
+                            mask_ptr, good_ptr, dist_th=DIST_TH):
+    """Enqueue p2p_recover_pose_batch (device addresses; mask_in_ptr None: all rows)."""
+    oh = np.ascontiguousarray(offsets_host, dtype=np.int64)
+    with torch.cuda.device(rows.device):
+        _lib.check(handle.lib.p2p_recover_pose_batch(
+            handle.h, C.c_void_p(rows.data_ptr()), row_stride, C.c_void_p(offsets.data_ptr()),
+            oh.ctypes.data_as(C.POINTER(C.c_int64)), oh.size - 1, n_dev, C.c_void_p(intr_ptr), C.c_void_p(E_ptr),
+            None if mask_in_ptr is None else C.c_void_p(mask_in_ptr), float(dist_th), C.c_void_p(Rt_ptr),
+            C.c_void_p(mask_ptr), C.c_void_p(good_ptr), handle.stream()))
+
+
+def _parse_batch(host, offsets, K, N):
+    """Per pair (E or None, E mask, n_good, R, t, pose mask) of a host pose batch buffer; raises on non-finite input."""
+    cnt = host[21 * K:22 * K].view(np.int32)
+    b = host[22 * K:].view(np.uint8)
+    out = []
+    for k in range(K):
+        if cnt[k] < 0:
+            raise ValueError(f'find_essential: a point coordinate is not finite (pair {k})')
+        o0, o1 = offsets[k], offsets[k + 1]
+        Rt = host[9 * K + 12 * k:9 * K + 12 * k + 12]
+        out.append((host[9 * k:9 * k + 9].reshape(3, 3).copy() if cnt[k] > 0 else None, b[o0:o1].astype(bool),
+                    int(cnt[K + k]), Rt[:9].reshape(3, 3).copy(), Rt[9:].reshape(3, 1).copy(),
+                    b[N + o0:N + o1].astype(bool)))
+    return out
+
+
+def find_essential_matrices(pts1_list, pts2_list, K1_list, K2_list, px_th, conf=0.999, max_iters=1000, seed=0):
+    """find_essential_matrix over a list of pairs in one batched call -> [(E, inlier mask)], element k equal to
+    find_essential_matrix(pts1_list[k], pts2_list[k], K1_list[k], K2_list[k], ...).  Numpy input crosses PCIe once
+    each way and raises ValueError when a pair has a non-finite coordinate; CUDA tensor input gives CUDA tensor views
+    without a sync."""
+    from .verify import pair_lists, upload
+    rows, offsets, is_np = pair_lists(pts1_list, pts2_list)
+    K, N = offsets.size - 1, int(offsets[-1])
+    intr = _intr_rows(K1_list, K2_list, K)
+    if K == 0:
+        return []
+    rows, offs, intr_d = upload(rows, offsets, is_np, intr)
+    out = torch.zeros(batch_out_size(K, N), dtype=torch.float64, device=rows.device)
+    p = _batch_ptrs(out, K, N)
+    find_essential_batch_into(_lib.default_handle(rows.device), rows, 4, offs, offsets, None, intr_d.data_ptr(), px_th,
+                              conf, max_iters, seed, p['E'], p['emask'], p['cnt'])
+    if is_np:
+        return [r[:2] for r in _parse_batch(out.cpu().numpy(), offsets, K, N)]
+    m = out[22 * K:].view(torch.uint8)
+    return [(out[9 * k:9 * k + 9].view(3, 3), m[offsets[k]:offsets[k + 1]].bool()) for k in range(K)]
+
+
+def recover_poses(E_list, pts1_list, pts2_list, K1_list, K2_list, mask_list=None, dist_th=DIST_TH):
+    """recover_pose over a list of pairs in one batched call -> [(n_good, R, t [3, 1], good mask)], element k equal to
+    recover_pose(E_list[k], pts1_list[k], pts2_list[k], K1_list[k], K2_list[k], mask_list[k], dist_th).  mask_list:
+    None, or one mask (or None) per pair."""
+    from .verify import _as_list, pair_lists, upload
+    rows, offsets, is_np = pair_lists(pts1_list, pts2_list)
+    K, N = offsets.size - 1, int(offsets[-1])
+    E_list = _as_list(E_list, 'E_list')
+    if len(E_list) != K:
+        raise ValueError(f'E_list must have one matrix per pair ({K}), got {len(E_list)}')
+    intr = _intr_rows(K1_list, K2_list, K)
+    for k, E in enumerate(E_list):
+        if (E.numel() if isinstance(E, torch.Tensor) else np.size(E)) != 9:
+            raise ValueError(f'pair {k}: E must be 3x3')
+    if mask_list is not None:
+        mask_list = _as_list(mask_list, 'mask_list')
+        if len(mask_list) != K:
+            raise ValueError(f'mask_list must have one mask (or None) per pair ({K}), got {len(mask_list)}')
+        for k, m in enumerate(mask_list):
+            if m is not None and (m.numel() if isinstance(m, torch.Tensor) else np.size(m)) != offsets[k + 1] - offsets[k]:
+                raise ValueError(f'pair {k}: mask has {np.size(m) if not isinstance(m, torch.Tensor) else m.numel()} '
+                                 f'entries for {offsets[k + 1] - offsets[k]} points')
+    if K == 0:
+        return []
+    if is_np:          # E and masks travel with the rows
+        Es = np.stack([np.asarray(E, dtype=np.float64).reshape(9) for E in E_list])
+        masks = None if mask_list is None else np.concatenate(
+            [np.ones(offsets[k + 1] - offsets[k]) if m is None else (np.asarray(m).reshape(-1) != 0)
+             for k, m in enumerate(mask_list)]).astype(np.float64)
+        extra = np.concatenate((intr.reshape(-1), Es.reshape(-1)) + (() if masks is None else (masks,)))
+        rows, offs, ex = upload(rows, offsets, is_np, extra)
+        Ed = ex[8 * K:17 * K]
+        md = None if masks is None else ex[17 * K:].to(torch.uint8)
+    else:
+        rows, offs, ex = upload(rows, offsets, is_np, intr)
+        Ed = torch.stack([torch.as_tensor(E, dtype=torch.float64).reshape(9).to(rows.device) for E in E_list])
+        md = None if mask_list is None else torch.cat(
+            [torch.ones(int(offsets[k + 1] - offsets[k]), dtype=torch.uint8, device=rows.device) if m is None else
+             (torch.as_tensor(m).reshape(-1) != 0).to(torch.uint8).to(rows.device) for k, m in enumerate(mask_list)])
+    dev = rows.device
+    out = torch.zeros(batch_out_size(K, N), dtype=torch.float64, device=dev)
+    p = _batch_ptrs(out, K, N)
+    recover_pose_batch_into(_lib.default_handle(dev), rows, 4, offs, offsets, None, ex.data_ptr(), Ed.data_ptr(),
+                            None if md is None else md.data_ptr(), p['Rt'], p['pmask'], p['good'], dist_th)
+    if is_np:
+        return [r[2:] for r in _parse_batch(out.cpu().numpy(), offsets, K, N)]
+    cnt = out[21 * K:22 * K].view(torch.int32)
+    m = out[22 * K:].view(torch.uint8)
+    return [(cnt[K + k], out[9 * K + 12 * k:9 * K + 12 * k + 9].view(3, 3),
+             out[9 * K + 12 * k + 9:9 * K + 12 * k + 12].view(3, 1), m[N + offsets[k]:N + offsets[k + 1]].bool())
+            for k in range(K)]
+
+
+def _match_lists(matches_list):
+    from .verify import _as_list
+    ms = [np.asarray(m, dtype=np.float64) for m in _as_list(matches_list, 'matches_list')]
+    for k, m in enumerate(ms):
+        if m.ndim != 2 or m.shape[1] < 4:
+            raise ValueError(f'pair {k}: matches must be [n, 4] (x1, y1, x2, y2), got {m.shape}')
+    return [m[:, :2] for m in ms], [m[:, 2:4] for m in ms]
+
+
+def matches2relapose_batch(matches_list, K1_list, K2_list, rthres=1):
+    """matches2relapose over a list of pairs: one E-RANSAC launch chain and one pose-recovery chain for every pair ->
+    [(E, inls, R, t)], element k equal to matches2relapose(m[:, :2], m[:, 2:4], K1_list[k], K2_list[k], rthres) for
+    m = matches_list[k].  One host->device and one device->host copy."""
+    from .verify import pair_lists, upload
+    p1, p2 = _match_lists(matches_list)
+    rows, offsets, _ = pair_lists(p1, p2)
+    K, N = offsets.size - 1, int(offsets[-1])
+    intr = _intr_rows(K1_list, K2_list, K, reference=True)
+    if K == 0:
+        return []
+    rows, offs, intr_d = upload(rows, offsets, True, intr)
+    h = _lib.default_handle(rows.device)
+    out = torch.zeros(batch_out_size(K, N), dtype=torch.float64, device=rows.device)
+    p = _batch_ptrs(out, K, N)
+    find_essential_batch_into(h, rows, 4, offs, offsets, None, intr_d.data_ptr(), rthres, 0.999, 1000, 0, p['E'],
+                              p['emask'], p['cnt'])
+    recover_pose_batch_into(h, rows, 4, offs, offsets, None, intr_d.data_ptr(), p['E'], p['emask'], p['Rt'], p['pmask'],
+                            p['good'])
+    return [(E, np.where(em)[0], R, t) for E, em, _, R, t, _ in _parse_batch(out.cpu().numpy(), offsets, K, N)]
+
+
+def matches2relapose_degensac_batch(matches_list, K1_list, K2_list, rthres=1):
+    """matches2relapose_degensac over a list of pairs -> [(E, inls, R, t)], element k equal to
+    matches2relapose_degensac(m[:, :2], m[:, 2:4], K1_list[k], K2_list[k], rthres) for m = matches_list[k]: the rows
+    rescaled per pair as the reference does, one DEGENSAC launch chain and one pose-recovery chain for every pair.  One
+    host->device and one device->host copy."""
+    from . import verify as V
+    p1, p2 = _match_lists(matches_list)
+    rows, offsets, _ = V.pair_lists(p1, p2)
+    K, N = offsets.size - 1, int(offsets[-1])
+    ref = _intr_rows(K1_list, K2_list, K, reference=True)          # f1, f1, cx1, cy1, f2, f2, cx2, cy2
+    if K == 0:
+        return []
+    f1, f2 = ref[:, 0], ref[:, 4]
+    # per pair: rescale (pc1 x2, f2, 1 / f1, pc2 x2), intr (f2, f2, 0, 0) x2, k = (f2, f2, 1)
+    z = np.zeros(K)
+    per_pair = np.stack((ref[:, 2], ref[:, 3], f2, 1.0 / f1, ref[:, 6], ref[:, 7]), 1)
+    intr = np.stack((f2, f2, z, z, f2, f2, z, z), 1)
+    kk = np.stack((f2, f2, np.ones(K)), 1)
+    rows, offs, ex = V.upload(rows, offsets, True, np.concatenate((per_pair.ravel(), intr.ravel(), kk.ravel())))
+    dev = rows.device
+    pp = ex[:6 * K].view(K, 6).repeat_interleave(torch.from_numpy(np.diff(offsets)).to(dev), dim=0)
+    # as matches2relapose_degensac: ((p1 - pc1) * f2) / f1 (a division by a host scalar runs as a multiplication by
+    # its reciprocal on the device), p2 - pc2
+    rows = torch.cat((((rows[:, 0:2] - pp[:, 0:2]) * pp[:, 2:3]) * pp[:, 3:4], rows[:, 2:4] - pp[:, 4:6]), 1).contiguous()
+    intr_d, k = ex[6 * K:14 * K], ex[14 * K:].view(K, 3)
+    h = _lib.default_handle(dev)
+    out = torch.zeros(batch_out_size(K, N) + V.batch_out_size(K, N), dtype=torch.float64, device=dev)
+    fout = out[batch_out_size(K, N):]
+    p, fb = _batch_ptrs(out, K, N), fout.data_ptr()
+    V.find_model_batch_into(h, V.MODEL_F_DEGENSAC, rows, 4, offs, offsets, None, rthres, 0.999, 10000, 0, fb,
+                            fb + 8 * (9 * K + (K + 1) // 2), fb + 72 * K)
+    out[:9 * K] = ((fout[:9 * K].view(K, 3, 3) * k[:, :, None]) * k[:, None, :]).reshape(-1)      # K^T F K per pair
+    recover_pose_batch_into(h, rows, 4, offs, offsets, None, intr_d.data_ptr(), p['E'],
+                            fb + 8 * (9 * K + (K + 1) // 2), p['Rt'], p['pmask'], p['good'])
+    host = out.cpu().numpy()
+    fres = V.parse_batch_host(host[batch_out_size(K, N):], offsets)
+    res = []
+    for k, (F, fmask) in enumerate(fres):
+        Rt = host[9 * K + 12 * k:9 * K + 12 * k + 12]
+        res.append((host[9 * k:9 * k + 9].reshape(3, 3).copy() if F is not None else None, np.where(fmask)[0],
+                    Rt[:9].reshape(3, 3).copy(), Rt[9:].reshape(3, 1).copy()))
+    return res

@@ -163,3 +163,138 @@ def first_degeneracy(pts1, pts2, px_th, count, seed=0):
         _lib.check(h.lib.p2p_test_degeneracy(h.h, _lib.ptr(rows), 4, int(rows.shape[0]), float(px_th),
                                              int(seed) & (2 ** 64 - 1), count, _lib.ptr(tri), _lib.ptr(H), h.stream()))
     return tri.cpu().numpy(), H.cpu().numpy()
+
+
+# ---- many pairs per call (p2p_find_model_batch) ----------------------------------------------------------------------
+def _as_list(x, name):
+    if isinstance(x, (np.ndarray, torch.Tensor)) or not hasattr(x, '__len__'):
+        raise TypeError(f'{name} must be a list of per-pair arrays')
+    return list(x)
+
+
+def pair_lists(pts1_list, pts2_list):
+    """Validate a batch of point-list pairs before any device work -> (per-pair [n, 4] rows (numpy float64 arrays, or
+    CUDA tensors of the caller's dtype), offsets int64 [K+1] on the host, whether the input was numpy)."""
+    pts1_list, pts2_list = _as_list(pts1_list, 'pts1_list'), _as_list(pts2_list, 'pts2_list')
+    if len(pts1_list) != len(pts2_list):
+        raise ValueError(f'pts1_list and pts2_list must have the same length, got {len(pts1_list)} and '
+                         f'{len(pts2_list)}')
+    kinds = {isinstance(p, torch.Tensor) for p in pts1_list + pts2_list}
+    if len(kinds) > 1:
+        raise TypeError('the point lists must all be numpy arrays or all be tensors')
+    is_np = not kinds or kinds == {False}
+    rows = []
+    for k, (p1, p2) in enumerate(zip(pts1_list, pts2_list)):
+        if is_np:
+            a = np.asarray(p1, dtype=np.float64).reshape(-1, 2)
+            b = np.asarray(p2, dtype=np.float64).reshape(-1, 2)
+            if a.shape != b.shape:
+                raise ValueError(f'pair {k}: pts1 and pts2 must have the same number of points, got {a.shape[0]} and '
+                                 f'{b.shape[0]}')
+            rows.append(np.concatenate((a, b), 1))
+        else:
+            if p1.device.type != 'cuda' or p2.device != p1.device or p1.device != pts1_list[0].device:
+                raise ValueError('tensor input must be on one CUDA device')
+            if p1.dim() != 2 or p1.shape[1] != 2 or p2.shape != p1.shape:
+                raise ValueError(f'pair {k}: pts1 and pts2 must both be [n, 2], got {tuple(p1.shape)} and '
+                                 f'{tuple(p2.shape)}')
+            rows.append((p1, p2))
+    offsets = np.zeros(len(rows) + 1, dtype=np.int64)
+    offsets[1:] = np.cumsum([r.shape[0] if is_np else r[0].shape[0] for r in rows])
+    if np.any(np.diff(offsets) > 1 << 26) or offsets[-1] >= 1 << 31:
+        raise ValueError('a pair has more than 2^26 rows or the batch has 2^31 rows or more')
+    return rows, offsets, is_np
+
+
+def upload(rows, offsets, is_np, extra=None, device=None):
+    """(rows [N, 4] float64, offsets int64 [K+1], extra float64 [...] or None) on the device.  Numpy input crosses PCIe
+    in one copy; tensor input is concatenated on its device (the offsets and `extra`, host arrays, are copied)."""
+    extra = None if extra is None else np.ascontiguousarray(extra, dtype=np.float64).reshape(-1)
+    n_ex = 0 if extra is None else extra.size
+    N, K1 = int(offsets[-1]), offsets.size
+    if is_np:
+        dev = device or torch.device('cuda', torch.cuda.current_device())
+        host = np.empty(4 * N + K1 + n_ex, dtype=np.float64)
+        if N:
+            host[:4 * N] = np.concatenate(rows, 0).reshape(-1)
+        host[4 * N:4 * N + K1] = offsets.view(np.float64)
+        if n_ex:
+            host[4 * N + K1:] = extra
+        d = torch.from_numpy(host).to(dev)
+        return (d[:4 * N].view(N, 4), d[4 * N:4 * N + K1].view(torch.int64),
+                None if extra is None else d[4 * N + K1:])
+    dev = rows[0][0].device
+    r = torch.cat([torch.cat(p, 1).to(torch.float64) for p in rows]).contiguous()
+    tail = np.concatenate((offsets.view(np.float64), extra if n_ex else np.empty(0)))
+    d = torch.from_numpy(tail).to(dev)
+    return r, d[:K1].view(torch.int64), None if extra is None else d[K1:]
+
+
+def find_model_batch_into(handle, model, rows, row_stride, offsets, offsets_host, n_dev, px_th, conf, max_iters, seed,
+                          models_ptr, mask_ptr, counts_ptr):
+    """Enqueue p2p_find_model_batch: `rows` a float64 device tensor, `offsets` an int64 device tensor [K+1] and
+    `offsets_host` the same values in numpy; the outputs are device addresses (models [K][9] float64, row-aligned uint8
+    mask, int32 counts [K]); `n_dev` an optional device address of K doubles."""
+    oh = np.ascontiguousarray(offsets_host, dtype=np.int64)
+    with torch.cuda.device(rows.device):
+        _lib.check(handle.lib.p2p_find_model_batch(
+            handle.h, model, C.c_void_p(rows.data_ptr()), row_stride, C.c_void_p(offsets.data_ptr()),
+            oh.ctypes.data_as(C.POINTER(C.c_int64)), oh.size - 1, n_dev, float(px_th), float(conf), int(max_iters),
+            int(seed) & (2 ** 64 - 1), C.c_void_p(models_ptr), C.c_void_p(mask_ptr), C.c_void_p(counts_ptr),
+            handle.stream()))
+
+
+def batch_out_size(K, N):
+    """float64 elements of a batch buffer: models [0:9K], int32 counts from element 9K, the uint8 mask after them."""
+    return 9 * K + (K + 1) // 2 + (N + 7) // 8
+
+
+def parse_batch_host(host, offsets, what='find_model'):
+    """[(model or None, bool mask)] from the host copy of a batch buffer; raises on a pair with non-finite input."""
+    K = offsets.size - 1
+    counts = host[9 * K:9 * K + (K + 1) // 2].view(np.int32)[:K]
+    masks = host[9 * K + (K + 1) // 2:].view(np.uint8)
+    out = []
+    for k in range(K):
+        if counts[k] < 0:
+            raise ValueError(f'{what}: a point coordinate is not finite (pair {k})')
+        out.append((host[9 * k:9 * k + 9].reshape(3, 3).copy() if counts[k] > 0 else None,
+                    masks[offsets[k]:offsets[k + 1]].astype(bool)))
+    return out
+
+
+def _find_batch(model, pts1_list, pts2_list, px_th, conf, max_iters, seed):
+    rows, offsets, is_np = pair_lists(pts1_list, pts2_list)
+    K, N = offsets.size - 1, int(offsets[-1])
+    if K == 0:
+        return []
+    rows, offs, _ = upload(rows, offsets, is_np)
+    out = torch.empty(batch_out_size(K, N), dtype=torch.float64, device=rows.device)
+    base = out.data_ptr()
+    find_model_batch_into(_lib.default_handle(rows.device), model, rows, 4, offs, offsets, None, px_th, conf, max_iters,
+                          seed, base, base + 8 * (9 * K + (K + 1) // 2), base + 72 * K)
+    if is_np:
+        return parse_batch_host(out.cpu().numpy(), offsets)
+    mask = out[9 * K + (K + 1) // 2:].view(torch.uint8)
+    return [(out[9 * k:9 * k + 9].view(3, 3), mask[offsets[k]:offsets[k + 1]].bool()) for k in range(K)]
+
+
+def find_fundamental_matrices(pts1_list, pts2_list, px_th, conf=0.999, max_iters=10000, seed=0, degeneracy_check=False):
+    """find_fundamental_matrix over a list of pairs in one batched call -> [(F, inlier mask)], element k equal to
+    find_fundamental_matrix(pts1_list[k], pts2_list[k], ...).  Numpy input crosses PCIe once each way and raises
+    ValueError when a pair has a non-finite coordinate; CUDA tensor input gives CUDA tensor views without a sync."""
+    return _find_batch(MODEL_F_DEGENSAC if degeneracy_check else MODEL_F, pts1_list, pts2_list, px_th, conf, max_iters,
+                       seed)
+
+
+def find_homographies(pts1_list, pts2_list, px_th, conf=0.999, max_iters=10000, seed=0):
+    """find_homography over a list of pairs in one batched call -> [(H, inlier mask)] (as find_fundamental_matrices)."""
+    return _find_batch(MODEL_H, pts1_list, pts2_list, px_th, conf, max_iters, seed)
+
+
+def batch_chunk_pairs(entry, device=None):
+    """Pairs per launch of a batched entry point (0 find_model, 1 find_essential, 2 recover_pose)."""
+    h = _lib.default_handle(device or torch.device('cuda', torch.cuda.current_device()))
+    v = C.c_int()
+    _lib.check(h.lib.p2p_batch_chunk_pairs(h.h, int(entry), C.byref(v)))
+    return v.value
