@@ -84,7 +84,11 @@ P2P_API int p2p_set_regressor_weights(p2p_handle_t h, int which, const p2p_regre
  * "nc_l2_mode" (layout of NC layer 2's block of hidden lines: 0 = chosen per shape, 1 = one haloed block per tile,
  * 2 = one block per column tap; bit-identical results), "unique_impl" (default 1: rank sort over the whole GPU for lists of
  * up to 8192 rows; 0: single-block bitonic network; identical results), "fc_impl" (default 1: the 512-512 and 512-256 Linear layers run on
- * the tensor cores, 3-pass; 0: fp32 CUDA-core FC kernel). */
+ * the tensor cores, 3-pass; 0: fp32 CUDA-core FC kernel), "share_windows" (default 1: in the mid stage's window-map
+ * 1-pass conv1, a half-group of 4 rows (rows 8g..8g+3 on image 2, 8g+4..8g+7 on image 1) with equal window origins
+ * computes that image's half of conv1 once; shared rows differ from 0 by one reordering of an fp32 sum, all other rows
+ * are bit-identical; 0: every row's whole conv1).  p2p_get_option also reads "shared_rows": the rows that shared a
+ * window half in the last mid-stage call (synchronises). */
 P2P_API int p2p_set_option(p2p_handle_t h, const char* key, int value);
 P2P_API int p2p_get_option(p2p_handle_t h, const char* key, int* value);
 /* Number of kernel launches enqueued by this handle since creation (bench.py's gpu_launches). */

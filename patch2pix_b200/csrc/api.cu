@@ -92,7 +92,11 @@ struct p2p_handle_s {
   int opt_fuse_gather = 3;  // conv1 A operand of the 1-pass launches: 3 (default): strided TMA boxes of a per-image window map
                             // (AMODE_WINDOW); 1 or 2: gathered by producer warps (AMODE_GATHER); 0: separate gather kernel +
                             // TMA of the patch tensor
+  int opt_share_windows = 1;  // mid stage, fuse_gather = 3, 1-pass: compute the conv1 half of an anchor window that a
+                              // half-group of 4 rows shares once (1, default), or every row's whole conv1 (0)
   const int* last_band_count = nullptr;  // device counter of the last risk-band subset
+  int* share_rows = nullptr;             // device: rows that shared a window half in the last sharing mid-stage call
+  bool last_mid_shared = false;          // the last mid-stage call shared windows (share_rows is its count)
   unsigned long long* band_totals = nullptr;   // device: {band rows, rows} summed over mid-stage calls
   bool nc_set = false;
   float *nc_w1p = nullptr, *nc_b1p = nullptr, *nc_w2p = nullptr;
@@ -402,6 +406,10 @@ int p2p_create(int device, p2p_handle_t* out) {
       cudaMemset(h->band_totals, 0, 2 * sizeof(unsigned long long));
     else
       h->band_totals = nullptr;
+    if (cudaMalloc(&h->share_rows, sizeof(int)) == cudaSuccess)
+      cudaMemset(h->share_rows, 0, sizeof(int));
+    else
+      h->share_rows = nullptr;
   }
   *out = h;
   return 0;
@@ -425,6 +433,7 @@ int p2p_destroy(p2p_handle_t h) {
   if (h->nc_w1p) cudaFree(h->nc_w1p);
   if (h->ncw.blob) cudaFree(h->ncw.blob);
   if (h->band_totals) cudaFree(h->band_totals);
+  if (h->share_rows) cudaFree(h->share_rows);
   if (h->uniq_rank) cudaFree(h->uniq_rank);
   for (int i = 0; i < 2; ++i)
     if (h->reg[i].blob) cudaFree(h->reg[i].blob);
@@ -484,6 +493,7 @@ static int* option_slot(p2p_handle_t h, const char* key) {
   if (!strcmp(key, "profile")) return &h->opt_profile;
   if (!strcmp(key, "mid_band")) return &h->opt_mid_band;
   if (!strcmp(key, "fuse_gather")) return &h->opt_fuse_gather;
+  if (!strcmp(key, "share_windows")) return &h->opt_share_windows;
   if (!strcmp(key, "fc_impl")) return &h->opt_fc_impl;
   if (!strcmp(key, "nc_impl")) return &h->opt_nc_impl;
   if (!strcmp(key, "nc_l2_mode")) return &h->opt_nc_l2_mode;
@@ -497,6 +507,7 @@ int p2p_set_option(p2p_handle_t h, const char* key, int value) {
   P2P_REQUIRE(s != nullptr, std::string("unknown option ") + key);
   if (s == &h->opt_mid_passes || s == &h->opt_fine_passes) P2P_REQUIRE(value == 1 || value == 3, "passes must be 1 or 3");
   if (s == &h->opt_corr_passes) P2P_REQUIRE(value == 0 || value == 1 || value == 3, "corr_passes must be 0, 1 or 3");
+  if (s == &h->opt_share_windows) P2P_REQUIRE(value == 0 || value == 1, "share_windows must be 0 or 1");
   P2P_REQUIRE(value >= 0, "option values are non-negative");
   *s = value;
   return 0;
@@ -510,6 +521,15 @@ int p2p_get_option(p2p_handle_t h, const char* key, int* value) {
       DeviceGuard g(h->device);
       P2P_CUDA_OK(cudaDeviceSynchronize());
       P2P_CUDA_OK(cudaMemcpy(value, h->last_band_count, sizeof(int), cudaMemcpyDeviceToHost));
+    }
+    return 0;
+  }
+  if (!strcmp(key, "shared_rows")) {  // rows whose conv1 shared a window half in the last mid-stage call (synchronises)
+    *value = 0;
+    if (h->last_mid_shared && h->share_rows != nullptr) {
+      DeviceGuard g(h->device);
+      P2P_CUDA_OK(cudaDeviceSynchronize());
+      P2P_CUDA_OK(cudaMemcpy(value, h->share_rows, sizeof(int), cudaMemcpyDeviceToHost));
     }
     return 0;
   }
@@ -889,8 +909,19 @@ struct RefineBuffers {
   __half *q_hi, *q_lo, *h1_hi, *h1_lo, *h2_hi, *h2_lo;   // tensor-core FC operands, rows padded to 128
   float *pooled, *raw;
   int *rowmap, *d_count;
+  int *sh_prefix, *sh_cont, *sh_unsh, *sh_cnt;   // launch_window_share_classify's lists and counts
+  float* part;                                    // share_windows: fp32 partial sums of the prefix launch
+  __half* r_unsh;                                 // share_windows: rgb im2col rows of the unshared rows
   int npad;
 };
+
+// The 36 conv1 k-steps of image si's window map (chunks 4 si .. 4 si + 3 of every tap), in tap-major order.
+int image_steps(const Regressor& R, int si, KStep* out) {
+  int k = 0;
+  for (int s = 0; s < 72; ++s)
+    if ((R.steps1[s].c0 >> 6) >> 2 == si) out[k++] = R.steps1[s];
+  return k;
+}
 
 // gather -> conv1 -> conv2 -> fc/parse for the rows selected by (rowmap, d_count) [all rows if null]
 int run_regressor(p2p_handle_s* h, Regressor& R, int which, int passes, const RefineBuffers& B, const void* matches_in,
@@ -903,6 +934,11 @@ int run_regressor(p2p_handle_s* h, Regressor& R, int which, int passes, const Re
   const bool fused = passes == 1 && rowmap == nullptr && h->opt_fuse_gather && h->opt_gemm_impl == 0 && !mapped;
   if (mapped) P2P_REQUIRE(h->pf[0].wmap != nullptr && h->pf[1].wmap != nullptr,
                           "fuse_gather = 3 needs p2p_refine_prepare to have run with the same option");
+  // Mid-stage anchor groups (shift_to_anchors): rows 8g..8g+3 share image 2's window, rows 8g+4..8g+7 image 1's.  conv1
+  // is linear in its input channels, so a shared window's 36 k-steps run once per half-group (prefix launch) and each
+  // row adds that partial sum to its own 37 (continuation launch); the other rows run all 73 k-steps as before.
+  const bool share = mapped && which == 0 && h->opt_share_windows;
+  if (which == 0 && rowmap == nullptr) h->last_mid_shared = share;
   if (!fused && !mapped) {
     ProfScope ps(h, kb, st);
     if ((rc = launch_patch_gather(h->pf[0], h->pf[1], matches_in, is_float, n, B.p_hi, lo ? B.p_lo : nullptr, B.r_hi,
@@ -979,13 +1015,54 @@ int run_regressor(p2p_handle_s* h, Regressor& R, int which, int passes, const Re
         }
         p.wm.matches = matches_in;
         p.wm.is_float = is_float;
-        // the rgb k-step's A operand (r_hi, read through a_rgb_hi); the main k-steps read the window maps directly
+        // the rgb k-step's A operand (r_hi, read through a_rgb_hi); the main k-steps read the window maps directly.
+        // Shared: the rows are classified first; r_hi holds the continuation order, r_unsh the unshared rows' order.
         ProfScope ps(h, kb, st);
-        if ((rc = launch_window_rgb(p.wm, n, B.npad, B.r_hi, st))) return rc;
+        if (share) {
+          P2P_REQUIRE(B.part != nullptr && B.r_unsh != nullptr, "share_windows: buffers not carved");
+          if ((rc = launch_window_share_classify(p.wm, n, B.sh_prefix, B.sh_cont, B.sh_unsh, B.sh_cnt, h->share_rows, st)))
+            return rc;
+          if ((rc = launch_window_rgb(p.wm, n, B.npad, B.r_hi, st, B.sh_cont, B.sh_cnt + 3))) return rc;
+          if ((rc = launch_window_rgb(p.wm, n, B.npad, B.r_unsh, st, B.sh_unsh, B.sh_cnt + 6))) return rc;
+        } else if ((rc = launch_window_rgb(p.wm, n, B.npad, B.r_hi, st))) {
+          return rc;
+        }
       }
       ProfScope ps(h, kb + 1, st);
       const int amode = mapped ? AMODE_WINDOW : (fused ? AMODE_GATHER : AMODE_TMA);
-      if ((rc = launch_umma_gemm(p, EPI_CONV1, passes, sms(h), st, amode))) return rc;
+      if (share) {
+        float* part = B.part;   // fp32 partial sums, [prefix slot][2][64][256]
+        KStep img[2][36];
+        image_steps(R, 0, img[0]);
+        image_steps(R, 1, img[1]);
+        UmmaGemmParams q = p;
+        // prefix: A half-groups (image 2's steps), then B half-groups (image 1's)
+        memcpy(q.steps, img[1], sizeof(img[1]));
+        memcpy(q.steps + 36, img[0], sizeof(img[0]));
+        q.nsteps = 36;
+        q.m_tiles = (n / 4 + 3) / 2;
+        q.d_units = B.sh_cnt;
+        q.ws = WindowShare{B.sh_prefix, B.sh_cnt + 1, 36, part, nullptr};
+        if ((rc = launch_umma_gemm(q, EPI_CONV1, passes, sms(h), st, amode))) return rc;
+        // continuation: A rows run image 1's steps + rgb, B rows image 2's + rgb
+        memcpy(q.steps, img[0], sizeof(img[0]));
+        q.steps[36] = R.steps1[72];
+        memcpy(q.steps + 37, img[1], sizeof(img[1]));
+        q.steps[73] = R.steps1[72];
+        q.nsteps = 37;
+        q.m_tiles = (n + 1) / 2;
+        q.d_units = B.sh_cnt + 3;
+        q.ws = WindowShare{B.sh_cont, B.sh_cnt + 4, 37, nullptr, part};
+        if ((rc = launch_umma_gemm(q, EPI_CONV1, passes, sms(h), st, amode))) return rc;
+        // unshared rows: all 73 steps, exactly as without sharing
+        q = p;
+        if ((rc = make_tmap_fp16(&q.a_rgb_hi, B.r_unsh, 5, rd, rs, abox))) return rc;
+        q.d_units = B.sh_cnt + 6;
+        q.ws = WindowShare{B.sh_unsh, nullptr, 0, nullptr, nullptr};
+        if ((rc = launch_umma_gemm(q, EPI_CONV1, passes, sms(h), st, amode))) return rc;
+      } else if ((rc = launch_umma_gemm(p, EPI_CONV1, passes, sms(h), st, amode))) {
+        return rc;
+      }
     }
     {  // conv2
       const uint64_t ad[5] = {512, 8, 8, 1, npad};
@@ -1073,8 +1150,12 @@ int p2p_refine(p2p_handle_t h, int which, const void* matches_in, int is_float, 
   const size_t pbytes = (size_t)npad * kPatchPos * kMainCh * 2, rbytes = (size_t)npad * 4096 * 2,
                ybytes = (size_t)npad * 64 * 512 * 2, qbytes = (size_t)npad * 512 * 4;
   const size_t n128 = align_up(n, 128);
+  const size_t shbytes = ((size_t)n * 2 + n / 4 + 2 + 8) * 4;
+  // share_windows: partial sums (one 128 KB unit per prefix slot, at most n / 4 + 1 slots) and the unshared rows' rgb
+  const bool share_bufs = which == 0 && h->opt_share_windows;
+  const size_t partbytes = share_bufs ? ((size_t)n / 4 + 2) * 64 * 512 * 4 : 0, runshbytes = share_bufs ? rbytes : 0;
   int rc = h->refine.reserve(2 * (pbytes + rbytes + ybytes) + qbytes + (size_t)n * 24 + n128 * (512 + 512 + 256) * 4 +
-                             (1 << 16));
+                             shbytes + partbytes + runshbytes + (1 << 16));
   if (rc) return rc;
   Arena& A = h->refine;
   RefineBuffers B;
@@ -1094,9 +1175,16 @@ int p2p_refine(p2p_handle_t h, int which, const void* matches_in, int is_float, 
   B.h2_lo = (__half*)A.take(n128 * 256 * 2);
   B.raw = (float*)A.take((size_t)n * 5 * 4);
   B.rowmap = (int*)A.take((size_t)n * 4 + 16);
+  B.sh_cnt = (int*)A.take(shbytes);
+  B.part = share_bufs ? (float*)A.take(partbytes) : nullptr;
+  B.r_unsh = share_bufs ? (__half*)A.take(runshbytes) : nullptr;
   P2P_REQUIRE(B.p_hi && B.p_lo && B.r_hi && B.r_lo && B.y_hi && B.y_lo && B.pooled && B.raw && B.rowmap && B.q_hi &&
-                  B.q_lo && B.h1_hi && B.h1_lo && B.h2_hi && B.h2_lo,
+                  B.q_lo && B.h1_hi && B.h1_lo && B.h2_hi && B.h2_lo && B.sh_cnt &&
+                  (!share_bufs || (B.part && B.r_unsh)),
               "scratch carve failed");
+  B.sh_prefix = B.sh_cnt + 8;
+  B.sh_cont = B.sh_prefix + n / 4 + 2;
+  B.sh_unsh = B.sh_cont + n;
   B.d_count = B.rowmap + n;
   if (which == 0) h->last_band_count = band ? B.d_count : nullptr;
   if (!band)

@@ -25,9 +25,46 @@ namespace p2p {
 // ------------------------------------------------------------------------------------------------
 // epilogues: consume one piece of 32 accumulator columns of one row
 // ------------------------------------------------------------------------------------------------
-template <int EPI>
-__device__ __forceinline__ void epilogue_piece(const UmmaEpilogue& e, int n_patches, int m_tile, int row, int col0,
-                                               const float* v) {
+// WindowShare partial sums of one staged piece (32 fp32 accumulators of one tile row, `srow` in shared memory): a prefix
+// launch stores them, a continuation adds its half-group's prefix to them in place, in shared memory: the consumers
+// hold the tile's other accumulators meanwhile, and a register copy of the piece beside the prefix would spill.
+// split_slot = first class-1 slot.
+// Partial-sum layout [unit][256-column half][64 rows][256]: what one 128 x 256 tile reads of one slot is one
+// contiguous 64 KB block, which the producer prefetches into L2 while the tile's main loop runs.
+__device__ __forceinline__ size_t part_offset(int unit, int row64, int col) {
+  return (((size_t)unit * 2 + (col >> 8)) * 64 + row64) * 256 + (col & 255);
+}
+__device__ __forceinline__ int part_unit(int slot, int split_slot, int split_unit) {
+  return slot < split_slot ? slot >> 2 : split_unit + ((slot - split_slot) >> 2);
+}
+__device__ __forceinline__ void share_piece(const WindowShare& ws, int split_slot, int split_unit, int n_patches, int m_tile,
+                                            int row, int col0, float* srow) {
+  const int n = m_tile * 2 + (row >> 6);
+  if (n >= n_patches) return;
+  if (ws.part_out != nullptr) {
+    float4* dst = reinterpret_cast<float4*>(ws.part_out + part_offset(n, row & 63, col0));
+#pragma unroll 1
+    for (int q = 0; q < 8; ++q) dst[q] = make_float4(srow[4 * q], srow[4 * q + 1], srow[4 * q + 2], srow[4 * q + 3]);
+  } else {
+    const float4* src = reinterpret_cast<const float4*>(ws.part_in + part_offset(part_unit(n, split_slot, split_unit), row & 63, col0));
+    float4 a8[8];                       // all 8 loads in flight at once (this piece's accumulators are staged already)
+#pragma unroll
+    for (int q = 0; q < 8; ++q) a8[q] = __ldg(src + q);
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+      const float4 a = a8[q];
+      srow[4 * q] += a.x;
+      srow[4 * q + 1] += a.y;
+      srow[4 * q + 2] += a.z;
+      srow[4 * q + 3] += a.w;
+    }
+  }
+}
+
+// SHARE (AMODE_WINDOW): the conv1 outputs go to row ws.slot_row[slot]
+template <int EPI, bool SHARE>
+__device__ __forceinline__ void epilogue_piece(const UmmaEpilogue& e, const WindowShare& ws, int n_patches, int m_tile,
+                                               int row, int col0, const float* v) {
   if (EPI == EPI_PLAIN) {
     const int r = m_tile * 128 + row;
     if (r < e.m_rows) {
@@ -39,6 +76,7 @@ __device__ __forceinline__ void epilogue_piece(const UmmaEpilogue& e, int n_patc
   } else if (EPI == EPI_CONV1) {
     const int n = m_tile * 2 + (row >> 6);
     if (n < n_patches) {
+      const int r = SHARE && ws.slot_row != nullptr ? __ldg(ws.slot_row + n) : n;   // the conv1 output row
       __align__(16) __half h[32];
       __align__(16) __half l[32];
 #pragma unroll
@@ -47,7 +85,7 @@ __device__ __forceinline__ void epilogue_piece(const UmmaEpilogue& e, int n_patc
         h[i] = __float2half_rn(y);
         l[i] = __float2half_rn(y - __half2float(h[i]));
       }
-      const size_t o = ((size_t)n * 64 + (row & 63)) * 512 + col0;
+      const size_t o = ((size_t)r * 64 + (row & 63)) * 512 + col0;
 #pragma unroll
       for (int q = 0; q < 4; ++q) reinterpret_cast<uint4*>(e.y_hi + o)[q] = reinterpret_cast<const uint4*>(h)[q];
       if (e.y_lo != nullptr) {
@@ -57,7 +95,7 @@ __device__ __forceinline__ void epilogue_piece(const UmmaEpilogue& e, int n_patc
       // zero this patch's slice of the max-pool accumulator that conv2's epilogue merges into with atomicMax
       // (replaces a cudaMemsetAsync between the two convolutions)
       if (e.pooled != nullptr && (row & 63) == 0) {
-        float4* z = reinterpret_cast<float4*>(e.pooled + (size_t)n * 512 + col0);
+        float4* z = reinterpret_cast<float4*>(e.pooled + (size_t)r * 512 + col0);
 #pragma unroll
         for (int q = 0; q < 8; ++q) z[q] = make_float4(0.f, 0.f, 0.f, 0.f);
       }
@@ -185,14 +223,19 @@ __device__ __forceinline__ void named_bar(int id, int threads) {
 // AMODE_WINDOW: window origin of patch n in padded map coordinates: window pixel (wy, wx) lives at (oy + wy, ox + wx).
 // Truncation = `.long()` (networks/utils.py:19); clamping the origin to [-7, W + 8] leaves every clamped window
 // pixel unchanged (beyond that all of them sit on the border pixel) and keeps the boxes inside the padded map.
-__device__ __forceinline__ int window_origin(const WindowMaps& wm, int n, int n_units, int j) {
-  if (n >= n_units) n = 0;      // past the end (odd patch counts): any valid patch, the epilogue discards the rows
+__device__ __forceinline__ int window_origin(const WindowMaps& wm, int n, int j) {
   int v;
   if (wm.is_float) v = (int)reinterpret_cast<const float*>(wm.matches)[(size_t)n * 4 + j];
   else v = (int)reinterpret_cast<const long long*>(wm.matches)[(size_t)n * 4 + j];
   const int lim = (j & 1) ? wm.H[j >> 1] : wm.W[j >> 1];
   v = v < -7 ? -7 : (v > lim + 8 ? lim + 8 : v);
   return v - 8 + kMapPad;
+}
+
+// AMODE_WINDOW: the matches row of patch slot s; past the end (odd patch counts) any valid row, the epilogue discards it
+__device__ __forceinline__ int window_row(const WindowShare& ws, int s, int n_units) {
+  if (s >= n_units) s = 0;
+  return ws.slot_row != nullptr ? __ldg(ws.slot_row + s) : s;
 }
 
 // Tile = 128 rows x BN columns (see GemmCfg); K chunk 64 (one 128-byte swizzle row)
@@ -240,6 +283,13 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, SEGMENTED, AMODE>::THREADS, 1)
   const int total_tiles = m_tiles * n_col_tiles;
   const int nsteps = p.nsteps;
   const int seg_len = SEGMENTED ? p.seg_len : nsteps;
+  // WindowShare: tiles from split_tile on are of class 1 and read steps[class_steps ..] (producer and fix-up warps only:
+  // both classes run nsteps k-steps, so every role walks the same stage sequence)
+  int split_tile = total_tiles, split_unit = 0;
+  if (AMODE == AMODE_WINDOW && p.ws.d_split != nullptr) {
+    split_tile = __ldg(p.ws.d_split);
+    split_unit = __ldg(p.ws.d_split + 1);
+  }
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&p.b_hi);
@@ -278,17 +328,28 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, SEGMENTED, AMODE>::THREADS, 1)
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         const int m_tile = tile / n_col_tiles, brow = (tile - m_tile * n_col_tiles) * BN;
         const int a4 = m_tile * p.a_units_per_tile;
+        const int kofs = m_tile < split_tile ? 0 : p.ws.class_steps;
+        if (AMODE == AMODE_WINDOW && p.ws.part_in != nullptr) {
+          // continuation: the tile's partial sums go to L2 now, so that its epilogue does not wait on HBM
+#pragma unroll 1
+          for (int pp = 0; pp < 2; ++pp)
+            if (m_tile * 2 + pp < n_units)
+              bulk_prefetch_l2(p.ws.part_in + part_offset(part_unit(m_tile * 2 + pp, 2 * split_tile, split_unit), 0, brow),
+                               64 * 256 * 4);
+        }
         int o[2][4];
         if (AMODE == AMODE_WINDOW) {
 #pragma unroll
-          for (int pp = 0; pp < 2; ++pp)
+          for (int pp = 0; pp < 2; ++pp) {
+            const int row = window_row(p.ws, m_tile * 2 + pp, n_units);
 #pragma unroll
-            for (int j = 0; j < 4; ++j) o[pp][j] = window_origin(p.wm, m_tile * 2 + pp, n_units, j);
+            for (int j = 0; j < 4; ++j) o[pp][j] = window_origin(p.wm, row, j);
+          }
         }
         for (int ks = 0; ks < nsteps; ++ks, ++it) {
           const int s = it % STAGES;
           mbar_wait(&empty_bar[s], ((uint32_t)(it / STAGES) & 1u) ^ 1u);
-          const KStep k = p.steps[ks];  // param space (constant bank)
+          const KStep k = p.steps[ks + kofs];  // param space (constant bank)
           uint8_t* st = smem + (size_t)s * STAGE_BYTES;
           if (AMODE == AMODE_GATHER) {
             mbar_expect_tx(&full_bar[s], B_BYTES);
@@ -327,12 +388,13 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, SEGMENTED, AMODE>::THREADS, 1)
       const int t = threadIdx.x - 32;                  // 0..95
       int it = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+        const int kofs = tile / n_col_tiles < split_tile ? 0 : p.ws.class_steps;
         for (int ks = 0; ks < nsteps; ++ks, ++it) {
           const int s = it % STAGES;
           // every fix-up warp follows every stage (wait + arrive): parity waits are only valid within one ring
           // revolution, so no warp may run ahead of -- or fall behind -- the pipeline
           mbar_wait(&full_bar[s], (uint32_t)(it / STAGES) & 1u);
-          const KStep k = p.steps[ks];
+          const KStep k = p.steps[ks + kofs];
           const bool zx = k.kind == 0 && !(k.plane & 1) && k.x < 0, zy = k.kind == 0 && !(k.plane & 2) && k.y < 0;
           if (zx || zy) {
             uint8_t* st = smem + (size_t)s * STAGE_BYTES;
@@ -430,10 +492,15 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, SEGMENTED, AMODE>::THREADS, 1)
           o[8 * kEpiPitch + 1] = d[3];
         }
         named_bar(1 + wg, 128);
+        if (AMODE == AMODE_WINDOW && (p.ws.part_out != nullptr || p.ws.part_in != nullptr)) {
+          share_piece(p.ws, 2 * split_tile, split_unit, n_units, m_tile, wg * 64 + er, col0 + c64 * 64 + ec,
+                      stg + er * kEpiPitch + ec);
+          if (p.ws.part_out != nullptr) continue;   // prefix launch: no BN, no y_hi, no pooled zeroing
+        }
         float v[32];
 #pragma unroll
         for (int i = 0; i < 32; ++i) v[i] = stg[er * kEpiPitch + ec + i];
-        epilogue_piece<EPI>(p.epi, n_units, m_tile, wg * 64 + er, col0 + c64 * 64 + ec, v);
+        epilogue_piece<EPI, AMODE == AMODE_WINDOW>(p.epi, p.ws, n_units, m_tile, wg * 64 + er, col0 + c64 * 64 + ec, v);
       }
     }
   } else if (AMODE == AMODE_GATHER) {
@@ -553,17 +620,23 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, SEGMENTED, AMODE>::THREADS, 1)
 // (54 used, rest zero), copied from the normalised rgb maps; window pixel -1 = conv zero padding, and the pad patch of
 // an odd count is all zero.  One thread per output pixel (row of 128 bytes).
 __global__ void __launch_bounds__(256) window_rgb_kernel(const __grid_constant__ WindowMaps wm, int n_units, int npad,
-                                                         __half* __restrict__ out) {
+                                                         __half* __restrict__ out, const int* __restrict__ slot_row,
+                                                         const int* __restrict__ d_count) {
   const int row = blockIdx.x * 256 + threadIdx.x;
   if (row >= npad * 64) return;
   const int n = row >> 6, oy = (row >> 3) & 7, ox = row & 7;
+  if (d_count != nullptr) {
+    n_units = __ldg(d_count);
+    if (n >= n_units + (n_units & 1)) return;      // beyond the pad slot: no tile reads it
+  }
   __align__(16) __half hv[64];
 #pragma unroll
   for (int i = 0; i < 64; ++i) hv[i] = __float2half_rn(0.f);
   if (n < n_units) {
+    const int r = slot_row != nullptr ? __ldg(slot_row + n) : n;
 #pragma unroll
     for (int si = 0; si < 2; ++si) {
-      const int bx = window_origin(wm, n, n_units, 2 * si), by = window_origin(wm, n, n_units, 2 * si + 1);
+      const int bx = window_origin(wm, r, 2 * si), by = window_origin(wm, r, 2 * si + 1);
       const int Wp = wm.W[si] + 2 * kMapPad;
 #pragma unroll
       for (int tap = 0; tap < 9; ++tap) {
@@ -583,10 +656,117 @@ __global__ void __launch_bounds__(256) window_rgb_kernel(const __grid_constant__
   for (int c = 0; c < 8; ++c) dst[c] = reinterpret_cast<const uint4*>(hv)[c];
 }
 
-int launch_window_rgb(const WindowMaps& wm, int n, int npad, __half* out, cudaStream_t st) {
+int launch_window_rgb(const WindowMaps& wm, int n, int npad, __half* out, cudaStream_t st, const int* slot_row,
+                      const int* d_count) {
   P2P_REQUIRE(n >= 0 && npad >= n, "window rgb: bad patch count");
   if (npad == 0) return 0;
-  window_rgb_kernel<<<(unsigned)cdiv(npad * 64, 256), 256, 0, st>>>(wm, n, npad, out);
+  window_rgb_kernel<<<(unsigned)cdiv(npad * 64, 256), 256, 0, st>>>(wm, n, npad, out, slot_row, d_count);
+  P2P_LAUNCH_OK();
+  return 0;
+}
+
+// Block-wide exclusive prefix sums of three counters per thread (1024 threads); tot receives the block totals.
+__device__ __forceinline__ void block_scan3(const int (&v)[3], int (&ex)[3], int (&tot)[3], int (*s_warp)[32]) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  int inc[3];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    inc[c] = v[c];
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int t = __shfl_up_sync(0xffffffffu, inc[c], o);
+      if (lane >= o) inc[c] += t;
+    }
+    if (lane == 31) s_warp[c][wid] = inc[c];
+  }
+  __syncthreads();
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    int woff = 0, t = 0;
+    for (int w = 0; w < 32; ++w) {
+      const int x = s_warp[c][w];
+      if (w < wid) woff += x;
+      t += x;
+    }
+    ex[c] = woff + inc[c] - v[c];
+    tot[c] = t;
+  }
+  __syncthreads();
+}
+
+// Half-group h (0: rows 8g..8g+3, compared on image 2; 1: rows 8g+4..8g+7, compared on image 1) of a complete group
+// is shared when its four window origins are equal.  Single block, one thread per group, order-preserving.
+__global__ void __launch_bounds__(1024) window_share_classify_kernel(const __grid_constant__ WindowMaps wm, int n,
+                                                                     int* __restrict__ prefix, int* __restrict__ cont,
+                                                                     int* __restrict__ unsh, int* __restrict__ cnt,
+                                                                     int* __restrict__ shared_out) {
+  __shared__ int s_warp[3][32];
+  __shared__ int s_base[3];   // A half-groups, B half-groups, unshared rows so far
+  __shared__ int s_na;
+  const int tid = threadIdx.x, groups = (n + 7) / 8;
+  auto shared_half = [&](int g, int h) {
+    if (8 * g + 8 > n) return 0;
+    const int si = 1 - h, r0 = 8 * g + 4 * h;
+    const int x = window_origin(wm, r0, 2 * si), y = window_origin(wm, r0, 2 * si + 1);
+    for (int i = 1; i < 4; ++i)
+      if (window_origin(wm, r0 + i, 2 * si) != x || window_origin(wm, r0 + i, 2 * si + 1) != y) return 0;
+    return 1;
+  };
+  if (tid == 0) s_na = s_base[0] = s_base[1] = s_base[2] = 0;
+  __syncthreads();
+  int na = 0;
+  for (int g = tid; g < groups; g += 1024) na += shared_half(g, 0);
+  atomicAdd(&s_na, na);
+  __syncthreads();
+  const int nA = s_na, ubase = nA + (nA & 1);
+  for (int g0 = 0; g0 < groups; g0 += 1024) {
+    const int g = g0 + tid;
+    int v[3] = {0, 0, 0};
+    if (g < groups) {
+      v[0] = shared_half(g, 0);
+      v[1] = shared_half(g, 1);
+      v[2] = min(8, n - 8 * g) - 4 * (v[0] + v[1]);
+    }
+    int ex[3], tot[3];
+    block_scan3(v, ex, tot, s_warp);
+    if (g < groups) {
+      const int ia = s_base[0] + ex[0], ib = s_base[1] + ex[1];
+      int iu = s_base[2] + ex[2];
+      if (v[0]) {
+        prefix[ia] = 8 * g;
+        for (int i = 0; i < 4; ++i) cont[4 * ia + i] = 8 * g + i;
+      }
+      if (v[1]) {
+        prefix[ubase + ib] = 8 * g + 4;
+        for (int i = 0; i < 4; ++i) cont[4 * (nA + ib) + i] = 8 * g + 4 + i;
+      }
+      for (int r = 8 * g; r < min(8 * g + 8, n); ++r)
+        if (!(r - 8 * g < 4 ? v[0] : v[1])) unsh[iu++] = r;
+    }
+    __syncthreads();
+    if (tid == 0)
+      for (int c = 0; c < 3; ++c) s_base[c] += tot[c];
+    __syncthreads();
+  }
+  if (tid == 0) {
+    const int nB = s_base[1];
+    if (nA & 1) prefix[nA] = prefix[nA - 1];   // pad slot: computed, never read
+    cnt[0] = ubase + nB;
+    cnt[1] = ubase / 2;
+    cnt[2] = 0;
+    cnt[3] = 4 * (nA + nB);
+    cnt[4] = 2 * nA;
+    cnt[5] = ubase;
+    cnt[6] = s_base[2];
+    cnt[7] = 0;
+    if (shared_out != nullptr) *shared_out = 4 * (nA + nB);
+  }
+}
+
+int launch_window_share_classify(const WindowMaps& wm, int n, int* prefix, int* cont, int* unsh, int* cnt, int* shared_out,
+                                 cudaStream_t st) {
+  P2P_REQUIRE(n >= 0, "window share: bad row count");
+  window_share_classify_kernel<<<1, 1024, 0, st>>>(wm, n, prefix, cont, unsh, cnt, shared_out);
   P2P_LAUNCH_OK();
   return 0;
 }

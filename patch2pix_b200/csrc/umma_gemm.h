@@ -51,6 +51,23 @@ struct WindowMaps {
   int is_float;
 };
 
+// AMODE_WINDOW launches of the mid stage's shared anchor windows (api.cu, run_regressor); all zero: patch slot s is
+// row s and every tile runs steps[0 .. nsteps).
+//   prefix launch:       one slot per shared half-group, k-steps of the shared image only; the epilogue stores the raw
+//                        fp32 accumulators to part_out[slot][2][64][256] (no BN, no y_hi, no pooled zeroing)
+//   continuation launch: the half-groups' rows, k-steps of the other image + rgb; the epilogue adds
+//                        part_in[unit][2][64][256] (4 consecutive slots per unit) before the BN, which the producer
+//                        prefetches into L2 at the start of each tile
+// Tiles from m-tile d_split[0] on are of class 1 and read steps[class_steps ..]; in the continuation the unit of
+// class-1 slot s is d_split[1] + (s - 2 * d_split[0]) / 4, of class-0 slot s it is s / 4.
+struct WindowShare {
+  const int* slot_row;   // patch slot -> row of wm.matches (window origins) and of the conv1 outputs (null: the slot)
+  const int* d_split;    // device {first class-1 m-tile, prefix unit of the first class-1 continuation slot}
+  int class_steps;
+  float* part_out;
+  const float* part_in;
+};
+
 struct UmmaGemmParams {
   CUtensorMap a_main_hi, a_main_lo, a_rgb_hi, a_rgb_lo, b_hi, b_lo;
   KStep steps[kMaxKSteps];
@@ -64,13 +81,27 @@ struct UmmaGemmParams {
   UmmaEpilogue epi;
   FusedGather fg;        // AMODE_GATHER
   WindowMaps wm;         // AMODE_WINDOW
+  WindowShare ws;        // AMODE_WINDOW
 };
 
 // estrides (optional): traversal strides; with stride s the box must be N * s to load N elements.
 int make_tmap_fp16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                    const uint32_t* box, const uint32_t* estrides = nullptr);
 int launch_umma_gemm(const UmmaGemmParams& p, int epi, int passes, int num_sms, cudaStream_t st, int amode = AMODE_TMA);
-// AMODE_WINDOW's rgb k-step operand: writes the [npad][64][64] fp16 im2col tensor of patches 0..n-1 (zeros beyond n)
-int launch_window_rgb(const WindowMaps& wm, int n, int npad, __half* out, cudaStream_t st);
+// AMODE_WINDOW's rgb k-step operand: writes the [npad][64][64] fp16 im2col tensor of patches 0..n-1 (zeros beyond n).
+// With slot_row / d_count (device): slot s < *d_count holds row slot_row[s]; an odd count's pad slot is zero and the
+// slots beyond it are not written.
+int launch_window_rgb(const WindowMaps& wm, int n, int npad, __half* out, cudaStream_t st, const int* slot_row = nullptr,
+                      const int* d_count = nullptr);
+// Anchor-window sharing of the mid stage's conv1 (WindowShare): over groups of 8 consecutive rows, half-group A (rows
+// 8g..8g+3) is shared when its four image-2 window origins are equal, half-group B (8g+4..8g+7) when its four image-1
+// origins are; a partial last group is never shared.  Writes, order-preserving:
+//   prefix[]: A representatives, one pad slot if their count nA is odd, then B representatives (from slot ubase)
+//   cont[]:   rows of the shared A half-groups, then those of the shared B half-groups
+//   unsh[]:   every other row, ascending
+//   cnt[8]:   {prefix slots, ubase / 2, 0, shared rows, 2 nA, ubase, unshared rows, 0}, ubase = nA rounded up to even
+// prefix needs n / 4 + 2 entries, cont and unsh n each.  shared_out (optional): receives the shared-row count too.
+int launch_window_share_classify(const WindowMaps& wm, int n, int* prefix, int* cont, int* unsh, int* cnt, int* shared_out,
+                                 cudaStream_t st);
 
 }  // namespace p2p

@@ -108,6 +108,10 @@ __device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, const void* s
                "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2)
                : "memory");
 }
+// bulk copy of global memory into L2 only (no shared-memory destination, no barrier); bytes: a multiple of 16
+__device__ __forceinline__ void bulk_prefetch_l2(const void* src, uint32_t bytes) {
+  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(reinterpret_cast<uint64_t>(src)), "r"(bytes) : "memory");
+}
 __device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void bulk_wait_group_read() {     // at most N groups still READING their shared source
