@@ -233,6 +233,27 @@ def synthetic_pair_shifted(pair_idx, height, width, noise=0.6):
     return im1, im2
 
 
+def synthetic_pair_sized(pair_idx, size1, size2, noise=0.6):
+    """Two overlapping views of one texture at their own sizes size1 = (H1, W1) and size2 = (H2, W2), built like
+    `synthetic_pair_shifted`: view 2's crop is offset from view 1's by a multiple of 16 px (shifted_pair_offset-style
+    draw) and carries independent noise.  This is what a portrait photo matched against a landscape one looks like
+    after load_im_flexible.  Returns im1 [1,3,H1,W1], im2 [1,3,H2,W2] fp32 on CPU."""
+    (h1, w1), (h2, w2) = (int(s) for s in size1), (int(s) for s in size2)
+    g = torch.Generator().manual_seed(3000 + int(pair_idx))
+    dx = 16 * int(torch.randint(-3, 4, (1,), generator=g))
+    dy = 16 * int(torch.randint(-2, 3, (1,), generator=g))
+    if dx == 0 and dy == 0:
+        dx = 16
+    height, width = max(h1, h2), max(w1, w2)
+    low = torch.randn(1, 3, height // 8 + 12, width // 8 + 12, generator=g)
+    base = F.interpolate(low, size=(height + 96, width + 96), mode='bicubic', align_corners=False)
+    base = base + 0.3 * torch.randn(1, 3, height + 96, width + 96, generator=g)
+    im1 = base[:, :, 48:48 + h1, 48:48 + w1].contiguous()
+    im2 = base[:, :, 48 + dy:48 + dy + h2, 48 + dx:48 + dx + w2].contiguous()
+    im2 = im2 + noise * torch.randn(im2.shape, generator=g)
+    return im1, im2
+
+
 def write_colmap_model(model_dir, cameras, images):
     """COLMAP binary model (little-endian) with the given cameras [(id, model_id, width, height, params)] and images
     [(id, qvec (w, x, y, z), tvec, camera_id, name)] or [(..., name, point3D_ids)]: cameras.bin and images.bin in
@@ -276,18 +297,25 @@ def synthetic_val_scene(root, scene, seed, sizes, ext='.png', missing=(), min_ov
     """One scene of a validation tree in the layout of the reference's PhotoTourism validation sets:
     root/scene/dense/images/<names>, dense/sparse/{cameras,images}.bin and dense/sparse/ov_pairs.npy
     ({min_overlap: pair names}).  Pair k is two views of one texture (synthetic_pair_shifted(seed * 1000 + k)) at
-    sizes[k] = (width, height) as 8-bit images, with a seeded SIMPLE_PINHOLE camera and pose per image (the poses do
-    not describe the textures: the matches are real, the pose errors are not meaningful).  Pair indices in `missing`
-    name a second image that is not written.  Returns the pair names."""
+    sizes[k] = (width, height) as 8-bit images, or, with sizes[k] = ((w1, h1), (w2, h2)), two views of different sizes
+    (synthetic_pair_sized(seed * 1000 + k)).  Each image has a seeded SIMPLE_PINHOLE camera of its own size and a
+    seeded pose (the poses do not describe the textures: the matches are real, the pose errors are not meaningful).
+    Pair indices in `missing` name a second image that is not written.  Returns the pair names."""
     from PIL import Image
     rng = np.random.default_rng([int(seed), 7])
     im_dir = os.path.join(root, scene, 'dense', 'images')
     os.makedirs(im_dir, exist_ok=True)
     cameras, images, pairs = [], [], []
-    for k, (w, h) in enumerate(sizes):
-        views = synthetic_pair_shifted(int(seed) * 1000 + k, h, w)
+    for k, size in enumerate(sizes):
+        if isinstance(size[0], (tuple, list)):
+            (w1, h1), (w2, h2) = size
+            views = synthetic_pair_sized(int(seed) * 1000 + k, (h1, w1), (h2, w2))
+        else:
+            w, h = size
+            views = synthetic_pair_shifted(int(seed) * 1000 + k, h, w)
         names = []
         for v, im in enumerate(views):
+            h, w = im.shape[2], im.shape[3]
             name = f'{scene}_{k:03d}_{v}{ext}'
             if not (v == 1 and k in missing):
                 rgb = (im[0].permute(1, 2, 0).numpy() * 48.0 + 128.0).clip(0, 255).astype(np.uint8)

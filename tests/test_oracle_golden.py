@@ -9,7 +9,7 @@ import pytest
 import torch
 
 from oracle import p2p_oracle as O
-from patch2pix_b200.synth import synthetic_pair, synthetic_pair_shifted
+from patch2pix_b200.synth import synthetic_pair, synthetic_pair_shifted, synthetic_pair_sized
 
 GOLD = os.path.join(os.path.dirname(__file__), 'golden')
 RTOL, ATOL = 2e-4, 2e-5
@@ -65,6 +65,47 @@ def test_train_forward_sequence(name, seeded_sd, consensus_sd):
         np.random.seed(int(g['np_seed']))
         fine, fine_p, mid, mid_p, anchors = O.train_forward_sequence(
             im1, im2, seeded_sd, ksize=2, ptmax=int(g['ptmax']), panc=8, return_all=True)
+    assert np.array_equal(anchors[0].numpy(), g['anchors'])
+    _close(mid[0], g['mid'], atol=1e-3)
+    _close(fine[0], g['fine'], atol=1e-3)
+    _close(mid_p[0], g['mid_p'], atol=1e-4)
+    _close(fine_p[0], g['fine_p'], atol=1e-4)
+
+
+@pytest.mark.parametrize('name', ['unequal_96x128_128x96', 'unequal_128x160_96x224'])
+def test_unequal_sizes_predict_fine(name, consensus_sd):
+    """Images of different sizes (transposed aspect; H1 > H2 with W1 < W2): every per-image size the reference uses --
+    the 4D volume's two grids, the patch gathers' clamps, the regressor outputs' clamps -- must be the right image's."""
+    g = np.load(os.path.join(GOLD, name + '.npz'))
+    im1, im2 = synthetic_pair_sized(int(g['pair_idx']), tuple(g['size1']), tuple(g['size2']))
+    assert im1.shape[2:] != im2.shape[2:]
+    with torch.no_grad():
+        f1 = O.backbone_forward_all(im1, consensus_sd)
+        f2 = O.backbone_forward_all(im2, consensus_sd)
+        st = {}
+        corr4d, delta4d = O.forward_coarse_match(f1[-1], f2[-1], consensus_sd, ksize=2, stages=st)
+        _close(st['pooled'], g['pooled'])
+        assert np.array_equal(np.stack([d.numpy() for d in delta4d]), g['delta'])
+        _close(st['ncn'], g['ncn'])
+        _close(corr4d, g['corr4d'])
+        cm, sc = O.cal_coarse_matches(corr4d, delta4d, ksize=2, upsample=8, center=True)
+        assert np.array_equal(cm.numpy(), g['cand_matches'])
+        _close(sc, g['cand_scores'])
+        fine, fine_p, mid, mid_p, coarse = O.predict_fine(im1, im2, consensus_sd, ksize=2, return_all=True)
+        assert np.array_equal(coarse[0].numpy(), g['coarse'])
+        _close(mid[0].reshape(-1, 4), g['mid'], atol=1e-3)
+        _close(fine[0].reshape(-1, 4), g['fine'], atol=1e-3)
+        _close(mid_p[0].reshape(-1), g['mid_p'], atol=1e-4)
+        _close(fine_p[0].reshape(-1), g['fine_p'], atol=1e-4)
+
+
+def test_unequal_sizes_train_forward_sequence(consensus_sd):
+    g = np.load(os.path.join(GOLD, 'unequal_trainseq_160x240_192x128.npz'))
+    im1, im2 = synthetic_pair_sized(int(g['pair_idx']), tuple(g['size1']), tuple(g['size2']))
+    with torch.no_grad():
+        np.random.seed(int(g['np_seed']))
+        fine, fine_p, mid, mid_p, anchors = O.train_forward_sequence(
+            im1, im2, consensus_sd, ksize=2, ptmax=int(g['ptmax']), panc=8, return_all=True)
     assert np.array_equal(anchors[0].numpy(), g['anchors'])
     _close(mid[0], g['mid'], atol=1e-3)
     _close(fine[0], g['fine'], atol=1e-3)
