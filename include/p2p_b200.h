@@ -87,8 +87,13 @@ P2P_API int p2p_set_regressor_weights(p2p_handle_t h, int which, const p2p_regre
  * the tensor cores, 3-pass; 0: fp32 CUDA-core FC kernel), "share_windows" (default 1: in the mid stage's window-map
  * 1-pass conv1, a half-group of 4 rows (rows 8g..8g+3 on image 2, 8g+4..8g+7 on image 1) with equal window origins
  * computes that image's half of conv1 once; shared rows differ from 0 by one reordering of an fp32 sum, all other rows
- * are bit-identical; 0: every row's whole conv1).  p2p_get_option also reads "shared_rows": the rows that shared a
- * window half in the last mid-stage call (synchronises). */
+ * are bit-identical; 0: every row's whole conv1), "epi_async" (default 1: the 256-wide 1-pass conv1 / conv2 launches
+ * take their epilogue straight from the wgmma fragments, conv1's fp16 output leaving by TMA store; 0: through the fp32
+ * shared-memory staging buffer; bit-identical results), "tile_trace" (default 0; 1: the conv GEMM launches and
+ * p2p_test_gemm record a per-tile phase trace, read with p2p_tile_trace_read; setting it clears the trace).
+ * p2p_get_option also reads "shared_rows": the rows that shared a window half in the last mid-stage call
+ * (synchronises), "frag_epi_launches": conv launches run with the fragment epilogues so far, and "tile_traces": the
+ * traced launches since tile_trace was set. */
 P2P_API int p2p_set_option(p2p_handle_t h, const char* key, int value);
 P2P_API int p2p_get_option(p2p_handle_t h, const char* key, int* value);
 /* Number of kernel launches enqueued by this handle since creation (bench.py's gpu_launches). */
@@ -337,6 +342,14 @@ P2P_API int p2p_batch_chunk_pairs(p2p_handle_t h, int entry, int* pairs_out);
  * a, b, c are DEVICE fp32; K % 64 == 0. */
 P2P_API int p2p_test_gemm(p2p_handle_t h, const float* a, const float* b, float* c, int M, int N, int K, int passes,
                   int seg_len, float in_scale, void* stream);
+
+/* ---- per-tile phase trace (option "tile_trace"): traced launch idx (0 .. "tile_traces" - 1) in launch order.  tag:
+ * stage * 8 + kind, stage 0 mid, 1 fine, 2 risk band; kind 0 conv1, 1 shared-window prefix, 2 continuation,
+ * 3 unshared rows, 4 conv2; tag 24 = p2p_test_gemm.  tiles: an upper bound of the launch's tiles.  out (optional,
+ * host, max_tiles >= tiles): 8 %globaltimer ns stamps per tile -- 0 producer's first load issued, 1 consumer tile
+ * start, 2 first stage ready, 3 last k-step issued, 4 accumulators drained, 5 epilogue done, 6 CTA index + 1 -- all
+ * zero for tiles the launch did not have.  Synchronises the device. */
+P2P_API int p2p_tile_trace_read(p2p_handle_t h, int idx, int* tag, int* tiles, unsigned long long* out, int max_tiles);
 
 #ifdef __cplusplus
 }

@@ -52,6 +52,7 @@ _SIGNATURES = {
     'p2p_preprocess_image': (_I, [_P, _P, _I, _I, _I, _I, _P, _P, _P]),
     'p2p_profile_read': (_I, [_P, C.POINTER(C.c_float), C.POINTER(_I), _I]),
     'p2p_test_gemm': (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _F, _P]),
+    'p2p_tile_trace_read': (_I, [_P, _I, C.POINTER(_I), C.POINTER(_I), _P, _I]),
     'p2p_find_model': (_I, [_P, _I, _P, _I, _I, _P, C.c_double, C.c_double, _I, C.c_ulonglong, _P, _P, _P, _P]),
     'p2p_sampson_distance': (_I, [_P, _P, _I, _I, _P, _P, _P]),
     'p2p_epipolar_histograms': (_I, [_P, _P, _I, _I, _P, _I, C.POINTER(C.c_double), _P, C.POINTER(C.c_double), _I, _P,
@@ -138,6 +139,19 @@ class Handle:
         v = C.c_int()
         check(self.lib.p2p_get_option(self.h, key.encode(), C.byref(v)))
         return v.value
+
+    def tile_traces(self):
+        """[(tag, stamps)] of the launches traced since option 'tile_trace' was set: stamps is [tiles][8] uint64
+        (p2p_tile_trace_read), rows of tiles the launch did not have are dropped.  Synchronises."""
+        import numpy as np
+        out = []
+        for i in range(self.get_option('tile_traces')):
+            tag, tiles = C.c_int(), C.c_int()
+            check(self.lib.p2p_tile_trace_read(self.h, i, C.byref(tag), C.byref(tiles), None, 0))
+            buf = np.zeros((tiles.value, 8), dtype=np.uint64)
+            check(self.lib.p2p_tile_trace_read(self.h, i, C.byref(tag), C.byref(tiles), buf.ctypes.data, tiles.value))
+            out.append((tag.value, buf[buf[:, 6] != 0]))
+        return out
 
     def launch_count(self):
         v = C.c_longlong()

@@ -94,6 +94,17 @@ struct p2p_handle_s {
                             // TMA of the patch tensor
   int opt_share_windows = 1;  // mid stage, fuse_gather = 3, 1-pass: compute the conv1 half of an anchor window that a
                               // half-group of 4 rows shares once (1, default), or every row's whole conv1 (0)
+  int opt_epi_async = 1;      // 256-wide conv1 / conv2 launches: epilogue straight from the wgmma fragments, conv1's
+                              // fp16 tile out by TMA store (1, default), or through the fp32 staging buffer (0); same bits
+  int frag_epi_launches = 0;  // conv launches run with the fragment epilogues so far
+  int opt_tile_trace = 0;     // 1: every umma_gemm launch of run_regressor / p2p_test_gemm records its per-tile phase trace
+  unsigned long long* trace_buf = nullptr;   // device, kTraceCap stamps
+  size_t trace_used = 0;
+  struct TraceRec {
+    int tag, tiles;
+    size_t off;
+  };
+  std::vector<TraceRec> traces;               // the traced launches since tile_trace was last set
   const int* last_band_count = nullptr;  // device counter of the last risk-band subset
   int* share_rows = nullptr;             // device: rows that shared a window half in the last sharing mid-stage call
   bool last_mid_shared = false;          // the last mid-stage call shared windows (share_rows is its count)
@@ -347,6 +358,24 @@ int pack_regressor(p2p_handle_s* h, Regressor& R, const p2p_regressor_weights_t&
 
 int sms(const p2p_handle_s* h) { return h->opt_num_sms > 0 ? h->opt_num_sms : h->num_sms; }
 
+constexpr size_t kTraceCap = (size_t)8 << 20;   // stamps (64 MB)
+
+// tile_trace: points p.trace at a zeroed region of the trace buffer for this launch (tag: see p2p_tile_trace_read), or
+// leaves it null when tracing is off or the buffer is full
+int set_trace(p2p_handle_s* h, UmmaGemmParams& p, int tag, cudaStream_t st) {
+  p.trace = nullptr;
+  if (!h->opt_tile_trace) return 0;
+  const int tiles = p.m_tiles * p.n_tiles * 2;   // an upper bound for 128- and 256-wide tiles
+  const size_t need = (size_t)tiles * kTraceStamps;
+  if (h->trace_buf == nullptr) P2P_CUDA_OK(cudaMalloc(&h->trace_buf, kTraceCap * sizeof(unsigned long long)));
+  if (h->trace_used + need > kTraceCap) return 0;
+  p.trace = h->trace_buf + h->trace_used;
+  P2P_CUDA_OK(cudaMemsetAsync(p.trace, 0, need * sizeof(unsigned long long), st));
+  h->traces.push_back({tag, tiles, h->trace_used});
+  h->trace_used += need;
+  return 0;
+}
+
 // Brackets a group of launches with CUDA events on the launching stream when profiling is on.
 struct ProfScope {
   p2p_handle_s* h;
@@ -434,6 +463,7 @@ int p2p_destroy(p2p_handle_t h) {
   if (h->ncw.blob) cudaFree(h->ncw.blob);
   if (h->band_totals) cudaFree(h->band_totals);
   if (h->share_rows) cudaFree(h->share_rows);
+  if (h->trace_buf) cudaFree(h->trace_buf);
   if (h->uniq_rank) cudaFree(h->uniq_rank);
   for (int i = 0; i < 2; ++i)
     if (h->reg[i].blob) cudaFree(h->reg[i].blob);
@@ -494,6 +524,8 @@ static int* option_slot(p2p_handle_t h, const char* key) {
   if (!strcmp(key, "mid_band")) return &h->opt_mid_band;
   if (!strcmp(key, "fuse_gather")) return &h->opt_fuse_gather;
   if (!strcmp(key, "share_windows")) return &h->opt_share_windows;
+  if (!strcmp(key, "epi_async")) return &h->opt_epi_async;
+  if (!strcmp(key, "tile_trace")) return &h->opt_tile_trace;
   if (!strcmp(key, "fc_impl")) return &h->opt_fc_impl;
   if (!strcmp(key, "nc_impl")) return &h->opt_nc_impl;
   if (!strcmp(key, "nc_l2_mode")) return &h->opt_nc_l2_mode;
@@ -508,6 +540,12 @@ int p2p_set_option(p2p_handle_t h, const char* key, int value) {
   if (s == &h->opt_mid_passes || s == &h->opt_fine_passes) P2P_REQUIRE(value == 1 || value == 3, "passes must be 1 or 3");
   if (s == &h->opt_corr_passes) P2P_REQUIRE(value == 0 || value == 1 || value == 3, "corr_passes must be 0, 1 or 3");
   if (s == &h->opt_share_windows) P2P_REQUIRE(value == 0 || value == 1, "share_windows must be 0 or 1");
+  if (s == &h->opt_epi_async) P2P_REQUIRE(value == 0 || value == 1, "epi_async must be 0 or 1");
+  if (s == &h->opt_tile_trace) {
+    P2P_REQUIRE(value == 0 || value == 1, "tile_trace must be 0 or 1");
+    h->traces.clear();
+    h->trace_used = 0;
+  }
   P2P_REQUIRE(value >= 0, "option values are non-negative");
   *s = value;
   return 0;
@@ -522,6 +560,14 @@ int p2p_get_option(p2p_handle_t h, const char* key, int* value) {
       P2P_CUDA_OK(cudaDeviceSynchronize());
       P2P_CUDA_OK(cudaMemcpy(value, h->last_band_count, sizeof(int), cudaMemcpyDeviceToHost));
     }
+    return 0;
+  }
+  if (!strcmp(key, "frag_epi_launches")) {
+    *value = h->frag_epi_launches;
+    return 0;
+  }
+  if (!strcmp(key, "tile_traces")) {
+    *value = (int)h->traces.size();
     return 0;
   }
   if (!strcmp(key, "shared_rows")) {  // rows whose conv1 shared a window half in the last mid-stage call (synchronises)
@@ -990,6 +1036,14 @@ int run_regressor(p2p_handle_s* h, Regressor& R, int which, int passes, const Re
       p.epi.y_lo = lo ? B.y_lo : nullptr;
       p.epi.pooled = B.pooled;       // conv1's epilogue zeroes the max-pool accumulator conv2 merges into
       p.epi.n_patches = n;
+      // 1-pass: conv1 and conv2 run on 256-wide tiles, which the fragment epilogues serve
+      p.frag_epi = !lo && !fused && h->opt_epi_async;
+      if (p.frag_epi) {
+        const uint64_t yd[3] = {512, 64, npad};
+        const uint64_t ys[2] = {1024, 65536};
+        const uint32_t yb[3] = {64, 64, 1};
+        if ((rc = make_tmap_fp16(&p.y_store, B.y_hi, 3, yd, ys, yb))) return rc;
+      }
       if (fused) {
         for (int s2 = 0; s2 < 2; ++s2) {
           p.fg.img[s2] = h->pf[s2].img;
@@ -1030,6 +1084,7 @@ int run_regressor(p2p_handle_s* h, Regressor& R, int which, int passes, const Re
       }
       ProfScope ps(h, kb + 1, st);
       const int amode = mapped ? AMODE_WINDOW : (fused ? AMODE_GATHER : AMODE_TMA);
+      const int tg = (rowmap != nullptr ? 2 : which) * 8;   // tile_trace tag: stage * 8 + launch kind
       if (share) {
         float* part = B.part;   // fp32 partial sums, [prefix slot][2][64][256]
         KStep img[2][36];
@@ -1043,6 +1098,7 @@ int run_regressor(p2p_handle_s* h, Regressor& R, int which, int passes, const Re
         q.m_tiles = (n / 4 + 3) / 2;
         q.d_units = B.sh_cnt;
         q.ws = WindowShare{B.sh_prefix, B.sh_cnt + 1, 36, part, nullptr};
+        if ((rc = set_trace(h, q, tg + 1, st))) return rc;
         if ((rc = launch_umma_gemm(q, EPI_CONV1, passes, sms(h), st, amode))) return rc;
         // continuation: A rows run image 1's steps + rgb, B rows image 2's + rgb
         memcpy(q.steps, img[0], sizeof(img[0]));
@@ -1053,16 +1109,20 @@ int run_regressor(p2p_handle_s* h, Regressor& R, int which, int passes, const Re
         q.m_tiles = (n + 1) / 2;
         q.d_units = B.sh_cnt + 3;
         q.ws = WindowShare{B.sh_cont, B.sh_cnt + 4, 37, nullptr, part};
+        if ((rc = set_trace(h, q, tg + 2, st))) return rc;
         if ((rc = launch_umma_gemm(q, EPI_CONV1, passes, sms(h), st, amode))) return rc;
         // unshared rows: all 73 steps, exactly as without sharing
         q = p;
         if ((rc = make_tmap_fp16(&q.a_rgb_hi, B.r_unsh, 5, rd, rs, abox))) return rc;
         q.d_units = B.sh_cnt + 6;
         q.ws = WindowShare{B.sh_unsh, nullptr, 0, nullptr, nullptr};
+        if ((rc = set_trace(h, q, tg + 3, st))) return rc;
         if ((rc = launch_umma_gemm(q, EPI_CONV1, passes, sms(h), st, amode))) return rc;
-      } else if ((rc = launch_umma_gemm(p, EPI_CONV1, passes, sms(h), st, amode))) {
-        return rc;
+      } else {
+        if ((rc = set_trace(h, p, tg, st))) return rc;
+        if ((rc = launch_umma_gemm(p, EPI_CONV1, passes, sms(h), st, amode))) return rc;
       }
+      h->frag_epi_launches += p.frag_epi ? (share ? 3 : 1) : 0;
     }
     {  // conv2
       const uint64_t ad[5] = {512, 8, 8, 1, npad};
@@ -1080,8 +1140,10 @@ int run_regressor(p2p_handle_s* h, Regressor& R, int which, int passes, const Re
       p.epi.scale = R.scale2;
       p.epi.bias = R.bias2;
       p.epi.pooled = B.pooled;
+      if ((rc = set_trace(h, p, (rowmap != nullptr ? 2 : which) * 8 + 4, st))) return rc;
       ProfScope ps(h, kb + 2, st);
       if ((rc = launch_umma_gemm(p, EPI_CONV2, passes, sms(h), st))) return rc;
+      h->frag_epi_launches += p.frag_epi;
     }
   }
   ProfScope ps(h, kb + 3, st);
@@ -1555,7 +1617,24 @@ int p2p_test_gemm(p2p_handle_t h, const float* a, const float* b, float* c, int 
   p.epi.m_rows = M;
   p.epi.n_cols = N;
   p.epi.alpha = 1.f / (in_scale * in_scale);
+  if ((rc = set_trace(h, p, 24, st))) return rc;
   return launch_umma_gemm(p, EPI_PLAIN, passes, sms(h), st);
+}
+
+int p2p_tile_trace_read(p2p_handle_t h, int idx, int* tag, int* tiles, unsigned long long* out, int max_tiles) {
+  P2P_ENTER(h);
+  P2P_REQUIRE(tag != nullptr && tiles != nullptr, "null argument");
+  P2P_REQUIRE(idx >= 0 && idx < (int)h->traces.size(), "tile trace index out of range");
+  const auto& t = h->traces[idx];
+  *tag = t.tag;
+  *tiles = t.tiles;
+  if (out != nullptr) {
+    P2P_REQUIRE(max_tiles >= t.tiles, "tile trace: output too small");
+    P2P_CUDA_OK(cudaDeviceSynchronize());
+    P2P_CUDA_OK(cudaMemcpy(out, h->trace_buf + t.off, (size_t)t.tiles * kTraceStamps * sizeof(unsigned long long),
+                           cudaMemcpyDeviceToHost));
+  }
+  return 0;
 }
 
 }  // extern "C"

@@ -165,6 +165,144 @@ __device__ __forceinline__ void epilogue_piece(const UmmaEpilogue& e, const Wind
   }
 }
 
+__device__ __forceinline__ void named_bar(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+
+// ------------------------------------------------------------------------------------------------
+// fragment epilogues of the 256-wide 1-pass conv launches: straight from the wgmma accumulators
+// ------------------------------------------------------------------------------------------------
+// Consumer warpgroup wg owns patch n = 2 m_tile + wg (its 64 rows).  Thread 32 wl + lane holds rows fr = 16 wl + lane / 4
+// and fr + 8, columns 8 j + fc, +1 (fc = 2 (lane % 4), j = 0..31) as acc[4 j + {0, 1, 2, 3}] (umma_ptx.cuh).  The
+// per-element arithmetic and the pooling max are epilogue_piece's, so both epilogues write identical bits; these skip
+// the fp32 staging round trip, its 8 named barriers per tile and the per-element scale / bias loads.
+constexpr int kFragBox = 64 * 128;   // one 128B-swizzled TMA box: 64 rows x 64 fp16
+
+// one step of a max reduce-scatter across lanes l and l ^ (H / 2): the lane with that bit set keeps the upper half
+template <int H>
+__device__ __forceinline__ void reduce_scatter_half(uint32_t* m, int lane) {
+  const bool up = (lane & (H / 2)) != 0;
+#pragma unroll
+  for (int i = 0; i < H; ++i) {
+    const uint32_t give = up ? m[i] : m[i + H], keep = up ? m[i + H] : m[i];
+    m[i] = max(keep, __shfl_xor_sync(0xffffffffu, give, H / 2));
+  }
+}
+
+// conv2: relu(BN), max over the patch's 64 rows, one atomicMax per column.  red: this warpgroup's [4 warps][256];
+// sb: the CTA's copy of scale[512] then bias[512] in shared memory.
+__device__ __forceinline__ void conv2_frag(const UmmaEpilogue& e, const float* acc, int n, int n_units, int col0,
+                                           uint32_t* red, const float* sb, int wg) {
+  const int lane = threadIdx.x & 31, wl = (threadIdx.x >> 5) & 3, fc = 2 * (lane & 3);
+  uint32_t m[64];   // m[2 j + b]: max over the thread's two rows of column 8 j + fc + b (as uint, like the atomicMax)
+#pragma unroll
+  for (int j = 0; j < 32; ++j) {
+    const float2 s = *reinterpret_cast<const float2*>(sb + col0 + 8 * j + fc);
+    const float2 b = *reinterpret_cast<const float2*>(sb + 512 + col0 + 8 * j + fc);
+    m[2 * j] = max(__float_as_uint(fmaxf(fmaf(acc[4 * j], s.x, b.x), 0.f)),
+                   __float_as_uint(fmaxf(fmaf(acc[4 * j + 2], s.x, b.x), 0.f)));
+    m[2 * j + 1] = max(__float_as_uint(fmaxf(fmaf(acc[4 * j + 1], s.y, b.y), 0.f)),
+                       __float_as_uint(fmaxf(fmaf(acc[4 * j + 3], s.y, b.y), 0.f)));
+  }
+  // reduce-scatter over the warp's 8 row pairs (lane bits 4, 3, 2): 32 + 16 + 8 shuffles, after which m[i], i < 8, is
+  // the warp's max of index 8 (lane / 4) + i, i.e. column 32 (lane / 4) + 8 (i / 2) + fc + i % 2
+  reduce_scatter_half<32>(m, lane);
+  reduce_scatter_half<16>(m, lane);
+  reduce_scatter_half<8>(m, lane);
+  named_bar(1 + wg, 128);   // the previous tile's reads of red are done
+#pragma unroll
+  for (int i = 0; i < 8; i += 2)
+    *reinterpret_cast<uint2*>(red + wl * 256 + 32 * (lane >> 2) + 4 * i + fc) = make_uint2(m[i], m[i + 1]);
+  named_bar(1 + wg, 128);
+  if (n < n_units) {
+    const int t = threadIdx.x & 127;
+    uint2 v = *reinterpret_cast<const uint2*>(red + 2 * t);
+#pragma unroll
+    for (int w = 1; w < 4; ++w) {
+      const uint2 u = *reinterpret_cast<const uint2*>(red + w * 256 + 2 * t);
+      v.x = max(v.x, u.x);
+      v.y = max(v.y, u.y);
+    }
+    unsigned int* dst = reinterpret_cast<unsigned int*>(e.pooled) + (size_t)n * 512 + col0 + 2 * t;
+    atomicMax(dst, v.x);
+    atomicMax(dst + 1, v.y);
+  }
+}
+
+// conv1: BN (* y_scale) to fp16 in the fragment layout, stmatrix into 128B-swizzled boxes, TMA store at the patch's
+// output row; the two 128-column halves go one after the other through one 16 KB buffer (buf) per warpgroup, whose
+// reuse waits until the previous store has read it.  A prefix launch (SHARE, part_out) stores its raw fp32 sums
+// instead, fragment-direct (8 lanes x 32 contiguous bytes per row); a continuation adds its prefix sums first.
+template <bool SHARE>
+__device__ __forceinline__ void conv1_frag(const UmmaGemmParams& p, float* acc, int n, int n_units, int split_slot,
+                                           int split_unit, int col0, uint8_t* buf) {
+  if (n >= n_units) return;   // warpgroup-uniform: the pad patch of an odd count
+  const int lane = threadIdx.x & 31, wl = (threadIdx.x >> 5) & 3, fc = 2 * (lane & 3), fr = 16 * wl + (lane >> 2);
+  const int wg = threadIdx.x / 128 - 1, t = threadIdx.x & 127;
+  const WindowShare& ws = p.ws;
+  if (SHARE && ws.part_out != nullptr) {   // prefix launch: no BN, no y_hi, no pooled zeroing
+    float* dst = ws.part_out + part_offset(n, 0, col0);
+#pragma unroll
+    for (int j = 0; j < 32; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        *reinterpret_cast<float2*>(dst + (fr + 8 * h) * 256 + 8 * j + fc) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+    return;
+  }
+  if (SHARE && ws.part_in != nullptr) {
+    const float* src = ws.part_in + part_offset(part_unit(n, split_slot, split_unit), 0, col0);
+#pragma unroll
+    for (int j0 = 0; j0 < 32; j0 += 8) {
+      float2 a[16];                     // 16 loads in flight at a time
+#pragma unroll
+      for (int i = 0; i < 16; ++i)
+        a[i] = __ldg(reinterpret_cast<const float2*>(src + (fr + 8 * (i & 1)) * 256 + 8 * (j0 + (i >> 1)) + fc));
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        acc[4 * (j0 + (i >> 1)) + 2 * (i & 1)] += a[i].x;
+        acc[4 * (j0 + (i >> 1)) + 2 * (i & 1) + 1] += a[i].y;
+      }
+    }
+  }
+  const int r = SHARE && ws.slot_row != nullptr ? __ldg(ws.slot_row + n) : n;   // the conv1 output row
+  // zero this patch's slice of the max-pool accumulator that conv2's epilogue merges into with atomicMax
+  if (p.epi.pooled != nullptr)
+    *reinterpret_cast<float2*>(p.epi.pooled + (size_t)r * 512 + col0 + 2 * t) = make_float2(0.f, 0.f);
+  const float ys = p.epi.y_scale;
+  const uint32_t sbuf = smem_u32(buf);
+  const int mi = lane >> 3, rr = lane & 7;           // this lane's stmatrix address: row rr of matrix mi
+  const uint32_t arow = sbuf + (uint32_t)(16 * wl + 8 * (mi & 1) + rr) * 128;
+#pragma unroll
+  for (int hf = 0; hf < 2; ++hf) {
+    if (t == 0) bulk_wait_group_read<0>();   // the previous store out of buf has read it
+    named_bar(1 + wg, 128);
+#pragma unroll
+    for (int j = 16 * hf; j < 16 * hf + 16; j += 2) {
+      uint32_t hv[4];                          // matrices (j, rows fr), (j, fr + 8), (j + 1, fr), (j + 1, fr + 8)
+#pragma unroll
+      for (int q = 0; q < 2; ++q) {
+        const float2 s = __ldg(reinterpret_cast<const float2*>(p.epi.scale + col0 + 8 * (j + q) + fc));
+        const float2 b = __ldg(reinterpret_cast<const float2*>(p.epi.bias + col0 + 8 * (j + q) + fc));
+        const float* d = acc + 4 * (j + q);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const __half2 y = __floats2half2_rn(fmaf(d[2 * h], s.x, b.x) * ys, fmaf(d[2 * h + 1], s.y, b.y) * ys);
+          hv[2 * q + h] = *reinterpret_cast<const uint32_t*>(&y);
+        }
+      }
+      const int jm = j + (mi >> 1);            // column group of this lane's matrix row
+      stmatrix_x4(arow + (uint32_t)((jm >> 3) & 1) * kFragBox + (uint32_t)(((jm & 7) ^ rr) << 4), hv[0], hv[1], hv[2], hv[3]);
+    }
+    fence_proxy_async();
+    named_bar(1 + wg, 128);
+    if (t == 0) {
+      tma_store_3d(&p.y_store, buf, col0 + 128 * hf, 0, r);
+      tma_store_3d(&p.y_store, buf + kFragBox, col0 + 128 * hf + 64, 0, r);
+      bulk_commit_group();
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // the kernel
 // ------------------------------------------------------------------------------------------------
@@ -216,10 +354,6 @@ __device__ __forceinline__ int fg_clamp(int v, int ds, int full) {   // ((x+dx)/
   return q < m ? q : m;
 }
 
-__device__ __forceinline__ void named_bar(int id, int threads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
-}
-
 // AMODE_WINDOW: window origin of patch n in padded map coordinates: window pixel (wy, wx) lives at (oy + wy, ox + wx).
 // Truncation = `.long()` (networks/utils.py:19); clamping the origin to [-7, W + 8] leaves every clamped window
 // pixel unchanged (beyond that all of them sit on the border pixel) and keeps the boxes inside the padded map.
@@ -261,6 +395,12 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, SEGMENTED, AMODE>::THREADS, 1)
   using Cfg = GemmCfg<PASSES, SEGMENTED, AMODE>;
   constexpr int STAGES = Cfg::STAGES, NOP = Cfg::NOP, STAGE_BYTES = Cfg::STAGE_BYTES;
   constexpr int BN = Cfg::BN, B_BYTES = Cfg::B_BYTES, NACC = BN / 2;
+  // 256-wide conv1 / conv2: p.frag_epi selects the fragment epilogues (conv1_frag / conv2_frag) over the staged one.
+  // They reuse the staging area: conv1 one 2-box buffer per warpgroup; conv2 a [4][256] max array per warpgroup and the
+  // CTA's scale and bias (4 KB), which do not fit beside conv1's buffers.
+  constexpr bool FRAG = BN == 256 && (EPI == EPI_CONV1 || EPI == EPI_CONV2);
+  static_assert(2 * kFragBox * 2 <= 2 * kEpiBytes && 3 * 1024 * 4 <= 2 * kEpiBytes && (STAGES * STAGE_BYTES) % 1024 == 0,
+                "fragment epilogue buffers");
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -303,6 +443,7 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, SEGMENTED, AMODE>::THREADS, 1)
       tma_prefetch_desc(&p.a_main_lo);
       tma_prefetch_desc(&p.b_lo);
     }
+    if (FRAG && EPI == EPI_CONV1 && p.frag_epi) tma_prefetch_desc(&p.y_store);
   }
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < STAGES; ++i) {
@@ -329,6 +470,10 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, SEGMENTED, AMODE>::THREADS, 1)
         const int m_tile = tile / n_col_tiles, brow = (tile - m_tile * n_col_tiles) * BN;
         const int a4 = m_tile * p.a_units_per_tile;
         const int kofs = m_tile < split_tile ? 0 : p.ws.class_steps;
+        if (p.trace != nullptr) {
+          mbar_wait(&empty_bar[it % STAGES], ((uint32_t)(it / STAGES) & 1u) ^ 1u);
+          p.trace[(size_t)tile * kTraceStamps] = globaltimer();
+        }
         if (AMODE == AMODE_WINDOW && p.ws.part_in != nullptr) {
           // continuation: the tile's partial sums go to L2 now, so that its epilogue does not wait on HBM
 #pragma unroll 1
@@ -417,6 +562,11 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, SEGMENTED, AMODE>::THREADS, 1)
     const bool leader = threadIdx.x % 128 == 0;    // arrives on empty_bar for the warpgroup
     uint64_t* ready = AMODE == AMODE_WINDOW ? ready_bar : full_bar;
     float* stg = epi_smem + wg * (64 * kEpiPitch);
+    if (FRAG && EPI == EPI_CONV2 && p.frag_epi) {   // scale, bias -> epi_smem[2048 ..), past both warpgroups' max arrays
+      const int t = threadIdx.x - 128;
+      for (int i = t; i < 1024; i += 256) epi_smem[2048 + i] = i < 512 ? __ldg(p.epi.scale + i) : __ldg(p.epi.bias + i - 512);
+      named_bar(4, 256);
+    }
     float acc[NACC];
     float tot[SEGMENTED ? NACC : 1];
     int it = 0;
@@ -425,6 +575,12 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, SEGMENTED, AMODE>::THREADS, 1)
       if (SEGMENTED) {
 #pragma unroll
         for (int i = 0; i < NACC; ++i) tot[i] = 0.f;
+      }
+      unsigned long long* tr = p.trace != nullptr && threadIdx.x == 128 ? p.trace + (size_t)tile * kTraceStamps : nullptr;
+      if (p.trace != nullptr) {   // the loop's own wait for this stage then returns at once
+        if (tr != nullptr) tr[1] = globaltimer();
+        mbar_wait(&ready[it % STAGES], (uint32_t)(it / STAGES) & 1u);
+        if (tr != nullptr) tr[2] = globaltimer();
       }
       // Each k-step's MMAs are one wgmma group.  wait_group 1 after issuing step ks retires step ks - 1, whose stage
       // is then released, so the tensor core always has the next group queued.  An interior segment end drains the
@@ -468,41 +624,57 @@ __global__ void __launch_bounds__(GemmCfg<PASSES, SEGMENTED, AMODE>::THREADS, 1)
         mbar_arrive_if(&empty_bar[(s + STAGES - 1) % STAGES], leader && prev_pending);
         mbar_arrive_if(&empty_bar[s], leader && seg_end);
       }
+      if (tr != nullptr) tr[3] = globaltimer();
       wgmma_wait<0>();
       wgmma_fence_regs<NACC>(acc);
+      if (tr != nullptr) tr[4] = globaltimer();
       mbar_arrive_if(&empty_bar[(it + STAGES - 1) % STAGES], leader);   // the tile's last k-step
       if (SEGMENTED) {
 #pragma unroll
         for (int i = 0; i < NACC; ++i) tot[i] += acc[i];
       }
-      const float* res = SEGMENTED ? tot : acc;
-      // fragment -> row-major staging, 64 columns at a time; then one row per thread
-      const int fr = 16 * wl + (lane >> 2), fc = 2 * (lane & 3);
-      const int er = (wl & 1) * 32 + lane, ec = (wl >> 1) * 32;
+      if (FRAG && p.frag_epi) {
+        if (EPI == EPI_CONV2)
+          conv2_frag(p.epi, acc, m_tile * 2 + wg, n_units, col0, reinterpret_cast<uint32_t*>(epi_smem) + wg * 1024,
+                     epi_smem + 2 * 1024, wg);
+        else
+          conv1_frag<AMODE == AMODE_WINDOW>(p, acc, m_tile * 2 + wg, n_units, 2 * split_tile, split_unit, col0,
+                                            reinterpret_cast<uint8_t*>(epi_smem) + wg * 2 * kFragBox);
+      } else {
+        const float* res = SEGMENTED ? tot : acc;
+        // fragment -> row-major staging, 64 columns at a time; then one row per thread
+        const int fr = 16 * wl + (lane >> 2), fc = 2 * (lane & 3);
+        const int er = (wl & 1) * 32 + lane, ec = (wl >> 1) * 32;
 #pragma unroll
-      for (int c64 = 0; c64 < BN / 64; ++c64) {
-        named_bar(1 + wg, 128);                 // the previous piece has been read
+        for (int c64 = 0; c64 < BN / 64; ++c64) {
+          named_bar(1 + wg, 128);                 // the previous piece has been read
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float* d = res + 4 * (c64 * 8 + j);
-          float* o = stg + fr * kEpiPitch + 8 * j + fc;
-          o[0] = d[0];
-          o[1] = d[1];
-          o[8 * kEpiPitch] = d[2];
-          o[8 * kEpiPitch + 1] = d[3];
+          for (int j = 0; j < 8; ++j) {
+            const float* d = res + 4 * (c64 * 8 + j);
+            float* o = stg + fr * kEpiPitch + 8 * j + fc;
+            o[0] = d[0];
+            o[1] = d[1];
+            o[8 * kEpiPitch] = d[2];
+            o[8 * kEpiPitch + 1] = d[3];
+          }
+          named_bar(1 + wg, 128);
+          if (AMODE == AMODE_WINDOW && (p.ws.part_out != nullptr || p.ws.part_in != nullptr)) {
+            share_piece(p.ws, 2 * split_tile, split_unit, n_units, m_tile, wg * 64 + er, col0 + c64 * 64 + ec,
+                        stg + er * kEpiPitch + ec);
+            if (p.ws.part_out != nullptr) continue;   // prefix launch: no BN, no y_hi, no pooled zeroing
+          }
+          float v[32];
+#pragma unroll
+          for (int i = 0; i < 32; ++i) v[i] = stg[er * kEpiPitch + ec + i];
+          epilogue_piece<EPI, AMODE == AMODE_WINDOW>(p.epi, p.ws, n_units, m_tile, wg * 64 + er, col0 + c64 * 64 + ec, v);
         }
-        named_bar(1 + wg, 128);
-        if (AMODE == AMODE_WINDOW && (p.ws.part_out != nullptr || p.ws.part_in != nullptr)) {
-          share_piece(p.ws, 2 * split_tile, split_unit, n_units, m_tile, wg * 64 + er, col0 + c64 * 64 + ec,
-                      stg + er * kEpiPitch + ec);
-          if (p.ws.part_out != nullptr) continue;   // prefix launch: no BN, no y_hi, no pooled zeroing
-        }
-        float v[32];
-#pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = stg[er * kEpiPitch + ec + i];
-        epilogue_piece<EPI, AMODE == AMODE_WINDOW>(p.epi, p.ws, n_units, m_tile, wg * 64 + er, col0 + c64 * 64 + ec, v);
+      }
+      if (tr != nullptr) {
+        tr[5] = globaltimer();
+        tr[6] = blockIdx.x + 1;
       }
     }
+    if (FRAG && EPI == EPI_CONV1 && p.frag_epi && threadIdx.x % 128 == 0) bulk_wait_group<0>();   // the last stores are complete
   } else if (AMODE == AMODE_GATHER) {
     // ===================== fused A-operand producers (warpgroup 3) =====================
     if constexpr (Cfg::AUX_REGS < Cfg::LAUNCH_REGS) setmaxnreg_dec<Cfg::AUX_REGS>();
@@ -877,6 +1049,11 @@ int launch_umma_gemm(const UmmaGemmParams& p, int epi, int passes, int num_sms, 
   P2P_REQUIRE(passes == 1 || passes == 3, "umma gemm: passes must be 1 or 3");
   P2P_REQUIRE(p.nsteps > 0 && p.m_tiles > 0 && p.n_tiles > 0, "umma gemm: empty problem");
   const bool seg = p.seg_len > 0 && p.seg_len < p.nsteps;
+  if (p.frag_epi) {
+    P2P_REQUIRE((epi == EPI_CONV1 || epi == EPI_CONV2) && passes == 1 && !seg && amode != AMODE_GATHER,
+                "umma gemm: the fragment epilogues serve the 256-wide conv1 / conv2 launches only");
+    P2P_REQUIRE(epi == EPI_CONV2 || p.epi.y_lo == nullptr, "umma gemm: the fragment conv1 epilogue writes y_hi only");
+  }
   if (amode != AMODE_TMA) {
     P2P_REQUIRE(epi == EPI_CONV1 && passes == 1 && !seg, "the fused A operand is available for 1-pass conv1 only");
     if (amode == AMODE_GATHER) return launch_one<1, false, EPI_CONV1, AMODE_GATHER>(p, num_sms, st);

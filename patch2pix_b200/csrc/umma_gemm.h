@@ -11,6 +11,7 @@ enum { EPI_PLAIN = 0, EPI_CONV1 = 1, EPI_CONV2 = 2, EPI_CORR = 3, EPI_FC = 4 };
 // the per-image window maps (conv1)
 enum { AMODE_TMA = 0, AMODE_GATHER = 1, AMODE_WINDOW = 2 };
 constexpr int kMaxKSteps = 96;
+constexpr int kTraceStamps = 8;
 
 struct UmmaEpilogue {
   // EPI_PLAIN / EPI_CORR output
@@ -70,6 +71,8 @@ struct WindowShare {
 
 struct UmmaGemmParams {
   CUtensorMap a_main_hi, a_main_lo, a_rgb_hi, a_rgb_lo, b_hi, b_lo;
+  // EPI_CONV1 with the fragment epilogue: TMA store of epi.y_hi as [rows][64 px][512 ch], box {64 ch, 64 px, 1 row}
+  CUtensorMap y_store;
   KStep steps[kMaxKSteps];
   int nsteps;
   int m_tiles;           // 128-row tiles
@@ -77,6 +80,15 @@ struct UmmaGemmParams {
                          // B tensor maps have 128-row boxes
   int a_units_per_tile;  // step of the outermost A coordinate per m-tile (2 patches, or 128 rows)
   int seg_len;           // k-steps accumulated by the tensor core before a drain (0 / >= nsteps: whole K)
+  // 1: the 256-wide (1-pass, unsegmented) EPI_CONV1 / EPI_CONV2 launches take their epilogue straight from the wgmma
+  // fragments (conv1: the fp16 tile leaves by TMA store through y_store) instead of through the fp32 staging buffer;
+  // both write identical bits
+  int frag_epi;
+  // optional per-tile phase trace (kTraceStamps %globaltimer stamps per tile, indexed by tile; zero-filled by the host):
+  //   0 producer: the tile's first stage is free and its loads are about to issue
+  //   1 consumer warpgroup 1: tile start   2 first stage ready   3 last k-step issued   4 accumulators drained
+  //   5 epilogue done   6 blockIdx.x + 1
+  unsigned long long* trace;
   const int* d_units;    // optional device count of A units (patches): m_tiles = ceil(*d_units / a_units_per_tile)
   UmmaEpilogue epi;
   FusedGather fg;        // AMODE_GATHER

@@ -117,6 +117,22 @@ template <int N>
 __device__ __forceinline__ void bulk_wait_group_read() {     // at most N groups still READING their shared source
   asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
 }
+template <int N>
+__device__ __forceinline__ void bulk_wait_group() {          // at most N groups not yet complete (writes done)
+  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
+}
+__device__ __forceinline__ unsigned long long globaltimer() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+// four 8x8 b16 matrices from the mma fragment layout (thread l holds row l / 4, columns 2 (l % 4), +1 of each) to
+// shared memory; lane l gives the address of row l % 8 of matrix l / 8
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1), "r"(r2),
+               "r"(r3)
+               : "memory");
+}
 
 // ---- warpgroup MMA (wgmma): one warpgroup (4 aligned warps) computes a 64-row x N tile, fp32 accumulators in
 // registers.  Fragment of thread t = 32 w + l: rows 16 w + l / 4 (+ 8), columns 8 j + 2 (l % 4) (+ 1), in the order
