@@ -169,14 +169,19 @@ P2P_API int p2p_select_anchor(p2p_handle_t h, const int64_t* rows, const float* 
 
 /* ---- refine: Patch2Pix.forward_fine_match for one batch item (networks/patch2pix.py:157-218):
  * select_local_patch_feats + L2 normalise + FeatRegressNet + parse_regressor_out.
- * feats1/feats2: HOST arrays of 4 DEVICE pointers: image [3,H,W], conv1-relu [64,H/2,W/2],
- * layer1 [64,H/4,W/4], layer2 [128,H/8,W/8] (ResNet.forward_all levels 0..3, networks/resnet.py:138-157).
+ * feats1/feats2: HOST arrays of 4 DEVICE pointers, the ResNet.forward_all levels 0..3 (networks/resnet.py:138-157) as
+ * the backbone produces them for an H x W image: image [3,H,W], conv1-relu [64,h1,w1], layer1 [64,h2,w2],
+ * layer2 [128,h3,w3] with the ceiling chain h1 = ceil(H/2), h2 = ceil(h1/2), h3 = ceil(h2/2) (same for w).  Any
+ * H, W >= 8 is accepted (below 8 the reference's level-3 clamp bound W // 8 - 1 is negative); only the top-left
+ * (H >> l) x (W >> l) of level l is read, the index range of the reference's per-level clamp.  For multiples of 8 the
+ * chain is H/2, H/4, H/8.
  * `p2p_refine_prepare` must be called once per image pair before p2p_refine (it builds channels-last
  * copies and norm maps); matches_in [n,4] int64 (is_float = 0) or fp32 (is_float = 1);
  * matches_out fp32 [n,4]; probs_out fp32 [n]. */
 P2P_API int p2p_refine_prepare(p2p_handle_t h, const float* const* feats1, const float* const* feats2, int H1, int W1,
                        int H2, int W2, void* stream);
-/* Same, with levels 1..3 as channels-last fp16 maps [h][w][C] (level 0, the image, stays [3,H,W] fp32). */
+/* Same, with levels 1..3 as channels-last fp16 maps [h][w][C] of the same ceiling-chain sizes (level 0, the image,
+ * stays [3,H,W] fp32). */
 P2P_API int p2p_refine_prepare_nhwc16(p2p_handle_t h, const void* const* feats1, const void* const* feats2, int H1, int W1,
                        int H2, int W2, void* stream);
 P2P_API int p2p_refine(p2p_handle_t h, int which, const void* matches_in, int is_float, int n, float* matches_out,
@@ -198,6 +203,12 @@ P2P_API int p2p_finalize_matches(p2p_handle_t h, const float* fine, const float*
  * (ht, wt) come from cal_rescale_size (preprocess.py:83-91), computed by the caller. */
 P2P_API int p2p_preprocess_image(p2p_handle_t h, const uint8_t* rgb_hwc, int ho, int wo, int ht, int wt, float* out_chw,
                          uint8_t* resized_hwc_out, void* stream);
+/* The same for load_im_tensor (utils/datasets/preprocess.py:7-30), the loader of the refiner entry point: (ht, wt) are
+ * the caller's int(round(ho * s)), int(round(wo * s)), or (ho, wo) when the image is not downscaled.  gray_hw
+ * (optional, may be NULL): DEVICE fp32 [ht][wt], Pillow's convert('L') of the resized 8-bit image
+ * ((19595 R + 38470 G + 7471 B + 0x8000) >> 16) divided by 255, written by the same launch as out_chw. */
+P2P_API int p2p_preprocess_image_gray(p2p_handle_t h, const uint8_t* rgb_hwc, int ho, int wo, int ht, int wt,
+                         float* out_chw, float* gray_hw, void* stream);
 
 /* ---- match verification: what every consumer of the match list does next in the reference -- pydegensac's
  * findFundamentalMatrix / findHomography in examples/visualize_matches.ipynb (first cell), the F / pose RANSAC of

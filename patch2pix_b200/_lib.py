@@ -50,6 +50,7 @@ _SIGNATURES = {
     'p2p_refine': (_I, [_P, _I, _P, _I, _I, _P, _P, _P]),
     'p2p_finalize_matches': (_I, [_P, _P, _P, _P, _I, _F, C.POINTER(C.c_double), _P, _P]),
     'p2p_preprocess_image': (_I, [_P, _P, _I, _I, _I, _I, _P, _P, _P]),
+    'p2p_preprocess_image_gray': (_I, [_P, _P, _I, _I, _I, _I, _P, _P, _P]),
     'p2p_profile_read': (_I, [_P, C.POINTER(C.c_float), C.POINTER(_I), _I]),
     'p2p_test_gemm': (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _F, _P]),
     'p2p_tile_trace_read': (_I, [_P, _I, C.POINTER(_I), C.POINTER(_I), _P, _I]),

@@ -893,8 +893,8 @@ static int refine_prepare_impl(p2p_handle_t h, const float* const* feats1, const
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   P2P_REQUIRE(feats1 && feats2, "null feature list");
   for (int l = 0; l < 4; ++l) P2P_REQUIRE(feats1[l] && feats2[l], "null feature level");
-  P2P_REQUIRE(H1 >= 8 && W1 >= 8 && H2 >= 8 && W2 >= 8 && H1 % 8 == 0 && W1 % 8 == 0 && H2 % 8 == 0 && W2 % 8 == 0,
-              "image sizes must be positive multiples of 8");
+  // below 8 px the reference's level-3 clamp bound W // 8 - 1 is -1 and its index wraps around
+  P2P_REQUIRE(H1 >= 8 && W1 >= 8 && H2 >= 8 && W2 >= 8, "image sizes must be at least 8 x 8");
   const int Hs[2] = {H1, H2}, Ws[2] = {W1, W2};
   size_t need = 1 << 16;
   for (int s = 0; s < 2; ++s) {
@@ -903,7 +903,7 @@ static int refine_prepare_impl(p2p_handle_t h, const float* const* feats1, const
   }
   const bool want_map = h->opt_fuse_gather == 3;
   if (want_map)
-    for (int s = 0; s < 2; ++s) need += (size_t)(Hs[s] + 2 * kMapPad) * (Ws[s] + 2 * kMapPad) * (512 + 8) + 4096;
+    for (int s = 0; s < 2; ++s) need += (size_t)(Hs[s] + 2 * kMapPad) * map_pitch(Ws[s]) * (512 + 8) + 4096;
   int rc = h->feat.reserve(need);
   if (rc) return rc;
   const int chans[3] = {64, 64, 128};
@@ -911,7 +911,7 @@ static int refine_prepare_impl(p2p_handle_t h, const float* const* feats1, const
     PairFeatures& pf = h->pf[s];
     for (int l = 0; l < 4; ++l) {
       const int ds = 1 << l;
-      pf.nsq[l] = (float*)h->feat.take((size_t)(Hs[s] / ds) * (Ws[s] / ds) * 4);
+      pf.nsq[l] = (float*)h->feat.take((size_t)(Hs[s] / ds) * (Ws[s] / ds) * 4);   // the floor-sized crop
       P2P_REQUIRE(pf.nsq[l] != nullptr, "scratch carve failed");
     }
     for (int l = 0; l < 3; ++l) {
@@ -922,7 +922,7 @@ static int refine_prepare_impl(p2p_handle_t h, const float* const* feats1, const
     }
     pf.wmap = pf.rgbn = nullptr;
     if (want_map) {
-      const size_t pxp = (size_t)(Hs[s] + 2 * kMapPad) * (Ws[s] + 2 * kMapPad);
+      const size_t pxp = (size_t)(Hs[s] + 2 * kMapPad) * map_pitch(Ws[s]);
       pf.wmap = (__half*)h->feat.take(pxp * 512);
       pf.rgbn = (__half*)h->feat.take(pxp * 8);
       P2P_REQUIRE(pf.wmap != nullptr && pf.rgbn != nullptr, "scratch carve failed");
@@ -1057,7 +1057,7 @@ int run_regressor(p2p_handle_s* h, Regressor& R, int which, int passes, const Re
       }
       if (mapped) {
         for (int s2 = 0; s2 < 2; ++s2) {
-          const uint64_t Wp = (uint64_t)h->pf[s2].W + 2 * kMapPad, Hp = (uint64_t)h->pf[s2].H + 2 * kMapPad;
+          const uint64_t Wp = (uint64_t)map_pitch(h->pf[s2].W), Hp = (uint64_t)h->pf[s2].H + 2 * kMapPad;
           const uint64_t md[3] = {256, Wp, Hp};
           const uint64_t ms[2] = {512, Wp * 512};
           const uint32_t mb[3] = {64, 16, 16};       // 8 elements at traversal stride 2 (box = N * stride)
@@ -1273,8 +1273,8 @@ int p2p_finalize_matches(p2p_handle_t h, const float* fine, const float* scores,
                                  reinterpret_cast<cudaStream_t>(stream));
 }
 
-int p2p_preprocess_image(p2p_handle_t h, const uint8_t* rgb_hwc, int ho, int wo, int ht, int wt, float* out_chw,
-                         uint8_t* resized_hwc_out, void* stream) {
+static int preprocess_impl(p2p_handle_t h, const uint8_t* rgb_hwc, int ho, int wo, int ht, int wt, float* out_chw,
+                           uint8_t* resized_hwc_out, float* gray_hw, void* stream) {
   P2P_ENTER(h);
   P2P_REQUIRE(rgb_hwc && out_chw && ho > 0 && wo > 0 && ht > 0 && wt > 0, "bad argument");
   P2P_REQUIRE((long long)ho * wo < (1ll << 28) && (long long)ht * wt < (1ll << 28), "image too large");
@@ -1298,7 +1298,18 @@ int p2p_preprocess_image(p2p_handle_t h, const uint8_t* rgb_hwc, int ho, int wo,
   uint8_t* tmp = (uint8_t*)h->pre.take((size_t)ho * wt * 3);
   P2P_REQUIRE(tmp != nullptr, "scratch carve failed");
   const float mean[3] = {0.485f, 0.456f, 0.406f}, stdv[3] = {0.229f, 0.224f, 0.225f};   // ImageNet, preprocess.py:93
-  return launch_preprocess(rgb_hwc, *C, mean, stdv, out_chw, resized_hwc_out, tmp, reinterpret_cast<cudaStream_t>(stream));
+  return launch_preprocess(rgb_hwc, *C, mean, stdv, out_chw, resized_hwc_out, gray_hw, tmp,
+                           reinterpret_cast<cudaStream_t>(stream));
+}
+
+int p2p_preprocess_image(p2p_handle_t h, const uint8_t* rgb_hwc, int ho, int wo, int ht, int wt, float* out_chw,
+                         uint8_t* resized_hwc_out, void* stream) {
+  return preprocess_impl(h, rgb_hwc, ho, wo, ht, wt, out_chw, resized_hwc_out, nullptr, stream);
+}
+
+int p2p_preprocess_image_gray(p2p_handle_t h, const uint8_t* rgb_hwc, int ho, int wo, int ht, int wt, float* out_chw,
+                              float* gray_hw, void* stream) {
+  return preprocess_impl(h, rgb_hwc, ho, wo, ht, wt, out_chw, nullptr, gray_hw, stream);
 }
 
 int p2p_find_model(p2p_handle_t h, int model, const double* rows, int row_stride, int n, const double* n_dev, double px_th,

@@ -59,7 +59,7 @@ struct PreprocessCoefs {
 };
 int preprocess_build_coefs(int ho, int wo, int ht, int wt, PreprocessCoefs& C);
 int launch_preprocess(const uint8_t* rgb, const PreprocessCoefs& C, const float mean[3], const float stdv[3], float* out,
-                      uint8_t* resized_u8, uint8_t* tmp, cudaStream_t st);
+                      uint8_t* resized_u8, float* gray, uint8_t* tmp, cudaStream_t st);
 
 // ---- refine.cu ---------------------------------------------------------------------------------
 // Activation scale applied before the fp16 hi/lo split of the L2-normalised patch features.
@@ -75,13 +75,16 @@ struct PairFeatures {             // per image: channels-last copies + squared-n
   float* nhwc[3];                 // levels 1..3: [h][w][C], C = 64, 64, 128
   __half* nhwc16[3];              // same, fp16, each pixel divided by its own level norm sqrt(nsq[l+1])
   float* nsq[4];                  // levels 0..3: [h][w]
-  int H, W;
+  int H, W;                       // level l is stored at (H >> l) x (W >> l), the index range the reference reads
   // full-resolution window map (fuse_gather = 3): every pixel's patch-normalised 256-channel vector, replicate-padded by
-  // kMapPad pixels, [H + 2 pad][W + 2 pad][256] fp16; rgbn: the normalised rgb triple [..][4] fp16
+  // kMapPad pixels, [H + 2 pad][map_pitch(W)][256] fp16; rgbn: the normalised rgb triple [..][4] fp16
   __half* wmap;
   __half* rgbn;
 };
 constexpr int kMapPad = 16;
+// Row pitch (pixels) of the window maps: W + 2 pad rounded up to 8, so that every 8-pixel run of the map kernel stays
+// in one row whatever W is.  The columns past W + 2 pad are never read.
+__host__ __device__ constexpr int map_pitch(int W) { return (W + 2 * kMapPad + 7) & ~7; }
 int launch_window_map(const PairFeatures pf[2], cudaStream_t st);
 
 int launch_feature_prep_pair(const float* const feats1[4], const float* const feats2[4], const int H[2], const int W[2],

@@ -14,6 +14,8 @@
 //     before the vertical pass.
 // ToTensor is float32(u8) / 255 and Normalize (x - mean) / std in float32 (torchvision), reproduced with
 // correctly rounded IEEE operations.
+// The optional grey image is Pillow's convert('L') of the (resized) 8-bit image, src/libImaging/Convert.c rgb2l:
+// L = (19595 R + 38470 G + 7471 B + 0x8000) >> 16 (ITU-R 601-2 luma in 16-bit fixed point), then ToTensor's / 255.
 #include <math.h>
 
 #include <vector>
@@ -94,10 +96,12 @@ __global__ void resample_h_kernel(const uint8_t* __restrict__ in, int H, int Win
   o[2] = clip8(s2);
 }
 
-// vertical pass + ToTensor + Normalize: tmp [Hin][W][3] u8 -> out [3][Hout][W] f32.  kk == nullptr: no resampling.
+// vertical pass + ToTensor + Normalize: tmp [Hin][W][3] u8 -> out [3][Hout][W] f32 and (optional) gray [Hout][W] f32.
+// kk == nullptr: no resampling.
 __global__ void resample_v_norm_kernel(const uint8_t* __restrict__ tmp, int Hin, int W, int Hout, const int* __restrict__ bounds,
                                        const int* __restrict__ kk, int ksize, float m0, float m1, float m2, float d0, float d1,
-                                       float d2, float* __restrict__ out, uint8_t* __restrict__ out_u8) {
+                                       float d2, float* __restrict__ out, uint8_t* __restrict__ out_u8,
+                                       float* __restrict__ gray) {
   const int xx = blockIdx.x * blockDim.x + threadIdx.x, yy = blockIdx.y;
   if (xx >= W) return;
   uint8_t px[3];
@@ -130,6 +134,10 @@ __global__ void resample_v_norm_kernel(const uint8_t* __restrict__ tmp, int Hin,
   out[o] = __fdiv_rn(__fsub_rn(__fdiv_rn((float)px[0], 255.f), m0), d0);
   out[plane + o] = __fdiv_rn(__fsub_rn(__fdiv_rn((float)px[1], 255.f), m1), d1);
   out[2 * plane + o] = __fdiv_rn(__fsub_rn(__fdiv_rn((float)px[2], 255.f), m2), d2);
+  if (gray != nullptr) {
+    const int l = (px[0] * 19595 + px[1] * 38470 + px[2] * 7471 + 0x8000) >> 16;
+    gray[o] = __fdiv_rn((float)l, 255.f);
+  }
 }
 
 // Coefficient tables of one (ho, wo) -> (ht, wt) geometry, uploaded once (synchronously) and cached by the handle.
@@ -152,9 +160,9 @@ int preprocess_build_coefs(int ho, int wo, int ht, int wt, PreprocessCoefs& C) {
 }
 
 // rgb: DEVICE u8 [ho][wo][3]; out: DEVICE f32 [3][ht][wt]; resized_u8 (optional): DEVICE u8 [ht][wt][3];
-// tmp: DEVICE scratch of ho*wt*3 bytes (horizontal-pass result).
+// gray (optional): DEVICE f32 [ht][wt]; tmp: DEVICE scratch of ho*wt*3 bytes (horizontal-pass result).
 int launch_preprocess(const uint8_t* rgb, const PreprocessCoefs& C, const float mean[3], const float stdv[3], float* out,
-                      uint8_t* resized_u8, uint8_t* tmp, cudaStream_t st) {
+                      uint8_t* resized_u8, float* gray, uint8_t* tmp, cudaStream_t st) {
   const int ho = C.ho, wo = C.wo, ht = C.ht, wt = C.wt;
   const uint8_t* src = rgb;
   if (C.ksx > 0) {
@@ -166,7 +174,7 @@ int launch_preprocess(const uint8_t* rgb, const PreprocessCoefs& C, const float 
   dim3 grid(cdiv(wt, 128), ht);
   resample_v_norm_kernel<<<grid, 128, 0, st>>>(src, ho, wt, ht, C.ksy > 0 ? C.d + C.o_by : nullptr,
                                                C.ksy > 0 ? C.d + C.o_ky : nullptr, C.ksy, mean[0], mean[1], mean[2], stdv[0],
-                                               stdv[1], stdv[2], out, resized_u8);
+                                               stdv[1], stdv[2], out, resized_u8, gray);
   P2P_LAUNCH_OK();
   return 0;
 }

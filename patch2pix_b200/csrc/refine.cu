@@ -19,13 +19,16 @@ namespace p2p {
 // ------------------------------------------------------------------------------------------------
 // One launch for both images and all four levels: segment = (image, level); level 0 (rgb, C = 3) only needs its
 // squared-norm map, levels 1..3 additionally get channels-last fp32 / level-normalised fp16 copies.
+// The backbone's level l is ceil-sized (each stride-2 layer rounds up); the reference only ever indexes the top-left
+// (H >> l) x (W >> l) of it (select_local_patch_feats clamps to W // ds - 1), so that crop is what gets written.
 struct PrepSegment {
-  const float* in;     // [C][npx] fp32, or (fmt 1) [npx][C] fp16
+  const float* in;     // [C][src_h][src_w] fp32, or (fmt 1) [src_h][src_w][C] fp16
   int fmt;             // 0: NCHW fp32 (reference layout); 1: channels-last fp16 (fp16 / channels_last backbone)
   float* out;          // [npx][C] (nullptr for level 0)
   __half* out16;       // [npx][C], every pixel divided by its own norm (nullptr for level 0)
   float* nsq;          // [npx]
-  int C, npx, block0;  // first block of this segment
+  int C, npx, block0;  // npx = w * (H >> l); block0 = first block of this segment
+  int w, src_w, src_plane;   // cropped row width, input row pitch, input channel stride (fmt 0) in pixels
 };
 struct PrepArgs {
   PrepSegment seg[8];
@@ -51,12 +54,13 @@ __global__ void __launch_bounds__(256) feature_prep_kernel(const __grid_constant
     for (int pp = wid; pp < 32; pp += 8) {
       const int px = px0 + pp;
       if (px >= npx) break;
+      const int sp = g.src_w == g.w ? px : (px / g.w) * g.src_w + px % g.w;
       float v[4] = {0.f, 0.f, 0.f, 0.f};
       if (per == 2) {
-        const float2 f = __half22float2(__ldg(reinterpret_cast<const __half2*>(in16 + (size_t)px * C) + lane));
+        const float2 f = __half22float2(__ldg(reinterpret_cast<const __half2*>(in16 + (size_t)sp * C) + lane));
         v[0] = f.x; v[1] = f.y;
       } else {
-        const uint2 u = __ldg(reinterpret_cast<const uint2*>(in16 + (size_t)px * C) + lane);
+        const uint2 u = __ldg(reinterpret_cast<const uint2*>(in16 + (size_t)sp * C) + lane);
         const float2 f0 = __half22float2(*reinterpret_cast<const __half2*>(&u.x)), f1 = __half22float2(*reinterpret_cast<const __half2*>(&u.y));
         v[0] = f0.x; v[1] = f0.y; v[2] = f1.x; v[3] = f1.y;
       }
@@ -76,9 +80,10 @@ __global__ void __launch_bounds__(256) feature_prep_kernel(const __grid_constant
     return;
   }
   const int px = px0 + lane;
+  const int sp = g.src_w == g.w ? px : (px / g.w) * g.src_w + px % g.w;   // crop only where the level is ceil-sized
   float s = 0.f;
   for (int c = wid; c < C; c += 8) {
-    const float v = px < npx ? __ldg(g.in + (size_t)c * npx + px) : 0.f;
+    const float v = px < npx ? __ldg(g.in + (size_t)c * g.src_plane + sp) : 0.f;
     tile[c * 33 + lane] = v;
     s = fmaf(v, v, s);
   }
@@ -114,13 +119,20 @@ int launch_feature_prep_pair(const float* const feats1[4], const float* const fe
     out[s].img = f[0];
     out[s].H = H[s];
     out[s].W = W[s];
+    int src_h = H[s], src_w = W[s];
     for (int l = 0; l < 4; ++l) {
       PrepSegment& g = a.seg[a.nseg++];
-      const int ds = 1 << l;
+      if (l > 0) {                          // ResNet's stride-2 layers: ceil(h / 2)
+        src_h = (src_h + 1) >> 1;
+        src_w = (src_w + 1) >> 1;
+      }
       g.in = f[l];
       g.fmt = l > 0 ? fmt : 0;              // the image (level 0) is always NCHW fp32
       g.C = chans[l];
-      g.npx = (H[s] / ds) * (W[s] / ds);
+      g.w = W[s] >> l;
+      g.src_w = src_w;
+      g.src_plane = src_h * src_w;
+      g.npx = (H[s] >> l) * g.w;
       g.nsq = out[s].nsq[l];
       g.out = l > 0 ? out[s].nhwc[l - 1] : nullptr;
       g.out16 = l > 0 ? out[s].nhwc16[l - 1] : nullptr;
@@ -135,11 +147,13 @@ int launch_feature_prep_pair(const float* const feats1[4], const float* const fe
 
 // ------------------------------------------------------------------------------------------------
 // Window map (fuse_gather = 3).  The 259-channel L2-normalised vector of a window pixel depends only on its absolute
-// (clamped) image position (select_local_patch_feats clamps per level, networks/utils.py:22-23, which equals clamping
-// the full-resolution coordinate first), so it is computed ONCE per image pixel: map[y + pad][x + pad][0..255] =
+// image position, so it is computed ONCE per image pixel: map[y + pad][x + pad][0..255] =
 // kActScale * concat(l1, l2, l3)(y, x) / sqrt(sum_c f^2 + 1e-6), replicate-padded.  The conv1 implicit GEMM then reads
-// every tap of every patch as one strided TMA box.  One warp per padded pixel; lane = one 16-byte channel chunk.
-// Arithmetic identical to the in-kernel producers of umma_conv1_fused_kernel (bit-identical A operand).
+// every tap of every patch as one strided TMA box.  One warp per 8 pixels of a padded row; lane = one 16-byte channel
+// chunk.  Arithmetic identical to the in-kernel producers of umma_conv1_fused_kernel (bit-identical A operand).
+// select_local_patch_feats clamps per level (networks/utils.py:22-23): level l reads min(x >> l, (W >> l) - 1) for the
+// full-resolution coordinate clamped to [0, W - 1].  The second bound only bites when 2^l does not divide W: for
+// W = 9, x = 8 gives level-1 index 3, not 8 >> 1 = 4.
 // ------------------------------------------------------------------------------------------------
 struct WindowMapArgs {
   const float* img[2];
@@ -151,7 +165,7 @@ struct WindowMapArgs {
   long long px0[3];     // first padded-pixel index of image 1; total
 };
 
-constexpr int kMapPxPerWarp = 8;     // consecutive pixels of one padded row (W is a multiple of 8, so is W + 2 * pad)
+constexpr int kMapPxPerWarp = 8;     // consecutive pixels of one padded row (map_pitch is a multiple of 8)
 
 __global__ void __launch_bounds__(256) window_map_kernel(const __grid_constant__ WindowMapArgs a) {
   const int lane = threadIdx.x & 31;
@@ -159,27 +173,30 @@ __global__ void __launch_bounds__(256) window_map_kernel(const __grid_constant__
   if (q0 >= (int)a.px0[2]) return;
   const int si = q0 >= (int)a.px0[1] ? 1 : 0;
   const int qb = q0 - (int)a.px0[si];
-  const int W = a.W[si], H = a.H[si], Wp = W + 2 * kMapPad;
+  const int W = a.W[si], H = a.H[si], Wp = map_pitch(W);
   const int yp = qb / Wp, xp0 = qb - yp * Wp;
   const int Y = min(max(yp - kMapPad, 0), H - 1);
   const int lvl = lane < 8 ? 0 : (lane < 16 ? 1 : 2);
   const int sh = lvl + 1, C = lvl == 2 ? 128 : 64;
   const int coff = (lane < 16 ? (lane & 7) : (lane - 16)) * 8;
+  const int W1 = W >> 1, W2 = W >> 2, W3 = W >> 3, Wl = W >> sh;
   const float* nsq0 = a.nsq[si][0] + (size_t)Y * W;
-  const float* nsq1 = a.nsq[si][1] + (size_t)(Y >> 1) * (W >> 1);
-  const float* nsq2 = a.nsq[si][2] + (size_t)(Y >> 2) * (W >> 2);
-  const float* nsq3 = a.nsq[si][3] + (size_t)(Y >> 3) * (W >> 3);
+  const float* nsq1 = a.nsq[si][1] + (size_t)min(Y >> 1, (H >> 1) - 1) * W1;
+  const float* nsq2 = a.nsq[si][2] + (size_t)min(Y >> 2, (H >> 2) - 1) * W2;
+  const float* nsq3 = a.nsq[si][3] + (size_t)min(Y >> 3, (H >> 3) - 1) * W3;
   const float* nsql = lvl == 0 ? nsq1 : (lvl == 1 ? nsq2 : nsq3);
-  const __half* frow = a.nhwc16[si][lvl] + (size_t)(Y >> sh) * (W >> sh) * C + coff;
+  const __half* frow = a.nhwc16[si][lvl] + (size_t)min(Y >> sh, (H >> sh) - 1) * Wl * C + coff;
   // phase 1: every load of the warp's 8 pixels in flight; phase 2: scale and store
   uint4 v[kMapPxPerWarp];
   float t[kMapPxPerWarp], nl[kMapPxPerWarp], rgb[kMapPxPerWarp];
 #pragma unroll
   for (int u = 0; u < kMapPxPerWarp; ++u) {
     const int X = min(max(xp0 + u - kMapPad, 0), W - 1);
-    t[u] = ((__ldg(nsq0 + X) + __ldg(nsq1 + (X >> 1))) + __ldg(nsq2 + (X >> 2))) + __ldg(nsq3 + (X >> 3));
-    nl[u] = __ldg(nsql + (X >> sh));
-    v[u] = __ldg(reinterpret_cast<const uint4*>(frow + (size_t)(X >> sh) * C));
+    const int xl = min(X >> sh, Wl - 1);
+    t[u] = ((__ldg(nsq0 + X) + __ldg(nsq1 + min(X >> 1, W1 - 1))) + __ldg(nsq2 + min(X >> 2, W2 - 1))) +
+           __ldg(nsq3 + min(X >> 3, W3 - 1));
+    nl[u] = __ldg(nsql + xl);
+    v[u] = __ldg(reinterpret_cast<const uint4*>(frow + (size_t)xl * C));
     rgb[u] = lane < 3 ? __ldg(a.img[si] + ((size_t)lane * H + Y) * W + X) : 0.f;
   }
   __half* wrow = a.wmap[si] + (size_t)qb * 256;
@@ -212,7 +229,7 @@ int launch_window_map(const PairFeatures pf[2], cudaStream_t st) {
     a.H[s] = pf[s].H;
     a.W[s] = pf[s].W;
     a.px0[s] = tot;
-    tot += (long long)(pf[s].H + 2 * kMapPad) * (pf[s].W + 2 * kMapPad);
+    tot += (long long)(pf[s].H + 2 * kMapPad) * map_pitch(pf[s].W);
   }
   a.px0[2] = tot;
   window_map_kernel<<<(unsigned)((tot + 8 * kMapPxPerWarp - 1) / (8 * kMapPxPerWarp)), 256, 0, st>>>(a);

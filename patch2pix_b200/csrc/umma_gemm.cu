@@ -809,7 +809,7 @@ __global__ void __launch_bounds__(256) window_rgb_kernel(const __grid_constant__
 #pragma unroll
     for (int si = 0; si < 2; ++si) {
       const int bx = window_origin(wm, r, 2 * si), by = window_origin(wm, r, 2 * si + 1);
-      const int Wp = wm.W[si] + 2 * kMapPad;
+      const int Wp = map_pitch(wm.W[si]);
 #pragma unroll
       for (int tap = 0; tap < 9; ++tap) {
         const int wx = 2 * ox - 1 + tap % 3, wy = 2 * oy - 1 + tap / 3;

@@ -45,8 +45,8 @@ struct FusedGather {
 // conv1 fed by strided TMA boxes of the per-image window maps (AMODE_WINDOW); the rgb k-step comes by TMA (a_rgb_hi)
 // from the im2col tensor launch_window_rgb builds out of rgbn
 struct WindowMaps {
-  CUtensorMap map[2];             // [H + 2 pad][W + 2 pad][256] fp16 per image; box = 64 ch x 8 (stride 2) x 8 (stride 2)
-  const __half* rgbn[2];          // [H + 2 pad][W + 2 pad][4]
+  CUtensorMap map[2];             // [H + 2 pad][map_pitch(W)][256] fp16 per image; box = 64 ch x 8 (stride 2) x 8 (stride 2)
+  const __half* rgbn[2];          // [H + 2 pad][map_pitch(W)][4]
   int H[2], W[2];
   const void* matches;
   int is_float;

@@ -165,3 +165,23 @@ def estimate_matches_from_files(net, im1_path, im2_path, ksize=2, ncn_thres=0.0,
     im2, sc2 = load_im_flexible(im2_path, ksize, net.upsample, imsize=imsize, device=net.device, handle=net._handle)
     return estimate_matches(net, im1.unsqueeze(0), im2.unsqueeze(0), sc1, sc2, ksize, ncn_thres, mutual, io_thres, eval_type,
                             verify)
+
+
+def refine_matches(im1_path, im2_path, net, coarse_matcher, io_thres=0.0, imsize=None, coarse_only=False):
+    """utils/eval/model_helper.py:111-127: Patch2Pix as the refiner of another matcher's coarse matches.  Both images
+    are loaded with load_im_tensor (any size; only the file decode runs on the host), `coarse_matcher(grey1, grey2)`
+    gets the [1,1,H,W] grey device tensors and returns [N,4] (x1, y1, x2, y2) rows in those images' pixels (numpy or
+    torch, int64 / float32 / float64), and net.refine_matches refines them.  -> (refined, scores, coarse): float64
+    matches in original-image pixels and float32 scores, filtered by `scores > io_thres` when io_thres > 0 (keeping
+    every row if none passes); coarse_only -> (coarse, None, None)."""
+    from .preprocess import load_im_tensor
+    im1, grey1, sc1 = load_im_tensor(im1_path, net.device, imsize, with_gray=True, handle=net._handle)
+    im2, grey2, sc2 = load_im_tensor(im2_path, net.device, imsize, with_gray=True, handle=net._handle)
+    upscale = np.array([sc1 + sc2])
+    coarse_matches = coarse_matcher(grey1, grey2)
+    if coarse_only:
+        cm = coarse_matches.cpu().numpy() if isinstance(coarse_matches, torch.Tensor) else np.asarray(coarse_matches)
+        return upscale * cm, None, None
+    with torch.no_grad():
+        refined, scores, coarse = net.refine_matches(im1, im2, coarse_matches, io_thres)
+    return upscale * refined, scores, upscale * coarse

@@ -331,6 +331,21 @@ class _RegressorParams(nn.Module):
         raise RuntimeError('regressor parameters are consumed by libp2p_b200; there is no eager path')
 
 
+def refine_level_shapes(H, W):
+    """Shapes of the pyramid levels 0..3 the refine stage reads for an H x W image, as the backbone produces them:
+    the image [3,H,W], then each stride-2 layer rounds up (h1 = ceil(H/2), h2 = ceil(h1/2), h3 = ceil(h2/2)).
+    Below 8 px the reference's level-3 clamp bound W // 8 - 1 is negative and its index wraps around, so such
+    sizes are refused."""
+    H, W = int(H), int(W)
+    if H < 8 or W < 8:
+        raise RuntimeError(f'the refine stage needs images of at least 8 x 8 pixels, got {H} x {W}')
+    shapes = [(3, H, W)]
+    for c in (64, 64, 128):
+        H, W = (H + 1) // 2, (W + 1) // 2
+        shapes.append((c, H, W))
+    return shapes
+
+
 def _host_f32(t):
     return t.detach().to('cpu', torch.float32).contiguous()
 
@@ -514,7 +529,7 @@ class Patch2PixB200(nn.Module):
         _, H1, W1 = lv1[0].shape
         _, H2, W2 = lv2[0].shape
         for lv, H, W in ((lv1, H1, W1), (lv2, H2, W2)):
-            exp = [(3, H, W), (64, H // 2, W // 2), (64, H // 4, W // 4), (128, H // 8, W // 8)]
+            exp = refine_level_shapes(H, W)
             if [tuple(t.shape) for t in lv] != exp:
                 raise RuntimeError(f'feature pyramid shapes {[tuple(t.shape) for t in lv]} do not match {exp}')
         a1 = (C.c_void_p * 4)(*[t.data_ptr() for t in lv1])
@@ -756,24 +771,37 @@ class Patch2PixB200(nn.Module):
         return self.match_from_feats(feats1, feats2, ksize, 0.0, True, ptmax, return_all)
 
     def refine_matches(self, im1, im2, coarse_matches, io_thres):
-        """networks/patch2pix.py:278-318."""
+        """networks/patch2pix.py:278-318.  coarse_matches [N,4] numpy or torch (any device), int64 or float; float64
+        rows are refined as float32, which is what the reference's parse_regressor_out computes in (`.float()`).
+        The refined rows, their scores and (for a device tensor) the coarse rows come back in one device->host copy."""
         if len(coarse_matches) == 0:
             return np.empty((0, 4)), np.empty((0,)), np.empty((0, 4))
+        host_cm = None
         if isinstance(coarse_matches, np.ndarray):
-            cm_ = torch.from_numpy(coarse_matches).to(self.device).unsqueeze(0)
+            host_cm = coarse_matches
+            cm_ = torch.from_numpy(coarse_matches).to(self.device)
         elif isinstance(coarse_matches, torch.Tensor):
-            cm_ = coarse_matches.to(self.device).unsqueeze(0)
-            coarse_matches = coarse_matches.cpu().data.numpy()
+            if not coarse_matches.is_cuda:
+                host_cm = coarse_matches.data.numpy()
+            cm_ = coarse_matches.to(self.device)
         else:
             raise RuntimeError('coarse_matches must be a numpy array or a torch tensor')
-        if cm_.dtype not in (torch.int64, torch.float32):
-            cm_ = cm_.float() if cm_.is_floating_point() else cm_.long()
+        cm_k = cm_
+        if cm_k.dtype not in (torch.int64, torch.float32):
+            cm_k = cm_k.float() if cm_k.is_floating_point() else cm_k.long()
         feats1 = self.extract.forward_all(im1, [], early_feat=True)
         feats2 = self.extract.forward_all(im2, [], early_feat=True)
-        mid, _ = self.forward_fine_match(feats1, feats2, cm_, self.psize[0], self.ptype[0], self.regress_mid)
+        mid, _ = self.forward_fine_match(feats1, feats2, [cm_k], self.psize[0], self.ptype[0], self.regress_mid)
         fine, fine_p = self.forward_fine_match(feats1, feats2, mid, self.psize[1], self.ptype[1], self.regress_fine)
-        both = torch.cat([fine[0].reshape(-1, 4), fine_p[0].reshape(-1, 1)], 1).cpu().numpy()   # one device->host copy
-        refined, scores = np.ascontiguousarray(both[:, :4]), np.ascontiguousarray(both[:, 4])
+        # float64 holds fp32 and the coarse rows (int64 below 2^53, fp32, fp64) exactly
+        cols = [fine[0].reshape(-1, 4).double(), fine_p[0].reshape(-1, 1).double()]
+        if host_cm is None:
+            cols.append(cm_.reshape(-1, 4).double())
+        both = torch.cat(cols, 1).cpu().numpy()          # one device->host copy
+        refined, scores = both[:, :4].astype(np.float32), both[:, 4].astype(np.float32)
+        if host_cm is None:
+            host_cm = both[:, 5:].astype(torch.empty(0, dtype=cm_.dtype).numpy().dtype)
+        coarse_matches = host_cm
         if io_thres > 0:
             pos = np.where(scores > io_thres)[0]
             if len(pos) > 0:

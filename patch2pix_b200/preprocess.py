@@ -59,3 +59,41 @@ def load_im_flexible(im_path, k_size=2, upsample=16, imsize=None, crop_square=Fa
         _, hh, ww = out.shape
         out = out[:, :ww, :]
     return out, scale
+
+
+def tensor_size(wo, ho, imsize=None):
+    """load_im_tensor's target size (utils/datasets/preprocess.py:11-16): downscale only when max(wo, ho) > imsize > 0,
+    to int(round(ho * s)) x int(round(wo * s)) with s = imsize / max(wo, ho) (Python's round); otherwise the image keeps
+    its own size.  -> (wt, ht)"""
+    if imsize and imsize > 0 and max(wo, ho) > imsize:
+        s = imsize / max(wo, ho)
+        return int(round(wo * s)), int(round(ho * s))
+    return wo, ho
+
+
+def load_im_tensor(im_path, device, imsize=None, with_gray=True, handle=None):
+    """utils/datasets/preprocess.py:7-30, the refiner's loader, with everything after the file decode on the GPU:
+    the Pillow-exact bicubic downscale, ToTensor + Normalize and the grey image (Pillow's convert('L') / 255) come out
+    of one launch chain.  -> (im [1,3,ht,wt], grey [1,1,ht,wt], (wo / wt, ho / ht)) on `device`, or (im, scale)
+    without `with_gray`.  Only RGB files are read (the reference's Normalize fails on any other mode)."""
+    from PIL import Image                        # host I/O only: file-format decoding
+    with Image.open(im_path) as im:
+        if im.mode != 'RGB':
+            raise RuntimeError(f'load_im_tensor reads RGB images only; {im_path} is {im.mode}')
+        rgb = np.asarray(im)
+    device = torch.device(device)
+    if device.type != 'cuda':
+        raise RuntimeError('load_im_tensor runs on a CUDA device (no CPU fallback)')
+    ho, wo = int(rgb.shape[0]), int(rgb.shape[1])
+    wt, ht = tensor_size(wo, ho, imsize)
+    if wt <= 0 or ht <= 0:
+        raise RuntimeError(f'imsize {imsize} shrinks the {wo}x{ho} image {im_path} to nothing')
+    h = handle or _lib.default_handle(device)
+    with torch.cuda.device(device):
+        src = torch.from_numpy(np.array(rgb, copy=True, order='C')).pin_memory().to(device, non_blocking=True)
+        out = torch.empty(1, 3, ht, wt, dtype=torch.float32, device=device)
+        gray = torch.empty(1, 1, ht, wt, dtype=torch.float32, device=device) if with_gray else None
+        _lib.check(h.lib.p2p_preprocess_image_gray(h.h, _lib.ptr(src), ho, wo, ht, wt, _lib.ptr(out), _lib.ptr(gray),
+                                                   h.stream()))
+    scale = (wo / wt, ho / ht)
+    return (out, gray, scale) if with_gray else (out, scale)

@@ -330,3 +330,36 @@ def synthetic_val_scene(root, scene, seed, sizes, ext='.png', missing=(), min_ov
     write_colmap_model(model_dir, cameras, images)
     np.save(os.path.join(model_dir, 'ov_pairs.npy'), {min_overlap: pairs})
     return pairs
+
+
+def synthetic_photo_pair(seed, size1, size2, shift=(8, 16)):
+    """Two 8-bit RGB views ([H,W,3] uint8 numpy) of one blocky texture at their own sizes size1 = (H1, W1) and
+    size2 = (H2, W2), view 2 cropped shift = (dy, dx) px further into it.  Integer arithmetic only, so every machine
+    writes the same pixels: the files the refiner's loader reads in tests and benchmarks."""
+    rng = np.random.default_rng(4000 + int(seed))
+    (h1, w1), (h2, w2) = (tuple(int(v) for v in s) for s in (size1, size2))
+    dy, dx = shift
+    H, W = max(h1, h2 + dy), max(w1, w2 + dx)
+    low = rng.integers(0, 256, size=(H // 8 + 2, W // 8 + 2, 3), dtype=np.int32)
+    base = np.repeat(np.repeat(low, 8, 0), 8, 1)[:H + 4, :W + 4]
+    base = (base[:H, :W] + base[4:H + 4, :W] + base[:H, 4:W + 4] + base[4:H + 4, 4:W + 4]) // 4
+    img = np.clip(base + rng.integers(-12, 13, size=base.shape), 0, 255).astype(np.uint8)
+    return img[:h1, :w1].copy(), img[dy:dy + h2, dx:dx + w2].copy()
+
+
+def grid_coarse_matcher(shift=(8, 16), step=12, dtype=torch.float32):
+    """Deterministic stand-in for a third-party coarse matcher (SuperPoint, SuperGlue, ...) in the refiner workflow:
+    called with the two grey images [1,1,H,W], it returns [N,4] (x1, y1, x2, y2) rows of `dtype` on their device, a
+    grid in image 1 shifted by shift = (dy, dx) into image 2, plus rows on and past the borders of each image."""
+    def matcher(grey1, grey2):
+        h1, w1 = grey1.shape[-2:]
+        h2, w2 = grey2.shape[-2:]
+        ys, xs = torch.meshgrid(torch.arange(2, h1 + 8, step, dtype=torch.float64),
+                                torch.arange(3, w1 + 8, step, dtype=torch.float64), indexing='ij')
+        x1, y1 = xs.flatten() + 0.375, ys.flatten() + 0.625
+        rows = torch.stack([x1, y1, x1 - shift[1], y1 - shift[0]], 1)
+        edge = torch.tensor([[0.0, 0.0, w2 - 1.0, h2 - 1.0], [w1 - 1.0, h1 - 1.0, 0.0, 0.0], [w1, h1, w2, h2],
+                             [w1 + 3.0, -2.5, 7.999, 8.0], [w1 / 2, h1 / 2, w2 + 20.0, h2 + 5.0],
+                             [-30.0, h1 + 9.0, w2 / 2, h2 / 2]], dtype=torch.float64)
+        return torch.cat([edge, rows]).to(dtype=dtype, device=grey1.device)
+    return matcher
