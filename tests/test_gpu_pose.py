@@ -9,6 +9,7 @@ import torch
 
 from oracle import pose_oracle as P
 from patch2pix_b200.synth import synthetic_two_view
+from test_gpu_verify import _dtoh
 
 pytestmark = pytest.mark.gpu
 BAND = 1e-4
@@ -193,15 +194,6 @@ def test_edge_cases():
     n, R, t, good = recover_pose(E, sc['pts1'], sc['pts2'], sc['K1'], sc['K2'], mask)
     assert n >= 0.95 * (mask & lab).sum()
     assert np.degrees(np.arccos(np.clip((np.trace(R.T @ sc['R']) - 1) / 2, -1, 1))) < 0.5
-
-
-def _dtoh(fn):
-    from torch.profiler import ProfilerActivity, profile
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
-        out = fn()
-        torch.cuda.synchronize()
-    return out, sum(1 for e in prof.events() if 'Memcpy DtoH' in e.name)
 
 
 def test_estimate_matches_pose_pipeline(consensus_sd):

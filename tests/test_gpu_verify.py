@@ -183,9 +183,15 @@ def test_sampson_distance_matches_oracle():
 
 
 def _dtoh(fn):
+    """fn()'s result and the device->host copies it made.  The profiler can drop the device activity a session records
+    first: on an H100, after earlier sessions in the same process, every other session lost a short call's kernels and
+    copy.  So the window opens with copy-free matmuls and fn() runs after them."""
     from torch.profiler import ProfilerActivity, profile
+    pad = torch.full((2048, 2048), 1.0 / 2048, device='cuda')
     torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+        for _ in range(60):
+            pad = pad @ pad
         out = fn()
         torch.cuda.synchronize()
     return out, sum(1 for e in prof.events() if 'Memcpy DtoH' in e.name)
