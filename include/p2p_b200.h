@@ -67,6 +67,13 @@ P2P_API int p2p_destroy(p2p_handle_t h);
  * w1 = ncn.conv.0.weight [3,16,1,3,3,3], b1 [16], w2 = ncn.conv.2.weight [3,1,16,3,3,3], b2 [1]. */
 P2P_API int p2p_set_ncn_weights(p2p_handle_t h, const float* w1, const float* b1, const float* w2, const float* b2);
 
+/* A general NeighConsensus stack (NCNet's ImMatchNet, networks/ncn/model.py:124-155), packed beside the Patch2Pix weights
+ * above: n_layers Conv4d layers (1..16), kernel_sizes[l] in {3, 5}, channels[l] in 1..16 with channels[n_layers-1] == 1.
+ * weights[l]: HOST fp32 in the reference's pre-permuted layout [k, Cout, Cin, k, k, k] (conv4d.py:118-120), Cin = 1 for
+ * layer 0 and channels[l-1] after; biases[l] [Cout].  symmetric != 0: conv(x) + conv(x^T)^T (symmetric_mode). */
+P2P_API int p2p_set_nc_stack_weights(p2p_handle_t h, int n_layers, const int* kernel_sizes, const int* channels,
+                                     const float* const* weights, const float* const* biases, int symmetric);
+
 /* which: 0 = regress_mid, 1 = regress_fine (networks/patch2pix.py:53-58). */
 P2P_API int p2p_set_regressor_weights(p2p_handle_t h, int which, const p2p_regressor_weights_t* w);
 
@@ -139,6 +146,13 @@ P2P_API int p2p_delta_pack(p2p_handle_t h, const int64_t* di, const int64_t* dj,
 P2P_API int p2p_mutual_matching(p2p_handle_t h, const float* in, int nA, int nB, float* out, void* stream);
 /* NeighConsensus alone (networks/ncn/model.py:145-155) on [hA,wA,hB,wB]. */
 P2P_API int p2p_neigh_consensus(p2p_handle_t h, const float* in, int hA, int wA, int hB, int wB, float* out, void* stream);
+/* The stack of p2p_set_nc_stack_weights alone on [hA,wA,hB,wB] fp32 (tensor cores; timed as P2P_PROF_NC). */
+P2P_API int p2p_nc_stack(p2p_handle_t h, const float* in, int hA, int wA, int hB, int wB, float* out, void* stream);
+/* ImMatchNet.forward_feat (networks/ncn/model.py:289-312) for one pair: L2-normalised features feat1 [c,h1,w1],
+ * feat2 [c,h2,w2] (c % 64 == 0) -> correlation, maxpool4d (ksize 2) -> MutualMatching -> the stack ->
+ * MutualMatching.  corr4d_out and delta_code_out as for p2p_coarse. */
+P2P_API int p2p_ncnet_coarse(p2p_handle_t h, const float* feat1, const float* feat2, int c, int h1, int w1, int h2, int w2,
+                             int ksize, float* corr4d_out, uint8_t* delta_code_out, void* stream);
 
 /* ---- proposals: Patch2Pix.cal_coarse_matches (networks/patch2pix.py:340-375, sort=False) over
  * corr_to_matches (networks/ncn/extract_ncmatches.py:6-94).  corr4d [hA*wA, hB*wB]; delta_code may be

@@ -42,6 +42,9 @@ _SIGNATURES = {
     'p2p_delta_pack': (_I, [_P, _P, _P, _P, _P, _LL, _I, _P, _P]),
     'p2p_mutual_matching': (_I, [_P, _P, _I, _I, _P, _P]),
     'p2p_neigh_consensus': (_I, [_P, _P, _I, _I, _I, _I, _P, _P]),
+    'p2p_set_nc_stack_weights': (_I, [_P, _I, _P, _P, _P, _P, _I]),
+    'p2p_nc_stack': (_I, [_P, _P, _I, _I, _I, _I, _P, _P]),
+    'p2p_ncnet_coarse': (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _P]),
     'p2p_proposals': (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P]),
     'p2p_unique_rows': (_I, [_P, _P, _I, _I, _P, _F, _P, _P, _P]),
     'p2p_select_anchor': (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P]),

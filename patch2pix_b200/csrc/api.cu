@@ -113,6 +113,8 @@ struct p2p_handle_s {
   float *nc_w1p = nullptr, *nc_b1p = nullptr, *nc_w2p = nullptr;
   float nc_b2 = 0.f;
   NcUmmaWeights ncw;            // tensor-core NC operand images
+  NcStackWeights ncs;           // general NeighConsensus stack (p2p_set_nc_stack_weights), beside the fixed stack above
+  bool ncs_set = false;
   void* dbg_nc[4] = {nullptr, nullptr, nullptr, nullptr};   // scratch of the last p2p_neigh_consensus call (debug hook below)
   int opt_unique_impl = 1;      // 1: rank sort over the whole GPU for lists <= 8192 rows; 0: single-block bitonic network
   int* uniq_rank = nullptr;     // zeroed scratch of the rank-sort path
@@ -461,6 +463,7 @@ int p2p_destroy(p2p_handle_t h) {
   for (auto e : h->event_pool) cudaEventDestroy(e);
   if (h->nc_w1p) cudaFree(h->nc_w1p);
   if (h->ncw.blob) cudaFree(h->ncw.blob);
+  nc_stack_release(h->ncs);
   if (h->band_totals) cudaFree(h->band_totals);
   if (h->share_rows) cudaFree(h->share_rows);
   if (h->trace_buf) cudaFree(h->trace_buf);
@@ -502,6 +505,16 @@ int p2p_set_ncn_weights(p2p_handle_t h, const float* w1, const float* b1, const 
     if (rc) return rc;
   }
   h->nc_set = true;
+  return 0;
+}
+
+int p2p_set_nc_stack_weights(p2p_handle_t h, int n_layers, const int* kernel_sizes, const int* channels,
+                              const float* const* weights, const float* const* biases, int symmetric) {
+  P2P_ENTER(h);
+  P2P_REQUIRE(kernel_sizes && channels && weights && biases, "null argument");
+  int rc = nc_stack_pack(n_layers, kernel_sizes, channels, weights, biases, symmetric, h->ncs);
+  if (rc) return rc;
+  h->ncs_set = true;
   return 0;
 }
 
@@ -778,6 +791,66 @@ int p2p_coarse_nhwc16(p2p_handle_t h, const void* feat1_nhwc16, const void* feat
                      h2, w2, ksize, corr4d_out, delta_code_out, pooled_out, ncn_out, stream);
 }
 
+int p2p_ncnet_coarse(p2p_handle_t h, const float* feat1, const float* feat2, int c, int h1, int w1, int h2, int w2, int ksize,
+                     float* corr4d_out, uint8_t* delta_code_out, void* stream) {
+  P2P_ENTER(h);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  P2P_REQUIRE(h->ncs_set, "p2p_set_nc_stack_weights has not been called");
+  P2P_REQUIRE(feat1 && feat2 && corr4d_out, "null tensor pointer");
+  P2P_REQUIRE(ksize == 1 || ksize == 2, "ksize must be 1 or 2");
+  P2P_REQUIRE(c > 0 && h1 > 0 && w1 > 0 && h2 > 0 && w2 > 0, "empty feature map");
+  P2P_REQUIRE(c % 64 == 0 && c / 64 <= kMaxKSteps, "the tensor-core correlation needs C % 64 == 0");
+  P2P_REQUIRE(h->opt_corr_passes > 0, "p2p_ncnet_coarse needs the tensor-core correlation (corr_passes 1 or 3)");
+  if (ksize == 2) {
+    P2P_REQUIRE(h1 % 2 == 0 && w1 % 2 == 0 && h2 % 2 == 0 && w2 % 2 == 0, "ksize 2 needs even feature sizes");
+    P2P_REQUIRE(delta_code_out != nullptr, "delta_code_out is required for ksize 2");
+  }
+  const int n1 = h1 * w1, n2 = h2 * w2;
+  const int hA = h1 / ksize, wA = w1 / ksize, hB = h2 / ksize, wB = w2 / ksize;
+  const int nA = hA * wA, nB = hB * wB;
+  const size_t V = (size_t)nA * nB;
+  const int n1pad = (int)align_up(n1, 128), n2pad = (int)align_up(n2, 256);
+  // pooled, m1, nc [V] f32; the stack's line buffers; MutualMatching maxima; the fp16 hi/lo correlation operands
+  const size_t need = 3 * V * 4 + nc_stack_scratch_bytes(V) + (size_t)(nA + nB) * 4 + (size_t)(n1pad + n2pad) * c * 4 +
+                      (1 << 16);
+  int rc = h->coarse.reserve(need);
+  if (rc) return rc;
+  Arena& A = h->coarse;
+  float* pooled = (float*)A.take(V * 4);
+  float* m1 = (float*)A.take(V * 4);
+  float* nc = (float*)A.take(V * 4);
+  __half* lines = (__half*)A.take(nc_stack_scratch_bytes(V));
+  float* rowmax = (float*)A.take((size_t)nA * 4);
+  unsigned int* colmax = (unsigned int*)A.take((size_t)nB * 4 + 16);
+  unsigned int* xmax = colmax != nullptr ? colmax + nB : nullptr;
+  __half* a_hi = (__half*)A.take((size_t)n1pad * c * 2);
+  __half* a_lo = (__half*)A.take((size_t)n1pad * c * 2);
+  __half* b_hi = (__half*)A.take((size_t)n2pad * c * 2);
+  __half* b_lo = (__half*)A.take((size_t)n2pad * c * 2);
+  P2P_REQUIRE(pooled && m1 && nc && lines && rowmax && colmax && a_hi && a_lo && b_hi && b_lo, "scratch carve failed");
+  const bool lo = h->opt_corr_passes == 3;
+  {
+    ProfScope ps(h, P2P_PROF_L2NORM, st);
+    if ((rc = launch_l2norm_perm_kmajor_pair(feat1, feat2, a_hi, lo ? a_lo : nullptr, b_hi, lo ? b_lo : nullptr, c, h1, w1,
+                                             h2, w2, ksize, st)))
+      return rc;
+  }
+  {
+    ProfScope ps(h, P2P_PROF_CORR, st);
+    if ((rc = corr_umma(h, a_hi, a_lo, b_hi, b_lo, c, n1, n2, n1pad, n2pad, ksize, pooled, delta_code_out, st))) return rc;
+  }
+  {
+    ProfScope ps(h, P2P_PROF_MUTUAL, st);
+    if ((rc = launch_mutual_matching(pooled, nA, nB, rowmax, colmax, m1, xmax, st))) return rc;
+  }
+  {
+    ProfScope ps(h, P2P_PROF_NC, st);
+    if ((rc = launch_nc_stack(m1, hA, wA, hB, wB, h->ncs, xmax, lines, nc, sms(h), st))) return rc;
+  }
+  ProfScope ps(h, P2P_PROF_MUTUAL, st);
+  return launch_mutual_matching(nc, nA, nB, rowmax, colmax, corr4d_out, nullptr, st);
+}
+
 int p2p_delta_unpack(p2p_handle_t h, const uint8_t* code, long long n, int ksize, int64_t* di, int64_t* dj,
                      int64_t* dk, int64_t* dl, void* stream) {
   P2P_ENTER(h);
@@ -826,6 +899,22 @@ int p2p_neigh_consensus(p2p_handle_t h, const float* in, int hA, int wA, int hB,
                                        nullptr, nullptr, h->opt_nc_l2_mode, sms(h), st);
   }
   return launch_neigh_consensus(in, hA, wA, hB, wB, h->nc_w1p, h->nc_b1p, h->nc_w2p, h->nc_b2, hidden, out, st);
+}
+
+int p2p_nc_stack(p2p_handle_t h, const float* in, int hA, int wA, int hB, int wB, float* out, void* stream) {
+  P2P_ENTER(h);
+  P2P_REQUIRE(h->ncs_set, "p2p_set_nc_stack_weights has not been called");
+  P2P_REQUIRE(in && out && hA > 0 && wA > 0 && hB > 0 && wB > 0, "bad argument");
+  const size_t V = (size_t)hA * wA * hB * wB;
+  int rc = h->misc.reserve(nc_stack_scratch_bytes(V) + 8192);
+  if (rc) return rc;
+  __half* lines = (__half*)h->misc.take(nc_stack_scratch_bytes(V));
+  unsigned int* xmax = (unsigned int*)h->misc.take(16);
+  P2P_REQUIRE(lines && xmax, "scratch carve failed");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  ProfScope ps(h, P2P_PROF_NC, st);
+  if ((rc = launch_absmax(in, V, xmax, st))) return rc;
+  return launch_nc_stack(in, hA, wA, hB, wB, h->ncs, xmax, lines, out, sms(h), st);
 }
 
 // Development hook (not part of include/p2p_b200.h): copies `bytes` of an intermediate of the last

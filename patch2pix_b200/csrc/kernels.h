@@ -51,6 +51,26 @@ int launch_neigh_consensus_umma(const float* x, int hA, int wA, int hB, int wB, 
                                 float b2, const unsigned int* xmax, uint32_t* xp, __half* hidden, float* partial,
                                 float* out, float* rowmax, unsigned int* colmax, int l2_mode, int num_sms, cudaStream_t st);
 
+// ---- nc_stack.cu: general NeighConsensus stack (NCNet ImMatchNet) on the tensor cores -----------------------
+constexpr int kNcStackMaxLayers = 16;
+struct NcStackWeights {
+  char* blob = nullptr;           // one allocation backing everything below
+  int n_layers = 0, symmetric = 1;
+  int ks[kNcStackMaxLayers] = {}, chans[kNcStackMaxLayers] = {};
+  float inv_sw[kNcStackMaxLayers] = {};           // 1 / power-of-two weight scale per layer
+  const __half* img[kNcStackMaxLayers] = {};     // per layer [k^2][k][k][32][64] swizzled operand images
+  const float* bias[kNcStackMaxLayers] = {};     // per layer [16], zero past the layer's channels
+  const float* bnd = nullptr;                     // [layers][2][16]: per channel sum |w| (x 1.0001), |b|
+};
+// weights[l]: HOST fp32 in the reference layout [k][Cout][Cin][k][k][k]; biases[l] [Cout].  Replaces S on success.
+int nc_stack_pack(int n_layers, const int* ks, const int* chans, const float* const* weights, const float* const* biases,
+                  int symmetric, NcStackWeights& S);
+void nc_stack_release(NcStackWeights& S);
+size_t nc_stack_scratch_bytes(size_t V);
+// x [hA*wA][hB*wB] -> out; xmax: device word holding the float bits of max |x|; scratch: nc_stack_scratch_bytes(V)
+int launch_nc_stack(const float* x, int hA, int wA, int hB, int wB, const NcStackWeights& W, const unsigned int* xmax,
+                    __half* scratch, float* out, int num_sms, cudaStream_t st);
+
 // ---- preprocess.cu: PIL-exact bicubic resize + ToTensor + Normalize (utils/datasets/preprocess.py:32-60) ----
 struct PreprocessCoefs {
   int ho = 0, wo = 0, ht = 0, wt = 0, ksx = 0, ksy = 0;

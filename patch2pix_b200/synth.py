@@ -363,3 +363,62 @@ def grid_coarse_matcher(shift=(8, 16), step=12, dtype=torch.float32):
                              [-30.0, h1 + 9.0, w2 / 2, h2 / 2]], dtype=torch.float64)
         return torch.cat([edge, rows]).to(dtype=dtype, device=grey1.device)
     return matcher
+
+
+# ---- NCNet (ImMatchNet) test data: regenerated from seeds, so fixtures store outputs only ----------------------------
+def ncnet_stack_weights(seed, kernel_sizes, channels):
+    """Conv4d weights in the reference's pre-permuted layout [k, Cout, Cin, k, k, k] and biases [Cout], fp32, scaled so
+    that activations stay O(1) and mostly positive through the ReLUs."""
+    g = torch.Generator().manual_seed(seed)
+    ws, bs = [], []
+    for i, (k, c) in enumerate(zip(kernel_sizes, channels)):
+        cin = 1 if i == 0 else channels[i - 1]
+        ws.append((torch.rand(k, c, cin, k, k, k, generator=g) - 0.35) / (cin * k ** 4) ** 0.5)
+        bs.append(0.05 * torch.randn(c, generator=g))
+    return ws, bs
+
+
+def ncnet_state_dict(seed, names_shapes, kernel_sizes, channels):
+    """A seeded ImMatchNet state_dict for the given (name, shape) list: ResNet101 convs He-scaled, BatchNorm near
+    identity, NeighConsensus from ncnet_stack_weights.  Names keep their order, so any holder of the same list
+    regenerates the same tensors."""
+    g = torch.Generator().manual_seed(seed)
+    ws, bs = ncnet_stack_weights(seed + 1, kernel_sizes, channels)
+    nc = {}
+    for i, (w, b) in enumerate(zip(ws, bs)):
+        nc[f'NeighConsensus.conv.{2 * i}.weight'], nc[f'NeighConsensus.conv.{2 * i}.bias'] = w, b
+    sd = {}
+    for name, shape in names_shapes:
+        shape = tuple(shape)
+        if name in nc:
+            sd[name] = nc[name]
+        elif name.endswith('num_batches_tracked'):
+            sd[name] = torch.zeros((), dtype=torch.int64)
+        elif len(shape) == 4:
+            fan_in = shape[1] * shape[2] * shape[3]
+            sd[name] = torch.randn(shape, generator=g) * (2.0 / fan_in) ** 0.5
+        elif name.endswith('running_var'):
+            sd[name] = 0.5 + torch.rand(shape, generator=g)
+        elif name.endswith('running_mean'):
+            sd[name] = 0.1 * torch.randn(shape, generator=g)
+        elif name.endswith('weight'):
+            sd[name] = 0.25 + 0.5 * torch.rand(shape, generator=g)
+        else:
+            sd[name] = 0.1 * torch.randn(shape, generator=g)
+    return sd
+
+
+def ncnet_features(seed, c, size1, size2):
+    """A pair of layer3-like feature maps [1, c, h, w] with a shared structure (so that matches are distinct)."""
+    g = torch.Generator().manual_seed(seed)
+    fa = torch.rand(1, c, *size1, generator=g)
+    fb = torch.rand(1, c, *size2, generator=g)
+    fa[:, :, : size1[0] // 2] += 2 * torch.rand(1, c, size1[0] // 2, size1[1], generator=g)
+    fb[:, :, : min(size2[0], size1[0]) // 2, : min(size2[1], size1[1])] += \
+        fa[:, :, : min(size2[0], size1[0]) // 2, : min(size2[1], size1[1])]
+    return fa, fb
+
+
+def ncnet_images(seed, size1, size2):
+    g = torch.Generator().manual_seed(seed)
+    return torch.rand(1, 3, *size1, generator=g), torch.rand(1, 3, *size2, generator=g)
