@@ -162,6 +162,18 @@ P2P_API int p2p_proposals(p2p_handle_t h, const float* corr4d, const uint8_t* de
                   int ksize, int upsample, int center, int do_softmax, int64_t* matches_out, float* scores_out,
                   void* stream);
 
+/* ---- top-k matches: corr_to_matches_topk (networks/ncn/extract_ncmatches.py:96-158) for a batch of b volumes in
+ * one launch.  corr4d fp32 [b][hA*wA][hB*wB]; delta_code NULL (ksize 1) or uint8 [b][hA*wA][hB*wB] packed as by
+ * p2p_delta_pack.  A slice is the cells matched against one cell: forward (invert 0) the hA*wA A cells of each of the
+ * N = hB*wB B cells, inverted the hB*wB B cells of each of the N = hA*wA A cells.  Each slice yields its topk best
+ * cells, ranked by the raw value, descending; exact ties go to the lowest flat cell index.  Outputs are int64 / fp32
+ * [b][topk * N] cell indices (index * ksize + delta with delta_code) and scores (exp(x - max) / sum over the slice,
+ * or x for do_softmax 0), rank-major forward (rank r of cell s at r * N + s), cell-major inverted (s * topk + r).
+ * Limits: slices of at most 32768 cells, 1 <= topk <= slice length, b <= 65535.  Timed as P2P_PROF_PROPOSALS. */
+P2P_API int p2p_proposals_topk(p2p_handle_t h, const float* corr4d, const uint8_t* delta_code, int b, int hA, int wA,
+                               int hB, int wB, int topk, int ksize, int do_softmax, int invert, int64_t* jA_out,
+                               int64_t* iA_out, int64_t* jB_out, int64_t* iB_out, float* scores_out, void* stream);
+
 /* ---- the np.unique part of filter_coarse (networks/utils.py:38-50): lexicographically sorted
  * first-occurrence indices of the distinct rows (mutual != 0: only rows occurring more than once).
  * rows int64 [n,4] with coordinates in [0,65535], n <= 4 Mi (lists beyond 16384 rows sort in global scratch); ids_out int32 [n]; count_out int32 [4] =

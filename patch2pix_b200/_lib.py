@@ -46,6 +46,7 @@ _SIGNATURES = {
     'p2p_nc_stack': (_I, [_P, _P, _I, _I, _I, _I, _P, _P]),
     'p2p_ncnet_coarse': (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _P]),
     'p2p_proposals': (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P]),
+    'p2p_proposals_topk': (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P]),
     'p2p_unique_rows': (_I, [_P, _P, _I, _I, _P, _F, _P, _P, _P]),
     'p2p_select_anchor': (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P]),
     'p2p_refine_prepare': (_I, [_P, C.POINTER(_P), C.POINTER(_P), _I, _I, _I, _I, _P]),

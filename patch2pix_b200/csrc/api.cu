@@ -940,6 +940,24 @@ int p2p_proposals(p2p_handle_t h, const float* corr4d, const uint8_t* delta_code
                           do_softmax, (long long*)matches_out, scores_out, reinterpret_cast<cudaStream_t>(stream));
 }
 
+int p2p_proposals_topk(p2p_handle_t h, const float* corr4d, const uint8_t* delta_code, int b, int hA, int wA, int hB,
+                       int wB, int topk, int ksize, int do_softmax, int invert, int64_t* jA_out, int64_t* iA_out,
+                       int64_t* jB_out, int64_t* iB_out, float* scores_out, void* stream) {
+  P2P_ENTER(h);
+  P2P_REQUIRE(corr4d && jA_out && iA_out && jB_out && iB_out && scores_out, "null tensor pointer");
+  P2P_REQUIRE(b > 0 && b <= 65535 && hA > 0 && wA > 0 && hB > 0 && wB > 0 && ksize >= 1 && ksize <= 3, "bad dims");
+  P2P_REQUIRE((long long)hA * wA <= INT32_MAX && (long long)hB * wB <= INT32_MAX, "bad dims");
+  const int n_slice = invert ? hB * wB : hA * wA;
+  P2P_REQUIRE(n_slice <= kTopkMaxSlice, "slice longer than 32768 cells");
+  P2P_REQUIRE(topk >= 1 && topk <= n_slice, "topk must be in 1..slice length");
+  P2P_REQUIRE(ksize == 1 || delta_code != nullptr, "delta_code is required for ksize > 1");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  ProfScope ps(h, P2P_PROF_PROPOSALS, st);
+  return launch_corr_topk(corr4d, ksize > 1 ? delta_code : nullptr, b, hA, wA, hB, wB, topk, ksize, do_softmax != 0,
+                          invert != 0, (long long*)jA_out, (long long*)iA_out, (long long*)jB_out, (long long*)iB_out,
+                          scores_out, st);
+}
+
 int p2p_unique_rows(p2p_handle_t h, const int64_t* rows, int n, int mutual, const float* scores, float thres,
                     int32_t* ids_out, int32_t* count_out, void* stream) {
   P2P_ENTER(h);

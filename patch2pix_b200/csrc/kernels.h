@@ -35,6 +35,13 @@ int launch_unique_rows(const long long* rows, int n, int mutual, const float* sc
 int launch_select_anchor(const long long* rows, const float* scores, const int* ids, const int* sel, int m, int panc,
                          int pshift, long long* matches_out, float* scores_out, long long* anchors_out, cudaStream_t st);
 
+// ---- topk.cu: corr_to_matches_topk ------------------------------------------------------------------------
+constexpr int kTopkMaxSlice = 32768;    // longest slice (cells matched against one cell) the top-k kernel stages
+// corr [b][hA*wA][hB*wB]; code NULL or [b][hA*wA][hB*wB] (ks 2..3); outputs [b][k * slices] in the reference's order
+int launch_corr_topk(const float* corr, const uint8_t* code, int b, int hA, int wA, int hB, int wB, int k, int ks,
+                     int do_softmax, int invert, long long* jA, long long* iA, long long* jB, long long* iB,
+                     float* score, cudaStream_t st);
+
 // ---- nc_umma.cu: NeighConsensus on the tensor cores -------------------------------------------------------
 struct NcUmmaWeights {
   char* blob = nullptr;           // one allocation backing the two operand images

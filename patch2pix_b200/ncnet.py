@@ -1,4 +1,5 @@
-"""NCNet's matcher (the reference's networks/ncn/model.py: ImMatchNet, NeighConsensus) on the tensor-core library.
+"""NCNet's matcher (the reference's networks/ncn/model.py: ImMatchNet, NeighConsensus, and
+networks/ncn/extract_ncmatches.py: corr_to_matches, corr_to_matches_topk) on the tensor-core library.
 
     -from networks.ncn.model import ImMatchNet
     +from patch2pix_b200.ncnet import ImMatchNet
@@ -14,7 +15,7 @@ import torch.nn as nn
 
 from . import _lib
 
-__all__ = ['ImMatchNet', 'NeighConsensus', 'corr_to_matches']
+__all__ = ['ImMatchNet', 'NeighConsensus', 'corr_to_matches', 'corr_to_matches_topk']
 
 
 def _as_ints(v, name):
@@ -247,3 +248,49 @@ def corr_to_matches(corr4d, delta4d=None, ksize=1, do_softmax=True, scale='posit
     xa, ya = _grid(wA * ksize, lo).to(dev), _grid(hA * ksize, lo).to(dev)
     xb, yb = _grid(wB * ksize, lo).to(dev), _grid(hB * ksize, lo).to(dev)
     return xa[jA], ya[iA], xb[jB], yb[iB], score
+
+
+TOPK_MAX_SLICE = 32768      # longest slice p2p_proposals_topk stages (kTopkMaxSlice in csrc/kernels.h)
+
+
+@torch.no_grad()
+def corr_to_matches_topk(corr4d, delta4d=None, topk=1, ksize=1, do_softmax=True, invert_matching_direction=False):
+    """networks/ncn/extract_ncmatches.py:96-158 on the GPU (p2p_proposals_topk, one launch for the batch).
+    corr4d [b, 1, hA, wA, hB, wB] fp32 CUDA; delta4d as for corr_to_matches (ksize is ignored without it).
+    -> (jA, iA, jB, iB, score): int64 indices and float32 scores, each [b, topk * N].  Forward, for each of the
+    N = hB*wB B cells the topk best A cells, rank-major (rank r of B cell s at r * N + s); inverted, for each of the
+    N = hA*wA A cells the topk best B cells, cell-major (s * topk + r).  Ranks follow the raw value, descending, and
+    exact ties go to the lowest flat cell index (the reference leaves their order to torch.topk)."""
+    if not (isinstance(corr4d, torch.Tensor) and corr4d.is_cuda and corr4d.dtype == torch.float32
+            and corr4d.dim() == 6 and corr4d.shape[1] == 1):
+        raise ValueError('corr_to_matches_topk expects a [b, 1, hA, wA, hB, wB] float32 CUDA tensor')
+    b, _, hA, wA, hB, wB = corr4d.shape
+    n_slice, n = (hB * wB, hA * wA) if invert_matching_direction else (hA * wA, hB * wB)
+    topk = int(topk)
+    if not 1 <= topk <= n_slice:
+        raise ValueError(f'topk must be in 1..{n_slice} (the cells of the other image), got {topk}')
+    if n_slice > TOPK_MAX_SLICE:
+        raise ValueError(f'slices of at most {TOPK_MAX_SLICE} cells are supported, got {n_slice}')
+    if b > 65535:
+        raise ValueError(f'batches of at most 65535 volumes are supported, got {b}')
+    from .model import _pack_delta
+    dev = corr4d.device
+    h = _lib.default_handle(dev)
+    code = None
+    if delta4d is not None:
+        if ksize not in (1, 2, 3):
+            raise ValueError('ksize must be 1, 2 or 3 with delta4d')
+        if len(delta4d) != 4 or any(tuple(d.shape) != tuple(corr4d.shape) for d in delta4d):
+            raise ValueError('delta4d must be four tensors shaped like corr4d')
+        delta4d = tuple(d.to(device=dev, dtype=torch.int64).contiguous() for d in delta4d)
+    corr4d = corr4d.contiguous()
+    out = [torch.empty(b, topk * n, dtype=torch.int64, device=dev) for _ in range(4)]
+    score = torch.empty(b, topk * n, dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        if delta4d is not None:
+            code = _pack_delta(delta4d, ksize, h)
+        _lib.check(h.lib.p2p_proposals_topk(h.h, _lib.ptr(corr4d), _lib.ptr(code), b, hA, wA, hB, wB, topk,
+                                            ksize if code is not None else 1, int(bool(do_softmax)),
+                                            int(bool(invert_matching_direction)), *[_lib.ptr(t) for t in out],
+                                            _lib.ptr(score), h.stream()))
+    return (*out, score)
