@@ -109,8 +109,8 @@ __global__ void __launch_bounds__(kDegenThreads, 1) verify_degen_kernel(VerifySt
   __shared__ int s_max[kDegenThreads / 32], s_first[kDegenThreads / 32];
   VerifyState* st = st_all + blockIdx.y;
   if (st->stop) return;
-  const double* models = models_all + blockIdx.y * kPairModels;
-  const int* counts = counts_all + blockIdx.y * kPairCounts;
+  const double* models = models_all + blockIdx.y * kPairModels<0>;
+  const int* counts = counts_all + blockIdx.y * kPairCounts<0>;
   const double* rows = rows_all + st->row0 * stride;
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, m0 = tid * kChunk;
   int mx = 0;
@@ -227,8 +227,8 @@ __global__ void __launch_bounds__(1024) verify_parallax_select_kernel(VerifyStat
                                                                       double conf, int max_iters) {
   st += blockIdx.y;
   if (!st->pending) return;
-  select_round(st, models + blockIdx.y * kPairModels, counts + blockIdx.y * kPairCounts, kRound, done, Kind<0>::kSample,
-               conf, max_iters, true);
+  select_round(st, models + blockIdx.y * kPairModels<0>, counts + blockIdx.y * kPairCounts<0>, kRound, done,
+               Kind<0>::kSample, conf, max_iters, true);
   if (threadIdx.x == 0) st->pending = 0;
 }
 
@@ -250,29 +250,28 @@ __global__ void verify_degen_hook_kernel(const VerifyState* __restrict__ st, con
 // every round; h_th = 2 px_th.
 int find_model_degensac(const PairBatch& B, double px_th, double conf, int max_iters, unsigned long long seed,
                         void* scratch, double* model_out, uint8_t* mask_out, int* count_out, cudaStream_t st) {
-  const Scratch s = carve(scratch, B.pairs, B.total, kRound);
-  const float th2 = (float)(px_th * px_th);
+  const Scratch s = carve<0>(scratch, B.pairs, B.total, kRound);
   const double h_th2 = (2.0 * px_th) * (2.0 * px_th);
   const dim3 one(1, B.pairs);
-  verify_prep_kernel<<<one, 1024, 0, st>>>(B, Kind<0>::kSample, s.rows32, s.st);
+  verify_prep_kernel<false><<<one, 1024, 0, st>>>(B, nullptr, {}, px_th, Kind<0>::kSample, s.rows32, s.st);
   P2P_LAUNCH_OK();
   for (int first = 0; first < max_iters; first += kRound) {
     const int count = min(kRound, max_iters - first);
-    int rc = enqueue_round<0>(s, B, first, count, seed, th2, 0, st);
+    int rc = enqueue_round<0>(s, B, first, count, seed, 0, st);
     if (rc) return rc;
     verify_degen_kernel<<<one, kDegenThreads, 0, st>>>(s.st, s.models, s.counts, count * 3, first, B.rows, B.stride, seed,
                                                        h_th2);
     P2P_LAUNCH_OK();
-    verify_select_kernel<<<one, 1024, 0, st>>>(s.st, s.models, s.counts, count * 3, first + count, Kind<0>::kSample, conf,
-                                               max_iters);
+    verify_select_kernel<<<one, 1024, 0, st>>>(s.st, s.models, s.counts, count * 3, first + count, Kind<0>::kSample,
+                                               Kind<0>::kPairSlots, conf, max_iters);
     P2P_LAUNCH_OK();
     verify_plane_kernel<<<one, kLoThreads, 0, st>>>(s.st, B.rows, B.stride, h_th2);
     P2P_LAUNCH_OK();
-    if ((rc = enqueue_round<2>(s, B, first, kRound, seed, th2, 0, st, h_th2))) return rc;
+    if ((rc = enqueue_round<2>(s, B, first, kRound, seed, 0, st, h_th2))) return rc;
     verify_parallax_select_kernel<<<one, 1024, 0, st>>>(s.st, s.models, s.counts, first + count, conf, max_iters);
     P2P_LAUNCH_OK();
   }
-  verify_lo_kernel<0><<<one, kLoThreads, 0, st>>>(s.st, s.rows32, B.rows, B.stride, th2, model_out, mask_out, count_out);
+  verify_lo_kernel<0><<<one, kLoThreads, 0, st>>>(s.st, s.rows32, B.rows, B.stride, model_out, mask_out, count_out);
   P2P_LAUNCH_OK();
   return 0;
 }
@@ -287,11 +286,11 @@ size_t verify_degeneracy_scratch_bytes(int n, int count) {
 int launch_test_degeneracy(const double* rows, int stride, int n, double px_th, unsigned long long seed, int count,
                            void* scratch, int* tri_out, double* H_out, cudaStream_t st) {
   const PairBatch B = single_pair(rows, stride, n, nullptr);
-  Scratch s = carve(scratch, 1, n, count);
+  Scratch s = carve<0>(scratch, 1, n, count);
   const double h_th2 = (2.0 * px_th) * (2.0 * px_th);
-  verify_prep_kernel<<<1, 1024, 0, st>>>(B, Kind<0>::kSample, s.rows32, s.st);
+  verify_prep_kernel<false><<<1, 1024, 0, st>>>(B, nullptr, {}, px_th, Kind<0>::kSample, s.rows32, s.st);
   P2P_LAUNCH_OK();
-  int rc = enqueue_round<0>(s, B, 0, count, seed, (float)(px_th * px_th), 1, st);
+  int rc = enqueue_round<0>(s, B, 0, count, seed, 1, st);
   if (rc) return rc;
   verify_degen_hook_kernel<<<cdiv(count * 3, 128), 128, 0, st>>>(s.st, s.models, s.counts, count * 3, rows, stride, seed,
                                                                  h_th2, tri_out, H_out);

@@ -1,13 +1,10 @@
 // Relative pose on the device: RANSAC for an essential matrix (5-point minimal solver) with local optimisation, and
 // pose recovery from E (cv2.findEssentialMat(..., RANSAC) + cv2.recoverPose semantics, utils/eval/geometry.py:32-48).
 //
-// p2p_find_essential enqueues, with no host sync:
-//   ess_prep_kernel     (1 block)  effective row count, finiteness, fp32 copy of the rows in camera coordinates
-//   ess_round_kernel    (x rounds) kRound hypotheses: 5-point sample -> up to 10 models (one thread each), then every
-//                                  (model, row) pair scored in fp32 (Sampson error) by warps over rows in shared memory
-//   ess_select_kernel   (x rounds) best model so far and the stopping bound, as verify.cu (s = 5)
-//   ess_lo_kernel       (1 block)  8-point refit on the winner's inliers projected onto the essential manifold while
-//                                  the count grows, final E, mask and count
+// p2p_find_essential runs the RANSAC kernels of verify_common.cuh as kind 3, with no host sync: the prep kernel maps
+// the rows to camera coordinates, each round draws 5-point samples -> up to 10 models (one thread each) and scores
+// every (model, row) pair in fp32 (Sampson error), and LO refits with the 8-point method projected onto the essential
+// manifold.  This file adds what only E needs: the 5-point solver, the projection, and pose recovery.
 // p2p_recover_pose enqueues:
 //   pose_decompose_kernel (1 thread)   SVD of E -> the four candidates [R1|t], [R2|t], [R1|-t], [R2|-t]
 //   pose_count_kernel     (kPoseBlocks) linear triangulation of every masked row against each candidate, cheirality and
@@ -22,38 +19,17 @@
 #include <math.h>
 
 #include "kernels.h"
-#include "ransac_common.cuh"
+#include "verify_common.cuh"
 
 namespace p2p {
 namespace {
 
-constexpr int kRound = 1024;        // hypotheses per round
-constexpr int kHypPerBlock = 8;     // hypotheses solved (one thread each) and scored per block
-constexpr int kScoreThreads = 256;  // 8 warps
-constexpr int kTile = 1024;         // rows staged in shared memory per pass (16 KB)
-constexpr int kSample = 5;
-constexpr int kSlots = 10;          // real roots of the degree-10 polynomial
-constexpr int kLoMin = 8;
-constexpr int kLoIters = 4;
-constexpr int kLoThreads = 256;
+constexpr int kMaxRoots = 10;       // real roots of the degree-10 polynomial
 constexpr int kBisect = 64;         // bisection steps per root
 constexpr int kNewton = 2;          // guarded Newton steps per root
 constexpr double kZMax = 1e6;       // roots are searched in (-kZMax, kZMax]
 constexpr int kPoseBlocks = 256;
 constexpr int kPoseThreads = 256;
-
-struct EssState {
-  double best[9];                   // best model so far, camera coordinates
-  Intrinsics K;                     // the pair's cameras
-  float th2;                        // squared inlier threshold in camera coordinates
-  int n;                            // effective row count
-  int bad;                          // a coordinate is not finite
-  int stop;                         // no further rounds are needed
-  int best_count;                   // 0: no model yet
-  int n_all;                        // rows of the pair (mask length)
-  long long row0;                   // first row of the pair in the row array and the mask
-  long long row32;                  // first row of the pair in rows32
-};
 
 struct PoseState {
   double R[2][9], t[3];             // R1, R2 row-major, t = U[:, 2]
@@ -64,9 +40,6 @@ struct PoseState {
   long long row0;                   // first row of the pair in the row array and the masks
   long long row32;                  // first row of the pair in the codes
 };
-
-constexpr size_t kPairModels = (size_t)kRound * kSlots * 9;   // round-model doubles per pair
-constexpr size_t kPairCounts = (size_t)kRound * kSlots;       // round-count ints per pair
 
 // ---- 5-point solver (one thread; restated in oracle/pose_oracle.py) ------------------------------------------------
 // Monomials of degree <= 3 in (x, y, z): x^3 y^3 x^2y xy^2 x^2z x^2 y^2z y^2 xyz xy | xz^2 xz x yz^2 yz y z^3 z^2 z 1.
@@ -191,7 +164,7 @@ __device__ __forceinline__ void row_polys(const double* be, const double* bf, do
 
 // 5-point solver on camera-coordinate rows (x1, y1, x2, y2): up to 10 essential matrices x2^T E x1 = 0 at unit
 // Frobenius norm, ascending in z.  M is this thread's 10 x 20 elimination matrix in shared memory.
-__device__ int solve_e5(const double (&p)[5][4], double (*M)[20], double (&out)[kSlots][9]) {
+__device__ int solve_e5(const double (&p)[5][4], double (*M)[20], double (&out)[kMaxRoots][9]) {
   double A[5][9], N[4][9];
   for (int i = 0; i < 5; ++i) {
     const double x1 = p[i][0], y1 = p[i][1], x2 = p[i][2], y2 = p[i][3];
@@ -386,276 +359,32 @@ __device__ __forceinline__ double det3m(const double (&m)[3][3]) {
          m[0][2] * (m[1][0] * m[2][1] - m[1][1] * m[2][0]);
 }
 
-__device__ __forceinline__ bool is_inlier_e(const float* m, float4 r, float th2) {
-  float dd, den;
-  sampson_terms<float>(m, r.x, r.y, r.z, r.w, dd, den);
-  return dd * dd < th2 * den;
-}
-
-__device__ __forceinline__ void to_camera(const double* p, const Intrinsics& K, double& x1, double& y1, double& x2,
-                                          double& y2) {
-  x1 = (p[0] - K.cx1) / K.fx1;
-  y1 = (p[1] - K.cy1) / K.fy1;
-  x2 = (p[2] - K.cx2) / K.fx2;
-  y2 = (p[3] - K.cy2) / K.fy2;
-}
-
-__device__ __forceinline__ int effective_rows(int n, const double* n_dev) {
-  int m = n;
-  if (n_dev != nullptr) {
-    const double v = *n_dev;
-    if (v >= 0.0 && v < (double)n) m = (int)v;
+// ---- E: kind 3 of the RANSAC kernels (verify_common.cuh) ---------------------------------------------------------
+// Camera coordinates throughout, scored as F.  kTile = 1024 rows (16 KB) leaves room for the 5-point solver's 12.8 KB
+// of shared elimination matrices: 2048 would put the round kernel 384 bytes under the 48 KB static shared-memory limit.
+template <> struct Kind<3> {
+  static constexpr int kSample = 5, kSlots = kMaxRoots, kPairSlots = kMaxRoots, kLoMin = 8, kScore = 0, kTile = 1024;
+  // Thread t < kHypPerBlock of a round block solves its hypothesis with s_M[t] as its elimination matrix.
+  static __device__ int solve(const VerifyState&, const double (&p)[5][4], double (&out)[kSlots][9]) {
+    __shared__ double s_M[kHypPerBlock][10][20];
+    return solve_e5(p, s_M[threadIdx.x], out);
   }
-  return m;
-}
-
-// Pair p's cameras: intr[8 p ..] (device), or K1 for a single pair (intr == nullptr).
-__device__ __forceinline__ Intrinsics pair_intrinsics(const double* intr, const Intrinsics& K1, int p) {
-  if (intr == nullptr) return K1;
-  const double* k = intr + 8 * (size_t)p;
-  return Intrinsics{k[0], k[1], k[2], k[3], k[4], k[5], k[6], k[7]};
-}
-
-// cv2.findEssentialMat's threshold in camera coordinates: px_th / ((fx + fy) / 2) of view 2, squared.
-__device__ __forceinline__ float ess_th2(double px_th, const Intrinsics& K) {
-  const double th = px_th / ((K.fx2 + K.fy2) / 2.0);
-  return (float)(th * th);
-}
-
-// ---- essential-matrix RANSAC kernels -------------------------------------------------------------------------------
-__global__ void __launch_bounds__(1024) ess_prep_kernel(PairBatch B, const double* __restrict__ intr, Intrinsics K1,
-                                                        double px_th, float4* __restrict__ rows32_all,
-                                                        EssState* __restrict__ st_all) {
-  __shared__ int s_n;
-  const int tid = threadIdx.x, p = blockIdx.y;
-  EssState* st = st_all + p;
-  const PairRange pr = pair_range(B, p);
-  const int n = pr.n, stride = B.stride;
-  const double* rows = B.rows + pr.row0 * stride;
-  float4* rows32 = rows32_all + (pr.row0 - B.base);
-  const Intrinsics K = pair_intrinsics(intr, K1, p);
-  if (tid == 0) s_n = effective_rows(n, B.n_dev == nullptr ? nullptr : B.n_dev + p);
-  __syncthreads();
-  const int m = s_n;
-  int bad = 0;
-  for (int r = tid; r < m; r += 1024) {
-    const double* p = rows + (size_t)r * stride;
-    bad |= !(isfinite(p[0]) && isfinite(p[1]) && isfinite(p[2]) && isfinite(p[3]));
-    double x1, y1, x2, y2;
-    to_camera(p, K, x1, y1, x2, y2);
-    rows32[r] = make_float4((float)x1, (float)y1, (float)x2, (float)y2);
-  }
-  bad = __syncthreads_or(bad);
-  if (tid == 0) {
-    for (int j = 0; j < 9; ++j) st->best[j] = 0.0;
-    st->n = m;
-    st->bad = bad;
-    st->stop = bad || m < kSample;
-    st->best_count = 0;
-    st->K = K;
-    st->th2 = ess_th2(px_th, K);
-    st->n_all = n;
-    st->row0 = pr.row0;
-    st->row32 = pr.row0 - B.base;
-  }
-}
-
-// Hypotheses first .. first + count - 1.  models [count * kSlots][9] fp64 (camera coordinates), counts
-// [count * kSlots] (-1: no model in that slot).
-__global__ void __launch_bounds__(kScoreThreads, 1) ess_round_kernel(const EssState* __restrict__ st_all,
-                                                                  const float4* __restrict__ rows32_all,
-                                                                  const double* __restrict__ rows_all, int stride,
-                                                                  int first, int count, unsigned long long seed,
-                                                                  int ignore_stop, double* __restrict__ models_all,
-                                                                  int* __restrict__ counts_all) {
-  constexpr int NM = kHypPerBlock * kSlots, NJ = NM / 8;
-  __shared__ float4 s_rows[kTile];
-  __shared__ double s_M[kHypPerBlock][10][20];
-  __shared__ float s_model[NM][9];
-  __shared__ int s_valid[NM];
-  const EssState* st = st_all + blockIdx.y;
-  if (!ignore_stop && st->stop) return;
-  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  const int n = st->n;
-  const Intrinsics K = st->K;
-  const float th2 = st->th2;
-  const double* rows = rows_all + st->row0 * stride;
-  const float4* rows32 = rows32_all + st->row32;
-  double* models = models_all + blockIdx.y * kPairModels;
-  int* counts = counts_all + blockIdx.y * kPairCounts;
-  if (tid < kHypPerBlock) {
-    const int local = blockIdx.x * kHypPerBlock + tid;
-    double out[kSlots][9];
-    int nm = 0;
-    if (local < count) {
-      int idx[kSample];
-      if (draw_sample<kSample>(seed, first + local, n, idx)) {
-        double p[kSample][4];
-#pragma unroll
-        for (int k = 0; k < kSample; ++k) to_camera(rows + (size_t)idx[k] * stride, K, p[k][0], p[k][1], p[k][2], p[k][3]);
-        nm = solve_e5(p, s_M[tid], out);
+  // The refit projected onto the essential manifold (singular values 1, 1, 0) at unit Frobenius norm.
+  static __device__ bool refit(const VerifyState&, double (&h)[9], double* out) {
+    double U[3][3], s[3], Vm[3][3];
+    if (!svd3(h, U, s, Vm)) return false;
+    double nrm = 0.0;
+    for (int i = 0; i < 3; ++i)
+      for (int j = 0; j < 3; ++j) {
+        const double v = U[i][0] * Vm[j][0] + U[i][1] * Vm[j][1];
+        out[3 * i + j] = v;
+        nrm += v * v;
       }
-    }
-    for (int k = 0; k < kSlots; ++k) {
-      const int slot = tid * kSlots + k;
-      s_valid[slot] = k < nm;
-      for (int j = 0; j < 9; ++j) {
-        s_model[slot][j] = k < nm ? (float)out[k][j] : 0.f;
-        if (local < count) models[((size_t)local * kSlots + k) * 9 + j] = k < nm ? out[k][j] : 0.0;
-      }
-    }
+    nrm = 1.0 / sqrt(nrm);
+    for (int j = 0; j < 9; ++j) out[j] *= nrm;
+    return true;
   }
-  int cnt[NJ];
-#pragma unroll
-  for (int j = 0; j < NJ; ++j) cnt[j] = 0;
-  for (int t0 = 0; t0 < n; t0 += kTile) {
-    const int tn = min(kTile, n - t0);
-    __syncthreads();
-    for (int r = tid; r < tn; r += kScoreThreads) s_rows[r] = rows32[t0 + r];
-    __syncthreads();
-#pragma unroll
-    for (int j = 0; j < NJ; ++j) {
-      const int mi = wid + 8 * j;
-      if (!s_valid[mi]) continue;
-      float m[9];
-#pragma unroll
-      for (int e = 0; e < 9; ++e) m[e] = s_model[mi][e];
-      for (int r0 = 0; r0 < tn; r0 += 32) {
-        const int r = r0 + lane;
-        const bool in = r < tn && is_inlier_e(m, s_rows[r < tn ? r : 0], th2);
-        cnt[j] += __popc(__ballot_sync(0xffffffffu, in));
-      }
-    }
-  }
-  if (lane == 0) {
-#pragma unroll
-    for (int j = 0; j < NJ; ++j) {
-      const int mi = wid + 8 * j;
-      const int local = blockIdx.x * kHypPerBlock + mi / kSlots;
-      if (local < count) counts[(size_t)blockIdx.x * NM + mi] = s_valid[mi] ? cnt[j] : -1;
-    }
-  }
-}
-
-__global__ void __launch_bounds__(1024) ess_select_kernel(EssState* __restrict__ st, const double* __restrict__ models,
-                                                          const int* __restrict__ counts, int nm, int done, double conf,
-                                                          int max_iters) {
-  select_round(st + blockIdx.y, models + blockIdx.y * kPairModels, counts + blockIdx.y * kPairCounts, nm, done, kSample,
-               conf, max_iters);
-}
-
-// Local optimisation + outputs: 8-point refit on the inliers (fp64 normal matrix, Jacobi), projected onto the essential
-// manifold (singular values 1, 1, 0) at unit Frobenius norm, kept while it has strictly more inliers.
-__global__ void __launch_bounds__(kLoThreads, 1) ess_lo_kernel(const EssState* __restrict__ st_all,
-                                                            const float4* __restrict__ rows32_all,
-                                                            const double* __restrict__ rows_all, int stride,
-                                                            double* __restrict__ E_out, uint8_t* __restrict__ mask_out,
-                                                            int* __restrict__ count_out) {
-  __shared__ double s_red[kLoThreads / 32][45];
-  __shared__ double s_cur[9], s_cand[9];
-  __shared__ float s_f32[9];
-  __shared__ int s_cnt[kLoThreads / 32], s_ok;
-  const EssState* st = st_all + blockIdx.y;
-  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  const int n = st->n, bad = st->bad, n_all = st->n_all;
-  const Intrinsics K = st->K;
-  const float th2 = st->th2;
-  const double* rows = rows_all + st->row0 * stride;
-  const float4* rows32 = rows32_all + st->row32;
-  E_out += 9 * blockIdx.y;
-  count_out += blockIdx.y;
-  mask_out += st->row0;
-  int cur_count = bad ? 0 : st->best_count;
-  if (tid < 9) s_cur[tid] = st->best[tid];
-  __syncthreads();
-
-  auto count_inliers = [&](const double* m64) -> int {    // block-wide, fixed order
-    if (tid < 9) s_f32[tid] = (float)m64[tid];
-    __syncthreads();
-    float m[9];
-#pragma unroll
-    for (int e = 0; e < 9; ++e) m[e] = s_f32[e];
-    int c = 0;
-    for (int r = tid; r < n; r += kLoThreads) c += is_inlier_e(m, rows32[r], th2);
-    for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
-    if (lane == 0) s_cnt[wid] = c;
-    __syncthreads();
-    int tot = 0;
-    for (int w = 0; w < kLoThreads / 32; ++w) tot += s_cnt[w];
-    __syncthreads();
-    return tot;
-  };
-
-  for (int it = 0; it < kLoIters && cur_count >= kLoMin; ++it) {
-    if (tid < 9) s_f32[tid] = (float)s_cur[tid];
-    __syncthreads();
-    float m[9];
-#pragma unroll
-    for (int e = 0; e < 9; ++e) m[e] = s_f32[e];
-    double acc[45];
-#pragma unroll
-    for (int e = 0; e < 45; ++e) acc[e] = 0.0;
-    for (int r = tid; r < n; r += kLoThreads) {
-      if (!is_inlier_e(m, rows32[r], th2)) continue;
-      double x, y, u, v;
-      to_camera(rows + (size_t)r * stride, K, x, y, u, v);
-      const double a[9] = {u * x, u * y, u, v * x, v * y, v, x, y, 1.0};
-      int e = 0;
-#pragma unroll
-      for (int i = 0; i < 9; ++i)
-#pragma unroll
-        for (int j = i; j < 9; ++j) acc[e++] += a[i] * a[j];
-    }
-#pragma unroll
-    for (int e = 0; e < 45; ++e) {
-      const double v = warp_sum_d(acc[e]);
-      if (lane == 0) s_red[wid][e] = v;
-    }
-    __syncthreads();
-    if (tid == 0) {
-      double M[9][9], h[9];
-      int e = 0;
-      for (int i = 0; i < 9; ++i)
-        for (int j = i; j < 9; ++j) {
-          double v = 0.0;
-          for (int w = 0; w < kLoThreads / 32; ++w) v += s_red[w][e];
-          M[i][j] = M[j][i] = v;
-          ++e;
-        }
-      jacobi_min_eigvec<9>(M, h);
-      double U[3][3], s[3], Vm[3][3];
-      bool ok = svd3(h, U, s, Vm);
-      if (ok) {
-        double nrm = 0.0;
-        for (int i = 0; i < 3; ++i)
-          for (int j = 0; j < 3; ++j) {
-            const double v = U[i][0] * Vm[j][0] + U[i][1] * Vm[j][1];
-            s_cand[3 * i + j] = v;
-            nrm += v * v;
-          }
-        nrm = 1.0 / sqrt(nrm);
-        for (int j = 0; j < 9; ++j) s_cand[j] *= nrm;
-      }
-      s_ok = ok;
-    }
-    __syncthreads();
-    if (!s_ok) break;
-    const int c = count_inliers(s_cand);
-    if (c <= cur_count) break;
-    cur_count = c;
-    if (tid < 9) s_cur[tid] = s_cand[tid];
-    __syncthreads();
-  }
-
-  if (tid < 9) E_out[tid] = bad ? __longlong_as_double(0x7ff8000000000000ll) : (cur_count > 0 ? s_cur[tid] : 0.0);
-  if (tid == 0) *count_out = bad ? -1 : cur_count;
-  if (tid < 9) s_f32[tid] = (float)s_cur[tid];
-  __syncthreads();
-  float m[9];
-#pragma unroll
-  for (int e = 0; e < 9; ++e) m[e] = s_f32[e];
-  for (int r = tid; r < n_all; r += kLoThreads) mask_out[r] = cur_count > 0 && r < n && is_inlier_e(m, rows32[r], th2);
-}
+};
 
 // ---- pose recovery kernels ----------------------------------------------------------------------------------------
 // cv2.decomposeEssentialMat: E = U S V^T with det U, det V^T made positive; R1 = U W V^T, R2 = U W^T V^T, t = U[:, 2].
@@ -670,7 +399,7 @@ __global__ void pose_decompose_kernel(PairBatch B, const double* __restrict__ in
   ps->n_all = pr.n;
   ps->row0 = pr.row0;
   ps->row32 = pr.row0 - B.base;
-  ps->n = effective_rows(pr.n, B.n_dev == nullptr ? nullptr : B.n_dev + p);
+  ps->n = effective_rows(B, p, pr.n);
   double e[9], amax = 0.0;
   bool fin = true;
   for (int j = 0; j < 9; ++j) {
@@ -797,35 +526,9 @@ __global__ void __launch_bounds__(1024) pose_select_kernel(const PoseState* __re
   for (int r = tid; r < n_all; r += 1024) mask_out[r] = valid && r < n && ((codes[r] >> b) & 1);
 }
 
-struct EssScratch {
-  EssState* st;
-  float4* rows32;
-  double* models;
-  int* counts;
-};
-
-// `pairs` states, `rows` fp32 rows, then nhyp hypotheses' models and counts per pair (nhyp = kRound: pair strides
-// kPairModels / kPairCounts).
-EssScratch carve_ess(void* base, int pairs, long long rows, int nhyp) {
-  char* p = (char*)base;
-  EssScratch s;
-  s.st = (EssState*)p;
-  p += align_up((size_t)pairs * sizeof(EssState), 1024);
-  s.rows32 = (float4*)p;
-  p += align_up((size_t)rows * sizeof(float4) + 16, 1024);
-  s.models = (double*)p;
-  p += align_up((size_t)pairs * nhyp * kSlots * 9 * sizeof(double), 1024);
-  s.counts = (int*)p;
-  return s;
-}
-
 }  // namespace
 
-size_t essential_scratch_bytes(int pairs, long long rows, bool rounds) {
-  return align_up((size_t)pairs * sizeof(EssState), 1024) + align_up((size_t)rows * sizeof(float4) + 16, 1024) +
-         (rounds ? align_up((size_t)pairs * kPairModels * sizeof(double), 1024) + (size_t)pairs * kPairCounts * sizeof(int)
-                 : 0);
-}
+size_t essential_scratch_bytes(int pairs, long long rows, bool rounds) { return scratch_bytes<3>(pairs, rows, rounds); }
 
 // states, per-block partial counts of every pair, then one code byte per row
 size_t pose_scratch_bytes(int pairs, long long rows) {
@@ -833,10 +536,7 @@ size_t pose_scratch_bytes(int pairs, long long rows) {
          (size_t)rows + 16;
 }
 
-int essential_chunk_pairs() {
-  const size_t per_pair = sizeof(EssState) + kPairModels * sizeof(double) + kPairCounts * sizeof(int);
-  return (int)std::min<size_t>(kMaxGridY, std::max<size_t>(1, kBatchScratchBudget / per_pair));
-}
+int essential_chunk_pairs() { return chunk_pairs<3>(); }
 
 int pose_chunk_pairs() {
   const size_t per_pair = sizeof(PoseState) + kPoseBlocks * 4 * sizeof(int);
@@ -846,34 +546,13 @@ int pose_chunk_pairs() {
 int launch_find_essential(const PairBatch& B, const double* intr, const Intrinsics& K1, double px_th, double conf,
                           int max_iters, unsigned long long seed, void* scratch, double* E_out, uint8_t* mask_out,
                           int* count_out, cudaStream_t st) {
-  const EssScratch s = carve_ess(scratch, B.pairs, B.total, kRound);
-  const dim3 one(1, B.pairs);
-  ess_prep_kernel<<<one, 1024, 0, st>>>(B, intr, K1, px_th, s.rows32, s.st);
-  P2P_LAUNCH_OK();
-  for (int first = 0; first < max_iters; first += kRound) {
-    const int count = min(kRound, max_iters - first);
-    ess_round_kernel<<<dim3(cdiv(count, kHypPerBlock), B.pairs), kScoreThreads, 0, st>>>(
-        s.st, s.rows32, B.rows, B.stride, first, count, seed, 0, s.models, s.counts);
-    P2P_LAUNCH_OK();
-    ess_select_kernel<<<one, 1024, 0, st>>>(s.st, s.models, s.counts, count * kSlots, first + count, conf, max_iters);
-    P2P_LAUNCH_OK();
-  }
-  ess_lo_kernel<<<one, kLoThreads, 0, st>>>(s.st, s.rows32, B.rows, B.stride, E_out, mask_out, count_out);
-  P2P_LAUNCH_OK();
-  return 0;
+  return find_model<3>(B, intr, K1, px_th, conf, max_iters, seed, scratch, E_out, mask_out, count_out, st);
 }
 
 int launch_test_essential_hypotheses(const double* rows, int stride, int n, const Intrinsics& K, double px_th,
                                      unsigned long long seed, int count, void* scratch, double* models_out,
                                      int* counts_out, cudaStream_t st) {
-  const PairBatch B = single_pair(rows, stride, n, nullptr);
-  const EssScratch s = carve_ess(scratch, 1, n, 0);
-  ess_prep_kernel<<<1, 1024, 0, st>>>(B, nullptr, K, px_th, s.rows32, s.st);
-  P2P_LAUNCH_OK();
-  ess_round_kernel<<<cdiv(count, kHypPerBlock), kScoreThreads, 0, st>>>(s.st, s.rows32, rows, stride, 0, count, seed, 1,
-                                                                        models_out, counts_out);
-  P2P_LAUNCH_OK();
-  return 0;
+  return test_hypotheses<3>(rows, stride, n, K, px_th, seed, count, scratch, models_out, counts_out, st);
 }
 
 int launch_recover_pose(const PairBatch& B, const double* intr, const Intrinsics& K1, const double* E,

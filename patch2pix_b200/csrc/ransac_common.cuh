@@ -1,6 +1,7 @@
-// Device helpers shared by the RANSAC estimators of verify.cu (F, H) and pose.cu (E): the counter-based sample
-// generator, fp64 null space and smallest-eigenvector solvers, the Sampson terms, fixed-order block sums and the
-// per-round select / stop rule.  Everything here is inlined into the calling kernels of each translation unit.
+// Device helpers of the RANSAC engine (verify_common.cuh), pose recovery (pose.cu) and the epipolar histograms
+// (eval.cu): a batch's row ranges, the counter-based sample generator, fp64 null space and smallest-eigenvector
+// solvers, the Sampson terms, fixed-order block sums and the per-round select / stop rule.  Everything here is inlined
+// into the calling kernels of each translation unit.
 #pragma once
 #include <math.h>
 
@@ -20,6 +21,14 @@ __device__ __forceinline__ PairRange pair_range(const PairBatch& B, int p) {
   if (B.offsets == nullptr) return PairRange{0, B.n1};
   const long long r0 = B.offsets[p];
   return PairRange{r0, (int)(B.offsets[p + 1] - r0)};
+}
+// Rows pair p uses of its n: n_dev[p] when that lies in [0, n), else n.
+__device__ __forceinline__ int effective_rows(const PairBatch& B, int p, int n) {
+  if (B.n_dev != nullptr) {
+    const double v = B.n_dev[p];
+    if (v >= 0.0 && v < (double)n) return (int)v;
+  }
+  return n;
 }
 
 // ---- stateless sample generator: index `draw` of hypothesis `hyp` (restated in oracle/verify_oracle.py) -------------

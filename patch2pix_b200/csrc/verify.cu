@@ -4,18 +4,17 @@
 //
 // One call enqueues, with no host sync:
 //   verify_prep_kernel     (1 block)  effective row count, finiteness, Hartley normalisation, fp32 copy of the rows
-//   verify_round_kernel    (x rounds) kRound hypotheses: minimal sample -> models (one thread each), then every
+//   verify_round_kernel<K> (x rounds) kRound hypotheses: minimal sample -> models (one thread each), then every
 //                                     (model, row) pair scored in fp32 by warps over rows staged in shared memory
 //   verify_select_kernel   (x rounds) best model so far (most inliers, ties to the lowest (hypothesis, root) index) and
 //                                     the stopping bound log(1-conf) / log(1-w^s); later rounds return at once past it
-//   verify_lo_kernel       (1 block)  non-minimal refit on the winner's inliers while the count grows, final mask
-// (verify_common.cuh; model 2, F with the DEGENSAC check, adds its launches in degensac.cu).  A batch of pairs runs the
-// same launches with the pair as grid dimension y: one block per pair for prep / select / LO, cdiv(count, 8) blocks per
-// pair for a round; a pair past its stopping bound returns at once from later rounds.
+//   verify_lo_kernel<K>    (1 block)  non-minimal refit on the winner's inliers while the count grows, final mask
+// (verify_common.cuh, kind K = 0 for F and 1 for H, which share one prep and one select kernel; E runs the same
+// kernels as kind 3 in pose.cu, and model 2, F with the DEGENSAC check, adds its launches to kind 0's in degensac.cu).
+// A batch of pairs runs the same launches with the pair as grid dimension y: one block per pair for prep / select / LO,
+// cdiv(count, 8) blocks per pair for a round; a pair past its stopping bound returns at once from later rounds.
 // Every reduction runs in a fixed order and no grid size depends on the device, so results are bit-reproducible.
 #include <math.h>
-
-#include <algorithm>
 
 #include "kernels.h"
 #include "verify_common.cuh"
@@ -33,64 +32,24 @@ __global__ void sampson_kernel(const double* __restrict__ rows, int stride, int 
   out[r] = sampson_distance(m, rows + (size_t)r * stride);
 }
 
-template <int KIND>
-int find_model(const PairBatch& B, double px_th, double conf, int max_iters, unsigned long long seed, void* scratch,
-               double* model_out, uint8_t* mask_out, int* count_out, cudaStream_t st) {
-  const Scratch s = carve(scratch, B.pairs, B.total, kRound);
-  const float th2 = (float)(px_th * px_th);
-  verify_prep_kernel<<<dim3(1, B.pairs), 1024, 0, st>>>(B, Kind<KIND>::kSample, s.rows32, s.st);
-  P2P_LAUNCH_OK();
-  for (int first = 0; first < max_iters; first += kRound) {
-    const int count = min(kRound, max_iters - first);
-    int rc = enqueue_round<KIND>(s, B, first, count, seed, th2, 0, st);
-    if (rc) return rc;
-    verify_select_kernel<<<dim3(1, B.pairs), 1024, 0, st>>>(s.st, s.models, s.counts, count * Kind<KIND>::kSlots,
-                                                            first + count, Kind<KIND>::kSample, conf, max_iters);
-    P2P_LAUNCH_OK();
-  }
-  verify_lo_kernel<KIND><<<dim3(1, B.pairs), kLoThreads, 0, st>>>(s.st, s.rows32, B.rows, B.stride, th2, model_out,
-                                                                  mask_out, count_out);
-  P2P_LAUNCH_OK();
-  return 0;
-}
-
-template <int KIND>
-int test_hypotheses(const double* rows, int stride, int n, double px_th, unsigned long long seed, int count, void* scratch,
-                    double* models_out, int* counts_out, cudaStream_t st) {
-  const PairBatch B = single_pair(rows, stride, n, nullptr);
-  Scratch s = carve(scratch, 1, n, 0);
-  s.models = models_out;
-  s.counts = counts_out;
-  verify_prep_kernel<<<1, 1024, 0, st>>>(B, Kind<KIND>::kSample, s.rows32, s.st);
-  P2P_LAUNCH_OK();
-  return enqueue_round<KIND>(s, B, 0, count, seed, (float)(px_th * px_th), 1, st);
-}
-
 }  // namespace
 
-size_t verify_scratch_bytes(int pairs, long long rows, bool rounds) {
-  return align_up((size_t)pairs * sizeof(VerifyState), 1024) + align_up((size_t)rows * sizeof(float4) + 16, 1024) +
-         (rounds ? align_up((size_t)pairs * kPairModels * sizeof(double), 1024) + (size_t)pairs * kPairCounts * sizeof(int)
-                 : 0);
-}
+size_t verify_scratch_bytes(int pairs, long long rows, bool rounds) { return scratch_bytes<0>(pairs, rows, rounds); }
 
-int verify_chunk_pairs() {
-  const size_t per_pair = sizeof(VerifyState) + kPairModels * sizeof(double) + kPairCounts * sizeof(int);
-  return (int)std::min<size_t>(kMaxGridY, std::max<size_t>(1, kBatchScratchBudget / per_pair));
-}
+int verify_chunk_pairs() { return chunk_pairs<0>(); }
 
 int launch_find_model(int model, const PairBatch& B, double px_th, double conf, int max_iters, unsigned long long seed,
                       void* scratch, double* model_out, uint8_t* mask_out, int* count_out, cudaStream_t st) {
   if (model == 2)
     return launch_find_model_degensac(B, px_th, conf, max_iters, seed, scratch, model_out, mask_out, count_out, st);
-  return model == 0 ? find_model<0>(B, px_th, conf, max_iters, seed, scratch, model_out, mask_out, count_out, st)
-                    : find_model<1>(B, px_th, conf, max_iters, seed, scratch, model_out, mask_out, count_out, st);
+  auto find = model == 0 ? find_model<0> : find_model<1>;
+  return find(B, nullptr, {}, px_th, conf, max_iters, seed, scratch, model_out, mask_out, count_out, st);
 }
 
 int launch_test_hypotheses(int model, const double* rows, int stride, int n, double px_th, unsigned long long seed,
                            int count, void* scratch, double* models_out, int* counts_out, cudaStream_t st) {
-  return model == 0 ? test_hypotheses<0>(rows, stride, n, px_th, seed, count, scratch, models_out, counts_out, st)
-                    : test_hypotheses<1>(rows, stride, n, px_th, seed, count, scratch, models_out, counts_out, st);
+  auto test = model == 0 ? test_hypotheses<0> : test_hypotheses<1>;
+  return test(rows, stride, n, {}, px_th, seed, count, scratch, models_out, counts_out, st);
 }
 
 int launch_sampson_distance(const double* rows, int stride, int n, const double* F, double* out, cudaStream_t st) {

@@ -1,12 +1,15 @@
-// RANSAC machinery shared by verify.cu (F / H, models 0 and 1) and degensac.cu (F with the DEGENSAC check, model 2):
-// the state, minimal solvers, scoring, and the prep / round / select / local-optimisation kernels.  Each translation
-// unit instantiates the kernels it launches.  See verify.cu for the launch sequence.
+// The RANSAC engine of verify.cu (F / H, kinds 0 and 1), degensac.cu (F with the DEGENSAC check: kind 0's launches plus
+// the plane-and-parallax round, kind 2) and pose.cu (E, kind 3): the state, the F / H minimal solvers, scoring, the
+// prep / round / select / local-optimisation kernels and their launch sequence (find_model).  Each translation unit
+// instantiates the kinds it launches; pose.cu defines Kind<3> before it does.
 //
 // Every kernel serves a batch of pairs: pair p is blockIdx.y and owns VerifyState st[p], its rows of the concatenated
 // row array (st[p].row0 ..), its fp32 rows (rows32 + st[p].row32) and its round models / counts (kPairModels /
 // kPairCounts per pair).  A pair's arithmetic does not depend on the other pairs.
 #pragma once
 #include <math.h>
+
+#include <algorithm>
 
 #include "kernels.h"
 #include "ransac_common.cuh"
@@ -18,7 +21,6 @@ namespace {
 constexpr int kRound = 1024;        // hypotheses per round
 constexpr int kHypPerBlock = 8;     // hypotheses solved (one thread each) and scored per block
 constexpr int kScoreThreads = 256;  // 8 warps
-constexpr int kTile = 2048;         // rows staged in shared memory per pass (32 KB)
 constexpr int kLoIters = 4;         // local-optimisation refits
 constexpr int kLoThreads = 256;
 constexpr int kDegenThreads = 256;  // records scan of one round: kRound * 3 slots over 256 threads
@@ -26,8 +28,8 @@ constexpr int kDegenMin = 5;        // a sample is H-degenerate when this many o
 constexpr unsigned long long kParallaxKey = 0x5851F42D4C957F2Dull;   // parallax draws use seed ^ kParallaxKey
 
 struct VerifyState {
-  double cx[2], cy[2], s[2];        // Hartley normalisation x' = s (x - c) of image 1 and image 2
-  double best[9];                   // best model so far, pixel coordinates
+  double cx[2], cy[2], s[2];        // F / H: Hartley normalisation x' = s (x - c) of image 1 and image 2
+  double best[9];                   // best model so far, in the scoring frame (pixels; E: camera coordinates)
   double plane[9];                  // DEGENSAC: H of the pending plane-and-parallax round, pixel coordinates
   int n;                            // effective row count
   int bad;                          // a coordinate is not finite
@@ -37,16 +39,44 @@ struct VerifyState {
   int n_all;                        // rows of the pair (mask length)
   long long row0;                   // first row of the pair in the row array and the mask
   long long row32;                  // first row of the pair in rows32
+  Intrinsics K;                     // E: the pair's cameras
+  float th2;                        // squared inlier threshold in the scoring frame
 };
 
-constexpr size_t kPairModels = (size_t)kRound * 3 * 9;   // round-model doubles per pair (3 slots per hypothesis)
-constexpr size_t kPairCounts = (size_t)kRound * 3;       // round-count ints per pair
+// Pair p's cameras: intr[8 p ..] (device), or K1 for a single pair (intr == nullptr).
+__device__ __forceinline__ Intrinsics pair_intrinsics(const double* intr, const Intrinsics& K1, int p) {
+  if (intr == nullptr) return K1;
+  const double* k = intr + 8 * (size_t)p;
+  return Intrinsics{k[0], k[1], k[2], k[3], k[4], k[5], k[6], k[7]};
+}
 
-// kScore: which inlier test scores the models.  Kind 2 is DEGENSAC's plane-and-parallax round: F from 2 rows and H.
-template <int KIND> struct Kind;
-template <> struct Kind<0> { static constexpr int kSample = 7, kSlots = 3, kLoMin = 8, kScore = 0; };   // F: up to 3 roots
-template <> struct Kind<1> { static constexpr int kSample = 4, kSlots = 1, kLoMin = 4, kScore = 1; };   // H
-template <> struct Kind<2> { static constexpr int kSample = 2, kSlots = 1, kScore = 0; };   // F = [e']x H
+// Pixels -> camera coordinates, (p - c) / f per axis: a subtraction, then a division (fp64, correctly rounded).
+__device__ __forceinline__ void to_camera(const double* p, const Intrinsics& K, double& x1, double& y1, double& x2,
+                                          double& y2) {
+  x1 = (p[0] - K.cx1) / K.fx1;
+  y1 = (p[1] - K.cy1) / K.fy1;
+  x2 = (p[2] - K.cx2) / K.fx2;
+  y2 = (p[3] - K.cy2) / K.fy2;
+}
+
+// cv2.findEssentialMat's threshold in camera coordinates: px_th / ((fx + fy) / 2) of view 2, squared.
+__device__ __forceinline__ float ess_th2(double px_th, const Intrinsics& K) {
+  const double th = px_th / ((K.fx2 + K.fy2) / 2.0);
+  return (float)(th * th);
+}
+
+// Row p in the solvers' frame: camera coordinates for E (kind 3), Hartley-normalised coordinates otherwise.
+template <int KIND>
+__device__ __forceinline__ void to_frame(const VerifyState& S, const double* p, double (&q)[4]) {
+  if constexpr (KIND == 3) {
+    to_camera(p, S.K, q[0], q[1], q[2], q[3]);
+  } else {
+    q[0] = (p[0] - S.cx[0]) * S.s[0];
+    q[1] = (p[1] - S.cy[0]) * S.s[0];
+    q[2] = (p[2] - S.cx[1]) * S.s[1];
+    q[3] = (p[3] - S.cy[1]) * S.s[1];
+  }
+}
 
 // ---- fp64 linear algebra (one thread) ----------------------------------------------------------------------------
 
@@ -187,6 +217,50 @@ __device__ int solve_h4(const double (&p)[4][4], double (&out)[1][9]) {
   return 1;
 }
 
+// ---- the kinds ----------------------------------------------------------------------------------------------------
+// kSample rows per minimal sample, up to kSlots models per sample, kPairSlots model slots per hypothesis in a pair's
+// round buffers (F's 3 for F, H and DEGENSAC, which share one scratch layout), LO refits from kLoMin inliers, kScore
+// the inlier test (0: Sampson, F and E; 1: transfer error, H), kTile rows staged in shared memory per scoring pass.
+// solve: a minimal sample in the solvers' frame -> models in the scoring frame.  refit: the smallest eigenvector of
+// LO's normal matrix -> a model in the scoring frame (false: none).  Kind 2 is DEGENSAC's plane-and-parallax round
+// (F from 2 rows and H, no solver); kind 3, E, is defined in pose.cu.
+template <int KIND> struct Kind;
+template <> struct Kind<0> {                                       // F: 7-point, up to 3 roots
+  static constexpr int kSample = 7, kSlots = 3, kPairSlots = 3, kLoMin = 8, kScore = 0, kTile = 2048;
+  static __device__ int solve(const VerifyState& S, const double (&p)[7][4], double (&out)[3][9]) {
+    double mn[3][9];
+    const int raw = solve_f7(p, mn);
+    int nm = 0;
+    for (int k = 0; k < raw; ++k)
+      if (denormalise<0>(S, mn[k], out[nm])) ++nm;
+    return nm;
+  }
+  // Rank 2: F <- F (I - e e^T), e the smallest right singular vector.
+  static __device__ bool refit(const VerifyState& S, double (&h)[9], double* out) {
+    double G[3][3], ev[3];
+    for (int i = 0; i < 3; ++i)
+      for (int j = 0; j < 3; ++j) G[i][j] = h[i] * h[j] + h[3 + i] * h[3 + j] + h[6 + i] * h[6 + j];
+    jacobi_min_eigvec<3>(G, ev);
+    for (int i = 0; i < 3; ++i) {
+      const double fe = h[3 * i] * ev[0] + h[3 * i + 1] * ev[1] + h[3 * i + 2] * ev[2];
+      for (int j = 0; j < 3; ++j) h[3 * i + j] -= fe * ev[j];
+    }
+    return denormalise<0>(S, h, out);
+  }
+};
+template <> struct Kind<1> {                                       // H: 4-point DLT
+  static constexpr int kSample = 4, kSlots = 1, kPairSlots = 3, kLoMin = 4, kScore = 1, kTile = 2048;
+  static __device__ int solve(const VerifyState& S, const double (&p)[4][4], double (&out)[1][9]) {
+    double mn[1][9];
+    return solve_h4(p, mn) && denormalise<1>(S, mn[0], out[0]);
+  }
+  static __device__ bool refit(const VerifyState& S, double (&h)[9], double* out) { return denormalise<1>(S, h, out); }
+};
+template <> struct Kind<2> { static constexpr int kSample = 2, kSlots = 1, kPairSlots = 3, kScore = 0, kTile = 2048; };
+
+template <int KIND> constexpr size_t kPairModels = (size_t)kRound * Kind<KIND>::kPairSlots * 9;   // doubles per pair
+template <int KIND> constexpr size_t kPairCounts = (size_t)kRound * Kind<KIND>::kPairSlots;       // ints per pair
+
 // ---- scoring ------------------------------------------------------------------------------------------------------
 // F: dd^2 / den < th^2.  H: |pi(H x1) - x2|^2 < th^2, never with a non-positive or vanishing third coordinate.
 template <int KIND>
@@ -267,57 +341,63 @@ __device__ bool parallax_model(const VerifyState& S, const double* rows, int str
 }
 
 // ---- kernels ------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(1024) verify_prep_kernel(PairBatch B, int min_rows, float4* __restrict__ rows32_all,
+// Effective row count, finiteness, the solvers' frame (F / H: the Hartley normalisation; E, CAMERA: the pair's
+// cameras), the scoring threshold, and the fp32 rows in the scoring frame (F / H: pixels; E: camera coordinates).  A
+// pair with fewer than min_rows rows, or a non-finite one, runs no rounds.
+template <bool CAMERA>
+__global__ void __launch_bounds__(1024) verify_prep_kernel(PairBatch B, const double* __restrict__ intr, Intrinsics K1,
+                                                           double px_th, int min_rows, float4* __restrict__ rows32_all,
                                                            VerifyState* __restrict__ st_all) {
   __shared__ double red[33];
-  __shared__ int s_n, s_bad;
+  __shared__ int s_n;
   const int tid = threadIdx.x;
   VerifyState* st = st_all + blockIdx.y;
   const PairRange pr = pair_range(B, blockIdx.y);
   const int n = pr.n, stride = B.stride;
   const double* rows = B.rows + pr.row0 * stride;
   float4* rows32 = rows32_all + (pr.row0 - B.base);
-  if (tid == 0) {
-    int m = n;
-    if (B.n_dev != nullptr) {
-      const double v = B.n_dev[blockIdx.y];
-      if (v >= 0.0 && v < (double)n) m = (int)v;
-    }
-    s_n = m;
-    s_bad = 0;
-  }
+  const Intrinsics K = pair_intrinsics(intr, K1, blockIdx.y);
+  if (tid == 0) s_n = effective_rows(B, blockIdx.y, n);
   __syncthreads();
   const int m = s_n;
   double sx[4] = {0.0, 0.0, 0.0, 0.0};
   int bad = 0;
   for (int r = tid; r < m; r += 1024) {
     const double* p = rows + (size_t)r * stride;
-    const double a = p[0], b = p[1], c = p[2], d = p[3];
-    bad |= !(isfinite(a) && isfinite(b) && isfinite(c) && isfinite(d));
-    sx[0] += a; sx[1] += b; sx[2] += c; sx[3] += d;
-    rows32[r] = make_float4((float)a, (float)b, (float)c, (float)d);
+    double q[4] = {p[0], p[1], p[2], p[3]};
+    bad |= !(isfinite(q[0]) && isfinite(q[1]) && isfinite(q[2]) && isfinite(q[3]));
+    if constexpr (CAMERA) to_camera(p, K, q[0], q[1], q[2], q[3]);
+    else for (int k = 0; k < 4; ++k) sx[k] += q[k];
+    rows32[r] = make_float4((float)q[0], (float)q[1], (float)q[2], (float)q[3]);
   }
-  if (bad) s_bad = 1;
-  double mean[4];
-  for (int k = 0; k < 4; ++k) mean[k] = block_sum_1024(sx[k], red) / (double)(m > 0 ? m : 1);
-  double dist[2] = {0.0, 0.0};
-  if (!s_bad)
-    for (int r = tid; r < m; r += 1024) {
-      const double* p = rows + (size_t)r * stride;
-      dist[0] += sqrt((p[0] - mean[0]) * (p[0] - mean[0]) + (p[1] - mean[1]) * (p[1] - mean[1]));
-      dist[1] += sqrt((p[2] - mean[2]) * (p[2] - mean[2]) + (p[3] - mean[3]) * (p[3] - mean[3]));
-    }
-  for (int k = 0; k < 2; ++k) dist[k] = block_sum_1024(dist[k], red) / (double)(m > 0 ? m : 1);
+  bad = __syncthreads_or(bad);
+  double mean[4], dist[2] = {0.0, 0.0};
+  if constexpr (!CAMERA) {
+    for (int k = 0; k < 4; ++k) mean[k] = block_sum_1024(sx[k], red) / (double)(m > 0 ? m : 1);
+    if (!bad)
+      for (int r = tid; r < m; r += 1024) {
+        const double* p = rows + (size_t)r * stride;
+        dist[0] += sqrt((p[0] - mean[0]) * (p[0] - mean[0]) + (p[1] - mean[1]) * (p[1] - mean[1]));
+        dist[1] += sqrt((p[2] - mean[2]) * (p[2] - mean[2]) + (p[3] - mean[3]) * (p[3] - mean[3]));
+      }
+    for (int k = 0; k < 2; ++k) dist[k] = block_sum_1024(dist[k], red) / (double)(m > 0 ? m : 1);
+  }
   if (tid == 0) {
-    for (int k = 0; k < 2; ++k) {
-      st->cx[k] = mean[2 * k];
-      st->cy[k] = mean[2 * k + 1];
-      st->s[k] = dist[k] > 0.0 ? 1.4142135623730951 / dist[k] : 1.0;
+    if constexpr (CAMERA) {
+      st->K = K;
+      st->th2 = ess_th2(px_th, K);
+    } else {
+      for (int k = 0; k < 2; ++k) {
+        st->cx[k] = mean[2 * k];
+        st->cy[k] = mean[2 * k + 1];
+        st->s[k] = dist[k] > 0.0 ? 1.4142135623730951 / dist[k] : 1.0;
+      }
+      st->th2 = (float)(px_th * px_th);
     }
     for (int j = 0; j < 9; ++j) st->best[j] = 0.0;
     st->n = m;
-    st->bad = s_bad;
-    st->stop = s_bad || m < min_rows;
+    st->bad = bad;
+    st->stop = bad || m < min_rows;
     st->best_count = 0;
     st->pending = 0;
     st->n_all = n;
@@ -326,17 +406,17 @@ __global__ void __launch_bounds__(1024) verify_prep_kernel(PairBatch B, int min_
   }
 }
 
-// Hypotheses first .. first + count - 1.  models [count * slots][9] fp64 (pixel coordinates), counts [count * slots]
+// Hypotheses first .. first + count - 1.  models [count * slots][9] fp64 (scoring frame), counts [count * slots]
 // (-1: no model in that slot).
 template <int KIND>
 __global__ void __launch_bounds__(kScoreThreads, 1) verify_round_kernel(const VerifyState* __restrict__ st_all,
                                                                      const float4* __restrict__ rows32_all,
                                                                      const double* __restrict__ rows_all, int stride,
                                                                      int first, int count, unsigned long long seed,
-                                                                     float th2, int ignore_stop, double h_th2,
+                                                                     int ignore_stop, double h_th2,
                                                                      double* __restrict__ models_all,
                                                                      int* __restrict__ counts_all) {
-  constexpr int S = Kind<KIND>::kSample, SL = Kind<KIND>::kSlots, NM = kHypPerBlock * SL;
+  constexpr int S = Kind<KIND>::kSample, SL = Kind<KIND>::kSlots, NM = kHypPerBlock * SL, kTile = Kind<KIND>::kTile;
   __shared__ float4 s_rows[kTile];
   __shared__ float s_model[NM][9];
   __shared__ int s_valid[NM];
@@ -344,35 +424,24 @@ __global__ void __launch_bounds__(kScoreThreads, 1) verify_round_kernel(const Ve
   if (KIND == 2 ? !st->pending : !ignore_stop && st->stop) return;
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   const int n = st->n;
+  const float th2 = st->th2;
   const double* rows = rows_all + st->row0 * stride;
   const float4* rows32 = rows32_all + st->row32;
-  double* models = models_all + blockIdx.y * kPairModels;
-  int* counts = counts_all + blockIdx.y * kPairCounts;
+  double* models = models_all + blockIdx.y * kPairModels<KIND>;
+  int* counts = counts_all + blockIdx.y * kPairCounts<KIND>;
   if (tid < kHypPerBlock) {
     const int local = blockIdx.x * kHypPerBlock + tid;
     double out[SL][9];
     int nm = 0;
-    if (KIND == 2) {
+    if constexpr (KIND == 2) {
       if (local < count && parallax_model(*st, rows, stride, seed, first + local, h_th2, out[0])) nm = 1;
     } else if (local < count) {
       int idx[S];
       if (draw_sample<S>(seed, first + local, n, idx)) {
         double p[S][4];
 #pragma unroll
-        for (int k = 0; k < S; ++k) {
-          const double* r = rows + (size_t)idx[k] * stride;
-          p[k][0] = (r[0] - st->cx[0]) * st->s[0];
-          p[k][1] = (r[1] - st->cy[0]) * st->s[0];
-          p[k][2] = (r[2] - st->cx[1]) * st->s[1];
-          p[k][3] = (r[3] - st->cy[1]) * st->s[1];
-        }
-        double mn[SL][9];
-        int raw;
-        if constexpr (KIND == 0) raw = solve_f7(p, mn);
-        else if constexpr (KIND == 1) raw = solve_h4(p, mn);
-        else raw = 0;
-        for (int k = 0; k < raw; ++k)
-          if (denormalise<KIND>(*st, mn[k], out[nm])) ++nm;
+        for (int k = 0; k < S; ++k) to_frame<KIND>(*st, rows + (size_t)idx[k] * stride, p[k]);
+        nm = Kind<KIND>::solve(*st, p, out);
       }
     }
     for (int k = 0; k < SL; ++k) {
@@ -416,23 +485,26 @@ __global__ void __launch_bounds__(kScoreThreads, 1) verify_round_kernel(const Ve
   }
 }
 
-// Best of this round's nm models -> state if strictly better than the best so far; then the stopping bound.
+// Best of this round's nm models -> state if strictly better than the best so far; then the stopping bound for samples
+// of `sample` rows.  Pair p's round models and counts start pair_slots * kRound slots after pair p - 1's.
 __global__ void __launch_bounds__(1024) verify_select_kernel(VerifyState* __restrict__ st, const double* __restrict__ models,
                                                              const int* __restrict__ counts, int nm, int done, int sample,
-                                                             double conf, int max_iters) {
-  select_round(st + blockIdx.y, models + blockIdx.y * kPairModels, counts + blockIdx.y * kPairCounts, nm, done, sample,
-               conf, max_iters);
+                                                             int pair_slots, double conf, int max_iters) {
+  const size_t slots = (size_t)blockIdx.y * kRound * pair_slots;
+  select_round(st + blockIdx.y, models + slots * 9, counts + slots, nm, done, sample, conf, max_iters);
 }
 
-// Local optimisation + outputs.  Refits on the inliers of the current model in normalised coordinates (F: 8-point with
-// rank-2 enforcement; H: DLT), keeps the refit while it has strictly more inliers, then writes model, mask and count.
-// Pair p writes model_out[9 p ..], count_out[p] and mask_out[row0 .. row0 + n_all).
+// Local optimisation + outputs.  Refits on the inliers of the current model in the solvers' frame (F: 8-point with
+// rank-2 enforcement; H: DLT; E: 8-point projected onto the essential manifold), keeps the refit while it has strictly
+// more inliers, then writes model, mask and count.  Pair p writes model_out[9 p ..], count_out[p] and
+// mask_out[row0 .. row0 + n_all).
 template <int KIND>
 __global__ void __launch_bounds__(kLoThreads, 1) verify_lo_kernel(const VerifyState* __restrict__ st_all,
                                                                const float4* __restrict__ rows32_all,
                                                                const double* __restrict__ rows_all, int stride,
-                                                               float th2, double* __restrict__ model_out,
+                                                               double* __restrict__ model_out,
                                                                uint8_t* __restrict__ mask_out, int* __restrict__ count_out) {
+  constexpr int SC = Kind<KIND>::kScore;
   __shared__ double s_red[kLoThreads / 32][45];
   __shared__ double s_cur[9], s_cand[9];
   __shared__ float s_f32[9];
@@ -440,6 +512,7 @@ __global__ void __launch_bounds__(kLoThreads, 1) verify_lo_kernel(const VerifySt
   const VerifyState* st = st_all + blockIdx.y;
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   const int n = st->n, bad = st->bad, n_all = st->n_all;
+  const float th2 = st->th2;
   const double* rows = rows_all + st->row0 * stride;
   const float4* rows32 = rows32_all + st->row32;
   model_out += 9 * blockIdx.y;
@@ -456,7 +529,7 @@ __global__ void __launch_bounds__(kLoThreads, 1) verify_lo_kernel(const VerifySt
 #pragma unroll
     for (int e = 0; e < 9; ++e) m[e] = s_f32[e];
     int c = 0;
-    for (int r = tid; r < n; r += kLoThreads) c += is_inlier<KIND>(m, rows32[r], th2);
+    for (int r = tid; r < n; r += kLoThreads) c += is_inlier<SC>(m, rows32[r], th2);
     for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
     if (lane == 0) s_cnt[wid] = c;
     __syncthreads();
@@ -475,12 +548,13 @@ __global__ void __launch_bounds__(kLoThreads, 1) verify_lo_kernel(const VerifySt
     double acc[45];
 #pragma unroll
     for (int e = 0; e < 45; ++e) acc[e] = 0.0;
-    const double c1x = st->cx[0], c1y = st->cy[0], s1 = st->s[0], c2x = st->cx[1], c2y = st->cy[1], s2 = st->s[1];
+    const VerifyState S = *st;                            // the frame, in registers for the row loop
     for (int r = tid; r < n; r += kLoThreads) {
-      if (!is_inlier<KIND>(m, rows32[r], th2)) continue;
-      const double* p = rows + (size_t)r * stride;
-      const double x = (p[0] - c1x) * s1, y = (p[1] - c1y) * s1, u = (p[2] - c2x) * s2, v = (p[3] - c2y) * s2;
-      if (KIND == 0) {
+      if (!is_inlier<SC>(m, rows32[r], th2)) continue;
+      double q[4];
+      to_frame<KIND>(S, rows + (size_t)r * stride, q);
+      const double x = q[0], y = q[1], u = q[2], v = q[3];
+      if (SC == 0) {
         const double a[9] = {u * x, u * y, u, v * x, v * y, v, x, y, 1.0};
         int e = 0;
 #pragma unroll
@@ -514,17 +588,7 @@ __global__ void __launch_bounds__(kLoThreads, 1) verify_lo_kernel(const VerifySt
           ++e;
         }
       jacobi_min_eigvec<9>(M, h);
-      if (KIND == 0) {                                     // rank 2: F <- F (I - e e^T), e the smallest right singular vector
-        double G[3][3], ev[3];
-        for (int i = 0; i < 3; ++i)
-          for (int j = 0; j < 3; ++j) G[i][j] = h[i] * h[j] + h[3 + i] * h[3 + j] + h[6 + i] * h[6 + j];
-        jacobi_min_eigvec<3>(G, ev);
-        for (int i = 0; i < 3; ++i) {
-          const double fe = h[3 * i] * ev[0] + h[3 * i + 1] * ev[1] + h[3 * i + 2] * ev[2];
-          for (int j = 0; j < 3; ++j) h[3 * i + j] -= fe * ev[j];
-        }
-      }
-      s_ok = denormalise<KIND>(*st, h, s_cand);
+      s_ok = Kind<KIND>::refit(S, h, s_cand);
     }
     __syncthreads();
     if (!s_ok) break;
@@ -543,7 +607,7 @@ __global__ void __launch_bounds__(kLoThreads, 1) verify_lo_kernel(const VerifySt
 #pragma unroll
   for (int e = 0; e < 9; ++e) m[e] = s_f32[e];
   for (int r = tid; r < n_all; r += kLoThreads)
-    mask_out[r] = cur_count > 0 && r < n && is_inlier<KIND>(m, rows32[r], th2);
+    mask_out[r] = cur_count > 0 && r < n && is_inlier<SC>(m, rows32[r], th2);
 }
 
 struct Scratch {
@@ -555,6 +619,7 @@ struct Scratch {
 
 // `pairs` states, `rows` fp32 rows, then nhyp hypotheses' models and counts per pair (nhyp = kRound: pair strides
 // kPairModels / kPairCounts).
+template <int KIND>
 Scratch carve(void* base, int pairs, long long rows, int nhyp) {
   char* p = (char*)base;
   Scratch s;
@@ -563,18 +628,72 @@ Scratch carve(void* base, int pairs, long long rows, int nhyp) {
   s.rows32 = (float4*)p;
   p += align_up((size_t)rows * sizeof(float4) + 16, 1024);
   s.models = (double*)p;
-  p += align_up((size_t)pairs * nhyp * 3 * 9 * sizeof(double), 1024);
+  p += align_up((size_t)pairs * nhyp * Kind<KIND>::kPairSlots * 9 * sizeof(double), 1024);
   s.counts = (int*)p;
   return s;
 }
 
+// Bytes carve<KIND> lays out for nhyp = kRound (rounds) or 0.
 template <int KIND>
-int enqueue_round(const Scratch& s, const PairBatch& B, int first, int count, unsigned long long seed, float th2,
-                  int ignore_stop, cudaStream_t st, double h_th2 = 0.0) {
+size_t scratch_bytes(int pairs, long long rows, bool rounds) {
+  return align_up((size_t)pairs * sizeof(VerifyState), 1024) + align_up((size_t)rows * sizeof(float4) + 16, 1024) +
+         (rounds ? align_up((size_t)pairs * kPairModels<KIND> * sizeof(double), 1024) +
+                       (size_t)pairs * kPairCounts<KIND> * sizeof(int)
+                 : 0);
+}
+
+// Pairs per launch within kBatchScratchBudget.
+template <int KIND>
+int chunk_pairs() {
+  const size_t per_pair = sizeof(VerifyState) + kPairModels<KIND> * sizeof(double) + kPairCounts<KIND> * sizeof(int);
+  return (int)std::min<size_t>(kMaxGridY, std::max<size_t>(1, kBatchScratchBudget / per_pair));
+}
+
+template <int KIND>
+int enqueue_round(const Scratch& s, const PairBatch& B, int first, int count, unsigned long long seed, int ignore_stop,
+                  cudaStream_t st, double h_th2 = 0.0) {
   verify_round_kernel<KIND><<<dim3(cdiv(count, kHypPerBlock), B.pairs), kScoreThreads, 0, st>>>(
-      s.st, s.rows32, B.rows, B.stride, first, count, seed, th2, ignore_stop, h_th2, s.models, s.counts);
+      s.st, s.rows32, B.rows, B.stride, first, count, seed, ignore_stop, h_th2, s.models, s.counts);
   P2P_LAUNCH_OK();
   return 0;
+}
+
+// RANSAC for F (kind 0), H (1) or E (3): prep, then per round of kRound hypotheses a round and a select, then LO.
+// intr / K1: the pairs' cameras for E, as launch_find_essential takes them; F and H ignore them.
+template <int KIND>
+int find_model(const PairBatch& B, const double* intr, const Intrinsics& K1, double px_th, double conf, int max_iters,
+               unsigned long long seed, void* scratch, double* model_out, uint8_t* mask_out, int* count_out,
+               cudaStream_t st) {
+  const Scratch s = carve<KIND>(scratch, B.pairs, B.total, kRound);
+  verify_prep_kernel<KIND == 3><<<dim3(1, B.pairs), 1024, 0, st>>>(B, intr, K1, px_th, Kind<KIND>::kSample, s.rows32,
+                                                                    s.st);
+  P2P_LAUNCH_OK();
+  for (int first = 0; first < max_iters; first += kRound) {
+    const int count = min(kRound, max_iters - first);
+    int rc = enqueue_round<KIND>(s, B, first, count, seed, 0, st);
+    if (rc) return rc;
+    verify_select_kernel<<<dim3(1, B.pairs), 1024, 0, st>>>(s.st, s.models, s.counts, count * Kind<KIND>::kSlots,
+                                                            first + count, Kind<KIND>::kSample, Kind<KIND>::kPairSlots,
+                                                            conf, max_iters);
+    P2P_LAUNCH_OK();
+  }
+  verify_lo_kernel<KIND><<<dim3(1, B.pairs), kLoThreads, 0, st>>>(s.st, s.rows32, B.rows, B.stride, model_out, mask_out,
+                                                                  count_out);
+  P2P_LAUNCH_OK();
+  return 0;
+}
+
+// Test hook: hypotheses 0 .. count-1 of a single pair without selection.
+template <int KIND>
+int test_hypotheses(const double* rows, int stride, int n, const Intrinsics& K, double px_th, unsigned long long seed,
+                    int count, void* scratch, double* models_out, int* counts_out, cudaStream_t st) {
+  const PairBatch B = single_pair(rows, stride, n, nullptr);
+  Scratch s = carve<KIND>(scratch, 1, n, 0);
+  s.models = models_out;
+  s.counts = counts_out;
+  verify_prep_kernel<KIND == 3><<<1, 1024, 0, st>>>(B, nullptr, K, px_th, Kind<KIND>::kSample, s.rows32, s.st);
+  P2P_LAUNCH_OK();
+  return enqueue_round<KIND>(s, B, 0, count, seed, 1, st);
 }
 
 }  // namespace
