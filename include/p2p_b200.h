@@ -144,7 +144,7 @@ P2P_API int p2p_delta_pack(p2p_handle_t h, const int64_t* di, const int64_t* dj,
 
 /* MutualMatching alone (networks/ncn/model.py:157-176) on [nA, nB]. */
 P2P_API int p2p_mutual_matching(p2p_handle_t h, const float* in, int nA, int nB, float* out, void* stream);
-/* NeighConsensus alone (networks/ncn/model.py:145-155) on [hA,wA,hB,wB]. */
+/* NeighConsensus alone (networks/ncn/model.py:145-155) on [hA,wA,hB,wB] (timed as P2P_PROF_NC). */
 P2P_API int p2p_neigh_consensus(p2p_handle_t h, const float* in, int hA, int wA, int hB, int wB, float* out, void* stream);
 /* The stack of p2p_set_nc_stack_weights alone on [hA,wA,hB,wB] fp32 (tensor cores; timed as P2P_PROF_NC). */
 P2P_API int p2p_nc_stack(p2p_handle_t h, const float* in, int hA, int wA, int hB, int wB, float* out, void* stream);

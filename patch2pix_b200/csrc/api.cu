@@ -681,12 +681,67 @@ static int corr_umma(p2p_handle_s* h, const __half* a_hi, const __half* a_lo, co
   return launch_umma_gemm(p, EPI_PLAIN, h->opt_corr_passes, sms(h), st);
 }
 
-static int coarse_impl(p2p_handle_t h, const float* feat1, const float* feat2, int fmt, int c, int h1, int w1, int h2, int w2,
-                       int ksize, float* corr4d_out, uint8_t* delta_code_out, float* pooled_out, float* ncn_out,
-                       void* stream) {
+// The NeighConsensus a coarse-stage or standalone call runs: Patch2Pix's fixed 2-layer stack on the tensor cores
+// (nc_umma.cu) or, with option nc_impl 0, on the fp32 kernels (coarse.cu); or NCNet's stack of
+// p2p_set_nc_stack_weights (nc_stack.cu).
+enum NcKind { kNcUmma, kNcFp32, kNcStack };
+
+// Fails unless the weights of the chosen NeighConsensus are set.
+static int pick_nc(const p2p_handle_s* h, bool ncnet, NcKind& kind) {
+  if (ncnet)
+    P2P_REQUIRE(h->ncs_set, "p2p_set_nc_stack_weights has not been called");
+  else
+    P2P_REQUIRE(h->nc_set, "p2p_set_ncn_weights has not been called");
+  kind = ncnet ? kNcStack : h->opt_nc_impl == 1 ? kNcUmma : kNcFp32;
+  return 0;
+}
+
+// NeighConsensus scratch.  hidden: fp16 hi/lo [V][64] (nc_umma), fp32 [nA][32][nB] (nc_impl 0) or the stack's lines;
+// partial [18][V] f32 and xp only for nc_umma.
+struct NcScratch {
+  void* hidden = nullptr;
+  float* partial = nullptr;
+  uint32_t* xp = nullptr;
+};
+
+static size_t nc_scratch_bytes(NcKind kind, int hA, int wA, int hB, int wB) {
+  const size_t V = (size_t)hA * wA * hB * wB;
+  if (kind == kNcUmma) return nc_umma_scratch_bytes(V) + nc_umma_xp_bytes(hA, wA, hB, wB);
+  return kind == kNcFp32 ? V * 128 : nc_stack_scratch_bytes(V);
+}
+
+static bool carve_nc(Arena& A, NcKind kind, int hA, int wA, int hB, int wB, NcScratch& s) {
+  const size_t V = (size_t)hA * wA * hB * wB;
+  s.hidden = A.take(kind == kNcStack ? nc_stack_scratch_bytes(V) : V * 128);
+  if (kind != kNcUmma) return s.hidden != nullptr;
+  s.partial = (float*)A.take(18 * V * 4);
+  s.xp = (uint32_t*)A.take(nc_umma_xp_bytes(hA, wA, hB, wB));
+  return s.hidden && s.partial && s.xp;
+}
+
+// xmax: max |x| (nc_umma, nc_stack).  rowmax / colmax: nc_umma's combine pass also yields the maxima of the
+// MutualMatching that follows (may be null).
+static int launch_nc(p2p_handle_s* h, NcKind kind, const float* x, int hA, int wA, int hB, int wB, const NcScratch& s,
+                     const unsigned int* xmax, float* out, float* rowmax, unsigned int* colmax, cudaStream_t st) {
+  if (kind == kNcUmma)
+    return launch_neigh_consensus_umma(x, hA, wA, hB, wB, h->ncw, h->nc_b1p, h->nc_b2, xmax, s.xp, (__half*)s.hidden,
+                                       s.partial, out, rowmax, colmax, h->opt_nc_l2_mode, sms(h), st);
+  if (kind == kNcFp32)
+    return launch_neigh_consensus(x, hA, wA, hB, wB, h->nc_w1p, h->nc_b1p, h->nc_w2p, h->nc_b2, (float*)s.hidden, out, st);
+  return launch_nc_stack(x, hA, wA, hB, wB, h->ncs, xmax, (__half*)s.hidden, out, sms(h), st);
+}
+
+// The coarse stage of one pair: L2-normalise, correlation (+ 4D max-pool for ksize 2), MutualMatching,
+// NeighConsensus, MutualMatching.  ncnet: NCNet's stack (fp32 NCHW features, tensor-core correlation only), else
+// Patch2Pix's fixed stack.  fmt 1: channels-last fp16 features.
+static int coarse_impl(p2p_handle_t h, bool ncnet, const float* feat1, const float* feat2, int fmt, int c, int h1, int w1,
+                       int h2, int w2, int ksize, float* corr4d_out, uint8_t* delta_code_out, float* pooled_out,
+                       float* ncn_out, void* stream) {
   P2P_ENTER(h);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  P2P_REQUIRE(h->nc_set, "p2p_set_ncn_weights has not been called");
+  NcKind kind;
+  int rc = pick_nc(h, ncnet, kind);
+  if (rc) return rc;
   P2P_REQUIRE(feat1 && feat2 && corr4d_out, "null tensor pointer");
   P2P_REQUIRE(ksize == 1 || ksize == 2, "ksize must be 1 or 2");
   P2P_REQUIRE(c > 0 && h1 > 0 && w1 > 0 && h2 > 0 && w2 > 0, "empty feature map");
@@ -694,161 +749,96 @@ static int coarse_impl(p2p_handle_t h, const float* feat1, const float* feat2, i
     P2P_REQUIRE(h1 % 2 == 0 && w1 % 2 == 0 && h2 % 2 == 0 && w2 % 2 == 0, "ksize 2 needs even feature sizes");
     P2P_REQUIRE(delta_code_out != nullptr, "delta_code_out is required for ksize 2");
   }
+  const bool tc = h->opt_corr_passes > 0;
+  if (ncnet) P2P_REQUIRE(tc, "p2p_ncnet_coarse needs the tensor-core correlation (corr_passes 1 or 3)");
+  if (tc) P2P_REQUIRE(c % 64 == 0 && c / 64 <= kMaxKSteps, "tensor-core correlation needs C % 64 == 0");
+  P2P_REQUIRE(fmt == 0 || tc, "channels-last fp16 features need the tensor-core correlation (corr_passes 1 or 3)");
   const int n1 = h1 * w1, n2 = h2 * w2;
   const int hA = h1 / ksize, wA = w1 / ksize, hB = h2 / ksize, wB = w2 / ksize;
   const int nA = hA * wA, nB = hB * wB;
   const size_t V = (size_t)nA * nB;
-  const bool tc = h->opt_corr_passes > 0;
-  if (tc) P2P_REQUIRE(c % 64 == 0 && c / 64 <= kMaxKSteps, "tensor-core correlation needs C % 64 == 0");
-  P2P_REQUIRE(fmt == 0 || tc, "channels-last fp16 features need the tensor-core correlation (corr_passes 1 or 3)");
   const int n1pad = (int)align_up(n1, 128), n2pad = (int)align_up(n2, 256);
-  size_t need = 4 * V * 4 + nc_umma_scratch_bytes(V) + nc_umma_xp_bytes(hA, wA, hB, wB) + (size_t)(nA + nB) * 8 + (1 << 16);
-  need += tc ? (size_t)(n1pad + n2pad) * c * 4 : (size_t)(n1 + n2) * c * 4;
-  int rc = h->coarse.reserve(need);
-  if (rc) return rc;
+  // pooled, m1, nc [V] f32; the NC scratch; MutualMatching maxima + xmax; the correlation operands (fp16 hi/lo, or fp32)
+  const size_t need = 3 * V * 4 + nc_scratch_bytes(kind, hA, wA, hB, wB) + (size_t)(nA + nB) * 4 + 16 +
+                      (size_t)(tc ? n1pad + n2pad : n1 + n2) * c * 4 + (1 << 16);
+  if ((rc = h->coarse.reserve(need))) return rc;
   Arena& A = h->coarse;
   float* pooled = pooled_out ? pooled_out : (float*)A.take(V * 4);
   float* m1 = (float*)A.take(V * 4);
   float* nc = ncn_out ? ncn_out : (float*)A.take(V * 4);
-  float* hidden = (float*)A.take(V * 128);               // fp32 [nA][32][nB] (nc_impl 0) or fp16 hi/lo [V][64] (nc_impl 1)
-  float* partial = (float*)A.take(18 * V * 4);
-  uint32_t* xp = (uint32_t*)A.take(nc_umma_xp_bytes(hA, wA, hB, wB));
+  NcScratch ns;
+  const bool nc_ok = carve_nc(A, kind, hA, wA, hB, wB, ns);
   float* rowmax = (float*)A.take((size_t)nA * 4);
   unsigned int* colmax = (unsigned int*)A.take((size_t)nB * 4 + 16);
   unsigned int* xmax = colmax != nullptr ? colmax + nB : nullptr;
+  __half *a_hi = nullptr, *a_lo = nullptr, *b_hi = nullptr, *b_lo = nullptr;   // tensor-core operands
+  float *fa = nullptr, *fb = nullptr;                                            // CUDA-core operands (corr_passes 0)
   if (tc) {
-    __half* a_hi = (__half*)A.take((size_t)n1pad * c * 2);
-    __half* a_lo = (__half*)A.take((size_t)n1pad * c * 2);
-    __half* b_hi = (__half*)A.take((size_t)n2pad * c * 2);
-    __half* b_lo = (__half*)A.take((size_t)n2pad * c * 2);
-    P2P_REQUIRE(a_hi && a_lo && b_hi && b_lo && hidden && colmax, "scratch carve failed");
-    const bool lo = h->opt_corr_passes == 3;
-    {
-      ProfScope ps(h, P2P_PROF_L2NORM, st);
-      if (fmt == 1)
-        rc = launch_l2norm_perm_kmajor_pair_nhwc16(reinterpret_cast<const __half*>(feat1), reinterpret_cast<const __half*>(feat2),
-                                                   a_hi, lo ? a_lo : nullptr, b_hi, lo ? b_lo : nullptr, c, h1, w1, h2, w2, ksize, st);
-      else
-        rc = launch_l2norm_perm_kmajor_pair(feat1, feat2, a_hi, lo ? a_lo : nullptr, b_hi, lo ? b_lo : nullptr, c, h1, w1, h2,
-                                            w2, ksize, st);
-      if (rc) return rc;
-    }
-    ProfScope ps(h, P2P_PROF_CORR, st);
-    if ((rc = corr_umma(h, a_hi, a_lo, b_hi, b_lo, c, n1, n2, n1pad, n2pad, ksize, pooled, delta_code_out, st)))
-      return rc;
+    a_hi = (__half*)A.take((size_t)n1pad * c * 2);
+    a_lo = (__half*)A.take((size_t)n1pad * c * 2);
+    b_hi = (__half*)A.take((size_t)n2pad * c * 2);
+    b_lo = (__half*)A.take((size_t)n2pad * c * 2);
   } else {
-    float* fa = (float*)A.take((size_t)n1 * c * 4);
-    float* fb = (float*)A.take((size_t)n2 * c * 4);
-    P2P_REQUIRE(fa && fb && hidden && colmax, "scratch carve failed");
-    {
-      ProfScope ps(h, P2P_PROF_L2NORM, st);
-      if ((rc = launch_l2norm_perm(feat1, fa, c, h1, w1, ksize, st))) return rc;
-      if ((rc = launch_l2norm_perm(feat2, fb, c, h2, w2, ksize, st))) return rc;
-    }
-    ProfScope ps(h, P2P_PROF_CORR, st);
-    if ((rc = launch_corr_pool_simt(fa, fb, c, n1, n2, ksize, pooled, delta_code_out, st))) return rc;
+    fa = (float*)A.take((size_t)n1 * c * 4);
+    fb = (float*)A.take((size_t)n2 * c * 4);
   }
-  P2P_REQUIRE(partial != nullptr && xmax != nullptr && xp != nullptr, "scratch carve failed");
-  if (h->opt_nc_impl == 1) {
-    {
-      ProfScope ps(h, P2P_PROF_MUTUAL, st);
-      if ((rc = launch_mutual_matching(pooled, nA, nB, rowmax, colmax, m1, xmax, st))) return rc;
+  P2P_REQUIRE(pooled && m1 && nc && nc_ok && rowmax && colmax && (tc ? a_hi && a_lo && b_hi && b_lo : fa && fb),
+              "scratch carve failed");
+  const bool lo = h->opt_corr_passes == 3;
+  {
+    ProfScope ps(h, P2P_PROF_L2NORM, st);
+    if (!tc) {
+      if ((rc = launch_l2norm_perm(feat1, fa, c, h1, w1, ksize, st))) return rc;
+      rc = launch_l2norm_perm(feat2, fb, c, h2, w2, ksize, st);
+    } else if (fmt == 1) {
+      rc = launch_l2norm_perm_kmajor_pair_nhwc16(reinterpret_cast<const __half*>(feat1), reinterpret_cast<const __half*>(feat2),
+                                                 a_hi, lo ? a_lo : nullptr, b_hi, lo ? b_lo : nullptr, c, h1, w1, h2, w2, ksize, st);
+    } else {
+      rc = launch_l2norm_perm_kmajor_pair(feat1, feat2, a_hi, lo ? a_lo : nullptr, b_hi, lo ? b_lo : nullptr, c, h1, w1, h2,
+                                          w2, ksize, st);
     }
-    {
-      // layer 1, layer 2 (tensor cores) and the combine pass, which also yields the maxima of the second MutualMatching
-      ProfScope ps(h, P2P_PROF_NC, st);
-      if ((rc = launch_neigh_consensus_umma(m1, hA, wA, hB, wB, h->ncw, h->nc_b1p, h->nc_b2, xmax, xp, (__half*)hidden, partial,
-                                            nc, rowmax, colmax, h->opt_nc_l2_mode, sms(h), st)))
-        return rc;
-    }
-    ProfScope ps(h, P2P_PROF_MUTUAL, st);
-    return launch_mutual_apply(nc, nA, nB, rowmax, colmax, corr4d_out, nullptr, st);
+    if (rc) return rc;
+  }
+  {
+    ProfScope ps(h, P2P_PROF_CORR, st);
+    rc = tc ? corr_umma(h, a_hi, a_lo, b_hi, b_lo, c, n1, n2, n1pad, n2pad, ksize, pooled, delta_code_out, st)
+            : launch_corr_pool_simt(fa, fb, c, n1, n2, ksize, pooled, delta_code_out, st);
+    if (rc) return rc;
   }
   {
     ProfScope ps(h, P2P_PROF_MUTUAL, st);
-    if ((rc = launch_mutual_matching(pooled, nA, nB, rowmax, colmax, m1, nullptr, st))) return rc;
+    if ((rc = launch_mutual_matching(pooled, nA, nB, rowmax, colmax, m1, kind == kNcFp32 ? nullptr : xmax, st))) return rc;
   }
+  const bool fused_max = kind == kNcUmma;
   {
     ProfScope ps(h, P2P_PROF_NC, st);
-    if ((rc = launch_neigh_consensus(m1, hA, wA, hB, wB, h->nc_w1p, h->nc_b1p, h->nc_w2p, h->nc_b2, hidden, nc, st)))
+    if ((rc = launch_nc(h, kind, m1, hA, wA, hB, wB, ns, xmax, nc, fused_max ? rowmax : nullptr,
+                        fused_max ? colmax : nullptr, st)))
       return rc;
   }
   ProfScope ps(h, P2P_PROF_MUTUAL, st);
-  if ((rc = launch_mutual_matching(nc, nA, nB, rowmax, colmax, corr4d_out, nullptr, st))) return rc;
-  return 0;
+  if (fused_max) return launch_mutual_apply(nc, nA, nB, rowmax, colmax, corr4d_out, nullptr, st);
+  return launch_mutual_matching(nc, nA, nB, rowmax, colmax, corr4d_out, nullptr, st);
 }
 
 int p2p_coarse(p2p_handle_t h, const float* feat1, const float* feat2, int c, int h1, int w1, int h2, int w2,
                int ksize, float* corr4d_out, uint8_t* delta_code_out, float* pooled_out, float* ncn_out,
                void* stream) {
-  return coarse_impl(h, feat1, feat2, 0, c, h1, w1, h2, w2, ksize, corr4d_out, delta_code_out, pooled_out, ncn_out, stream);
+  return coarse_impl(h, false, feat1, feat2, 0, c, h1, w1, h2, w2, ksize, corr4d_out, delta_code_out, pooled_out, ncn_out,
+                     stream);
 }
 
 int p2p_coarse_nhwc16(p2p_handle_t h, const void* feat1_nhwc16, const void* feat2_nhwc16, int c, int h1, int w1, int h2, int w2,
                       int ksize, float* corr4d_out, uint8_t* delta_code_out, float* pooled_out, float* ncn_out,
                       void* stream) {
-  return coarse_impl(h, reinterpret_cast<const float*>(feat1_nhwc16), reinterpret_cast<const float*>(feat2_nhwc16), 1, c, h1, w1,
-                     h2, w2, ksize, corr4d_out, delta_code_out, pooled_out, ncn_out, stream);
+  return coarse_impl(h, false, reinterpret_cast<const float*>(feat1_nhwc16), reinterpret_cast<const float*>(feat2_nhwc16), 1,
+                     c, h1, w1, h2, w2, ksize, corr4d_out, delta_code_out, pooled_out, ncn_out, stream);
 }
 
 int p2p_ncnet_coarse(p2p_handle_t h, const float* feat1, const float* feat2, int c, int h1, int w1, int h2, int w2, int ksize,
                      float* corr4d_out, uint8_t* delta_code_out, void* stream) {
-  P2P_ENTER(h);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  P2P_REQUIRE(h->ncs_set, "p2p_set_nc_stack_weights has not been called");
-  P2P_REQUIRE(feat1 && feat2 && corr4d_out, "null tensor pointer");
-  P2P_REQUIRE(ksize == 1 || ksize == 2, "ksize must be 1 or 2");
-  P2P_REQUIRE(c > 0 && h1 > 0 && w1 > 0 && h2 > 0 && w2 > 0, "empty feature map");
-  P2P_REQUIRE(c % 64 == 0 && c / 64 <= kMaxKSteps, "the tensor-core correlation needs C % 64 == 0");
-  P2P_REQUIRE(h->opt_corr_passes > 0, "p2p_ncnet_coarse needs the tensor-core correlation (corr_passes 1 or 3)");
-  if (ksize == 2) {
-    P2P_REQUIRE(h1 % 2 == 0 && w1 % 2 == 0 && h2 % 2 == 0 && w2 % 2 == 0, "ksize 2 needs even feature sizes");
-    P2P_REQUIRE(delta_code_out != nullptr, "delta_code_out is required for ksize 2");
-  }
-  const int n1 = h1 * w1, n2 = h2 * w2;
-  const int hA = h1 / ksize, wA = w1 / ksize, hB = h2 / ksize, wB = w2 / ksize;
-  const int nA = hA * wA, nB = hB * wB;
-  const size_t V = (size_t)nA * nB;
-  const int n1pad = (int)align_up(n1, 128), n2pad = (int)align_up(n2, 256);
-  // pooled, m1, nc [V] f32; the stack's line buffers; MutualMatching maxima; the fp16 hi/lo correlation operands
-  const size_t need = 3 * V * 4 + nc_stack_scratch_bytes(V) + (size_t)(nA + nB) * 4 + (size_t)(n1pad + n2pad) * c * 4 +
-                      (1 << 16);
-  int rc = h->coarse.reserve(need);
-  if (rc) return rc;
-  Arena& A = h->coarse;
-  float* pooled = (float*)A.take(V * 4);
-  float* m1 = (float*)A.take(V * 4);
-  float* nc = (float*)A.take(V * 4);
-  __half* lines = (__half*)A.take(nc_stack_scratch_bytes(V));
-  float* rowmax = (float*)A.take((size_t)nA * 4);
-  unsigned int* colmax = (unsigned int*)A.take((size_t)nB * 4 + 16);
-  unsigned int* xmax = colmax != nullptr ? colmax + nB : nullptr;
-  __half* a_hi = (__half*)A.take((size_t)n1pad * c * 2);
-  __half* a_lo = (__half*)A.take((size_t)n1pad * c * 2);
-  __half* b_hi = (__half*)A.take((size_t)n2pad * c * 2);
-  __half* b_lo = (__half*)A.take((size_t)n2pad * c * 2);
-  P2P_REQUIRE(pooled && m1 && nc && lines && rowmax && colmax && a_hi && a_lo && b_hi && b_lo, "scratch carve failed");
-  const bool lo = h->opt_corr_passes == 3;
-  {
-    ProfScope ps(h, P2P_PROF_L2NORM, st);
-    if ((rc = launch_l2norm_perm_kmajor_pair(feat1, feat2, a_hi, lo ? a_lo : nullptr, b_hi, lo ? b_lo : nullptr, c, h1, w1,
-                                             h2, w2, ksize, st)))
-      return rc;
-  }
-  {
-    ProfScope ps(h, P2P_PROF_CORR, st);
-    if ((rc = corr_umma(h, a_hi, a_lo, b_hi, b_lo, c, n1, n2, n1pad, n2pad, ksize, pooled, delta_code_out, st))) return rc;
-  }
-  {
-    ProfScope ps(h, P2P_PROF_MUTUAL, st);
-    if ((rc = launch_mutual_matching(pooled, nA, nB, rowmax, colmax, m1, xmax, st))) return rc;
-  }
-  {
-    ProfScope ps(h, P2P_PROF_NC, st);
-    if ((rc = launch_nc_stack(m1, hA, wA, hB, wB, h->ncs, xmax, lines, nc, sms(h), st))) return rc;
-  }
-  ProfScope ps(h, P2P_PROF_MUTUAL, st);
-  return launch_mutual_matching(nc, nA, nB, rowmax, colmax, corr4d_out, nullptr, st);
+  return coarse_impl(h, true, feat1, feat2, 0, c, h1, w1, h2, w2, ksize, corr4d_out, delta_code_out, nullptr, nullptr,
+                     stream);
 }
 
 int p2p_delta_unpack(p2p_handle_t h, const uint8_t* code, long long n, int ksize, int64_t* di, int64_t* dj,
@@ -879,47 +869,38 @@ int p2p_mutual_matching(p2p_handle_t h, const float* in, int nA, int nB, float* 
   return launch_mutual_matching(in, nA, nB, rowmax, colmax, out, nullptr, reinterpret_cast<cudaStream_t>(stream));
 }
 
-int p2p_neigh_consensus(p2p_handle_t h, const float* in, int hA, int wA, int hB, int wB, float* out, void* stream) {
+// NeighConsensus alone on [hA, wA, hB, wB]: Patch2Pix's fixed stack (p2p_neigh_consensus) or NCNet's (p2p_nc_stack).
+static int nc_alone(p2p_handle_t h, bool ncnet, const float* in, int hA, int wA, int hB, int wB, float* out, void* stream) {
   P2P_ENTER(h);
-  P2P_REQUIRE(h->nc_set, "p2p_set_ncn_weights has not been called");
-  P2P_REQUIRE(in && out && hA > 0 && wA > 0 && hB > 0 && wB > 0, "bad argument");
-  const size_t V = (size_t)hA * wA * hB * wB;
-  int rc = h->misc.reserve(nc_umma_scratch_bytes(V) + nc_umma_xp_bytes(hA, wA, hB, wB) + 8192);
+  NcKind kind;
+  int rc = pick_nc(h, ncnet, kind);
   if (rc) return rc;
-  float* hidden = (float*)h->misc.take(V * 128);
-  float* partial = (float*)h->misc.take(18 * V * 4);
-  uint32_t* xp = (uint32_t*)h->misc.take(nc_umma_xp_bytes(hA, wA, hB, wB));
+  P2P_REQUIRE(in && out && hA > 0 && wA > 0 && hB > 0 && wB > 0, "bad argument");
+  if ((rc = h->misc.reserve(nc_scratch_bytes(kind, hA, wA, hB, wB) + 8192))) return rc;
+  NcScratch ns;
+  const bool nc_ok = carve_nc(h->misc, kind, hA, wA, hB, wB, ns);
   unsigned int* xmax = (unsigned int*)h->misc.take(16);
-  P2P_REQUIRE(hidden && partial && xmax && xp, "scratch carve failed");
-  h->dbg_nc[0] = hidden; h->dbg_nc[1] = partial; h->dbg_nc[2] = xp; h->dbg_nc[3] = xmax;
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (h->opt_nc_impl == 1) {
-    if ((rc = launch_absmax(in, V, xmax, st))) return rc;
-    return launch_neigh_consensus_umma(in, hA, wA, hB, wB, h->ncw, h->nc_b1p, h->nc_b2, xmax, xp, (__half*)hidden, partial, out,
-                                       nullptr, nullptr, h->opt_nc_l2_mode, sms(h), st);
+  P2P_REQUIRE(nc_ok && xmax, "scratch carve failed");
+  if (!ncnet) {
+    h->dbg_nc[0] = ns.hidden; h->dbg_nc[1] = ns.partial; h->dbg_nc[2] = ns.xp; h->dbg_nc[3] = xmax;
   }
-  return launch_neigh_consensus(in, hA, wA, hB, wB, h->nc_w1p, h->nc_b1p, h->nc_w2p, h->nc_b2, hidden, out, st);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  ProfScope ps(h, P2P_PROF_NC, st);
+  if (kind != kNcFp32 && (rc = launch_absmax(in, (size_t)hA * wA * hB * wB, xmax, st))) return rc;
+  return launch_nc(h, kind, in, hA, wA, hB, wB, ns, xmax, out, nullptr, nullptr, st);
+}
+
+int p2p_neigh_consensus(p2p_handle_t h, const float* in, int hA, int wA, int hB, int wB, float* out, void* stream) {
+  return nc_alone(h, false, in, hA, wA, hB, wB, out, stream);
 }
 
 int p2p_nc_stack(p2p_handle_t h, const float* in, int hA, int wA, int hB, int wB, float* out, void* stream) {
-  P2P_ENTER(h);
-  P2P_REQUIRE(h->ncs_set, "p2p_set_nc_stack_weights has not been called");
-  P2P_REQUIRE(in && out && hA > 0 && wA > 0 && hB > 0 && wB > 0, "bad argument");
-  const size_t V = (size_t)hA * wA * hB * wB;
-  int rc = h->misc.reserve(nc_stack_scratch_bytes(V) + 8192);
-  if (rc) return rc;
-  __half* lines = (__half*)h->misc.take(nc_stack_scratch_bytes(V));
-  unsigned int* xmax = (unsigned int*)h->misc.take(16);
-  P2P_REQUIRE(lines && xmax, "scratch carve failed");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  ProfScope ps(h, P2P_PROF_NC, st);
-  if ((rc = launch_absmax(in, V, xmax, st))) return rc;
-  return launch_nc_stack(in, hA, wA, hB, wB, h->ncs, xmax, lines, out, sms(h), st);
+  return nc_alone(h, true, in, hA, wA, hB, wB, out, stream);
 }
 
 // Development hook (not part of include/p2p_b200.h): copies `bytes` of an intermediate of the last
 // p2p_neigh_consensus call to the host -- which = 0 hidden [V][64] fp16, 1 partial [18][V] f32, 2 xp (padded hi|lo
-// words), 3 xmax word.
+// words), 3 xmax word.  Under nc_impl 0 only 0 (hidden, fp32 [nA][32][nB]) and 3 are set.
 P2P_API int p2p_debug_nc_scratch(p2p_handle_t h, int which, void* host_dst, size_t bytes) {
   P2P_ENTER(h);
   P2P_REQUIRE(which >= 0 && which < 4 && host_dst != nullptr && h->dbg_nc[which] != nullptr, "bad argument");

@@ -264,6 +264,37 @@ def _pack_delta(delta4d, ksize, h):
     return code
 
 
+def _unpack_delta(code, ksize, h):
+    """maxpool4d's four int64 delta tensors (max_i, max_j, max_k, max_l), shaped like code, from the packed code."""
+    ds = [torch.empty(code.shape, dtype=torch.int64, device=code.device) for _ in range(4)]
+    with torch.cuda.device(code.device):
+        _lib.check(h.lib.p2p_delta_unpack(h.h, _lib.ptr(code), code.numel(), ksize, *[_lib.ptr(d) for d in ds],
+                                          h.stream()))
+    return ds
+
+
+def _coarse_volume(feat1, feat2, ksize, dtype=torch.float32):
+    """An uninitialised [b, 1, h1 // ksize, w1 // ksize, h2 // ksize, w2 // ksize] volume on feat1's device."""
+    b, _, h1, w1 = feat1.shape
+    _, _, h2, w2 = feat2.shape
+    return torch.empty(b, 1, h1 // ksize, w1 // ksize, h2 // ksize, w2 // ksize, dtype=dtype, device=feat1.device)
+
+
+def _coarse_per_pair(h, entry, feat1, feat2, ksize, *taps):
+    """Runs a coarse-stage C entry (p2p_coarse, p2p_coarse_nhwc16, p2p_ncnet_coarse) on each pair of the batch
+    -> (corr4d f32, packed delta code uint8 | None for ksize 1), both _coarse_volume-shaped.  taps: the entry's
+    arguments after delta_code_out (p2p_coarse's pooled_out, ncn_out), _coarse_volume-shaped tensors or None."""
+    b, c, h1, w1 = feat1.shape
+    _, _, h2, w2 = feat2.shape
+    corr4d = _coarse_volume(feat1, feat2, ksize)
+    code = _coarse_volume(feat1, feat2, ksize, torch.uint8) if ksize > 1 else None
+    with torch.cuda.device(feat1.device):
+        for i in range(b):
+            _lib.check(entry(h.h, _lib.ptr(feat1[i]), _lib.ptr(feat2[i]), c, h1, w1, h2, w2, ksize, _lib.ptr(corr4d[i]),
+                             *[_lib.ptr(t[i]) if t is not None else None for t in (code, *taps)], h.stream()))
+    return corr4d, code
+
+
 class _FeatList(list):
     """Feature pyramid list that remembers the CUDA-graph instance whose static buffers it views."""
     graph_inst = None
@@ -454,20 +485,8 @@ class Patch2PixB200(nn.Module):
         if fmt == 0:
             feat1, feat2 = feat1.contiguous(), feat2.contiguous()
         entry = h.lib.p2p_coarse if fmt == 0 else h.lib.p2p_coarse_nhwc16
-        b, c, h1, w1 = feat1.shape
-        _, _, h2, w2 = feat2.shape
-        hA, wA, hB, wB = h1 // ksize, w1 // ksize, h2 // ksize, w2 // ksize
-        dev = feat1.device
-        corr4d = torch.empty(b, 1, hA, wA, hB, wB, dtype=torch.float32, device=dev)
-        code = torch.empty(b, 1, hA, wA, hB, wB, dtype=torch.uint8, device=dev) if ksize > 1 else None
-        pooled = torch.empty_like(corr4d) if return_stages else None
-        ncn = torch.empty_like(corr4d) if return_stages else None
-        with torch.cuda.device(dev):
-            for i in range(b):
-                _lib.check(entry(h.h, _lib.ptr(feat1[i]), _lib.ptr(feat2[i]), c, h1, w1, h2, w2, ksize,
-                                            _lib.ptr(corr4d[i]), _lib.ptr(code[i]) if code is not None else None,
-                                            _lib.ptr(pooled[i]) if pooled is not None else None,
-                                            _lib.ptr(ncn[i]) if ncn is not None else None, h.stream()))
+        pooled, ncn = [_coarse_volume(feat1, feat2, ksize) if return_stages else None for _ in range(2)]
+        corr4d, code = _coarse_per_pair(h, entry, feat1, feat2, ksize, pooled, ncn)
         if return_stages:
             return corr4d, code, {'pooled': pooled, 'ncn': ncn}
         return corr4d, code
@@ -476,14 +495,9 @@ class Patch2PixB200(nn.Module):
         """networks/patch2pix.py:120-136 -> (corr4d [b,1,hA,wA,hB,wB] f32, delta4d 4 x int64 | None)."""
         r = self._coarse_raw(feat1, feat2, ksize, return_stages)
         corr4d, code = r[0], r[1]
-        h = self._handle
         delta4d = None
         if ksize > 1:
-            with torch.cuda.device(corr4d.device):
-                ds = [torch.empty(code.shape, dtype=torch.int64, device=code.device) for _ in range(4)]
-                _lib.check(h.lib.p2p_delta_unpack(h.h, _lib.ptr(code), code.numel(), ksize, *[_lib.ptr(d) for d in ds],
-                                                  h.stream()))
-            delta4d = _DeltaTuple(ds)
+            delta4d = _DeltaTuple(_unpack_delta(code, ksize, self._handle))
             delta4d.code = code
         if return_stages:
             return corr4d, delta4d, r[2]

@@ -182,26 +182,14 @@ class ImMatchNet(nn.Module):
         for t, n in ((featA, 'featA'), (featB, 'featB')):
             if not (t.is_cuda and t.dim() == 4):
                 raise ValueError(f'{n} must be a [b, C, h, w] CUDA tensor')
+        from .model import _coarse_per_pair, _unpack_delta
         featA, featB = featA.float().contiguous(), featB.float().contiguous()
-        b, c, h1, w1 = featA.shape
-        _, _, h2, w2 = featB.shape
         k = max(1, self.relocalization_k_size)
-        hA, wA, hB, wB = h1 // k, w1 // k, h2 // k, w2 // k
-        dev = featA.device
-        nc = self.NeighConsensus
-        h = nc._handle(dev)
-        corr4d = torch.empty(b, 1, hA, wA, hB, wB, dtype=torch.float32, device=dev)
-        code = torch.empty(b, 1, hA, wA, hB, wB, dtype=torch.uint8, device=dev) if k > 1 else None
-        with torch.cuda.device(dev):
-            for i in range(b):
-                _lib.check(h.lib.p2p_ncnet_coarse(h.h, _lib.ptr(featA[i]), _lib.ptr(featB[i]), c, h1, w1, h2, w2, k,
-                                                  _lib.ptr(corr4d[i]), _lib.ptr(code[i]) if code is not None else None,
-                                                  h.stream()))
-            if k == 1:
-                return corr4d
-            ds = [torch.empty(code.shape, dtype=torch.int64, device=dev) for _ in range(4)]
-            _lib.check(h.lib.p2p_delta_unpack(h.h, _lib.ptr(code), code.numel(), k, *[_lib.ptr(d) for d in ds],
-                                              h.stream()))
+        h = self.NeighConsensus._handle(featA.device)
+        corr4d, code = _coarse_per_pair(h, h.lib.p2p_ncnet_coarse, featA, featB, k)
+        if k == 1:
+            return corr4d
+        ds = _unpack_delta(code, k, h)
         return corr4d, (ds[0].float(), ds[1].float(), ds[2].float(), ds[3])
 
     @torch.no_grad()
