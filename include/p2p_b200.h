@@ -287,6 +287,22 @@ P2P_API int p2p_sampson_distance(p2p_handle_t h, const double* rows, int row_str
 P2P_API int p2p_epipolar_histograms(p2p_handle_t h, const double* rows, int row_stride, int n, const double* n_dev,
                                     int coarse_col, const double* F, const uint8_t* mask, const double* edges,
                                     int n_edges, int32_t* counts_out, void* stream);
+/* The per-pair statistics of the HPatches evaluation (patch2pix_b200/hpatches.py), in one launch and without a host
+ * sync.  rows / row_stride / n / n_dev as p2p_find_model: m = min(n, *n_dev) rows (x1, y1, x2, y2) in columns 0..3
+ * (row_stride 9 reads the packed_out of p2p_finalize_matches in place).  H_gt HOST double [9] (row-major, image 1 ->
+ * image 2) and thresholds HOST double [n_thr] (1 <= n_thr <= 16, finite, > 0, strictly increasing; anything else
+ * returns -1) are passed by value to the kernel.  A row's reprojection error is d = |pi(H_gt [x1, y1, 1]^T) - (x2, y2)|
+ * in fp64, every product and sum rounded on its own ((h0 x + h1 y) + h2, no fused multiply-add), correctly rounded
+ * division and square root; it counts at threshold t iff d <= t, so NaN and inf never count.  counts_out DEVICE int32
+ * [n_thr + 1]: the count at each threshold, then m.  H_pred is a DEVICE p2p_find_model output buffer (model at doubles
+ * 0..8, int32 inlier count at byte 72).  corner_err_out DEVICE double [1]: the mean over the corners (0, 0),
+ * (width-1, 0), (0, height-1), (width-1, height-1) of |pi(H_gt c) - pi(H_pred c)|, summed in that order and divided
+ * by 4; +inf when the inlier count is <= 0, when a corner projects with w = 0 under either H, or when the mean is not
+ * finite.  Both outputs are written with plain stores (no zeroing needed) and are identical across runs. */
+P2P_API int p2p_homography_errors(p2p_handle_t h, const double* rows, int row_stride, int n, const double* n_dev,
+                                  const double* H_gt, const double* H_pred, int width, int height,
+                                  const double* thresholds, int n_thr, int32_t* counts_out, double* corner_err_out,
+                                  void* stream);
 /* The image-overlap matrix of the reference's validation-pair precompute (utils/colmap/data_loading.py:54-70,
  * cal_overlap_scores), in two launches and without a host sync.  Image i's keypoints are point3D_ids[offsets[i] ..
  * offsets[i+1]-1] (DEVICE int64; offsets DEVICE int64 [n_images+1], offsets_host the same values on the HOST, checked

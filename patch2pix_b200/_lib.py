@@ -62,6 +62,8 @@ _SIGNATURES = {
     'p2p_sampson_distance': (_I, [_P, _P, _I, _I, _P, _P, _P]),
     'p2p_epipolar_histograms': (_I, [_P, _P, _I, _I, _P, _I, C.POINTER(C.c_double), _P, C.POINTER(C.c_double), _I, _P,
                                      _P]),
+    'p2p_homography_errors': (_I, [_P, _P, _I, _I, _P, C.POINTER(C.c_double), _P, _I, _I, C.POINTER(C.c_double), _I,
+                                   _P, _P, _P]),
     'p2p_overlap_scores': (_I, [_P, _P, _P, C.POINTER(C.c_int64), _I, _I, _P, _P, _P, _P]),
     'p2p_test_hypotheses': (_I, [_P, _I, _P, _I, _I, C.c_double, C.c_ulonglong, _I, _P, _P, _P]),
     'p2p_test_degeneracy': (_I, [_P, _P, _I, _I, C.c_double, C.c_ulonglong, _I, _P, _P, _P]),

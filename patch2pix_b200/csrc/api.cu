@@ -1514,6 +1514,29 @@ int p2p_epipolar_histograms(p2p_handle_t h, const double* rows, int row_stride, 
                                     reinterpret_cast<cudaStream_t>(stream));
 }
 
+int p2p_homography_errors(p2p_handle_t h, const double* rows, int row_stride, int n, const double* n_dev,
+                          const double* H_gt, const double* H_pred, int width, int height, const double* thresholds,
+                          int n_thr, int32_t* counts_out, double* corner_err_out, void* stream) {
+  P2P_ENTER(h);
+  P2P_REQUIRE(H_gt && H_pred && thresholds && counts_out && corner_err_out && (rows || n == 0), "null pointer");
+  P2P_REQUIRE(n >= 0 && row_stride >= 4, "bad row count or stride");
+  P2P_REQUIRE(width >= 1 && height >= 1, "width and height must be positive");
+  P2P_REQUIRE(n_thr >= 1 && n_thr <= kMaxHomThresholds, "n_thr must be in 1..16");
+  HomErrArgs a{};
+  for (int j = 0; j < 9; ++j) a.H[j] = H_gt[j];
+  for (int i = 0; i < kMaxHomThresholds; ++i) a.thr[i] = NAN;     // no row passes a padding entry
+  for (int i = 0; i < n_thr; ++i) {
+    P2P_REQUIRE(std::isfinite(thresholds[i]) && thresholds[i] > 0.0 && (i == 0 || thresholds[i] > thresholds[i - 1]),
+                "thresholds must be finite, positive and strictly increasing");
+    a.thr[i] = thresholds[i];
+  }
+  a.n_thr = n_thr;
+  a.width = width;
+  a.height = height;
+  return launch_homography_errors(rows, row_stride, n, n_dev, a, H_pred, counts_out, corner_err_out,
+                                  reinterpret_cast<cudaStream_t>(stream));
+}
+
 int p2p_overlap_scores(p2p_handle_t h, const int64_t* point3D_ids, const int64_t* offsets,
                        const int64_t* offsets_host, int n_images, int words, uint32_t* bits_out, int32_t* counts_out,
                        double* scores_out, void* stream) {

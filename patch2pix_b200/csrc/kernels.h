@@ -180,6 +180,18 @@ struct EpiHistArgs {
 };
 int launch_epipolar_histograms(const double* rows, int stride, int n, const double* n_dev, int coarse_col,
                                const uint8_t* mask, const EpiHistArgs& a, int* counts_out, cudaStream_t st);
+// ---- hpatches.cu: HPatches statistics against a ground-truth H (passed by value): counts_out [n_thr + 1] = rows
+// with reprojection error d <= thr[j], then the rows considered; corner_err_out [1] = mean corner distance of H and the
+// model of a find_model output buffer H_pred (model at doubles 0..8, int32 count at byte 72), +inf when there is none.
+constexpr int kMaxHomThresholds = 16;
+struct HomErrArgs {
+  double H[9];
+  double thr[kMaxHomThresholds];   // finite, > 0, strictly increasing; NaN from n_thr on (no row passes those)
+  int n_thr;                       // 1 .. kMaxHomThresholds
+  int width, height;               // image 1's size, for the corners
+};
+int launch_homography_errors(const double* rows, int stride, int n, const double* n_dev, const HomErrArgs& a,
+                             const double* H_pred, int* counts_out, double* corner_err_out, cudaStream_t st);
 // ---- overlap.cu: cal_overlap_scores' matrix.  ids: flat point3D_ids, image i at offsets[i] .. offsets[i+1]-1 (device);
 // bits [n][words] and counts [n] are written by the pack kernel, scores [n][n] (every entry) by the count kernel.
 constexpr int kMaxOverlapImages = 1 << 20;

@@ -365,6 +365,76 @@ def grid_coarse_matcher(shift=(8, 16), step=12, dtype=torch.float32):
     return matcher
 
 
+# ---- HPatches-layout sequences -----------------------------------------------------------------------------------------
+def _hpatches_h(rng, split, w1, h1, w2, h2):
+    """A mild random homography from a (w1, h1) image to a (w2, h2) one, about the image centres: near identity for
+    'i' (illumination) sequences, rotation, scale, shear and perspective for 'v' (viewpoint) ones.  H[2][2] = 1."""
+    if split == 'i':
+        th, s, sh, persp, t = rng.uniform(-0.01, 0.01), rng.uniform(0.99, 1.01), 0.0, (0.0, 0.0), rng.uniform(-3, 3, 2)
+    else:
+        th, s, sh = rng.uniform(-0.25, 0.25), rng.uniform(0.8, 1.2), rng.uniform(-0.05, 0.05)
+        persp = rng.uniform(-0.25, 0.25, 2) / max(w1, h1)
+        t = rng.uniform(-0.05, 0.05, 2) * (w2, h2)
+    A = s * np.array([[math.cos(th), -math.sin(th)], [math.sin(th), math.cos(th)]]) @ np.array([[1.0, sh], [0.0, 1.0]])
+    M = np.eye(3)
+    M[:2, :2] = A
+    M[2, :2] = persp
+    T1 = np.array([[1.0, 0, -(w1 - 1) / 2], [0, 1.0, -(h1 - 1) / 2], [0, 0, 1.0]])
+    T2 = np.array([[1.0, 0, (w2 - 1) / 2 + t[0]], [0, 1.0, (h2 - 1) / 2 + t[1]], [0, 0, 1.0]])
+    H = T2 @ M @ T1
+    return H / H[2, 2]
+
+
+def synthetic_hpatches_tree(root, seed, seqs):
+    """HPatches-sequences layout under `root` from a seed, for tests and benchmarks: per sequence, root/name/1.ppm ..
+    6.ppm and H_1_2 .. H_1_6.  `seqs` lists names (split from the i_ / v_ prefix, seeded size) or (name, (w, h)).
+    1.ppm is a blocky 8-bit texture cropped from a larger canvas; k.ppm is the canvas warped by H_1_k (fp64 numpy inverse
+    mapping, nearest pixel, 0 outside the canvas): a near-identity H and a brightness change for i_ sequences, rotation,
+    scale, shear and perspective (and a size of its own) for v_ ones.  H_1_k is written with %.17g, so np.loadtxt reads
+    back exactly the H used.  -> {name: [H_1_2 .. H_1_6]}"""
+    from PIL import Image
+    out = {}
+    for idx, item in enumerate(seqs):
+        name, size = (item, None) if isinstance(item, str) else (item[0], item[1])
+        split = name[:1]
+        rng = np.random.default_rng([int(seed), 5, idx])
+        w1, h1 = (int(v) for v in size) if size is not None else (int(rng.integers(160, 321)), int(rng.integers(128, 257)))
+        m = max(w1, h1) // 2
+        cw, ch = w1 + 2 * m, h1 + 2 * m
+        low = rng.integers(0, 256, size=(ch // 8 + 2, cw // 8 + 2, 3), dtype=np.int32)
+        base = np.repeat(np.repeat(low, 8, 0), 8, 1)[:ch + 4, :cw + 4]
+        base = (base[:ch, :cw] + base[4:ch + 4, :cw] + base[:ch, 4:cw + 4] + base[4:ch + 4, 4:cw + 4]) // 4
+        canvas = np.clip(base + rng.integers(-12, 13, size=base.shape), 0, 255).astype(np.uint8)
+        d = os.path.join(root, name)
+        os.makedirs(d, exist_ok=True)
+        Image.fromarray(canvas[m:m + h1, m:m + w1].copy()).save(os.path.join(d, '1.ppm'))
+        Hs = []
+        for k in range(2, 7):
+            if split == 'v':
+                w2, h2 = int(w1 * rng.uniform(0.85, 1.15)), int(h1 * rng.uniform(0.85, 1.15))
+            else:
+                w2, h2 = w1, h1
+            H = _hpatches_h(rng, split, w1, h1, w2, h2)
+            Hi = np.linalg.inv(H)
+            v, u = np.mgrid[0:h2, 0:w2].astype(np.float64)
+            q = Hi[2, 0] * u + Hi[2, 1] * v + Hi[2, 2]
+            with np.errstate(all='ignore'):
+                x = (Hi[0, 0] * u + Hi[0, 1] * v + Hi[0, 2]) / q
+                y = (Hi[1, 0] * u + Hi[1, 1] * v + Hi[1, 2]) / q
+            xi, yi = np.floor(x + 0.5) + m, np.floor(y + 0.5) + m
+            ok = (q > 0) & (xi >= 0) & (xi < cw) & (yi >= 0) & (yi < ch)
+            img = np.zeros((h2, w2, 3), dtype=np.uint8)
+            img[ok] = canvas[yi[ok].astype(np.int64), xi[ok].astype(np.int64)]
+            if split == 'i':
+                gain, bias = rng.uniform(0.6, 1.4), rng.uniform(-20, 20)
+                img = np.clip(np.floor(img * gain + bias), 0, 255).astype(np.uint8)
+            Image.fromarray(img).save(os.path.join(d, f'{k}.ppm'))
+            np.savetxt(os.path.join(d, f'H_1_{k}'), H, fmt='%.17g')
+            Hs.append(H)
+        out[name] = Hs
+    return out
+
+
 # ---- NCNet (ImMatchNet) test data: regenerated from seeds, so fixtures store outputs only ----------------------------
 def ncnet_stack_weights(seed, kernel_sizes, channels):
     """Conv4d weights in the reference's pre-permuted layout [k, Cout, Cin, k, k, k] and biases [Cout], fp32, scaled so
