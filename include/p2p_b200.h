@@ -212,6 +212,19 @@ P2P_API int p2p_refine_prepare_nhwc16(p2p_handle_t h, const void* const* feats1,
                        int H2, int W2, void* stream);
 P2P_API int p2p_refine(p2p_handle_t h, int which, const void* matches_in, int is_float, int n, float* matches_out,
                float* probs_out, void* stream);
+/* Test access: copies the intermediate buffers of the handle's last p2p_refine call, as they stand after its last pass,
+ * into the caller's DEVICE buffers (each may be NULL).  Valid until the next p2p_refine on the handle; synchronises
+ * `stream` after a risk-band call.  info_out HOST int32 [4] = {m: rows of the last pass, passes of the last pass (1 or 3),
+ * 1 if the last pass was the risk band's 3-pass subset, 1 if the FC ran on the tensor cores}.  After a risk-band call the
+ * buffers hold the band's m flagged rows, slot s holding row rows_out[s] (ascending); otherwise slot s is row s of the n.
+ * scales_out HOST float [4]: the power-of-two scales the buffers carry: y_scale, then the FC operand scales of
+ * pooled, h1 and h2.  rows_out int32 [m]; y_hi / y_lo fp16 [m][64][512], the conv1 output (BN folded) times y_scale
+ * at output pixel y * 8 + x, y_hi + y_lo after a 3-pass pass (y_lo NULL after a 1-pass one); pooled fp32 [m][512]
+ * (unscaled); h1_hi / h1_lo fp16 [m][512] and h2_hi / h2_lo fp16 [m][256], the FC hidden layers times their scales
+ * (tensor-core FC only); raw_out fp32 [n][5], the regressor outputs of every row (the band's rows from its 3-pass pass). */
+P2P_API int p2p_refine_taps(p2p_handle_t h, int32_t* info_out, float* scales_out, int32_t* rows_out, void* y_hi, void* y_lo,
+                            float* pooled, void* h1_hi, void* h1_lo, void* h2_hi, void* h2_lo, float* raw_out,
+                            void* stream);
 
 /* ---- tail of estimate_matches (utils/eval/model_helper.py:97-109): inlier filter `scores > io_thres` ("keep everything
  * if nothing passes"), row order preserved, and `upscale * matches` in float64, so that ONE device->host copy returns

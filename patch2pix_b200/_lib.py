@@ -52,6 +52,7 @@ _SIGNATURES = {
     'p2p_refine_prepare': (_I, [_P, C.POINTER(_P), C.POINTER(_P), _I, _I, _I, _I, _P]),
     'p2p_refine_prepare_nhwc16': (_I, [_P, C.POINTER(_P), C.POINTER(_P), _I, _I, _I, _I, _P]),
     'p2p_refine': (_I, [_P, _I, _P, _I, _I, _P, _P, _P]),
+    'p2p_refine_taps': (_I, [_P, C.POINTER(C.c_int32), C.POINTER(_F), _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     'p2p_finalize_matches': (_I, [_P, _P, _P, _P, _I, _F, C.POINTER(C.c_double), _P, _P]),
     'p2p_preprocess_image': (_I, [_P, _P, _I, _I, _I, _I, _P, _P, _P]),
     'p2p_preprocess_image_gray': (_I, [_P, _P, _I, _I, _I, _I, _P, _P, _P]),

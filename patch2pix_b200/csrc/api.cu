@@ -72,6 +72,7 @@ struct Regressor {
   // tensor-core FC path: K-major fp16 hi/lo weights [out][in] with per-row pow2 scale, 1/(act*w scale), bias
   __half *f1_hi = nullptr, *f1_lo = nullptr, *f2_hi = nullptr, *f2_lo = nullptr;
   float *fa1 = nullptr, *fa2 = nullptr;
+  float fc_scale[3] = {1.f, 1.f, 1.f};   // power-of-two scales of the FC operands: pooled, h1, h2
   KStep steps1[kConv1Steps];
   KStep steps2[kConv2Steps];
   KStep *d_steps1 = nullptr, *d_steps2 = nullptr;
@@ -109,6 +110,13 @@ struct p2p_handle_s {
   int* share_rows = nullptr;             // device: rows that shared a window half in the last sharing mid-stage call
   bool last_mid_shared = false;          // the last mid-stage call shared windows (share_rows is its count)
   unsigned long long* band_totals = nullptr;   // device: {band rows, rows} summed over mid-stage calls
+  struct RefineTap {            // the buffers of the last p2p_refine call's last pass (p2p_refine_taps)
+    const __half *y_hi = nullptr, *y_lo = nullptr, *h1_hi = nullptr, *h1_lo = nullptr, *h2_hi = nullptr, *h2_lo = nullptr;
+    const float *pooled = nullptr, *raw = nullptr;
+    const int *rowmap = nullptr, *d_count = nullptr;   // risk-band subset: slot -> row, and the slot count
+    int n = 0, passes = 0, fc_tc = 0;
+    float scales[4] = {1.f, 1.f, 1.f, 1.f};            // y_scale, then the pooled, h1 and h2 operand scales
+  } tap;
   bool nc_set = false;
   float *nc_w1p = nullptr, *nc_b1p = nullptr, *nc_w2p = nullptr;
   float nc_b2 = 0.f;
@@ -204,6 +212,7 @@ int pack_regressor(p2p_handle_s* h, Regressor& R, const p2p_regressor_weights_t&
   std::vector<float> sc1(512), sc2(512), bi1(b1), bi2(b2);
   float max_bound = 0.f;
   std::vector<float> sw1(512), sw2(512);
+  std::vector<double> ybound(512);   // |conv1 output| of each channel, for any L2-normalised input
   for (int o = 0; o < 512; ++o) {
     const float* wo = w.conv0_weight + (size_t)o * 518 * 9;
     float m = 0.f;
@@ -217,6 +226,7 @@ int pack_regressor(p2p_handle_s* h, Regressor& R, const p2p_regressor_weights_t&
     float bound = fabsf(b1[o]);
     for (int t = 0; t < 9; ++t) bound += 1.41421357f * (float)sqrt(tapn[t]);
     max_bound = fmaxf(max_bound, bound);
+    ybound[o] = bound;
     sw1[o] = pow2_floor_scale(m, 1024.f);
     sc1[o] = 1.f / (kActScale * sw1[o]);
     __half* dh = w1h.data() + (size_t)o * K1;
@@ -277,6 +287,31 @@ int pack_regressor(p2p_handle_s* h, Regressor& R, const p2p_regressor_weights_t&
     for (int k = 0; k < 256; ++k) f3t[k * 5 + o] = w.fc6_weight[o * 256 + k];
     f3b[o] = w.fc6_bias[o];
   }
+  // Activation bounds of the FC operands, continuing conv1's: pooled[o] = max relu(conv2) <= P[o] (conv1 outputs of
+  // either sign), h1[o] = relu(bias + W1 pooled) <= relu(bias + sum_k max(W1[o][k], 0) P[k]) as pooled >= 0, h2 likewise
+  // from h1 >= 0.  Each operand is scaled by the power of two that puts its bound in [2^14, 2^15), so the fp16 hi
+  // part never saturates (the epilogues' clip at 65504 stays out of reach) while O(1) activations keep their lo bits.
+  std::vector<double> pb(512), h1b(512), h2b(256);
+  for (int o = 0; o < 512; ++o) {
+    const float* wo = w.conv2_weight + (size_t)o * 512 * 9;
+    double a = b2[o];
+    for (int c = 0; c < 512; ++c)
+      for (int t = 0; t < 9; ++t) a += fabs((double)wo[c * 9 + t] * g2[o]) * ybound[c];
+    pb[o] = std::max(a, 0.0);
+  }
+  for (int o = 0; o < 512; ++o) {
+    double a = f1b[o];
+    for (int k = 0; k < 512; ++k) a += std::max((double)f1t[(size_t)k * 512 + o], 0.0) * pb[k];
+    h1b[o] = std::max(a, 0.0);
+  }
+  for (int o = 0; o < 256; ++o) {
+    double a = f2b[o];
+    for (int k = 0; k < 512; ++k) a += std::max((double)f2t[(size_t)k * 256 + o], 0.0) * h1b[k];
+    h2b[o] = std::max(a, 0.0);
+  }
+  const float fc_bound[3] = {(float)*std::max_element(pb.begin(), pb.end()), (float)*std::max_element(h1b.begin(), h1b.end()),
+                             (float)*std::max_element(h2b.begin(), h2b.end())};
+  for (int i = 0; i < 3; ++i) R.fc_scale[i] = pow2_floor_scale(fc_bound[i], 32768.f);
   // tensor-core FC operands
   std::vector<__half> f1h((size_t)512 * 512), f1l((size_t)512 * 512), f2h((size_t)256 * 512), f2l((size_t)256 * 512);
   std::vector<float> fa1(512), fa2(256);
@@ -284,7 +319,7 @@ int pack_regressor(p2p_handle_s* h, Regressor& R, const p2p_regressor_weights_t&
     float m = 0.f;
     for (int k = 0; k < 512; ++k) m = fmaxf(m, fabsf(w.fc0_weight[(size_t)o * 512 + k] * gf1[o]));
     const float sw = pow2_floor_scale(m, 1024.f);
-    fa1[o] = 1.f / (kFcActScale * sw);
+    fa1[o] = 1.f / (R.fc_scale[0] * sw);
     for (int k = 0; k < 512; ++k)
       split_half(w.fc0_weight[(size_t)o * 512 + k] * gf1[o] * sw, f1h[(size_t)o * 512 + k], f1l[(size_t)o * 512 + k]);
   }
@@ -292,7 +327,7 @@ int pack_regressor(p2p_handle_s* h, Regressor& R, const p2p_regressor_weights_t&
     float m = 0.f;
     for (int k = 0; k < 512; ++k) m = fmaxf(m, fabsf(w.fc3_weight[(size_t)o * 512 + k] * gf2[o]));
     const float sw = pow2_floor_scale(m, 1024.f);
-    fa2[o] = 1.f / (kFcActScale * sw);
+    fa2[o] = 1.f / (R.fc_scale[1] * sw);
     for (int k = 0; k < 512; ++k)
       split_half(w.fc3_weight[(size_t)o * 512 + k] * gf2[o] * sw, f2h[(size_t)o * 512 + k], f2l[(size_t)o * 512 + k]);
   }
@@ -1239,7 +1274,7 @@ int run_regressor(p2p_handle_s* h, Regressor& R, int which, int passes, const Re
     return launch_fc_parse(B.pooled, R.fc, matches_in, is_float, n, h->pf[0].W, h->pf[0].H, h->pf[1].W, h->pf[1].H,
                            matches_out, probs_out, raw_out, rowmap, d_count, st);
   // tensor-core FC: split -> Linear(512,512)+BN+ReLU -> Linear(512,256)+BN+ReLU (3-pass, segmented) -> Linear(256,5)+parse
-  if ((rc = launch_pooled_split(B.pooled, n, B.q_hi, B.q_lo, d_count, st))) return rc;
+  if ((rc = launch_pooled_split(B.pooled, n, R.fc_scale[0], B.q_hi, B.q_lo, d_count, st))) return rc;
   const uint64_t m128 = align_up(n, 128);
   const uint32_t abx[5] = {64, 1, 1, 1, 128};
   const uint32_t bbx[2] = {64, 128};
@@ -1268,14 +1303,14 @@ int run_regressor(p2p_handle_s* h, Regressor& R, int which, int passes, const Re
     p.d_units = d_count;
     p.epi.scale = layer == 0 ? R.fa1 : R.fa2;
     p.epi.bias = layer == 0 ? R.fc.b1 : R.fc.b2;
-    p.epi.y_scale = kFcActScale;
+    p.epi.y_scale = R.fc_scale[layer + 1];
     p.epi.y_hi = layer == 0 ? B.h1_hi : B.h2_hi;
     p.epi.y_lo = layer == 0 ? B.h1_lo : B.h2_lo;
     p.epi.ldc = nout;
     p.epi.n_patches = n;
     if ((rc = launch_umma_gemm(p, EPI_FC, 3, sms(h), st))) return rc;
   }
-  return launch_fc3_parse(B.h2_hi, B.h2_lo, R.fc.w3t, R.fc.b3, matches_in, is_float, n, h->pf[0].W, h->pf[0].H,
+  return launch_fc3_parse(B.h2_hi, B.h2_lo, 1.f / R.fc_scale[2], R.fc.w3t, R.fc.b3, matches_in, is_float, n, h->pf[0].W, h->pf[0].H,
                           h->pf[1].W, h->pf[1].H, matches_out, probs_out, raw_out, rowmap, d_count, st);
 }
 
@@ -1337,9 +1372,25 @@ int p2p_refine(p2p_handle_t h, int which, const void* matches_in, int is_float, 
   B.sh_unsh = B.sh_cont + n;
   B.d_count = B.rowmap + n;
   if (which == 0) h->last_band_count = band ? B.d_count : nullptr;
+  auto& T = h->tap;
+  T.y_hi = B.y_hi;
+  T.y_lo = B.y_lo;
+  T.pooled = B.pooled;
+  T.h1_hi = B.h1_hi;
+  T.h1_lo = B.h1_lo;
+  T.h2_hi = B.h2_hi;
+  T.h2_lo = B.h2_lo;
+  T.raw = B.raw;
+  T.rowmap = band ? B.rowmap : nullptr;
+  T.d_count = band ? B.d_count : nullptr;
+  T.n = n;
+  T.passes = passes;
+  T.fc_tc = h->opt_fc_impl != 0 && h->opt_gemm_impl == 0;
+  T.scales[0] = R.y_scale;
+  for (int i = 0; i < 3; ++i) T.scales[i + 1] = R.fc_scale[i];
   if (!band)
     return run_regressor(h, R, which, passes, B, matches_in, is_float, n, nullptr, nullptr, matches_out, probs_out,
-                         nullptr, st);
+                         B.raw, st);
   if ((rc = run_regressor(h, R, which, 1, B, matches_in, is_float, n, nullptr, nullptr, matches_out, probs_out, B.raw,
                           st)))
     return rc;
@@ -1350,7 +1401,49 @@ int p2p_refine(p2p_handle_t h, int which, const void* matches_in, int is_float, 
       return rc;
   }
   return run_regressor(h, R, which, 3, B, matches_in, is_float, n, B.rowmap, B.d_count, matches_out, probs_out,
-                       nullptr, st);
+                       B.raw, st);
+}
+
+int p2p_refine_taps(p2p_handle_t h, int32_t* info_out, float* scales_out, int32_t* rows_out, void* y_hi, void* y_lo,
+                    float* pooled, void* h1_hi, void* h1_lo, void* h2_hi, void* h2_lo, float* raw_out, void* stream) {
+  P2P_ENTER(h);
+  P2P_REQUIRE(info_out && scales_out, "null info / scales pointer");
+  const auto& T = h->tap;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  int m = T.n;
+  if (T.d_count != nullptr) {
+    P2P_CUDA_OK(cudaStreamSynchronize(st));
+    P2P_CUDA_OK(cudaMemcpy(&m, T.d_count, sizeof(int), cudaMemcpyDeviceToHost));
+  }
+  info_out[0] = m;
+  info_out[1] = T.passes;
+  info_out[2] = T.d_count != nullptr;
+  info_out[3] = T.fc_tc;
+  for (int i = 0; i < 4; ++i) scales_out[i] = T.scales[i];
+  if (T.n == 0) return 0;
+  P2P_REQUIRE(!y_lo || T.passes == 3, "y_lo is written by 3-pass passes only");
+  P2P_REQUIRE(!(h1_hi || h1_lo || h2_hi || h2_lo) || T.fc_tc, "h1 / h2 are written by the tensor-core FC only");
+#define TAP(dst, src, bytes) \
+  if (dst) P2P_CUDA_OK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, st))
+  if (rows_out) {
+    if (T.rowmap != nullptr) {
+      TAP(rows_out, T.rowmap, (size_t)m * 4);
+    } else {
+      std::vector<int32_t> id(m);
+      for (int i = 0; i < m; ++i) id[i] = i;
+      P2P_CUDA_OK(cudaMemcpy(rows_out, id.data(), (size_t)m * 4, cudaMemcpyHostToDevice));
+    }
+  }
+  TAP(y_hi, T.y_hi, (size_t)m * 64 * 512 * 2);
+  TAP(y_lo, T.y_lo, (size_t)m * 64 * 512 * 2);
+  TAP(pooled, T.pooled, (size_t)m * 512 * 4);
+  TAP(h1_hi, T.h1_hi, (size_t)m * 512 * 2);
+  TAP(h1_lo, T.h1_lo, (size_t)m * 512 * 2);
+  TAP(h2_hi, T.h2_hi, (size_t)m * 256 * 2);
+  TAP(h2_lo, T.h2_lo, (size_t)m * 256 * 2);
+  TAP(raw_out, T.raw, (size_t)T.n * 5 * 4);
+#undef TAP
+  return 0;
 }
 
 int p2p_finalize_matches(p2p_handle_t h, const float* fine, const float* scores, const int64_t* coarse, int n, float io_thres,

@@ -227,10 +227,10 @@ int launch_recover_pose(const PairBatch& B, const double* intr, const Intrinsics
                         const uint8_t* mask_in, double dist_th, void* scratch, double* Rt_out, uint8_t* mask_out,
                         int* count_out, cudaStream_t st);
 
-// Tensor-core FC path helpers: pooled fp32 -> fp16 hi/lo A operand; final Linear(256,5) + parse_regressor_out.
-constexpr float kFcActScale = 16.f;
-int launch_pooled_split(const float* pooled, int n, __half* hi, __half* lo, const int* d_count, cudaStream_t st);
-int launch_fc3_parse(const __half* h2_hi, const __half* h2_lo, const float* w3t, const float* b3, const void* matches_in,
+// Tensor-core FC path helpers: pooled fp32 -> fp16 hi/lo A operand (times `scale`); final Linear(256,5) +
+// parse_regressor_out of h2 = (h2_hi + h2_lo) * inv_scale.
+int launch_pooled_split(const float* pooled, int n, float scale, __half* hi, __half* lo, const int* d_count, cudaStream_t st);
+int launch_fc3_parse(const __half* h2_hi, const __half* h2_lo, float inv_scale, const float* w3t, const float* b3, const void* matches_in,
                      int is_float, int N, int W1, int H1, int W2, int H2, float* matches_out, float* probs_out,
                      float* raw_out, const int* rowmap, const int* d_count, cudaStream_t st);
 

@@ -500,20 +500,20 @@ int launch_fc_parse(const float* pooled, const FcWeights& fc, const void* matche
 // Tensor-core FC path: the two big Linear layers run on umma_gemm_kernel<EPI_FC> (3-pass, fp32-grade);
 // these two kernels are its prologue (pooled -> fp16 hi/lo) and tail (Linear(256,5) + parse_regressor_out).
 // ------------------------------------------------------------------------------------------------
-__global__ void pooled_split_kernel(const float* __restrict__ pooled, int n, __half* __restrict__ hi,
+__global__ void pooled_split_kernel(const float* __restrict__ pooled, int n, float scale, __half* __restrict__ hi,
                                     __half* __restrict__ lo, const int* __restrict__ d_count) {
   if (d_count != nullptr) n = *d_count;
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (size_t)n * 512) return;
-  const float v = fminf(pooled[i] * kFcActScale, 65504.f);   // pooled >= 0 (post-ReLU); saturate, never inf/NaN
+  const float v = fminf(pooled[i] * scale, 65504.f);   // pooled >= 0 (post-ReLU); saturate, never inf/NaN
   const __half h = __float2half_rn(v);
   hi[i] = h;
   lo[i] = __float2half_rn(v - __half2float(h));
 }
 
-int launch_pooled_split(const float* pooled, int n, __half* hi, __half* lo, const int* d_count, cudaStream_t st) {
+int launch_pooled_split(const float* pooled, int n, float scale, __half* hi, __half* lo, const int* d_count, cudaStream_t st) {
   if (n == 0) return 0;
-  pooled_split_kernel<<<(unsigned)(((size_t)n * 512 + 255) / 256), 256, 0, st>>>(pooled, n, hi, lo, d_count);
+  pooled_split_kernel<<<(unsigned)(((size_t)n * 512 + 255) / 256), 256, 0, st>>>(pooled, n, scale, hi, lo, d_count);
   P2P_LAUNCH_OK();
   return 0;
 }
@@ -521,7 +521,7 @@ int launch_pooled_split(const float* pooled, int n, __half* hi, __half* lo, cons
 // one warp per row: 5 dot products of length 256, then parse_regressor_out (networks/patch2pix.py:138-155)
 template <bool IS_FLOAT>
 __global__ void __launch_bounds__(256) fc3_parse_kernel(const __half* __restrict__ h2_hi, const __half* __restrict__ h2_lo,
-                                                       const float* __restrict__ w3t, const float* __restrict__ b3,
+                                                       float inv_scale, const float* __restrict__ w3t, const float* __restrict__ b3,
                                                        const void* __restrict__ matches_in, int N, float W1, float H1,
                                                        float W2, float H2, float* __restrict__ matches_out,
                                                        float* __restrict__ probs_out, float* __restrict__ raw_out,
@@ -534,8 +534,7 @@ __global__ void __launch_bounds__(256) fc3_parse_kernel(const __half* __restrict
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
     const int k = lane + 32 * i;
-    const float x = (__half2float(h2_hi[(size_t)slot * 256 + k]) + __half2float(h2_lo[(size_t)slot * 256 + k])) *
-                    (1.f / kFcActScale);
+    const float x = (__half2float(h2_hi[(size_t)slot * 256 + k]) + __half2float(h2_lo[(size_t)slot * 256 + k])) * inv_scale;
 #pragma unroll
     for (int o = 0; o < 5; ++o) acc[o] = fmaf(x, __ldg(w3t + k * 5 + o), acc[o]);
   }
@@ -561,16 +560,16 @@ __global__ void __launch_bounds__(256) fc3_parse_kernel(const __half* __restrict
   }
 }
 
-int launch_fc3_parse(const __half* h2_hi, const __half* h2_lo, const float* w3t, const float* b3, const void* matches_in,
+int launch_fc3_parse(const __half* h2_hi, const __half* h2_lo, float inv_scale, const float* w3t, const float* b3, const void* matches_in,
                      int is_float, int N, int W1, int H1, int W2, int H2, float* matches_out, float* probs_out,
                      float* raw_out, const int* rowmap, const int* d_count, cudaStream_t st) {
   if (N == 0) return 0;
   if (is_float)
-    fc3_parse_kernel<true><<<cdiv(N, 8), 256, 0, st>>>(h2_hi, h2_lo, w3t, b3, matches_in, N, (float)W1, (float)H1,
+    fc3_parse_kernel<true><<<cdiv(N, 8), 256, 0, st>>>(h2_hi, h2_lo, inv_scale, w3t, b3, matches_in, N, (float)W1, (float)H1,
                                                       (float)W2, (float)H2, matches_out, probs_out, raw_out, rowmap,
                                                       d_count);
   else
-    fc3_parse_kernel<false><<<cdiv(N, 8), 256, 0, st>>>(h2_hi, h2_lo, w3t, b3, matches_in, N, (float)W1, (float)H1,
+    fc3_parse_kernel<false><<<cdiv(N, 8), 256, 0, st>>>(h2_hi, h2_lo, inv_scale, w3t, b3, matches_in, N, (float)W1, (float)H1,
                                                        (float)W2, (float)H2, matches_out, probs_out, raw_out, rowmap,
                                                        d_count);
   P2P_LAUNCH_OK();
