@@ -399,6 +399,31 @@ P2P_API int p2p_recover_pose_batch(p2p_handle_t h, const double* rows, int row_s
                                    uint8_t* mask_out, int32_t* n_good_out, void* stream);
 /* E DEVICE double [K][9], mask_in row-aligned or NULL (all rows), Rt_out DEVICE double [K][12], n_good_out DEVICE int32
  * [K]: per pair as p2p_recover_pose. */
+/* p2p_find_essential_batch with one threshold per pair: px_th DEVICE double [K], pair k's px_th (positive and finite
+ * are the caller's contract: not read back).  Pair k's result is bit-identical to p2p_find_essential on its rows with
+ * px_th[k]; with every entry equal to x it is p2p_find_essential_batch's with px_th = x. */
+P2P_API int p2p_find_essential_batch_th(p2p_handle_t h, const double* rows, int row_stride, const int64_t* offsets,
+                                        const int64_t* offsets_host, int K, const double* n_dev, const double* intr,
+                                        const double* px_th, double conf, int max_iters, unsigned long long seed,
+                                        double* E_out, uint8_t* mask_out, int32_t* n_inliers_out, void* stream);
+/* The per-pair statistics of the relative-pose evaluation (patch2pix_b200/relpose.py) for K pairs in one launch, no host
+ * sync.  rows / row_stride / offsets / offsets_host / n_dev / intr as p2p_find_essential_batch (m_k = min(n_k,
+ * n_dev[k]) rows (x1, y1, x2, y2) in columns 0..3).  Rt_gt and Rt_est DEVICE double [K][12]: R row-major then t
+ * (x1 = R x0 + t, view 0 -> view 1; t need not be normalised), Rt_est as p2p_recover_pose_batch writes it; n_inliers
+ * DEVICE int32 [K], the E-RANSAC inlier counts (<= 0: no model).  thresholds HOST double [n_thr] (1 <= n_thr <= 16,
+ * finite, > 0, strictly increasing; anything else returns -1), passed by value to the kernel.  Pair k writes
+ * out[k * out_stride ..] (DEVICE, out_stride >= 2 + (n_thr + 2) / 2 doubles):
+ *   double [0] = clip((tr(R_gt^T R) - 1) / 2, -1, 1), double [1] = clip(t_gt . t / (|t_gt| |t|), -1, 1), both NaN
+ *   when n_inliers[k] <= 0 (the caller takes the arccos, which the device does not round correctly);
+ *   then int32 [n_thr + 1] from double 2 on: the rows whose symmetric epipolar error in camera coordinates,
+ *   e = (x1^T E x0)^2 (1 / ((E x0)_0^2 + (E x0)_1^2) + 1 / ((E^T x1)_0^2 + (E^T x1)_1^2)) with E = [t_gt]x R_gt and
+ *   x = ((x - cx) / fx, (y - cy) / fy, 1), is < thresholds[j] (NaN never is), then m_k.
+ * Every fp64 product, sum, quotient and square root is rounded on its own (no fused multiply-add; order in
+ * csrc/relpose.cu), so a numpy restatement gives the same bits.  Integer counts: identical across runs and devices. */
+P2P_API int p2p_relpose_errors_batch(p2p_handle_t h, const double* rows, int row_stride, const int64_t* offsets,
+                                     const int64_t* offsets_host, int K, const double* n_dev, const double* intr,
+                                     const double* Rt_gt, const double* Rt_est, const int32_t* n_inliers,
+                                     const double* thresholds, int n_thr, double* out, int out_stride, void* stream);
 /* Pairs per launch of the batched entry points: entry 0 = p2p_find_model_batch, 1 = p2p_find_essential_batch,
  * 2 = p2p_recover_pose_batch. */
 P2P_API int p2p_batch_chunk_pairs(p2p_handle_t h, int entry, int* pairs_out);

@@ -75,6 +75,10 @@ _SIGNATURES = {
                                   C.c_ulonglong, _P, _P, _P, _P]),
     'p2p_find_essential_batch': (_I, [_P, _P, _I, _P, C.POINTER(C.c_int64), _I, _P, _P, C.c_double, C.c_double, _I,
                                       C.c_ulonglong, _P, _P, _P, _P]),
+    'p2p_find_essential_batch_th': (_I, [_P, _P, _I, _P, C.POINTER(C.c_int64), _I, _P, _P, _P, C.c_double, _I,
+                                         C.c_ulonglong, _P, _P, _P, _P]),
+    'p2p_relpose_errors_batch': (_I, [_P, _P, _I, _P, C.POINTER(C.c_int64), _I, _P, _P, _P, _P, _P,
+                                      C.POINTER(C.c_double), _I, _P, _I, _P]),
     'p2p_recover_pose_batch': (_I, [_P, _P, _I, _P, C.POINTER(C.c_int64), _I, _P, _P, _P, _P, C.c_double, _P, _P, _P,
                                     _P]),
     'p2p_batch_chunk_pairs': (_I, [_P, _I, C.POINTER(_I)]),

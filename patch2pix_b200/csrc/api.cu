@@ -1701,18 +1701,19 @@ int p2p_find_essential(p2p_handle_t h, const double* rows, int row_stride, int n
   int rc = h->verify.reserve(essential_scratch_bytes(1, n, true) + 4096);
   if (rc) return rc;
   void* scratch = h->verify.take(essential_scratch_bytes(1, n, true));
-  return launch_find_essential(single_pair(rows, row_stride, n, n_dev), nullptr, K, px_th, conf, max_iters, seed, scratch,
-                               E_out, mask_out, n_inliers_out, reinterpret_cast<cudaStream_t>(stream));
+  return launch_find_essential(single_pair(rows, row_stride, n, n_dev), nullptr, K, px_th, nullptr, conf, max_iters,
+                               seed, scratch, E_out, mask_out, n_inliers_out, reinterpret_cast<cudaStream_t>(stream));
 }
 
-int p2p_find_essential_batch(p2p_handle_t h, const double* rows, int row_stride, const int64_t* offsets,
-                             const int64_t* offsets_host, int K, const double* n_dev, const double* intr, double px_th,
-                             double conf, int max_iters, unsigned long long seed, double* E_out, uint8_t* mask_out,
-                             int32_t* n_inliers_out, void* stream) {
-  P2P_ENTER(h);
+// p2p_find_essential_batch with one px_th for every pair (px_th_dev null), or with pair k's at px_th_dev[k].
+static int find_essential_batch(p2p_handle_t h, const double* rows, int row_stride, const int64_t* offsets,
+                                const int64_t* offsets_host, int K, const double* n_dev, const double* intr,
+                                double px_th, const double* px_th_dev, double conf, int max_iters,
+                                unsigned long long seed, double* E_out, uint8_t* mask_out, int32_t* n_inliers_out,
+                                void* stream) {
   int rc = check_batch(rows, row_stride, offsets, offsets_host, K);
   if (rc) return rc;
-  P2P_REQUIRE(px_th > 0.0 && isfinite(px_th), "px_th must be positive");
+  P2P_REQUIRE(px_th_dev != nullptr || (px_th > 0.0 && isfinite(px_th)), "px_th must be positive");
   P2P_REQUIRE(conf > 0.0 && conf < 1.0, "conf must lie in (0, 1)");
   P2P_REQUIRE(max_iters > 0 && max_iters <= (1 << 24), "max_iters must lie in [1, 2^24]");
   if (K == 0) return 0;
@@ -1724,12 +1725,32 @@ int p2p_find_essential_batch(p2p_handle_t h, const double* rows, int row_stride,
   void* scratch = h->verify.take(need);
   for (int k0 = 0; k0 < K; k0 += chunk) {
     const PairBatch B = batch_chunk(rows, row_stride, offsets, offsets_host, n_dev, k0, std::min(chunk, K - k0));
-    if ((rc = launch_find_essential(B, intr + 8 * (size_t)k0, Intrinsics{}, px_th, conf, max_iters, seed, scratch,
+    if ((rc = launch_find_essential(B, intr + 8 * (size_t)k0, Intrinsics{}, px_th,
+                                    px_th_dev ? px_th_dev + k0 : nullptr, conf, max_iters, seed, scratch,
                                     E_out + 9 * (size_t)k0, mask_out, n_inliers_out + k0,
                                     reinterpret_cast<cudaStream_t>(stream))))
       return rc;
   }
   return 0;
+}
+
+int p2p_find_essential_batch(p2p_handle_t h, const double* rows, int row_stride, const int64_t* offsets,
+                             const int64_t* offsets_host, int K, const double* n_dev, const double* intr, double px_th,
+                             double conf, int max_iters, unsigned long long seed, double* E_out, uint8_t* mask_out,
+                             int32_t* n_inliers_out, void* stream) {
+  P2P_ENTER(h);
+  return find_essential_batch(h, rows, row_stride, offsets, offsets_host, K, n_dev, intr, px_th, nullptr, conf,
+                              max_iters, seed, E_out, mask_out, n_inliers_out, stream);
+}
+
+int p2p_find_essential_batch_th(p2p_handle_t h, const double* rows, int row_stride, const int64_t* offsets,
+                                const int64_t* offsets_host, int K, const double* n_dev, const double* intr,
+                                const double* px_th, double conf, int max_iters, unsigned long long seed,
+                                double* E_out, uint8_t* mask_out, int32_t* n_inliers_out, void* stream) {
+  P2P_ENTER(h);
+  P2P_REQUIRE(px_th != nullptr, "null px_th pointer");
+  return find_essential_batch(h, rows, row_stride, offsets, offsets_host, K, n_dev, intr, 0.0, px_th, conf, max_iters,
+                              seed, E_out, mask_out, n_inliers_out, stream);
 }
 
 int p2p_recover_pose(p2p_handle_t h, const double* rows, int row_stride, int n, const double* n_dev, const double* intr,
@@ -1770,6 +1791,30 @@ int p2p_recover_pose_batch(p2p_handle_t h, const double* rows, int row_stride, c
       return rc;
   }
   return 0;
+}
+
+int p2p_relpose_errors_batch(p2p_handle_t h, const double* rows, int row_stride, const int64_t* offsets,
+                             const int64_t* offsets_host, int K, const double* n_dev, const double* intr,
+                             const double* Rt_gt, const double* Rt_est, const int32_t* n_inliers,
+                             const double* thresholds, int n_thr, double* out, int out_stride, void* stream) {
+  P2P_ENTER(h);
+  int rc = check_batch(rows, row_stride, offsets, offsets_host, K);
+  if (rc) return rc;
+  P2P_REQUIRE(thresholds != nullptr, "null thresholds pointer");
+  P2P_REQUIRE(n_thr >= 1 && n_thr <= kMaxRelposeThresholds, "n_thr must be in 1..16");
+  P2P_REQUIRE(out_stride >= 2 + (n_thr + 2) / 2, "out_stride must hold 2 doubles and n_thr + 1 int32 counts");
+  RelposeErrArgs a{};
+  for (int i = 0; i < kMaxRelposeThresholds; ++i) a.thr[i] = NAN;     // no row passes a padding entry
+  for (int i = 0; i < n_thr; ++i) {
+    P2P_REQUIRE(std::isfinite(thresholds[i]) && thresholds[i] > 0.0 && (i == 0 || thresholds[i] > thresholds[i - 1]),
+                "thresholds must be finite, positive and strictly increasing");
+    a.thr[i] = thresholds[i];
+  }
+  a.n_thr = n_thr;
+  if (K == 0) return 0;
+  P2P_REQUIRE(intr && Rt_gt && Rt_est && n_inliers && out, "null tensor pointer");
+  return launch_relpose_errors(batch_chunk(rows, row_stride, offsets, offsets_host, n_dev, 0, K), intr, Rt_gt, Rt_est,
+                               n_inliers, a, out, out_stride, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int p2p_test_essential_hypotheses(p2p_handle_t h, const double* rows, int row_stride, int n, const double* intr,

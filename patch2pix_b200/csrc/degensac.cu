@@ -253,7 +253,7 @@ int find_model_degensac(const PairBatch& B, double px_th, double conf, int max_i
   const Scratch s = carve<0>(scratch, B.pairs, B.total, kRound);
   const double h_th2 = (2.0 * px_th) * (2.0 * px_th);
   const dim3 one(1, B.pairs);
-  verify_prep_kernel<false><<<one, 1024, 0, st>>>(B, nullptr, {}, px_th, Kind<0>::kSample, s.rows32, s.st);
+  verify_prep_kernel<false><<<one, 1024, 0, st>>>(B, nullptr, {}, px_th, nullptr, Kind<0>::kSample, s.rows32, s.st);
   P2P_LAUNCH_OK();
   for (int first = 0; first < max_iters; first += kRound) {
     const int count = min(kRound, max_iters - first);
@@ -288,7 +288,7 @@ int launch_test_degeneracy(const double* rows, int stride, int n, double px_th, 
   const PairBatch B = single_pair(rows, stride, n, nullptr);
   Scratch s = carve<0>(scratch, 1, n, count);
   const double h_th2 = (2.0 * px_th) * (2.0 * px_th);
-  verify_prep_kernel<false><<<1, 1024, 0, st>>>(B, nullptr, {}, px_th, Kind<0>::kSample, s.rows32, s.st);
+  verify_prep_kernel<false><<<1, 1024, 0, st>>>(B, nullptr, {}, px_th, nullptr, Kind<0>::kSample, s.rows32, s.st);
   P2P_LAUNCH_OK();
   int rc = enqueue_round<0>(s, B, 0, count, seed, 1, st);
   if (rc) return rc;

@@ -210,14 +210,14 @@ int launch_test_degeneracy(const double* rows, int stride, int n, double px_th, 
 // ---- pose.cu: essential-matrix RANSAC (5-point) and pose recovery ------------------------------------------------
 struct Intrinsics { double fx1, fy1, cx1, cy1, fx2, fy2, cx2, cy2; };   // pixels -> camera coordinates of both views
 // Batches as launch_find_model.  intr: DEVICE double [pairs][8] (fx1, fy1, cx1, cy1, fx2, fy2, cx2, cy2), or nullptr:
-// K1 for the single pair.
+// K1 for the single pair.  px_th_dev: DEVICE double [pairs], pair p's px_th, or nullptr: px_th for every pair.
 size_t essential_scratch_bytes(int pairs, long long rows, bool rounds);
 size_t pose_scratch_bytes(int pairs, long long rows);
 int essential_chunk_pairs();
 int pose_chunk_pairs();
-int launch_find_essential(const PairBatch& B, const double* intr, const Intrinsics& K1, double px_th, double conf,
-                          int max_iters, unsigned long long seed, void* scratch, double* E_out, uint8_t* mask_out,
-                          int* count_out, cudaStream_t st);
+int launch_find_essential(const PairBatch& B, const double* intr, const Intrinsics& K1, double px_th,
+                          const double* px_th_dev, double conf, int max_iters, unsigned long long seed, void* scratch,
+                          double* E_out, uint8_t* mask_out, int* count_out, cudaStream_t st);
 // Hypotheses 0 .. count-1 without selection: models_out [count*10][9], counts_out [count*10] (-1: no model).
 int launch_test_essential_hypotheses(const double* rows, int stride, int n, const Intrinsics& K, double px_th,
                                      unsigned long long seed, int count, void* scratch, double* models_out,
@@ -226,6 +226,16 @@ int launch_test_essential_hypotheses(const double* rows, int stride, int n, cons
 int launch_recover_pose(const PairBatch& B, const double* intr, const Intrinsics& K1, const double* E,
                         const uint8_t* mask_in, double dist_th, void* scratch, double* Rt_out, uint8_t* mask_out,
                         int* count_out, cudaStream_t st);
+// ---- relpose.cu: relative-pose statistics of a batch (one block per pair, pairs = B.pairs, any count): pair p writes
+// out[p * out_stride ..] = cos of the rotation and translation-direction errors of Rt_est [p] against Rt_gt [p]
+// (NaN when n_inliers[p] <= 0), then int32 [n_thr + 1]: rows with symmetric epipolar error < thr[j], rows considered.
+constexpr int kMaxRelposeThresholds = 16;
+struct RelposeErrArgs {
+  double thr[kMaxRelposeThresholds];   // finite, > 0, strictly increasing; NaN from n_thr on (no row passes those)
+  int n_thr;                           // 1 .. kMaxRelposeThresholds
+};
+int launch_relpose_errors(const PairBatch& B, const double* intr, const double* Rt_gt, const double* Rt_est,
+                          const int* n_inliers, const RelposeErrArgs& a, double* out, int out_stride, cudaStream_t st);
 
 // Tensor-core FC path helpers: pooled fp32 -> fp16 hi/lo A operand (times `scale`); final Linear(256,5) +
 // parse_regressor_out of h2 = (h2_hi + h2_lo) * inv_scale.

@@ -543,10 +543,10 @@ int pose_chunk_pairs() {
   return (int)std::min<size_t>(kMaxGridY, std::max<size_t>(1, kBatchScratchBudget / per_pair));
 }
 
-int launch_find_essential(const PairBatch& B, const double* intr, const Intrinsics& K1, double px_th, double conf,
-                          int max_iters, unsigned long long seed, void* scratch, double* E_out, uint8_t* mask_out,
-                          int* count_out, cudaStream_t st) {
-  return find_model<3>(B, intr, K1, px_th, conf, max_iters, seed, scratch, E_out, mask_out, count_out, st);
+int launch_find_essential(const PairBatch& B, const double* intr, const Intrinsics& K1, double px_th,
+                          const double* px_th_dev, double conf, int max_iters, unsigned long long seed, void* scratch,
+                          double* E_out, uint8_t* mask_out, int* count_out, cudaStream_t st) {
+  return find_model<3>(B, intr, K1, px_th, px_th_dev, conf, max_iters, seed, scratch, E_out, mask_out, count_out, st);
 }
 
 int launch_test_essential_hypotheses(const double* rows, int stride, int n, const Intrinsics& K, double px_th,

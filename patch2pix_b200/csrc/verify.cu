@@ -43,7 +43,7 @@ int launch_find_model(int model, const PairBatch& B, double px_th, double conf, 
   if (model == 2)
     return launch_find_model_degensac(B, px_th, conf, max_iters, seed, scratch, model_out, mask_out, count_out, st);
   auto find = model == 0 ? find_model<0> : find_model<1>;
-  return find(B, nullptr, {}, px_th, conf, max_iters, seed, scratch, model_out, mask_out, count_out, st);
+  return find(B, nullptr, {}, px_th, nullptr, conf, max_iters, seed, scratch, model_out, mask_out, count_out, st);
 }
 
 int launch_test_hypotheses(int model, const double* rows, int stride, int n, double px_th, unsigned long long seed,

@@ -343,10 +343,12 @@ __device__ bool parallax_model(const VerifyState& S, const double* rows, int str
 // ---- kernels ------------------------------------------------------------------------------------------------------
 // Effective row count, finiteness, the solvers' frame (F / H: the Hartley normalisation; E, CAMERA: the pair's
 // cameras), the scoring threshold, and the fp32 rows in the scoring frame (F / H: pixels; E: camera coordinates).  A
-// pair with fewer than min_rows rows, or a non-finite one, runs no rounds.
+// pair with fewer than min_rows rows, or a non-finite one, runs no rounds.  px_th_dev (device, nullable): pair p's
+// threshold is px_th_dev[p] instead of px_th.
 template <bool CAMERA>
 __global__ void __launch_bounds__(1024) verify_prep_kernel(PairBatch B, const double* __restrict__ intr, Intrinsics K1,
-                                                           double px_th, int min_rows, float4* __restrict__ rows32_all,
+                                                           double px_th, const double* __restrict__ px_th_dev,
+                                                           int min_rows, float4* __restrict__ rows32_all,
                                                            VerifyState* __restrict__ st_all) {
   __shared__ double red[33];
   __shared__ int s_n;
@@ -383,6 +385,7 @@ __global__ void __launch_bounds__(1024) verify_prep_kernel(PairBatch B, const do
     for (int k = 0; k < 2; ++k) dist[k] = block_sum_1024(dist[k], red) / (double)(m > 0 ? m : 1);
   }
   if (tid == 0) {
+    if (px_th_dev != nullptr) px_th = px_th_dev[blockIdx.y];
     if constexpr (CAMERA) {
       st->K = K;
       st->th2 = ess_th2(px_th, K);
@@ -659,14 +662,15 @@ int enqueue_round(const Scratch& s, const PairBatch& B, int first, int count, un
 }
 
 // RANSAC for F (kind 0), H (1) or E (3): prep, then per round of kRound hypotheses a round and a select, then LO.
-// intr / K1: the pairs' cameras for E, as launch_find_essential takes them; F and H ignore them.
+// intr / K1: the pairs' cameras for E, as launch_find_essential takes them; F and H ignore them.  px_th_dev (device,
+// nullable): one threshold per pair of the launch, in place of px_th.
 template <int KIND>
-int find_model(const PairBatch& B, const double* intr, const Intrinsics& K1, double px_th, double conf, int max_iters,
-               unsigned long long seed, void* scratch, double* model_out, uint8_t* mask_out, int* count_out,
-               cudaStream_t st) {
+int find_model(const PairBatch& B, const double* intr, const Intrinsics& K1, double px_th, const double* px_th_dev,
+               double conf, int max_iters, unsigned long long seed, void* scratch, double* model_out, uint8_t* mask_out,
+               int* count_out, cudaStream_t st) {
   const Scratch s = carve<KIND>(scratch, B.pairs, B.total, kRound);
-  verify_prep_kernel<KIND == 3><<<dim3(1, B.pairs), 1024, 0, st>>>(B, intr, K1, px_th, Kind<KIND>::kSample, s.rows32,
-                                                                    s.st);
+  verify_prep_kernel<KIND == 3><<<dim3(1, B.pairs), 1024, 0, st>>>(B, intr, K1, px_th, px_th_dev, Kind<KIND>::kSample,
+                                                                    s.rows32, s.st);
   P2P_LAUNCH_OK();
   for (int first = 0; first < max_iters; first += kRound) {
     const int count = min(kRound, max_iters - first);
@@ -691,7 +695,8 @@ int test_hypotheses(const double* rows, int stride, int n, const Intrinsics& K, 
   Scratch s = carve<KIND>(scratch, 1, n, 0);
   s.models = models_out;
   s.counts = counts_out;
-  verify_prep_kernel<KIND == 3><<<1, 1024, 0, st>>>(B, nullptr, K, px_th, Kind<KIND>::kSample, s.rows32, s.st);
+  verify_prep_kernel<KIND == 3><<<1, 1024, 0, st>>>(B, nullptr, K, px_th, nullptr, Kind<KIND>::kSample, s.rows32,
+                                                     s.st);
   P2P_LAUNCH_OK();
   return enqueue_round<KIND>(s, B, 0, count, seed, 1, st);
 }

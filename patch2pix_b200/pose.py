@@ -300,6 +300,18 @@ def find_essential_batch_into(handle, rows, row_stride, offsets, offsets_host, n
             handle.stream()))
 
 
+def find_essential_batch_th_into(handle, rows, row_stride, offsets, offsets_host, n_dev, intr_ptr, px_th_ptr, conf,
+                                 max_iters, seed, E_ptr, mask_ptr, counts_ptr):
+    """Enqueue p2p_find_essential_batch_th (as pose.find_essential_batch_into, px_th_ptr: DEVICE double [K])."""
+    oh = np.ascontiguousarray(offsets_host, dtype=np.int64)
+    with torch.cuda.device(rows.device):
+        _lib.check(handle.lib.p2p_find_essential_batch_th(
+            handle.h, C.c_void_p(rows.data_ptr()), row_stride, C.c_void_p(offsets.data_ptr()),
+            oh.ctypes.data_as(C.POINTER(C.c_int64)), oh.size - 1, n_dev, C.c_void_p(intr_ptr), C.c_void_p(px_th_ptr),
+            float(conf), int(max_iters), int(seed) & (2 ** 64 - 1), C.c_void_p(E_ptr), C.c_void_p(mask_ptr),
+            C.c_void_p(counts_ptr), handle.stream()))
+
+
 def recover_pose_batch_into(handle, rows, row_stride, offsets, offsets_host, n_dev, intr_ptr, E_ptr, mask_in_ptr, Rt_ptr,
                             mask_ptr, good_ptr, dist_th=DIST_TH):
     """Enqueue p2p_recover_pose_batch (device addresses; mask_in_ptr None: all rows)."""
@@ -330,20 +342,31 @@ def _parse_batch(host, offsets, K, N):
 
 def find_essential_matrices(pts1_list, pts2_list, K1_list, K2_list, px_th, conf=0.999, max_iters=1000, seed=0):
     """find_essential_matrix over a list of pairs in one batched call -> [(E, inlier mask)], element k equal to
-    find_essential_matrix(pts1_list[k], pts2_list[k], K1_list[k], K2_list[k], ...).  Numpy input crosses PCIe once
-    each way and raises ValueError when a pair has a non-finite coordinate; CUDA tensor input gives CUDA tensor views
-    without a sync."""
+    find_essential_matrix(pts1_list[k], pts2_list[k], K1_list[k], K2_list[k], px_th_k, ...), px_th_k = px_th, or
+    px_th[k] when px_th is a sequence of one threshold per pair (p2p_find_essential_batch_th).  Numpy input crosses
+    PCIe once each way and raises ValueError when a pair has a non-finite coordinate; CUDA tensor input gives CUDA
+    tensor views without a sync."""
     from .verify import pair_lists, upload
     rows, offsets, is_np = pair_lists(pts1_list, pts2_list)
     K, N = offsets.size - 1, int(offsets[-1])
     intr = _intr_rows(K1_list, K2_list, K)
+    per_pair = np.ndim(px_th) > 0
+    if per_pair:
+        px = np.asarray(px_th, dtype=np.float64).reshape(-1)
+        if px.size != K or not (np.all(np.isfinite(px)) and np.all(px > 0)):
+            raise ValueError(f'px_th must be one positive threshold, or {K} (one per pair), got {px.size} values')
     if K == 0:
         return []
-    rows, offs, intr_d = upload(rows, offsets, is_np, intr)
+    rows, offs, ex = upload(rows, offsets, is_np, np.concatenate((intr.reshape(-1), px)) if per_pair else intr)
     out = torch.zeros(batch_out_size(K, N), dtype=torch.float64, device=rows.device)
     p = _batch_ptrs(out, K, N)
-    find_essential_batch_into(_lib.default_handle(rows.device), rows, 4, offs, offsets, None, intr_d.data_ptr(), px_th,
-                              conf, max_iters, seed, p['E'], p['emask'], p['cnt'])
+    h = _lib.default_handle(rows.device)
+    if per_pair:
+        find_essential_batch_th_into(h, rows, 4, offs, offsets, None, ex.data_ptr(), ex.data_ptr() + 64 * K, conf,
+                                     max_iters, seed, p['E'], p['emask'], p['cnt'])
+    else:
+        find_essential_batch_into(h, rows, 4, offs, offsets, None, ex.data_ptr(), px_th, conf, max_iters, seed, p['E'],
+                                  p['emask'], p['cnt'])
     if is_np:
         return [r[:2] for r in _parse_batch(out.cpu().numpy(), offsets, K, N)]
     m = out[22 * K:].view(torch.uint8)

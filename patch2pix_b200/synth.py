@@ -435,6 +435,89 @@ def synthetic_hpatches_tree(root, seed, seqs):
     return out
 
 
+# ---- relative-pose pair lists (SuperGlue's text format, LoFTR's scene-info .npz) ------------------------------------
+def synthetic_relpose_pair(seed, size=(320, 240)):
+    """A seeded two-view scene of a textured plane for the relative-pose evaluation: cameras as synthetic_two_view's
+    (principal points at the image centres, camera 1 rotated up to 0.09 rad per axis and translated by ~1 unit, the
+    plane 5-7 units away), each with its own focal length (0.8-1.2 x the width), so f_mean differs from view 1's mean
+    focal length.  Image 0 is a blocky 8-bit texture cropped from a larger canvas; image 1 is the canvas seen through the
+    plane's homography K1 (R + t n^T / d) K0^-1 (fp64 inverse mapping, nearest pixel, 0 outside), so the ground-truth
+    pose is exact for every pixel.  size = (w, h) of both images.
+    -> dict(img0, img1 [h, w, 3] uint8, K0, K1 (3x3), T_0to1 (4x4: x1 = R x0 + t))."""
+    rng = np.random.default_rng([int(seed), 11])
+    w, h = (int(v) for v in size)
+    K0, K1 = (np.array([[f, 0, w / 2], [0, f, h / 2], [0, 0, 1.0]]) for f in rng.uniform(0.8, 1.2, 2) * w)
+    R = _rotation(rng.uniform(-0.09, 0.09, 3))
+    t = np.array([rng.uniform(0.6, 1.0) * rng.choice([-1, 1]), rng.uniform(-0.3, 0.3), rng.uniform(-0.2, 0.2)])
+    normal = np.array([rng.uniform(-0.2, 0.2), rng.uniform(-0.2, 0.2), 1.0])
+    normal /= np.linalg.norm(normal)
+    d = rng.uniform(5.0, 7.0)
+    m = max(w, h) // 2
+    cw, ch = w + 2 * m, h + 2 * m
+    low = rng.integers(0, 256, size=(ch // 8 + 2, cw // 8 + 2, 3), dtype=np.int32)
+    base = np.repeat(np.repeat(low, 8, 0), 8, 1)[:ch + 4, :cw + 4]
+    base = (base[:ch, :cw] + base[4:ch + 4, :cw] + base[:ch, 4:cw + 4] + base[4:ch + 4, 4:cw + 4]) // 4
+    canvas = np.clip(base + rng.integers(-12, 13, size=base.shape), 0, 255).astype(np.uint8)
+    Hi = np.linalg.inv(K1 @ (R + np.outer(t, normal) / d) @ np.linalg.inv(K0))
+    v, u = np.mgrid[0:h, 0:w].astype(np.float64)
+    q = Hi[2, 0] * u + Hi[2, 1] * v + Hi[2, 2]
+    with np.errstate(all='ignore'):
+        x = (Hi[0, 0] * u + Hi[0, 1] * v + Hi[0, 2]) / q
+        y = (Hi[1, 0] * u + Hi[1, 1] * v + Hi[1, 2]) / q
+    xi, yi = np.floor(x + 0.5) + m, np.floor(y + 0.5) + m
+    ok = (q > 0) & (xi >= 0) & (xi < cw) & (yi >= 0) & (yi < ch)
+    img1 = np.zeros((h, w, 3), dtype=np.uint8)
+    img1[ok] = canvas[yi[ok].astype(np.int64), xi[ok].astype(np.int64)]
+    T = np.eye(4)
+    T[:3, :3], T[:3, 3] = R, t
+    return dict(img0=canvas[m:m + h, m:m + w].copy(), img1=img1, K0=K0, K1=K1, T_0to1=T)
+
+
+def synthetic_relpose_tree(root, seed, n_pairs, fmt='txt', size=(320, 240)):
+    """Seeded pair list and images for the relative-pose evaluation under `root`: pair k's images are
+    images/pair{k:03d}_0.png and _1.png (synthetic_relpose_pair(seed * 1000 + k, size)), listed in
+      fmt 'txt': root/pairs.txt, SuperGlue's format (name0 name1 0 0 K0 (9) K1 (9) T_0to1 (16), written with %.17g,
+        so it reads back exactly);
+      fmt 'npz': root/scene_info.npz, the layout patch2pix_b200.relpose.read_pairs_npz reads: image_paths (object array
+        of paths relative to root), intrinsics [2n, 3, 3], poses [2n, 4, 4] world -> camera (a seeded pose for image 0
+        of each pair, T_0to1 @ it for image 1) and pair_infos (object array of ((2k, 2k + 1), overlap, an empty [0, 2]
+        array of central matches)).
+    -> (pair-list path, [dict(K0, K1, T_0to1)] per pair)."""
+    from PIL import Image
+    if fmt not in ('txt', 'npz'):
+        raise ValueError("fmt must be 'txt' or 'npz'")
+    os.makedirs(os.path.join(root, 'images'), exist_ok=True)
+    gts, names = [], []
+    for k in range(n_pairs):
+        sc = synthetic_relpose_pair(int(seed) * 1000 + k, size)
+        nm = [f'images/pair{k:03d}_{i}.png' for i in range(2)]
+        for i in range(2):
+            Image.fromarray(sc[f'img{i}']).save(os.path.join(root, nm[i]))
+        gts.append(dict(K0=sc['K0'], K1=sc['K1'], T_0to1=sc['T_0to1']))
+        names.append(nm)
+    if fmt == 'txt':
+        path = os.path.join(root, 'pairs.txt')
+        with open(path, 'w') as f:
+            for nm, g in zip(names, gts):
+                vals = np.concatenate([g['K0'].reshape(-1), g['K1'].reshape(-1), g['T_0to1'].reshape(-1)])
+                f.write(' '.join([nm[0], nm[1], '0', '0'] + ['%.17g' % v for v in vals]) + '\n')
+        return path, gts
+    rng = np.random.default_rng([int(seed), 12])
+    paths = np.empty(2 * n_pairs, dtype=object)
+    Ks, poses = np.zeros((2 * n_pairs, 3, 3)), np.zeros((2 * n_pairs, 4, 4))
+    infos = np.empty(n_pairs, dtype=object)
+    for k, (nm, g) in enumerate(zip(names, gts)):
+        T0 = np.eye(4)
+        T0[:3, :3], T0[:3, 3] = _rotation(rng.uniform(-1.0, 1.0, 3)), rng.uniform(-5.0, 5.0, 3)
+        paths[2 * k], paths[2 * k + 1] = nm
+        Ks[2 * k], Ks[2 * k + 1] = g['K0'], g['K1']
+        poses[2 * k], poses[2 * k + 1] = T0, g['T_0to1'] @ T0
+        infos[k] = ((2 * k, 2 * k + 1), float(rng.uniform(0.1, 0.7)), np.zeros((0, 2)))
+    path = os.path.join(root, 'scene_info.npz')
+    np.savez(path, image_paths=paths, intrinsics=Ks, poses=poses, pair_infos=infos)
+    return path, gts
+
+
 # ---- NCNet (ImMatchNet) test data: regenerated from seeds, so fixtures store outputs only ----------------------------
 def ncnet_stack_weights(seed, kernel_sizes, channels):
     """Conv4d weights in the reference's pre-permuted layout [k, Cout, Cin, k, k, k] and biases [Cout], fp32, scaled so
