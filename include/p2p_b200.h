@@ -425,8 +425,52 @@ P2P_API int p2p_relpose_errors_batch(p2p_handle_t h, const double* rows, int row
                                      const double* Rt_gt, const double* Rt_est, const int32_t* n_inliers,
                                      const double* thresholds, int n_thr, double* out, int out_stride, void* stream);
 /* Pairs per launch of the batched entry points: entry 0 = p2p_find_model_batch, 1 = p2p_find_essential_batch,
- * 2 = p2p_recover_pose_batch. */
+ * 2 = p2p_recover_pose_batch, 3 = p2p_find_absolute_pose_batch (queries). */
 P2P_API int p2p_batch_chunk_pairs(p2p_handle_t h, int entry, int* pairs_out);
+
+/* ---- absolute pose from 2D-3D matches (patch2pix_b200/localize.py): RANSAC over K queries in one launch chain, no
+ * host sync.  rows: ONE fp64 row array, row = (u, v, X, Y, Z) in columns 0..4 (the pixel in the query, the world
+ * point), row_stride >= 5; offsets / offsets_host / n_dev as p2p_find_model_batch (query k owns rows offsets[k] ..
+ * offsets[k+1]-1 and uses min(n_k, n_dev[k]) of them).  intr DEVICE double [K][4] = (fx, fy, cx, cy), a pinhole camera
+ * without distortion per query (finite, positive focal lengths: the caller's contract, not read back).  px_th_dev
+ * DEVICE double [K] (query k's pixel threshold, positive and finite by contract) or NULL: px_th for every query.
+ *
+ * Per query: the world points are centred on their mean (fp32 scoring stays accurate far from the origin); rounds of
+ * 1024 hypotheses draw 3 distinct rows (the p2p_find_model generator) and solve Grunert's P3P quartic in fp64 (Ferrari,
+ * two Newton steps per root, up to 4 poses); a row is an inlier iff its depth is > 0 and its squared reprojection
+ * error is < px_th^2, scored in fp32.  Selection, tie rule and stopping bound (s = 3) as p2p_find_model.  The winner is
+ * refined by Gauss-Newton on the 6-DoF pose over its inliers (3 steps per refit, rotation through the exponential
+ * map), each refit kept while the inlier count strictly grows, at most 4 refits.
+ * Rt_out DEVICE double [K][12]: R row-major then t, x_cam = R X + t, in world coordinates; mask_out DEVICE uint8,
+ * row-aligned; n_inliers_out DEVICE int32 [K].  A query with fewer than 4 rows, or without a model, gets count 0; one
+ * with a non-finite value gets -1; both get a NaN pose and a zero mask, and neither affects the other queries.  Query
+ * k's result is bit-identical to the same call on its rows alone, and with px_th_dev all equal to x, to the call with
+ * px_th = x. */
+P2P_API int p2p_find_absolute_pose_batch(p2p_handle_t h, const double* rows, int row_stride, const int64_t* offsets,
+                                         const int64_t* offsets_host, int K, const double* n_dev, const double* intr,
+                                         double px_th, const double* px_th_dev, double conf, int max_iters,
+                                         unsigned long long seed, double* Rt_out, uint8_t* mask_out,
+                                         int32_t* n_inliers_out, void* stream);
+/* Test hook: hypotheses 0 .. count-1 (count <= 2^20) of one query (n >= 4 rows, intr HOST double [4]) without
+ * selection.  models_out DEVICE double [count*4][12]: poses in the centred frame (x_cam = R (X - mean) + t, mean the
+ * row-order fixed-tree sum of the world points over n), zero where a slot has none; counts_out DEVICE int32 [count*4]
+ * (-1: no pose).  A sample's poses fill its first slots in ascending order of the quartic's root. */
+P2P_API int p2p_test_absolute_pose_hypotheses(p2p_handle_t h, const double* rows, int row_stride, int n,
+                                              const double* intr, double px_th, unsigned long long seed, int count,
+                                              double* models_out, int32_t* counts_out, void* stream);
+/* Lift one database cutout's matches to world points (hloc's interpolate_scan + the scan alignment).  scan DEVICE fp64
+ * [height][width][3] (the cutout's XYZcut, NaN holes), align HOST double [16] (4x4 row-major, finite), matches DEVICE
+ * fp64 rows (xq, yq, xdb, ydb) in columns 0..3, match_stride >= 4, n rows or min(n, *n_dev) (n_dev DEVICE double,
+ * nullable).  Per match in order: a database pixel outside [0, width-1] x [0, height-1] (or NaN) is dropped; else the
+ * scan is sampled there as grid_sample(align_corners=True) does, bilinear (in-bounds corners only), and a NaN channel
+ * takes the nearest pixel's value (round half to even); a point still not finite is dropped; a kept point becomes
+ * A[:3, :3] p + A[:3, 3], every product and sum rounded on its own.  Kept rows (xq, yq, X, Y, Z) are written to rows_out
+ * (DEVICE, row_stride >= 5) from row *count_dev on, in match order, at most up to row capacity, and *count_dev (DEVICE
+ * double: the running count, p2p_find_absolute_pose_batch's n_dev entry) grows by their number.  One block; n = 0
+ * enqueues nothing. */
+P2P_API int p2p_lift_scan(p2p_handle_t h, const double* scan, int height, int width, const double* align,
+                          const double* matches, int match_stride, int n, const double* n_dev, double* rows_out,
+                          int row_stride, long long capacity, double* count_dev, void* stream);
 
 /* ---- bring-up / accuracy probe: C[M,N] = alpha * A[M,K] B[N,K]^T on the wgmma path with the
  * same operand format as the hot path (fp32 inputs are split to fp16 hi/lo on the device).

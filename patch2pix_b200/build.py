@@ -10,7 +10,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 OUT = os.path.join(HERE, 'libp2p_b200.so')
 SOURCES = ['api.cu', 'coarse.cu', 'refine.cu', 'umma_gemm.cu', 'nc_umma.cu', 'preprocess.cu', 'verify.cu', 'pose.cu', 'degensac.cu',
-           'eval.cu', 'hpatches.cu', 'overlap.cu', 'nc_stack.cu', 'topk.cu', 'relpose.cu']
+           'eval.cu', 'hpatches.cu', 'overlap.cu', 'nc_stack.cu', 'topk.cu', 'relpose.cu',
+           'abspose.cu']
 HEADERS = ['common.cuh', 'kernels.h', 'ransac_common.cuh', 'verify_common.cuh', 'umma_gemm.h', 'umma_ptx.cuh',
            os.path.join('..', '..', 'include', 'p2p_b200.h')]
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',

@@ -1548,8 +1548,12 @@ static size_t batch_scratch(const int64_t* offsets_host, int K, int chunk, size_
 int p2p_batch_chunk_pairs(p2p_handle_t h, int entry, int* pairs_out) {
   P2P_ENTER(h);
   P2P_REQUIRE(pairs_out != nullptr, "null pointer");
-  P2P_REQUIRE(entry >= 0 && entry <= 2, "entry must be 0 (find_model), 1 (find_essential) or 2 (recover_pose)");
-  *pairs_out = entry == 0 ? verify_chunk_pairs() : entry == 1 ? essential_chunk_pairs() : pose_chunk_pairs();
+  P2P_REQUIRE(entry >= 0 && entry <= 3,
+              "entry must be 0 (find_model), 1 (find_essential), 2 (recover_pose) or 3 (find_absolute_pose)");
+  *pairs_out = entry == 0   ? verify_chunk_pairs()
+               : entry == 1 ? essential_chunk_pairs()
+               : entry == 2 ? pose_chunk_pairs()
+                            : abspose_chunk_queries();
   return 0;
 }
 
@@ -1831,6 +1835,67 @@ int p2p_test_essential_hypotheses(p2p_handle_t h, const double* rows, int row_st
   void* scratch = h->verify.take(essential_scratch_bytes(1, n, false));
   return launch_test_essential_hypotheses(rows, row_stride, n, K, px_th, seed, count, scratch, models_out, counts_out,
                                           reinterpret_cast<cudaStream_t>(stream));
+}
+
+int p2p_find_absolute_pose_batch(p2p_handle_t h, const double* rows, int row_stride, const int64_t* offsets,
+                                 const int64_t* offsets_host, int K, const double* n_dev, const double* intr,
+                                 double px_th, const double* px_th_dev, double conf, int max_iters,
+                                 unsigned long long seed, double* Rt_out, uint8_t* mask_out, int32_t* n_inliers_out,
+                                 void* stream) {
+  P2P_ENTER(h);
+  P2P_REQUIRE(row_stride >= 5, "row_stride must be at least 5");
+  int rc = check_batch(rows, row_stride, offsets, offsets_host, K);
+  if (rc) return rc;
+  P2P_REQUIRE(px_th_dev != nullptr || (px_th > 0.0 && isfinite(px_th)), "px_th must be positive");
+  P2P_REQUIRE(conf > 0.0 && conf < 1.0, "conf must lie in (0, 1)");
+  P2P_REQUIRE(max_iters > 0 && max_iters <= (1 << 24), "max_iters must lie in [1, 2^24]");
+  if (K == 0) return 0;
+  P2P_REQUIRE(intr && Rt_out && mask_out && n_inliers_out, "null tensor pointer");
+  const int chunk = abspose_chunk_queries();
+  const size_t need =
+      batch_scratch(offsets_host, K, chunk, [](int p, long long r) { return abspose_scratch_bytes(p, r, true); });
+  if ((rc = h->verify.reserve(need + 4096))) return rc;
+  void* scratch = h->verify.take(need);
+  for (int k0 = 0; k0 < K; k0 += chunk) {
+    const PairBatch B = batch_chunk(rows, row_stride, offsets, offsets_host, n_dev, k0, std::min(chunk, K - k0));
+    if ((rc = launch_find_absolute_pose(B, intr + 4 * (size_t)k0, px_th, px_th_dev ? px_th_dev + k0 : nullptr, conf,
+                                        max_iters, seed, scratch, Rt_out + 12 * (size_t)k0, mask_out,
+                                        n_inliers_out + k0, reinterpret_cast<cudaStream_t>(stream))))
+      return rc;
+  }
+  return 0;
+}
+
+int p2p_test_absolute_pose_hypotheses(p2p_handle_t h, const double* rows, int row_stride, int n, const double* intr,
+                                      double px_th, unsigned long long seed, int count, double* models_out,
+                                      int32_t* counts_out, void* stream) {
+  P2P_ENTER(h);
+  P2P_REQUIRE(rows && models_out && counts_out && count > 0 && count <= (1 << 20) && row_stride >= 5, "bad argument");
+  P2P_REQUIRE(n >= 4 && n <= (1 << 26), "fewer than 4 rows");
+  P2P_REQUIRE(intr != nullptr && isfinite(intr[0]) && isfinite(intr[1]) && isfinite(intr[2]) && isfinite(intr[3]) &&
+                  intr[0] > 0.0 && intr[1] > 0.0,
+              "intr must be 4 finite values with positive focal lengths");
+  P2P_REQUIRE(px_th > 0.0 && isfinite(px_th), "px_th must be positive");
+  int rc = h->verify.reserve(abspose_scratch_bytes(1, n, false) + 4096);
+  if (rc) return rc;
+  void* scratch = h->verify.take(abspose_scratch_bytes(1, n, false));
+  return launch_test_absolute_pose_hypotheses(rows, row_stride, n, intr, px_th, seed, count, scratch, models_out,
+                                              counts_out, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int p2p_lift_scan(p2p_handle_t h, const double* scan, int height, int width, const double* align,
+                  const double* matches, int match_stride, int n, const double* n_dev, double* rows_out,
+                  int row_stride, long long capacity, double* count_dev, void* stream) {
+  P2P_ENTER(h);
+  P2P_REQUIRE(height >= 1 && width >= 1 && (size_t)height * width <= ((size_t)1 << 31), "bad scan size");
+  P2P_REQUIRE(match_stride >= 4 && row_stride >= 5, "match_stride must be at least 4 and row_stride at least 5");
+  P2P_REQUIRE(n >= 0 && n <= (1 << 26) && capacity >= 0, "bad match count or capacity");
+  P2P_REQUIRE(align != nullptr, "null alignment");
+  for (int i = 0; i < 16; ++i) P2P_REQUIRE(std::isfinite(align[i]), "the alignment must be finite");
+  P2P_REQUIRE(scan && count_dev && (matches || n == 0) && (rows_out || capacity == 0), "null pointer");
+  if (n == 0) return 0;
+  return launch_lift_scan(scan, height, width, align, matches, match_stride, n, n_dev, rows_out, row_stride, capacity,
+                          count_dev, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int p2p_test_gemm(p2p_handle_t h, const float* a, const float* b, float* c, int M, int N, int K, int passes,

@@ -226,6 +226,24 @@ int launch_test_essential_hypotheses(const double* rows, int stride, int n, cons
 int launch_recover_pose(const PairBatch& B, const double* intr, const Intrinsics& K1, const double* E,
                         const uint8_t* mask_in, double dist_th, void* scratch, double* Rt_out, uint8_t* mask_out,
                         int* count_out, cudaStream_t st);
+// ---- abspose.cu: absolute-pose RANSAC (P3P, Gauss-Newton LO) and the scan lift -------------------------------------
+// Rows (u, v, X, Y, Z) in columns 0..4, batches as launch_find_model (a pair is a query).  intr: DEVICE double
+// [queries][4] (fx, fy, cx, cy); px_th_dev: DEVICE double [queries] or nullptr (px_th for every query).  Rt_out
+// [queries][12] (R row-major, t; x_cam = R X + t), mask_out indexed by row, count_out [queries].
+size_t abspose_scratch_bytes(int queries, long long rows, bool rounds);
+int abspose_chunk_queries();
+int launch_find_absolute_pose(const PairBatch& B, const double* intr, double px_th, const double* px_th_dev,
+                              double conf, int max_iters, unsigned long long seed, void* scratch, double* Rt_out,
+                              uint8_t* mask_out, int* count_out, cudaStream_t st);
+// Hypotheses 0 .. count-1 of one query without selection: intr HOST double [4]; models_out [count*4][12] (centred
+// frame), counts_out [count*4] (-1: no pose).
+int launch_test_absolute_pose_hypotheses(const double* rows, int stride, int n, const double* intr, double px_th,
+                                         unsigned long long seed, int count, void* scratch, double* models_out,
+                                         int* counts_out, cudaStream_t st);
+// align: HOST double [12], the top 3x4 of the cutout's alignment, row-major.
+int launch_lift_scan(const double* scan, int H, int W, const double* align, const double* matches, int match_stride,
+                     int n, const double* n_dev, double* rows_out, int row_stride, long long cap, double* count_dev,
+                     cudaStream_t st);
 // ---- relpose.cu: relative-pose statistics of a batch (one block per pair, pairs = B.pairs, any count): pair p writes
 // out[p * out_stride ..] = cos of the rotation and translation-direction errors of Rt_est [p] against Rt_gt [p]
 // (NaN when n_inliers[p] <= 0), then int32 [n_thr + 1]: rows with symmetric epipolar error < thr[j], rows considered.

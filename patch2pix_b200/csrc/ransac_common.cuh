@@ -180,9 +180,10 @@ __device__ __forceinline__ double block_sum_1024(double v, double* red) {   // f
 
 // ---- per-round selection (one block of 1024 threads) --------------------------------------------------------------
 // Best of this round's nm models -> state if strictly better than the best so far (most inliers, ties to the lowest
-// (hypothesis, root) index); then the stopping bound log(1-conf) / log(1-w^s).  State has best[9], n, stop, best_count.
-// `past_stop` selects even when an earlier select of the same round has set stop (extra candidates of that round).
-template <typename State>
+// (hypothesis, root) index); then the stopping bound log(1-conf) / log(1-w^s).  State has best[L], n, stop, best_count;
+// models holds L doubles per model (9 for F / H / E, 12 for an absolute pose).  `past_stop` selects even when an earlier
+// select of the same round has set stop (extra candidates of that round).
+template <int L = 9, typename State>
 __device__ __forceinline__ void select_round(State* __restrict__ st, const double* __restrict__ models,
                                              const int* __restrict__ counts, int nm, int done, int sample, double conf,
                                              int max_iters, bool past_stop = false) {
@@ -212,7 +213,7 @@ __device__ __forceinline__ void select_round(State* __restrict__ st, const doubl
   if (c > st->best_count) {
     const int m = (int)(0xFFFFFFFFull - (key & 0xFFFFFFFFull));
     st->best_count = c;
-    for (int j = 0; j < 9; ++j) st->best[j] = models[(size_t)m * 9 + j];
+    for (int j = 0; j < L; ++j) st->best[j] = models[(size_t)m * L + j];
   }
   double needed = HUGE_VAL;
   if (st->best_count > 0) {

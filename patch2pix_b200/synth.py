@@ -575,3 +575,165 @@ def ncnet_features(seed, c, size1, size2):
 def ncnet_images(seed, size1, size2):
     g = torch.Generator().manual_seed(seed)
     return torch.rand(1, 3, *size1, generator=g), torch.rand(1, 3, *size2, generator=g)
+
+
+# ---- absolute pose and InLoc-layout trees ------------------------------------------------------------------------------
+def synthetic_abspose(seed, n, outlier_ratio, noise_px, width=1024, height=768, focal=900.0):
+    """Seeded 2D-3D correspondences with a known pose, for absolute-pose RANSAC: a pinhole camera (focal `focal`,
+    principal point at the image centre) with a random orientation, its centre about 100 units from the world origin (so
+    the world coordinates are far from zero, as InLoc's are), round(n * (1 - outlier_ratio)) world points 2-20 units in
+    front of it projected into the image with N(0, noise_px^2) pixel noise, and outliers pairing uniform pixels with
+    world points drawn like the true ones, shuffled.
+    -> dict(pts2d [n, 2], pts3d [n, 3] float64, K (3x3), R, t (x_cam = R X + t), inlier [n] bool)."""
+    rng = np.random.default_rng([int(seed), 21])
+    K = np.array([[focal, 0, width / 2], [0, focal, height / 2], [0, 0, 1.0]])
+    R = _rotation(rng.normal(0.0, 1.0, 3))
+    C = rng.uniform(-10.0, 10.0, 3) + np.array([100.0, -60.0, 25.0])
+    t = -R @ C
+
+    def points(m):
+        uv = rng.uniform([0, 0], [width, height], (m, 2))
+        ray = np.linalg.solve(K, np.concatenate([uv, np.ones((m, 1))], 1).T).T
+        return uv, (ray * rng.uniform(2.0, 20.0, m)[:, None] - t) @ R
+    n_in = int(round(n * (1.0 - outlier_ratio)))
+    uv, X = points(n_in)
+    uv = uv + rng.normal(0.0, noise_px, uv.shape)
+    _, Xo = points(n - n_in)
+    uvo = rng.uniform([0, 0], [width, height], (n - n_in, 2))
+    perm = rng.permutation(n)
+    return dict(pts2d=np.concatenate([uv, uvo])[perm], pts3d=np.concatenate([X, Xo])[perm], K=K, R=R, t=t,
+                inlier=np.concatenate([np.ones(n_in, bool), np.zeros(n - n_in, bool)])[perm])
+
+
+INLOC_FOCAL = 4032.0 * 28.0 / 36.0    # hloc's focal length of InLoc's iPhone 7 queries
+
+
+def _look_at(C, target, roll):
+    z = target - C
+    z = z / np.linalg.norm(z)
+    x = np.cross(np.array([0.0, 0.0, 1.0]), z)
+    x /= np.linalg.norm(x)
+    y = np.cross(z, x)
+    R = np.stack([x, y, z])                                  # rows: camera axes in world coordinates
+    return _rotation(np.array([0.0, 0.0, roll])) @ R
+
+
+def _render_plane(scene, K, R, t, w, h):
+    """World points [h, w, 3] of the plane seen through each pixel centre (NaN off the textured area or behind the
+    camera) and the image [h, w, 3] uint8 (nearest texel, 0 where NaN)."""
+    O, e1, e2, nrm, texel, canvas = (scene[k] for k in ('O', 'e1', 'e2', 'n', 'texel', 'canvas'))
+    v, u = np.mgrid[0:h, 0:w].astype(np.float64)
+    ray = np.stack([(u - K[0, 2]) / K[0, 0], (v - K[1, 2]) / K[1, 1], np.ones_like(u)], -1) @ R   # world directions
+    C = -R.T @ t
+    lam = ((O - C) @ nrm) / (ray @ nrm)
+    X = C + lam[..., None] * ray
+    a = ((X - O) @ e1) / texel + canvas.shape[1] / 2
+    b = ((X - O) @ e2) / texel + canvas.shape[0] / 2
+    ai, bi = np.floor(a + 0.5), np.floor(b + 0.5)
+    ok = (lam > 0) & (ai >= 0) & (ai < canvas.shape[1]) & (bi >= 0) & (bi < canvas.shape[0])
+    img = np.zeros((h, w, 3), dtype=np.uint8)
+    img[ok] = canvas[bi[ok].astype(np.int64), ai[ok].astype(np.int64)]
+    X[~ok] = np.nan
+    return X, img
+
+
+def _quat(R):
+    from .localize import rotmat_to_qvec
+    return rotmat_to_qvec(R)
+
+
+def synthetic_inloc_tree(root, seed, n_queries, n_db, size=(320, 240)):
+    """Seeded InLoc-layout tree under `root`, in the layout patch2pix_b200.localize reads: a textured plane about 100
+    units from the world origin, seen by
+      query/iphone7/IMG_{k:04d}.JPG: query k, focal INLOC_FOCAL, principal point at the image centre;
+      database/cutouts/DUC1/{s:03d}/DUC_cutout_{s:03d}_{30 j}_0.jpg (+ .jpg.mat): n_db cutouts per query from nearby
+        cameras, each with its scan `XYZcut` [h, w, 3] in the scan's own frame (NaN off the plane and in a few seeded
+        rectangular holes);
+      database/alignments/DUC1/transformations/DUC_trans_{s:03d}.txt: the scan-to-world transform, 4x4 rows on lines
+        7-10 (counted from 0) after a header;
+      pairs.txt: hloc's retrieval list ('query db' per line, grouped by query);
+      gt_poses.txt: the queries' poses as localize writes them (name qw qx qy qz tx ty tz, world -> camera).
+    Images are size = (w, h) PNG data behind .JPG / .jpg names (PIL reads either).
+    -> dict(pairs, gt (paths), queries {query name: (K, R, t)}, db {db name: (K, R, t)}, scene)."""
+    from PIL import Image
+    from scipy.io import savemat
+    rng = np.random.default_rng([int(seed), 31])
+    w, h = (int(v) for v in size)
+    canvas_px = 1024
+    low = rng.integers(0, 256, size=(canvas_px // 8 + 2, canvas_px // 8 + 2, 3), dtype=np.int32)
+    base = np.repeat(np.repeat(low, 8, 0), 8, 1)[:canvas_px + 4, :canvas_px + 4]
+    base = (base[:canvas_px, :canvas_px] + base[4:, :canvas_px] + base[:canvas_px, 4:] + base[4:, 4:]) // 4
+    canvas = np.clip(base + rng.integers(-12, 13, size=base.shape), 0, 255).astype(np.uint8)
+    nrm = np.array([rng.uniform(-0.2, 0.2), 1.0, rng.uniform(-0.1, 0.1)])
+    nrm /= np.linalg.norm(nrm)
+    e1 = np.cross(np.array([0.0, 0.0, 1.0]), nrm)
+    e1 /= np.linalg.norm(e1)
+    scene = dict(O=np.array([120.0, -40.0, 30.0]), n=nrm, e1=e1, e2=np.cross(nrm, e1), texel=0.002, canvas=canvas)
+    K = np.array([[INLOC_FOCAL, 0, w / 2], [0, INLOC_FOCAL, h / 2], [0, 0, 1.0]])
+
+    def camera(center_off, target_off, dist):
+        C = scene['O'] + scene['n'] * dist + scene['e1'] * center_off[0] + scene['e2'] * center_off[1]
+        T = scene['O'] + scene['e1'] * target_off[0] + scene['e2'] * target_off[1]
+        R = _look_at(C, T, rng.uniform(-0.1, 0.1))
+        return R, -R @ C
+    for d in ('query/iphone7', 'database/cutouts/DUC1', 'database/alignments/DUC1/transformations'):
+        os.makedirs(os.path.join(root, d), exist_ok=True)
+    queries, db, lines, gt_lines = {}, {}, [], []
+    for k in range(n_queries):
+        qname = f'query/iphone7/IMG_{k:04d}.JPG'
+        tgt = rng.uniform(-0.4, 0.4, 2)
+        R, t = camera(tgt + rng.uniform(-0.5, 0.5, 2), tgt, rng.uniform(5.0, 7.0))
+        _, img = _render_plane(scene, K, R, t, w, h)
+        Image.fromarray(img).save(os.path.join(root, qname), format='PNG')
+        queries[qname] = (K, R, t)
+        q = _quat(R)
+        gt_lines.append(' '.join([os.path.basename(qname)] + ['%.17g' % v for v in np.concatenate([q, t])]))
+        for j in range(n_db):
+            s = k * n_db + j
+            dname = f'database/cutouts/DUC1/{s:03d}/DUC_cutout_{s:03d}_{30 * j}_0.jpg'
+            os.makedirs(os.path.dirname(os.path.join(root, dname)), exist_ok=True)
+            Rd, td = camera(tgt + rng.uniform(-0.5, 0.5, 2), tgt + rng.uniform(-0.03, 0.03, 2), rng.uniform(5.0, 7.0))
+            X, img = _render_plane(scene, K, Rd, td, w, h)
+            Image.fromarray(img).save(os.path.join(root, dname), format='PNG')
+            Ta = np.eye(4)
+            Ta[:3, :3], Ta[:3, 3] = _rotation(np.array([0.0, 0.0, rng.uniform(-np.pi, np.pi)])), rng.uniform(-50, 50, 3)
+            Xl = (X - Ta[:3, 3]) @ Ta[:3, :3]                  # the scan's own frame: X = Ta[:3, :3] Xl + Ta[:3, 3]
+            for _ in range(3):
+                y0, x0 = int(rng.integers(0, h - 8)), int(rng.integers(0, w - 8))
+                Xl[y0:y0 + int(rng.integers(2, 9)), x0:x0 + int(rng.integers(2, 9))] = np.nan
+            savemat(os.path.join(root, dname + '.mat'), {'XYZcut': Xl})
+            with open(os.path.join(root, 'database/alignments/DUC1/transformations', f'DUC_trans_{s:03d}.txt'),
+                      'w') as f:
+                f.write(f'DUC_scan_{s:03d}.ptx\n\nAfter general icp:\n')
+                f.write('\n'.join(' '.join('%.17g' % v for v in row) for row in np.eye(4)) + '\n')
+                f.write('\n'.join(' '.join('%.17g' % v for v in row) for row in Ta) + '\n')
+            db[dname] = (K, Rd, td)
+            lines.append(f'{qname} {dname}')
+    pairs = os.path.join(root, 'pairs.txt')
+    with open(pairs, 'w') as f:
+        f.write('\n'.join(lines) + '\n')
+    gt = os.path.join(root, 'gt_poses.txt')
+    with open(gt, 'w') as f:
+        f.write('\n'.join(gt_lines) + '\n')
+    return dict(pairs=pairs, gt=gt, queries=queries, db=db, scene=scene)
+
+
+def inloc_gt_matcher(tree, step=8):
+    """Callable (query_path, db_path) -> [N, 4] (xq, yq, xdb, ydb) ground-truth matches of a synthetic_inloc_tree: a
+    pixel grid of the query, its plane points projected into the cutout, kept inside the cutout."""
+    def matcher(qpath, dpath):
+        qn = next(k for k in tree['queries'] if qpath.endswith(k))
+        dn = next(k for k in tree['db'] if dpath.endswith(k))
+        K, R, t = tree['queries'][qn]
+        Kd, Rd, td = tree['db'][dn]
+        w, h = int(round(2 * K[0, 2])), int(round(2 * K[1, 2]))
+        X, _ = _render_plane(tree['scene'], K, R, t, w, h)
+        v, u = np.mgrid[0:h:step, 0:w:step]
+        X = X[v, u].reshape(-1, 3)
+        P = X @ Rd.T + td
+        with np.errstate(invalid='ignore'):
+            xd = Kd[0, 0] * P[:, 0] / P[:, 2] + Kd[0, 2]
+            yd = Kd[1, 1] * P[:, 1] / P[:, 2] + Kd[1, 2]
+            ok = np.isfinite(xd) & (xd >= 0) & (xd <= w - 1) & (yd >= 0) & (yd <= h - 1)
+        return np.stack([u.reshape(-1), v.reshape(-1), xd, yd], 1)[ok].astype(np.float64)
+    return matcher
