@@ -472,6 +472,61 @@ P2P_API int p2p_lift_scan(p2p_handle_t h, const double* scan, int height, int wi
                           const double* matches, int match_stride, int n, const double* n_dev, double* rows_out,
                           int row_stride, long long capacity, double* count_dev, void* stream);
 
+/* ---- triangulation against known poses (sfm.cu; the protocol in patch2pix_b200/sfm.py).  All DEVICE arrays unless
+ * named HOST; ids come from sorted keys, so every output is independent of grid shape and scheduling.
+ *
+ * p2p_sfm_keypoints: matches fp64 [n_matches][4] (x0, y0, x1, y1), pair p owning rows offsets[p] .. offsets[p+1]
+ * (int64 [n_pairs + 1], offsets[0] = 0), pair_img int32 [n_pairs][2] (image index < 2^20 of each side).  Endpoint e is
+ * side e & 1 of match e >> 1 when both_sides, else side 0 of match e.  An endpoint that is not finite, is negative, or
+ * whose cell (floor(x / merge_px), floor(y / merge_px)) reaches 2^22 is dropped.  Keypoints are the distinct keys
+ * image << 44 | cell_y << 22 | cell_x, ids in key order; kp_xy [.][2] is the mean of the key's endpoints summed in
+ * endpoint order, kp_key [.] the key; kp_of_ep [endpoints] the keypoint of each endpoint or -1.  Capacity of the
+ * keypoint arrays: the endpoint count.  counts int64 [2] = keypoints, dropped endpoints.  No host sync. */
+P2P_API int p2p_sfm_keypoints(p2p_handle_t h, const double* matches, long long n_matches, const int64_t* offsets,
+                              int n_pairs, const int32_t* pair_img, int both_sides, double merge_px, double* kp_xy,
+                              uint64_t* kp_key, int32_t* kp_of_ep, int64_t* counts, void* stream);
+/* Pixels -> undistorted normalised coordinates of keypoints 0 .. min(capacity, *n_dev) - 1 (n_dev nullable): image =
+ * kp_key >> 44, camera cams [img_cam[image]] = (model, fx, fy, cx, cy, k1, k2, 0), COLMAP's radial distortion
+ * u (1 + k1 r^2 + k2 r^4) inverted by 12 Newton steps from the distorted point. */
+P2P_API int p2p_sfm_undistort(p2p_handle_t h, const double* xy, const uint64_t* kp_key, long long capacity,
+                              const int64_t* n_dev, const int32_t* img_cam, const double* cams, double* xy_out,
+                              void* stream);
+/* Edges and tracks of a p2p_sfm_keypoints(both_sides = 1) result.  A match is an edge candidate iff it is the first
+ * match of its pair, in match order, for its keypoint on side 0 and also for its keypoint on side 1; it is kept iff
+ * its Sampson error under E [n_pairs][9] (row-major, x1^T E x0 = 0 in the normalised coordinates kp_n) is at most
+ * thr [n_pairs].  Equal edges collapse.  labels int32 [n_kp]: the smallest keypoint id of each connected component.
+ * obs_kp int32 [n_kp]: keypoints sorted by (label, id); a track is a run of 2 .. 2^16 equal labels, track t at
+ * obs_kp[track_start[t]] .. + track_len[t] (capacity n_kp), in label order.  counts (DEVICE and HOST int64 [6]) =
+ * unique kept edges, tracks, observations in tracks, rejected components over 2^16, first-in-pair matches, 0.
+ * Synchronises once (hooking converged), then copies the counts to counts_host. */
+P2P_API int p2p_sfm_tracks(p2p_handle_t h, const int32_t* kp_of_ep, long long n_matches, const int64_t* offsets,
+                           int n_pairs, const double* E, const double* thr, const double* kp_n, long long n_kp,
+                           int32_t* labels, int32_t* obs_kp, int32_t* track_start, int32_t* track_len,
+                           int64_t* counts_dev, int64_t* counts_host, void* stream);
+/* Multi-view triangulation of each track (rounds of hypotheses, selection, Gauss-Newton, acceptance; sfm.py states
+ * them).  images fp64 [.][15] = R row-major, t, centre; cameras as p2p_sfm_undistort; a reprojection error is measured
+ * in original (distorted) pixels.  Points are numbered by (track, round): points [.][3], point_len int32 (inlier
+ * observations), point_err (their mean error in pixels), capacity n_tracks * 8; kp_point int32 [n_kp] the point of each
+ * keypoint or -1.  counts int64 [1] = points.  No host sync. */
+P2P_API int p2p_sfm_triangulate(p2p_handle_t h, const int32_t* obs_kp, const int32_t* track_start,
+                                const int32_t* track_len, int n_tracks, long long n_kp, const double* kp_xy,
+                                const double* kp_n, const uint64_t* kp_key, const double* images,
+                                const int32_t* img_cam, const double* cams, double reproj_px, double cos_min_angle,
+                                double* points, int32_t* point_len, double* point_err, int32_t* kp_point,
+                                int64_t* counts, void* stream);
+/* 2D-3D rows of a chunk of queries.  matches / offsets / pair_img as p2p_sfm_keypoints with pair_img = (query index,
+ * database image); qkp_* the p2p_sfm_keypoints(both_sides = 0) and p2p_sfm_undistort results of the same matches.
+ * Each database endpoint takes the nearest keypoint of its image, among the 3x3 cells around its own, that has a
+ * point and lies within merge_px (ties to the lower id); rows fp64 [.][5] = (fx xn + cx, fy yn + cy, X, Y, Z) with
+ * q_intr [n_queries][4] = (fx, fy, cx, cy), one per distinct (query keypoint, point), ordered by that pair; q_offsets
+ * int64 [n_queries + 1] the rows of each query (the p2p_find_absolute_pose_batch layout).  No host sync. */
+P2P_API int p2p_sfm_query_rows(p2p_handle_t h, const double* matches, long long n_matches, const int64_t* offsets,
+                               int n_pairs, const int32_t* pair_img, int n_queries, double merge_px,
+                               const int32_t* qkp_of_ep, const uint64_t* qkp_key, const double* qkp_n,
+                               const double* q_intr, const uint64_t* kp_key, const double* kp_xy,
+                               const int32_t* kp_point, long long n_kp, const double* points, double* rows,
+                               int64_t* q_offsets, void* stream);
+
 /* ---- bring-up / accuracy probe: C[M,N] = alpha * A[M,K] B[N,K]^T on the wgmma path with the
  * same operand format as the hot path (fp32 inputs are split to fp16 hi/lo on the device).
  * a, b, c are DEVICE fp32; K % 64 == 0. */

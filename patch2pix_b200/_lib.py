@@ -87,6 +87,13 @@ _SIGNATURES = {
     'p2p_lift_scan': (_I, [_P, _P, _I, _I, C.POINTER(C.c_double), _P, _I, _I, _P, _P, _I, _LL, _P, _P]),
     'p2p_test_absolute_pose_hypotheses': (_I, [_P, _P, _I, _I, C.POINTER(C.c_double), C.c_double, C.c_ulonglong, _I, _P,
                                                _P, _P]),
+    'p2p_sfm_keypoints': (_I, [_P, _P, _LL, _P, _I, _P, _I, C.c_double, _P, _P, _P, _P, _P]),
+    'p2p_sfm_undistort': (_I, [_P, _P, _P, _LL, _P, _P, _P, _P, _P]),
+    'p2p_sfm_tracks': (_I, [_P, _P, _LL, _P, _I, _P, _P, _P, _LL, _P, _P, _P, _P, _P, C.POINTER(C.c_int64), _P]),
+    'p2p_sfm_triangulate': (_I, [_P, _P, _P, _P, _I, _LL, _P, _P, _P, _P, _P, _P, C.c_double, C.c_double, _P, _P, _P,
+                                 _P, _P, _P]),
+    'p2p_sfm_query_rows': (_I, [_P, _P, _LL, _P, _I, _P, _I, C.c_double, _P, _P, _P, _P, _P, _P, _P, _LL, _P, _P, _P,
+                                _P]),
 }
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
 PROF_KINDS = ('l2norm', 'corr', 'mutual', 'nc', 'proposals', 'prep', 'gather_mid', 'conv1_mid', 'conv2_mid', 'fc_mid',

@@ -11,11 +11,13 @@ CSRC = os.path.join(HERE, 'csrc')
 OUT = os.path.join(HERE, 'libp2p_b200.so')
 SOURCES = ['api.cu', 'coarse.cu', 'refine.cu', 'umma_gemm.cu', 'nc_umma.cu', 'preprocess.cu', 'verify.cu', 'pose.cu', 'degensac.cu',
            'eval.cu', 'hpatches.cu', 'overlap.cu', 'nc_stack.cu', 'topk.cu', 'relpose.cu',
-           'abspose.cu']
+           'abspose.cu', 'sfm.cu']
 HEADERS = ['common.cuh', 'kernels.h', 'ransac_common.cuh', 'verify_common.cuh', 'umma_gemm.h', 'umma_ptx.cuh',
            os.path.join('..', '..', 'include', 'p2p_b200.h')]
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
               '-Xcompiler', '-fPIC,-O2,-fvisibility=hidden', '--threads', '4']
+# sfm.cu rounds every product and sum on its own so that its numpy oracle reproduces it bit for bit
+FILE_FLAGS = {'sfm.cu': ['-fmad=false']}
 
 
 def _nvcc():
@@ -41,7 +43,7 @@ def build(force=False, verbose=False):
     os.makedirs(os.path.join(HERE, 'build'), exist_ok=True)
     for s in SOURCES:
         o = os.path.join(HERE, 'build', s.replace('.cu', '.o'))
-        cmd = [_nvcc()] + NVCC_FLAGS + (['-Xptxas', '-v'] if verbose else []) + ['-c', os.path.join(CSRC, s), '-o', o]
+        cmd = [_nvcc()] + NVCC_FLAGS + FILE_FLAGS.get(s, []) + (['-Xptxas', '-v'] if verbose else []) + ['-c', os.path.join(CSRC, s), '-o', o]
         procs.append((s, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))
         objs.append(o)
     failed = False

@@ -129,7 +129,7 @@ struct p2p_handle_s {
   int opt_nc_l2_mode = 0;       // NC layer 2 block layout: 0 auto, 1 one haloed block per tile, 2 one block per column tap
   int opt_nc_impl = 1;          // 1: NeighConsensus on the tensor cores (nc_umma.cu); 0: fp32 CUDA-core kernels (shape-capped)
   Regressor reg[2];
-  Arena coarse, refine, feat, misc, uniq, pre, verify;
+  Arena coarse, refine, feat, misc, uniq, pre, verify, sfm;
   std::vector<PreprocessCoefs> pre_coefs;   // cached resampling tables, one per image geometry
   PairFeatures pf[2];
   bool prepared = false;
@@ -492,6 +492,7 @@ int p2p_destroy(p2p_handle_t h) {
   h->uniq.release();
   h->pre.release();
   h->verify.release();
+  h->sfm.release();
   for (auto& c : h->pre_coefs)
     if (c.d) cudaFree(c.d);
   for (auto& e : h->prof) { cudaEventDestroy(e.a); cudaEventDestroy(e.b); }
@@ -1896,6 +1897,82 @@ int p2p_lift_scan(p2p_handle_t h, const double* scan, int height, int width, con
   if (n == 0) return 0;
   return launch_lift_scan(scan, height, width, align, matches, match_stride, n, n_dev, rows_out, row_stride, capacity,
                           count_dev, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int p2p_sfm_keypoints(p2p_handle_t h, const double* matches, long long n_matches, const int64_t* offsets, int n_pairs,
+                      const int32_t* pair_img, int both_sides, double merge_px, double* kp_xy, uint64_t* kp_key,
+                      int32_t* kp_of_ep, int64_t* counts, void* stream) {
+  P2P_ENTER(h);
+  P2P_REQUIRE(n_matches >= 0 && n_matches <= (1ll << 30) && n_pairs >= 1 && n_pairs < (1 << 30), "bad match count");
+  P2P_REQUIRE(both_sides == 0 || both_sides == 1, "both_sides must be 0 or 1");
+  P2P_REQUIRE(merge_px > 0.0 && std::isfinite(merge_px), "merge_px must be positive");
+  P2P_REQUIRE(offsets && pair_img && counts && kp_xy && kp_key && kp_of_ep && (matches || n_matches == 0),
+              "null pointer");
+  return launch_sfm_keypoints(h->sfm, matches, n_matches, (const long long*)offsets, n_pairs, pair_img, both_sides,
+                              merge_px, kp_xy, (unsigned long long*)kp_key, kp_of_ep, (long long*)counts,
+                              reinterpret_cast<cudaStream_t>(stream));
+}
+
+int p2p_sfm_undistort(p2p_handle_t h, const double* xy, const uint64_t* kp_key, long long capacity,
+                      const int64_t* n_dev, const int32_t* img_cam, const double* cams, double* xy_out, void* stream) {
+  P2P_ENTER(h);
+  P2P_REQUIRE(capacity >= 0 && capacity <= (1ll << 31), "bad capacity");
+  P2P_REQUIRE((xy && kp_key && img_cam && cams && xy_out) || capacity == 0, "null pointer");
+  return launch_sfm_undistort(xy, (const unsigned long long*)kp_key, capacity, (const long long*)n_dev, img_cam, cams,
+                              xy_out, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int p2p_sfm_tracks(p2p_handle_t h, const int32_t* kp_of_ep, long long n_matches, const int64_t* offsets, int n_pairs,
+                   const double* E, const double* thr, const double* kp_n, long long n_kp, int32_t* labels,
+                   int32_t* obs_kp, int32_t* track_start, int32_t* track_len, int64_t* counts_dev, int64_t* counts_host,
+                   void* stream) {
+  P2P_ENTER(h);
+  P2P_REQUIRE(n_matches >= 0 && n_matches <= (1ll << 30) && n_pairs >= 1 && n_kp >= 0 && n_kp < (1ll << 31) - 1,
+              "bad sizes");
+  P2P_REQUIRE(offsets && counts_dev && counts_host && (n_matches == 0 || (kp_of_ep && E && thr && kp_n)) &&
+                  (n_kp == 0 || (labels && obs_kp && track_start && track_len)),
+              "null pointer");
+  return launch_sfm_tracks(h->sfm, kp_of_ep, n_matches, (const long long*)offsets, n_pairs, E, thr, kp_n, n_kp, labels,
+                           obs_kp, track_start, track_len, (long long*)counts_dev, (long long*)counts_host,
+                           reinterpret_cast<cudaStream_t>(stream));
+}
+
+int p2p_sfm_triangulate(p2p_handle_t h, const int32_t* obs_kp, const int32_t* track_start, const int32_t* track_len,
+                        int n_tracks, long long n_kp, const double* kp_xy, const double* kp_n, const uint64_t* kp_key,
+                        const double* images, const int32_t* img_cam, const double* cams, double reproj_px,
+                        double cos_min_angle, double* points, int32_t* point_len, double* point_err, int32_t* kp_point,
+                        int64_t* counts, void* stream) {
+  P2P_ENTER(h);
+  P2P_REQUIRE(n_tracks >= 0 && n_tracks <= (1 << 27) && n_kp >= 0 && n_kp < (1ll << 31) - 1, "bad sizes");
+  P2P_REQUIRE(reproj_px > 0.0 && std::isfinite(reproj_px), "reproj_px must be positive");
+  P2P_REQUIRE(cos_min_angle > -1.0 && cos_min_angle <= 1.0, "cos_min_angle must lie in (-1, 1]");
+  P2P_REQUIRE(counts && (n_kp == 0 || kp_point) &&
+                  (n_tracks == 0 || (obs_kp && track_start && track_len && kp_xy && kp_n && kp_key && images &&
+                                     img_cam && cams && points && point_len && point_err)),
+              "null pointer");
+  return launch_sfm_triangulate(h->sfm, obs_kp, track_start, track_len, n_tracks, n_kp, kp_xy, kp_n,
+                                (const unsigned long long*)kp_key, images, img_cam, cams, reproj_px,
+                                cos_min_angle, points, point_len, point_err, kp_point,
+                                (long long*)counts, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int p2p_sfm_query_rows(p2p_handle_t h, const double* matches, long long n_matches, const int64_t* offsets, int n_pairs,
+                       const int32_t* pair_img, int n_queries, double merge_px, const int32_t* qkp_of_ep,
+                       const uint64_t* qkp_key, const double* qkp_n, const double* q_intr, const uint64_t* kp_key,
+                       const double* kp_xy, const int32_t* kp_point, long long n_kp, const double* points, double* rows,
+                       int64_t* q_offsets, void* stream) {
+  P2P_ENTER(h);
+  P2P_REQUIRE(n_matches >= 0 && n_matches <= (1ll << 30) && n_pairs >= 1 && n_queries >= 1 &&
+                  n_queries < (1 << 20) && n_kp >= 0 && n_kp < (1ll << 31) - 1,
+              "bad sizes");
+  P2P_REQUIRE(merge_px > 0.0 && std::isfinite(merge_px), "merge_px must be positive");
+  P2P_REQUIRE(q_offsets && (n_matches == 0 || (matches && offsets && pair_img && qkp_of_ep && qkp_key && qkp_n &&
+                                               q_intr && rows && (n_kp == 0 || (kp_key && kp_xy && kp_point && points)))),
+              "null pointer");
+  return launch_sfm_query_rows(h->sfm, matches, n_matches, (const long long*)offsets, n_pairs, pair_img, n_queries,
+                               merge_px, qkp_of_ep, (const unsigned long long*)qkp_key, qkp_n, q_intr,
+                               (const unsigned long long*)kp_key, kp_xy, kp_point, n_kp, points, rows,
+                               (long long*)q_offsets, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int p2p_test_gemm(p2p_handle_t h, const float* a, const float* b, float* c, int M, int N, int K, int passes,

@@ -244,6 +244,28 @@ int launch_test_absolute_pose_hypotheses(const double* rows, int stride, int n, 
 int launch_lift_scan(const double* scan, int H, int W, const double* align, const double* matches, int match_stride,
                      int n, const double* n_dev, double* rows_out, int row_stride, long long cap, double* count_dev,
                      cudaStream_t st);
+// ---- sfm.cu: keypoints, tracks and triangulation against known poses, query 2D-3D rows (semantics in
+// include/p2p_b200.h, p2p_sfm_*).  Scratch comes from `ar` (reserved here, which resets it).
+constexpr int kMaxSfmTrackPoints = 8;   // points (and rounds) per track
+int launch_sfm_keypoints(Arena& ar, const double* m4, long long M, const long long* offsets, int P,
+                         const int* pair_img, int both, double px, double* kp_xy, unsigned long long* kp_key,
+                         int* kp_of_ep, long long* counts, cudaStream_t st);
+int launch_sfm_undistort(const double* xy, const unsigned long long* key, long long cap, const long long* n_dev,
+                         const int* img_cam, const double* cams, double* out, cudaStream_t st);
+// Synchronises once (the hooking convergence check) and copies counts_dev [6] to counts_host.
+int launch_sfm_tracks(Arena& ar, const int* kp_of_ep, long long M, const long long* offsets, int P, const double* E,
+                      const double* thr, const double* kp_n, long long n_kp, int* labels, int* obs_kp, int* start,
+                      int* tlen, long long* counts_dev, long long* counts_host, cudaStream_t st);
+int launch_sfm_triangulate(Arena& ar, const int* obs_kp, const int* start, const int* tlen, int n_tracks,
+                           long long n_kp, const double* kp_xy, const double* kp_n, const unsigned long long* kp_key,
+                           const double* img, const int* img_cam, const double* cams, double reproj_px,
+                           double cos_min, double* pts, int* pt_len, double* pt_err, int* kp_point, long long* counts,
+                           cudaStream_t st);
+int launch_sfm_query_rows(Arena& ar, const double* m4, long long M, const long long* offsets, int P,
+                          const int* pair_img, int n_queries, double px, const int* qkp_of_ep,
+                          const unsigned long long* qkp_key, const double* qkp_n, const double* q_intr,
+                          const unsigned long long* kp_key, const double* kp_xy, const int* kp_point, long long n_kp,
+                          const double* pts, double* rows, long long* q_offsets, cudaStream_t st);
 // ---- relpose.cu: relative-pose statistics of a batch (one block per pair, pairs = B.pairs, any count): pair p writes
 // out[p * out_stride ..] = cos of the rotation and translation-direction errors of Rt_est [p] against Rt_gt [p]
 // (NaN when n_inliers[p] <= 0), then int32 [n_thr + 1]: rows with symmetric epipolar error < thr[j], rows considered.

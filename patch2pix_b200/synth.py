@@ -737,3 +737,138 @@ def inloc_gt_matcher(tree, step=8):
             ok = np.isfinite(xd) & (xd >= 0) & (xd <= w - 1) & (yd >= 0) & (yd <= h - 1)
         return np.stack([u.reshape(-1), v.reshape(-1), xd, yd], 1)[ok].astype(np.float64)
     return matcher
+
+
+def _radial_undistort(f, cx, cy, k, x, y, iters=20):
+    """Normalised rays of distorted pixels under SIMPLE_RADIAL (f, cx, cy, k): Newton on u (1 + k r^2) = x."""
+    xd, yd = (x - cx) / f, (y - cy) / f
+    u, v = xd.copy(), yd.copy()
+    for _ in range(iters):
+        r2 = u * u + v * v
+        a = 1.0 + k * r2
+        fu, fv = u * a - xd, v * a - yd
+        j00, j11, j01 = a + 2 * k * u * u, a + 2 * k * v * v, 2 * k * u * v
+        det = j00 * j11 - j01 * j01
+        u, v = u - (j11 * fu - j01 * fv) / det, v - (j00 * fv - j01 * fu) / det
+    return u, v
+
+
+def _radial_project(cam, R, t, X):
+    f, cx, cy, k = cam
+    P = X @ R.T + t
+    with np.errstate(invalid='ignore', divide='ignore'):
+        u, v = P[..., 0] / P[..., 2], P[..., 1] / P[..., 2]
+    r2 = u * u + v * v
+    return f * u * (1 + k * r2) + cx, f * v * (1 + k * r2) + cy, P[..., 2]
+
+
+def _radial_plane_points(scene, cam, R, t, x, y):
+    """World points on the scene plane seen through distorted pixels (x, y) (NaN behind the camera or off the plane)."""
+    u, v = _radial_undistort(*cam, x, y)
+    ray = np.stack([u, v, np.ones_like(u)], -1) @ R
+    C = -R.T @ t
+    lam = ((scene['O'] - C) @ scene['n']) / (ray @ scene['n'])
+    X = C + lam[..., None] * ray
+    X[lam <= 0] = np.nan
+    return X
+
+
+def synthetic_aachen_tree(root, seed, n_db, n_queries, size=(320, 240), focal=180.0, k=-0.05, db_neighbours=3,
+                          query_neighbours=3):
+    """Seeded Aachen-layout tree under `root`, in metres: a textured plane 10 m wide through the origin, seen from 5-7 m
+    by SIMPLE_RADIAL cameras (f = focal, principal point at the centre, k != 0), written as
+      images/db/{i:04d}.png, images/query/{k:04d}.png: PNG images rendered with the distortion;
+      model/cameras.bin, images.bin: the database cameras and poses (write_colmap_model; no 2D points);
+      db_pairs.txt: each database image with its next db_neighbours along the row of cameras;
+      query_pairs.txt: each query with its query_neighbours nearest database images (camera centres);
+      queries.txt: 'name SIMPLE_RADIAL w h f cx cy k' per query;  gt_poses.txt: the queries' poses (localize's format,
+      file names without their directory).
+    -> dict(images, model, db_pairs, query_pairs, queries, gt, cams {name: (f, cx, cy, k)}, poses {name: (R, t)},
+    scene)."""
+    from PIL import Image
+    rng = np.random.default_rng([int(seed), 47])
+    w, h = (int(v) for v in size)
+    canvas_px = 1024
+    low = rng.integers(0, 256, size=(canvas_px // 8 + 2, canvas_px // 8 + 2, 3), dtype=np.int32)
+    base = np.repeat(np.repeat(low, 8, 0), 8, 1)[:canvas_px + 4, :canvas_px + 4]
+    base = (base[:canvas_px, :canvas_px] + base[4:, :canvas_px] + base[:canvas_px, 4:] + base[4:, 4:]) // 4
+    canvas = np.clip(base + rng.integers(-12, 13, size=base.shape), 0, 255).astype(np.uint8)
+    nrm = np.array([rng.uniform(-0.1, 0.1), 1.0, rng.uniform(-0.1, 0.1)])
+    nrm /= np.linalg.norm(nrm)
+    e1 = np.cross(np.array([0.0, 0.0, 1.0]), nrm)
+    e1 /= np.linalg.norm(e1)
+    scene = dict(O=np.zeros(3), n=nrm, e1=e1, e2=np.cross(nrm, e1), texel=10.0 / canvas_px, canvas=canvas)
+    cam = (float(focal), w / 2.0, h / 2.0, float(k))
+    root = str(root)
+    for d in ('images/db', 'images/query', 'model'):
+        os.makedirs(os.path.join(root, d), exist_ok=True)
+    v, u = np.mgrid[0:h, 0:w].astype(np.float64)
+
+    def render(R, t):
+        X = _radial_plane_points(scene, cam, R, t, u, v)
+        a = ((X - scene['O']) @ scene['e1']) / scene['texel'] + canvas_px / 2
+        b = ((X - scene['O']) @ scene['e2']) / scene['texel'] + canvas_px / 2
+        with np.errstate(invalid='ignore'):
+            ai, bi = np.floor(a + 0.5), np.floor(b + 0.5)
+            ok = (ai >= 0) & (ai < canvas_px) & (bi >= 0) & (bi < canvas_px)
+        img = np.zeros((h, w, 3), dtype=np.uint8)
+        img[ok] = canvas[bi[ok].astype(np.int64), ai[ok].astype(np.int64)]
+        return img
+
+    def camera(off):
+        C = scene['n'] * rng.uniform(5.0, 7.0) + scene['e1'] * off[0] + scene['e2'] * off[1]
+        T = scene['e1'] * (0.6 * off[0]) + scene['e2'] * (0.6 * off[1]) + rng.uniform(-0.2, 0.2, 3)
+        R = _look_at(C, T, rng.uniform(-0.1, 0.1))
+        return R, -R @ C
+    poses, cams, db_imgs, centres = {}, {}, [], []
+    for i in range(n_db):
+        name = f'db/{i:04d}.png'
+        off = np.array([-2.0 + 4.0 * i / max(n_db - 1, 1), rng.uniform(-0.5, 0.5)])
+        R, t = camera(off)
+        Image.fromarray(render(R, t)).save(os.path.join(root, 'images', name), format='PNG')
+        poses[name], cams[name] = (R, t), cam
+        db_imgs.append((i + 1, _quat(R), t, 1, name))
+        centres.append(-R.T @ t)
+    write_colmap_model(os.path.join(root, 'model'), [(1, 2, w, h, list(cam))], db_imgs)
+    names = [d[4] for d in db_imgs]
+    with open(os.path.join(root, 'db_pairs.txt'), 'w') as f:
+        for i in range(n_db):
+            for j in range(i + 1, min(n_db, i + 1 + db_neighbours)):
+                f.write(f'{names[i]} {names[j]}\n')
+    qlines, plines, glines = [], [], []
+    centres = np.array(centres)
+    for q in range(n_queries):
+        name = f'query/{q:04d}.png'
+        R, t = camera(np.array([rng.uniform(-1.6, 1.6), rng.uniform(-0.4, 0.4)]))
+        Image.fromarray(render(R, t)).save(os.path.join(root, 'images', name), format='PNG')
+        poses[name], cams[name] = (R, t), cam
+        qlines.append(f'{name} SIMPLE_RADIAL {w} {h} ' + ' '.join('%.17g' % x for x in cam))
+        near = np.argsort(np.linalg.norm(centres - (-R.T @ t), axis=1), kind='stable')[:query_neighbours]
+        plines += [f'{name} {names[j]}' for j in near]
+        glines.append(' '.join([os.path.basename(name)] + ['%.17g' % x for x in np.concatenate([_quat(R), t])]))
+    out = dict(images=os.path.join(root, 'images'), model=os.path.join(root, 'model'),
+               db_pairs=os.path.join(root, 'db_pairs.txt'), query_pairs=os.path.join(root, 'query_pairs.txt'),
+               queries=os.path.join(root, 'queries.txt'), gt=os.path.join(root, 'gt_poses.txt'), cams=cams,
+               poses=poses, scene=scene)
+    for key, lines in (('query_pairs', plines), ('queries', qlines), ('gt', glines)):
+        with open(out[key], 'w') as f:
+            f.write('\n'.join(lines) + '\n')
+    return out
+
+
+def aachen_gt_matcher(tree, step=8):
+    """Callable (path0, path1) -> [N, 4] exact correspondences of a synthetic_aachen_tree: a pixel grid of image 0,
+    its plane points projected, with the distortion, into image 1 and kept inside it."""
+    def matcher(p0, p1):
+        n0 = next(k for k in tree['poses'] if p0.endswith(k))
+        n1 = next(k for k in tree['poses'] if p1.endswith(k))
+        c0, c1 = tree['cams'][n0], tree['cams'][n1]
+        w, h = int(round(2 * c0[1])), int(round(2 * c0[2]))
+        v, u = np.mgrid[0:h:step, 0:w:step].astype(np.float64)
+        u, v = u.reshape(-1) + 0.5, v.reshape(-1) + 0.5
+        X = _radial_plane_points(tree['scene'], c0, *tree['poses'][n0], u, v)
+        x1, y1, z1 = _radial_project(c1, *tree['poses'][n1], X)
+        with np.errstate(invalid='ignore'):
+            ok = np.isfinite(x1) & (z1 > 0) & (x1 >= 0) & (x1 <= 2 * c1[1] - 1) & (y1 >= 0) & (y1 <= 2 * c1[2] - 1)
+        return np.stack([u, v, x1, y1], 1)[ok]
+    return matcher
