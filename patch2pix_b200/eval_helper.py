@@ -7,11 +7,14 @@ in one kernel and the result crosses PCIe in ONE copy.  `estimate_matches_from_f
 file-format decode stays on the host, resize / ToTensor / Normalize run on the GPU (patch2pix_b200.preprocess).
 """
 from argparse import Namespace
+from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import torch
 
 from .model import Patch2PixB200
+
+MAX_THRESHOLDS = 16       # kMaxHomThresholds / kMaxRelposeThresholds of the statistics kernels
 
 
 def load_model(state_dict, regressor_config=None, device='cuda:0', method='patch2pix'):
@@ -165,6 +168,91 @@ def estimate_matches_from_files(net, im1_path, im2_path, ksize=2, ncn_thres=0.0,
     im2, sc2 = load_im_flexible(im2_path, ksize, net.upsample, imsize=imsize, device=net.device, handle=net._handle)
     return estimate_matches(net, im1.unsqueeze(0), im2.unsqueeze(0), sc1, sc2, ksize, ncn_thres, mutual, io_thres, eval_type,
                             verify)
+
+
+# ---- the evaluation protocols' pair runner -------------------------------------------------------------------------
+def check_thresholds(values, what='thresholds'):
+    """A threshold list as float64: 1..MAX_THRESHOLDS finite, positive, strictly increasing values, else ValueError."""
+    t = np.asarray([float(v) for v in values], dtype=np.float64)
+    if not (1 <= t.size <= MAX_THRESHOLDS and np.all(np.isfinite(t)) and np.all(t > 0) and np.all(np.diff(t) > 0)):
+        raise ValueError(f'{what} must be 1..{MAX_THRESHOLDS} finite, positive, strictly increasing values, got '
+                         f'{list(values)}')
+    return t
+
+
+def as_rows(out, dev):
+    """Matches as a matcher returns them (numpy or a tensor, or a tuple whose first element is those) -> contiguous
+    [N, 4] float64 rows on `dev`; ValueError on any other shape."""
+    if isinstance(out, tuple):
+        out = out[0]
+    if isinstance(out, torch.Tensor):
+        rows = out.detach().to(device=dev, dtype=torch.float64)
+    else:
+        rows = torch.from_numpy(np.ascontiguousarray(out, dtype=np.float64)).to(dev)
+    if rows.numel() == 0:
+        rows = rows.reshape(0, 4)
+    if rows.dim() != 2 or rows.shape[1] != 4:
+        raise ValueError(f'matches must be [N, 4] rows (x0, y0, x1, y1), got shape {tuple(rows.shape)}')
+    return rows.contiguous()
+
+
+def prefetch(items, load):
+    """Yields (i, load(items[i]), or the exception it raised) for the items in order; `load` runs on one worker thread,
+    one item ahead of the item being yielded."""
+    items = list(items)
+    with ThreadPoolExecutor(max_workers=1) as pool:
+        nxt = pool.submit(load, items[0]) if items else None
+        for i in range(len(items)):
+            cur = nxt
+            nxt = pool.submit(load, items[i + 1]) if i + 1 < len(items) else None
+            try:
+                got = cur.result()
+            except Exception as e:
+                got = e
+            yield i, got
+
+
+class PairRunner:
+    """Runs a matcher on image pairs for the evaluation protocols: a Patch2PixB200 (put in eval mode) as
+    estimate_matches_from_files(..., ksize, ncn_thres, True, io_thres, eval_type, imsize) runs it, or any callable
+    (path0, path1) -> [N, 4] rows.  `dev` and `h` are the device and handle the protocol's own launches use."""
+
+    def __init__(self, matcher, ksize=2, eval_type='fine', io_thres=0.25, ncn_thres=0.0, imsize=1024):
+        from . import _lib
+        self.matcher = matcher
+        self.is_net = isinstance(matcher, Patch2PixB200)
+        self.ksize, self.eval_type, self.io_thres, self.ncn_thres, self.imsize = (ksize, eval_type, io_thres,
+                                                                                  ncn_thres, imsize)
+        if self.is_net:
+            matcher.eval()
+            self.dev, self.h = matcher.device, matcher._handle
+        else:
+            self.dev = torch.device('cuda', torch.cuda.current_device())
+            self.h = _lib.default_handle(self.dev)
+
+    def decode(self, paths):
+        """The image files as pinned RGB uint8 tensors [H, W, 3] for the net; None for a callable, which reads its
+        own files."""
+        if not self.is_net:
+            return None
+        from PIL import Image
+        return [torch.from_numpy(np.array(Image.open(p).convert('RGB'))).pin_memory() for p in paths]
+
+    def prepare(self, rgb):
+        """A decoded image -> (x [1, 3, H, W] on the device, scale), the input of match."""
+        from .preprocess import preprocess_image
+        x, scale = preprocess_image(rgb, self.ksize, self.matcher.upsample, self.imsize, self.dev, self.h)
+        return x.unsqueeze(0), scale
+
+    def match(self, a, b, verify=None):
+        """match_device on two prepared images -> (packed, n), without a host sync."""
+        packed, n, _ = match_device(self.matcher, a[0], b[0], a[1], b[1], self.ksize, self.ncn_thres, True,
+                                    self.io_thres, self.eval_type, verify)
+        return packed, n
+
+    def call(self, path0, path1):
+        """The callable on two image files -> [N, 4] float64 rows on the device."""
+        return as_rows(self.matcher(path0, path1), self.dev)
 
 
 def refine_matches(im1_path, im2_path, net, coarse_matcher, io_thres=0.0, imsize=None, coarse_only=False):

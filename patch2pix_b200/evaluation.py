@@ -18,13 +18,13 @@ import os
 import struct
 import time
 from argparse import Namespace
-from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import torch
 
 from . import _lib
 from . import pose as P
+from .eval_helper import PairRunner, prefetch
 from .verify import epipolar_histograms_into
 
 EVAL_BINS = [0, 1e-2, 1, 5, 10, 25, 50, 100, 2500, 1e5]      # eval_epoch_immatch.py:85
@@ -230,46 +230,33 @@ def _rec_len(n_edges):
     return _REC_POSE + (3 * n_edges + 1) // 2
 
 
-def _decode(paths):
-    from PIL import Image
-    return [torch.from_numpy(np.array(Image.open(p).convert('RGB'))).pin_memory() for p in paths]
-
-
 def eval_pairs(net, pairs, ksize=2, eval_type='fine', io_thres=0.5, ncn_thres=0.0, imsize=1024, rthres=0.5,
                bins=EVAL_BINS):
     """The per-pair work of eval_epoch_immatch.py:39-80 on an explicit pair list [(im1_path, im2_path, im1, im2)], im1
     and im2 the load_model_ims records -> one Namespace per pair: status ('ok', 'match_failed', 'geo_failed'), N,
     n_inls, R, t, counts (int32 [3, len(bins)]: cdist, fdist, indist histograms, each ending with its sample size),
     terr, qerr (degrees; None where the reference has none)."""
-    from .eval_helper import match_device
-    from .preprocess import preprocess_image
-    dev = net.device
-    h = net._handle
+    run = PairRunner(net, ksize, eval_type, io_thres, ncn_thres, imsize)
     n_edges = len(bins)
-    table = torch.zeros(len(pairs), _rec_len(n_edges), dtype=torch.float64, device=dev)
+    table = torch.zeros(len(pairs), _rec_len(n_edges), dtype=torch.float64, device=run.dev)
     gts, failed = [], set()
-    with ThreadPoolExecutor(max_workers=1) as pool:
-        nxt = pool.submit(_decode, pairs[0][:2]) if pairs else None
-        for i, (p1, p2, im1, im2) in enumerate(pairs):
-            t_gt, q_gt = P.abs2relapose(im1.c, im2.c, im1.q, im2.q)
-            F = P.pose2fund(im1.K, im2.K, P.quat2mat(q_gt), t_gt)
-            gts.append((t_gt, q_gt))
-            cur = nxt
-            nxt = pool.submit(_decode, pairs[i + 1][:2]) if i + 1 < len(pairs) else None
-            try:
-                rgb1, rgb2 = cur.result()
-                x1, sc1 = preprocess_image(rgb1, ksize, net.upsample, imsize, dev, h)
-                x2, sc2 = preprocess_image(rgb2, ksize, net.upsample, imsize, dev, h)
-                packed, n, _ = match_device(net, x1.unsqueeze(0), x2.unsqueeze(0), sc1, sc2, ksize, ncn_thres, True,
-                                            io_thres, eval_type, ('E', rthres, im1.K, im2.K))
-            except Exception:
-                failed.add(i)
-                continue
-            rec = table[i]
-            epipolar_histograms_into(h, packed, 9, n, C.c_void_p(packed.data_ptr() + n * 9 * 8), 5, F,
-                                     C.c_void_p(packed.data_ptr() + (n * 9 + 1) * 8 + 184), bins,
-                                     C.c_void_p(rec.data_ptr() + _REC_POSE * 8))
-            rec[:_REC_POSE].copy_(packed[n * 9:n * 9 + _REC_POSE])
+    for i, ims in prefetch(pairs, lambda p: run.decode(p[:2])):
+        _, _, im1, im2 = pairs[i]
+        t_gt, q_gt = P.abs2relapose(im1.c, im2.c, im1.q, im2.q)
+        F = P.pose2fund(im1.K, im2.K, P.quat2mat(q_gt), t_gt)
+        gts.append((t_gt, q_gt))
+        try:
+            if isinstance(ims, Exception):
+                raise ims
+            packed, n = run.match(run.prepare(ims[0]), run.prepare(ims[1]), ('E', rthres, im1.K, im2.K))
+        except Exception:
+            failed.add(i)
+            continue
+        rec = table[i]
+        epipolar_histograms_into(run.h, packed, 9, n, C.c_void_p(packed.data_ptr() + n * 9 * 8), 5, F,
+                                 C.c_void_p(packed.data_ptr() + (n * 9 + 1) * 8 + 184), bins,
+                                 C.c_void_p(rec.data_ptr() + _REC_POSE * 8))
+        rec[:_REC_POSE].copy_(packed[n * 9:n * 9 + _REC_POSE])
     host = table.cpu().numpy()                        # the run's one copy of the records
     return [parse_record(None if i in failed else host[i], t_gt, q_gt, n_edges) for i, (t_gt, q_gt) in enumerate(gts)]
 

@@ -28,16 +28,16 @@ import ctypes as C
 import os
 import time
 from argparse import Namespace
-from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import torch
 
 from . import _lib
+from . import verify as V
+from .eval_helper import PairRunner, as_rows, check_thresholds, prefetch
 
 D2NET_EXCLUDED = ('i_contruction', 'i_crownnight', 'i_dc', 'i_pencils', 'i_whitebuilding', 'v_artisans',
                   'v_astronautis', 'v_talent')
-MAX_THRESHOLDS = 16
 
 # A record is one float64 row of the device table: the kept-match count N, the find_model buffer up to its int32
 # inlier count (H [9], count in the low half of element 10), the corner error, then the int32 counts [n_thr + 1] of
@@ -88,14 +88,6 @@ def read_hpatches(data_root, exclude=D2NET_EXCLUDED):
     return seqs
 
 
-def _thresholds(thresholds, what='thresholds'):
-    t = np.asarray([float(v) for v in thresholds], dtype=np.float64)
-    if not (1 <= t.size <= MAX_THRESHOLDS and np.all(np.isfinite(t)) and np.all(t > 0) and np.all(np.diff(t) > 0)):
-        raise ValueError(f'{what} must be 1..{MAX_THRESHOLDS} finite, positive, strictly increasing values, got '
-                         f'{list(thresholds)}')
-    return t
-
-
 def homography_errors_into(handle, rows, row_stride, n, n_dev, H_gt, H_pred_ptr, width, height, thresholds,
                            counts_ptr, corner_ptr):
     """Enqueue p2p_homography_errors on `rows` (a float64 device tensor, row r at offset r * row_stride) with H_gt and
@@ -123,7 +115,7 @@ def homography_errors(rows, H_gt, H_pred_buf, width, height, thresholds=range(1,
             and H_pred_buf.is_contiguous() and H_pred_buf.numel() >= 10 and H_pred_buf.device == rows.device):
         raise ValueError('H_pred_buf must be a contiguous CUDA float64 find_model buffer of at least 10 elements on '
                          'the device of rows')
-    t = _thresholds(thresholds)
+    t = check_thresholds(thresholds)
     rows = rows.contiguous()
     n, stride = int(rows.shape[0]), int(rows.shape[1])
     counts = torch.empty(t.size + 1, dtype=torch.int32, device=rows.device)
@@ -135,11 +127,6 @@ def homography_errors(rows, H_gt, H_pred_buf, width, height, thresholds=range(1,
     return counts, corner
 
 
-def _decode(paths):
-    from PIL import Image
-    return [torch.from_numpy(np.array(Image.open(p).convert('RGB'))).pin_memory() for p in paths]
-
-
 def _record_into(h, rec, rows, row_stride, n, n_dev, seq, k, buf, thresholds):
     """The pair's statistics into its table row `rec`: p2p_homography_errors on the rows, then the count and the
     find_model buffer (`buf`: N followed by that buffer) copied device to device."""
@@ -147,77 +134,6 @@ def _record_into(h, rec, rows, row_stride, n, n_dev, seq, k, buf, thresholds):
                            seq.size[0], seq.size[1], thresholds, C.c_void_p(rec.data_ptr() + _REC_COUNTS * 8),
                            C.c_void_p(rec.data_ptr() + _REC_CORNER * 8))
     rec[:_REC_CORNER].copy_(buf[:_REC_CORNER])
-
-
-def _eval_net(net, pairs, table, ksize, eval_type, io_thres, ncn_thres, imsize, ransac_thres, thresholds):
-    """Patch2PixB200: image 1 of a sequence is decoded and preprocessed once; every decode runs on a worker thread one
-    pair ahead; each pair goes through match_device(verify=('H', ransac_thres)) and p2p_homography_errors reads the
-    packed rows in place.  -> {pair index: error text} of the pairs whose matcher raised."""
-    from .eval_helper import match_device
-    from .preprocess import preprocess_image
-    dev, h = net.device, net._handle
-    failed = {}
-    jobs = [seq.paths[:1] + [seq.paths[k - 1]] if k == 2 else [seq.paths[k - 1]] for seq, k in pairs]
-    x1 = sc1 = None
-    with ThreadPoolExecutor(max_workers=1) as pool:
-        nxt = pool.submit(_decode, jobs[0]) if jobs else None
-        for i, (seq, k) in enumerate(pairs):
-            cur = nxt
-            nxt = pool.submit(_decode, jobs[i + 1]) if i + 1 < len(jobs) else None
-            if k == 2:
-                x1 = sc1 = None
-            try:
-                ims = cur.result()
-                if k == 2:
-                    x1, sc1 = preprocess_image(ims[0], ksize, net.upsample, imsize, dev, h)
-                if x1 is None:
-                    raise RuntimeError(f'{seq.paths[0]} could not be loaded')
-                x2, sc2 = preprocess_image(ims[-1], ksize, net.upsample, imsize, dev, h)
-                packed, n, _ = match_device(net, x1.unsqueeze(0), x2.unsqueeze(0), sc1, sc2, ksize, ncn_thres, True,
-                                            io_thres, eval_type, ('H', ransac_thres))
-            except Exception as e:
-                failed[i] = f'{type(e).__name__}: {e}'
-                continue
-            _record_into(h, table[i], packed, 9, n, C.c_void_p(packed.data_ptr() + n * 9 * 8), seq, k,
-                         packed[n * 9:], thresholds)
-    return failed
-
-
-def _as_rows(out, dev):
-    """A matcher's return value -> [N, 4] float64 rows on `dev`."""
-    if isinstance(out, tuple):
-        out = out[0]
-    if isinstance(out, torch.Tensor):
-        rows = out.detach().to(device=dev, dtype=torch.float64)
-    else:
-        rows = torch.from_numpy(np.ascontiguousarray(out, dtype=np.float64)).to(dev)
-    if rows.numel() == 0:
-        rows = rows.reshape(0, 4)
-    if rows.dim() != 2 or rows.shape[1] != 4:
-        raise ValueError(f'a matcher returns [N, 4] rows (x1, y1, x2, y2), got shape {tuple(rows.shape)}')
-    return rows.contiguous()
-
-
-def _eval_callable(matcher, pairs, table, ransac_thres, thresholds):
-    """Any callable (im1_path, im2_path) -> [N, 4] rows: the rows go through find_model_into(MODEL_H) and
-    p2p_homography_errors.  -> {pair index: error text} of the pairs whose matcher raised."""
-    from . import verify as V
-    dev = table.device
-    h = _lib.default_handle(dev)
-    failed = {}
-    for i, (seq, k) in enumerate(pairs):
-        try:
-            out = matcher(seq.paths[0], seq.paths[k - 1])
-        except Exception as e:
-            failed[i] = f'{type(e).__name__}: {e}'
-            continue
-        rows = _as_rows(out, dev)
-        n = int(rows.shape[0])
-        buf = torch.empty(1 + V.out_size(n), dtype=torch.float64, device=dev)
-        buf[0].fill_(float(n))
-        V.find_model_into(h, V.MODEL_H, rows, 4, n, None, ransac_thres, 0.999, 10000, 0, buf[1:])
-        _record_into(h, table[i], rows, 4, n, None, seq, k, buf, thresholds)
-    return failed
 
 
 def parse_record(row, seq, k, n_thr, failed=False):
@@ -263,29 +179,51 @@ def eval_hpatches(matcher, data_root, ksize=2, eval_type='fine', io_thres=0.25, 
     -> dict(mma={'all', 'i', 'v'} -> float64 [len(thresholds)], h_acc={'all', 'i', 'v'} -> float64
     [len(h_thresholds)], n_pairs, h_failed (pairs without a finite corner error), records: one Namespace per pair
     (seq, k, N, n_inliers, corner_err, counts, match_failed), thresholds, h_thresholds, time)."""
-    from .model import Patch2PixB200
-    thr = _thresholds(thresholds)
-    h_thr = _thresholds(h_thresholds, 'h_thresholds')
+    thr = check_thresholds(thresholds)
+    h_thr = check_thresholds(h_thresholds, 'h_thresholds')
     if not (ransac_thres > 0 and np.isfinite(ransac_thres)):
         raise ValueError('ransac_thres must be positive')
     seqs = read_hpatches(data_root, exclude)
     pairs = [(seq, k) for seq in seqs for k in range(2, 7)]
-    is_net = isinstance(matcher, Patch2PixB200)
+    run = PairRunner(matcher, ksize, eval_type, io_thres, ncn_thres, imsize)
     n_i = sum(s.split == 'i' for s in seqs)
     lprint_(f'\n>>Eval on HPatches: {len(seqs)} sequences ({n_i} i / {len(seqs) - n_i} v), {len(pairs)} pairs, '
-            + (f'eval_type={eval_type} ksize={ksize} io={io_thres} nc={ncn_thres} im={imsize} ' if is_net else '')
+            + (f'eval_type={eval_type} ksize={ksize} io={io_thres} nc={ncn_thres} im={imsize} ' if run.is_net else '')
             + f'rthres={ransac_thres}')
-    if is_net:
-        matcher.eval()
-        dev = matcher.device
-    else:
-        dev = torch.device('cuda', torch.cuda.current_device())
     start = time.time()
-    table = torch.zeros(len(pairs), _rec_len(thr.size), dtype=torch.float64, device=dev)
-    if is_net:
-        failed = _eval_net(matcher, pairs, table, ksize, eval_type, io_thres, ncn_thres, imsize, ransac_thres, thr)
-    else:
-        failed = _eval_callable(matcher, pairs, table, ransac_thres, thr)
+    table = torch.zeros(len(pairs), _rec_len(thr.size), dtype=torch.float64, device=run.dev)
+    failed = {}
+    x1 = None
+
+    def load(pair):             # image 1 is decoded, and prepared, once per sequence
+        seq, k = pair
+        return run.decode(seq.paths[:1] + [seq.paths[k - 1]] if k == 2 else [seq.paths[k - 1]])
+    for i, ims in prefetch(pairs, load):
+        seq, k = pairs[i]
+        if k == 2:
+            x1 = None
+        try:
+            if isinstance(ims, Exception):
+                raise ims
+            if run.is_net:          # the packed rows, their device count and the RANSAC buffer, read in place
+                if k == 2:
+                    x1 = run.prepare(ims[0])
+                if x1 is None:
+                    raise RuntimeError(f'{seq.paths[0]} could not be loaded')
+                rows, n = run.match(x1, run.prepare(ims[-1]), ('H', ransac_thres))
+                stride, n_dev, buf = 9, C.c_void_p(rows.data_ptr() + n * 9 * 8), rows[n * 9:]
+            else:
+                rows = matcher(seq.paths[0], seq.paths[k - 1])
+        except Exception as e:
+            failed[i] = f'{type(e).__name__}: {e}'
+            continue
+        if not run.is_net:          # rows of the wrong shape raise rather than fail the pair
+            rows = as_rows(rows, run.dev)
+            n, stride, n_dev = int(rows.shape[0]), 4, None
+            buf = torch.empty(1 + V.out_size(n), dtype=torch.float64, device=run.dev)
+            buf[0].fill_(float(n))
+            V.find_model_into(run.h, V.MODEL_H, rows, 4, n, None, ransac_thres, 0.999, 10000, 0, buf[1:])
+        _record_into(run.h, table[i], rows, stride, n, n_dev, seq, k, buf, thr)
     host = table.cpu().numpy()                        # the run's one copy of the records
     runtime = time.time() - start
     records = [parse_record(host[i], seq.name, k, thr.size, i in failed) for i, (seq, k) in enumerate(pairs)]

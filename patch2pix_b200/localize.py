@@ -30,12 +30,12 @@ come back in one copy at the end.  The result does not depend on chunk_queries.
 import ctypes as C
 import os
 import time
-from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import torch
 
 from . import _lib
+from .eval_helper import PairRunner, prefetch
 
 INLOC_FOCAL = 4032.0 * 28.0 / 36.0
 ENTRY_ABSPOSE = 3                  # p2p_batch_chunk_pairs entry of p2p_find_absolute_pose_batch
@@ -353,19 +353,61 @@ def eval_localization(results, gt, thresholds=((0.25, 10), (0.5, 10), (1.0, 10))
 
 
 # ---- the protocol ------------------------------------------------------------------------------------------------------
-def _load_query(data_root, q, net):
-    from PIL import Image
-    im = Image.open(os.path.join(data_root, q))
-    w, h = im.size
-    return (w, h), (np.asarray(im.convert('RGB')) if net else None)
+class AbsPoseTable:
+    """The absolute-pose records of nq queries on the device, one float64 row each: R|t [12], then the int32 inlier
+    count in element 12 (0 or less: no model)."""
+
+    def __init__(self, nq, dev):
+        self.table = torch.zeros(max(nq, 1), 13, dtype=torch.float64, device=dev)
+
+    def solve(self, k0, handle, rows, offsets, offsets_host, n_dev, intr_ptr, px_th, conf, max_iters):
+        """find_absolute_pose_batch_into on the queries k0 .. k0 + K - 1 of a chunk (rows of stride 5, K + 1 offsets,
+        intrinsics [K][4] at intr_ptr) into their records, without a host sync."""
+        K, dev = len(offsets_host) - 1, self.table.device
+        mask = torch.empty(int(offsets_host[-1]) + 1, dtype=torch.uint8, device=dev)
+        cnt = torch.empty(K, dtype=torch.int32, device=dev)
+        rt = torch.empty(K, 12, dtype=torch.float64, device=dev)
+        find_absolute_pose_batch_into(handle, rows, 5, offsets, offsets_host, n_dev, intr_ptr, px_th, None, conf,
+                                      max_iters, 0, rt.data_ptr(), mask.data_ptr(), cnt.data_ptr())
+        self.table[k0:k0 + K, :12].copy_(rt)
+        self.table[k0:k0 + K, 12:13].view(torch.int32)[:, 0].copy_(cnt)
+
+    def finish(self, queries, failed, results_path):
+        """One copy of the table -> {file name: (R, t, n_inliers)} of the queries (paths, in table order), written to
+        the results file.  A query without a model is added to `failed` ({index: reason}) as 'no model'; every failed
+        query gets the identity pose."""
+        host = self.table.cpu().numpy()
+        poses, out = {}, []
+        for i, q in enumerate(queries):
+            cnt = int(host[i, 12:13].view(np.int32)[0])
+            R, t = host[i, :9].reshape(3, 3).copy(), host[i, 9:12].copy()
+            if i not in failed and cnt <= 0:
+                failed[i] = 'no model'
+            if i in failed:
+                R, t = np.eye(3), np.zeros(3)
+            name = os.path.basename(q)
+            poses[name] = (R, t, cnt)
+            out.append((name, R, t))
+        write_results(results_path, out)
+        return poses
 
 
-def _load_db(data_root, db, net):
+def _load_query(data_root, q, run):
+    """((width, height), the decoded image for the net or None)."""
     from PIL import Image
+    path = os.path.join(data_root, q)
+    if run.is_net:
+        rgb = run.decode([path])[0]
+        return (int(rgb.shape[1]), int(rgb.shape[0])), rgb
+    with Image.open(path) as im:
+        return im.size, None
+
+
+def _load_db(data_root, db, run):
     scan = torch.from_numpy(read_scan(os.path.join(data_root, db + '.mat'))).pin_memory()
     align = read_alignment(alignment_path(data_root, db))
-    img = np.asarray(Image.open(os.path.join(data_root, db)).convert('RGB')) if net else None
-    return scan, align, img
+    img = run.decode([os.path.join(data_root, db)])
+    return scan, align, None if img is None else img[0]
 
 
 class _Block:
@@ -396,27 +438,20 @@ def localize_inloc(matcher, data_root, pairs, results_path, ksize=2, eval_type='
     those).  `pairs` is a retrieval-list file or a list as read_retrieval returns it.
 
     -> dict(poses={query name: (R, t, n_inliers)}, failed=[(query, reason)], n_queries, time)."""
-    from .model import Patch2PixB200
     if not (ransac_thres > 0 and np.isfinite(ransac_thres)):
         raise ValueError('ransac_thres must be positive')
     if int(chunk_queries) < 1:
         raise ValueError('chunk_queries must be at least 1')
     retrieval = read_retrieval(pairs) if isinstance(pairs, (str, os.PathLike)) else list(pairs)
-    is_net = isinstance(matcher, Patch2PixB200)
-    if is_net:
-        matcher.eval()
-        dev = matcher.device
-    else:
-        dev = torch.device('cuda', torch.cuda.current_device())
+    run = PairRunner(matcher, ksize, eval_type, io_thres, 0.0, imsize)
+    dev = run.dev
     lprint_(f'\n>>Localize InLoc: {len(retrieval)} queries, {sum(len(d) for _, d in retrieval)} pairs, '
             f'rthres={ransac_thres}')
     start = time.time()
-    h = matcher._handle if is_net else _lib.default_handle(dev)
     nq = len(retrieval)
-    table = torch.zeros(max(nq, 1), 13, dtype=torch.float64, device=dev)     # R|t [12], int32 count in element 12
+    table = AbsPoseTable(nq, dev)
     failed = {}
-    jobs = [(i, db) for i, (_, dbs) in enumerate(retrieval) for db in dbs]
-    chunk = []
+    chunk, k0 = [], 0
 
     def flush(k0):
         K = len(chunk)
@@ -430,84 +465,52 @@ def localize_inloc(matcher, data_root, pairs, results_path, ksize=2, eval_type='
         n_t = torch.cat([b.count for b, _ in chunk])
         intr = np.stack([c for _, c in chunk]).reshape(-1)
         ex = torch.from_numpy(np.concatenate([intr, offsets.view(np.float64)])).pin_memory().to(dev, non_blocking=True)
-        mask = torch.empty(N + 1, dtype=torch.uint8, device=dev)
-        cnt = torch.empty(K, dtype=torch.int32, device=dev)
-        rt = torch.empty(K, 12, dtype=torch.float64, device=dev)
-        find_absolute_pose_batch_into(h, rows, 5, ex[4 * K:].view(torch.int64), offsets, C.c_void_p(n_t.data_ptr()),
-                                      ex.data_ptr(), ransac_thres, None, conf, max_iters, 0, rt.data_ptr(),
-                                      mask.data_ptr(), cnt.data_ptr())
-        table[k0:k0 + K, :12].copy_(rt)
-        table[k0:k0 + K, 12:13].view(torch.int32)[:, 0].copy_(cnt)
+        table.solve(k0, run.h, rows, ex[4 * K:].view(torch.int64), offsets, C.c_void_p(n_t.data_ptr()),
+                    ex.data_ptr(), ransac_thres, conf, max_iters)
         chunk.clear()
 
-    with ThreadPoolExecutor(max_workers=1) as pool:
-        qfut = {0: pool.submit(_load_query, data_root, retrieval[0][0], is_net)} if nq else {}
-        dfut = [pool.submit(_load_db, data_root, jobs[0][1], is_net)] if jobs else []
-        j = 0
-        k0 = 0
-        for i, (q, dbs) in enumerate(retrieval):
-            if i + 1 < nq:
-                qfut[i + 1] = pool.submit(_load_query, data_root, retrieval[i + 1][0], is_net)
-            block = _Block(dev)
-            xq = scq = None
+    # one job per query (None) followed by one per database image; a load runs one job ahead on the worker
+    jobs = [(i, db) for i, (_, dbs) in enumerate(retrieval) for db in [None] + list(dbs)]
+
+    def load(job):
+        i, db = job
+        return _load_query(data_root, retrieval[i][0], run) if db is None else _load_db(data_root, db, run)
+    for j, got in prefetch(jobs, load):
+        i, db = jobs[j]
+        if db is None:
+            block, xq, cam = _Block(dev), None, np.array([INLOC_FOCAL, INLOC_FOCAL, 0.5, 0.5])
+        if i not in failed:
             try:
-                (w, hgt), qimg = qfut.pop(i).result()
-                cam = np.array([INLOC_FOCAL, INLOC_FOCAL, 0.5 * w, 0.5 * hgt])
-                if is_net:
-                    from .preprocess import preprocess_image
-                    xq, scq = preprocess_image(qimg, ksize, matcher.upsample, imsize, dev, h)
-            except Exception as e:
-                failed[i] = f'{type(e).__name__}: {e}'
-                cam = np.array([INLOC_FOCAL, INLOC_FOCAL, 0.5, 0.5])
-            for _ in dbs:
-                cur = dfut.pop(0)
-                if j + 1 < len(jobs):
-                    dfut.append(pool.submit(_load_db, data_root, jobs[j + 1][1], is_net))
-                db = jobs[j][1]
-                j += 1
-                if i in failed:
-                    continue
-                try:
-                    scan_h, align, dimg = cur.result()
-                    if is_net:
-                        from .eval_helper import match_device
-                        from .preprocess import preprocess_image
-                        xd, scd = preprocess_image(dimg, ksize, matcher.upsample, imsize, dev, h)
-                        packed, n, _ = match_device(matcher, xq.unsqueeze(0), xd.unsqueeze(0), scq, scd, ksize, 0.0,
-                                                    True, io_thres, eval_type, None)
+                if isinstance(got, Exception):
+                    raise got
+                if db is None:
+                    (w, hgt), qimg = got
+                    if run.is_net:
+                        xq = run.prepare(qimg)
+                    cam = np.array([INLOC_FOCAL, INLOC_FOCAL, 0.5 * w, 0.5 * hgt])
+                else:
+                    scan_h, align, dimg = got
+                    if run.is_net:
+                        packed, n = run.match(xq, run.prepare(dimg))
                         mt, stride, n_dev = packed, 9, C.c_void_p(packed.data_ptr() + 72 * n)
                     else:
-                        from .hpatches import _as_rows
-                        mt = _as_rows(matcher(os.path.join(data_root, q), os.path.join(data_root, db)), dev)
+                        mt = run.call(os.path.join(data_root, retrieval[i][0]), os.path.join(data_root, db))
                         n, stride, n_dev = int(mt.shape[0]), 4, None
                     if n:
                         scan = scan_h.to(dev, non_blocking=True)
                         block.reserve(n)
-                        lift_scan_into(h, scan, align, mt, stride, n, n_dev, block.rows, 5, block.cap,
+                        lift_scan_into(run.h, scan, align, mt, stride, n, n_dev, block.rows, 5, block.cap,
                                        block.count.data_ptr())
-                except Exception as e:
-                    failed[i] = f'{type(e).__name__}: {e}'
-            if i in failed:
-                block = _Block(dev)
-            chunk.append((block, cam))
+            except Exception as e:
+                failed[i] = f'{type(e).__name__}: {e}'
+        if j + 1 == len(jobs) or jobs[j + 1][1] is None:        # the query's last job
+            chunk.append((_Block(dev) if i in failed else block, cam))
             if len(chunk) == int(chunk_queries):
                 flush(k0)
                 k0 = i + 1
-        flush(k0)
-    host = table.cpu().numpy()                       # the run's one copy of the poses
+    flush(k0)
+    poses = table.finish([q for q, _ in retrieval], failed, results_path)
     runtime = time.time() - start
-    poses, out = {}, []
-    for i, (q, _) in enumerate(retrieval):
-        cnt = int(host[i, 12:13].view(np.int32)[0])
-        R, t = host[i, :9].reshape(3, 3).copy(), host[i, 9:12].copy()
-        if i not in failed and cnt <= 0:
-            failed[i] = 'no model'
-        if i in failed:
-            R, t = np.eye(3), np.zeros(3)
-        name = os.path.basename(q)
-        poses[name] = (R, t, cnt)
-        out.append((name, R, t))
-    write_results(results_path, out)
     lprint_(f'localized {nq - len(failed)} / {nq} queries, time={runtime:.2f}s -> {results_path}')
     return dict(poses=poses, failed=[(retrieval[i][0], failed[i]) for i in sorted(failed)], n_queries=nq,
                 time=runtime)

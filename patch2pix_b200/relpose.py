@@ -35,14 +35,13 @@ import ctypes as C
 import os
 import time
 from argparse import Namespace
-from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import torch
 
 from . import _lib
+from .eval_helper import PairRunner, check_thresholds, prefetch
 
-MAX_THRESHOLDS = 16
 DIST_TH = 1e9             # the protocol's recoverPose(..., 1e9, mask)
 
 # A record is one float64 row of the device table: int32 E-RANSAC inlier count and int32 good-point count in element 0,
@@ -146,14 +145,6 @@ def pair_arrays(pairs, ransac_thres):
     return intr, Rt, px
 
 
-def _thresholds(thresholds, what):
-    t = np.asarray([float(v) for v in thresholds], dtype=np.float64)
-    if not (1 <= t.size <= MAX_THRESHOLDS and np.all(np.isfinite(t)) and np.all(t > 0) and np.all(np.diff(t) > 0)):
-        raise ValueError(f'{what} must be 1..{MAX_THRESHOLDS} finite, positive, strictly increasing values, got '
-                         f'{list(thresholds)}')
-    return t
-
-
 # ---- device entry points -------------------------------------------------------------------------------------------
 def relpose_errors_batch_into(handle, rows, row_stride, offsets, offsets_host, n_dev, intr_ptr, Rt_gt_ptr, Rt_est_ptr,
                               n_inliers_ptr, thresholds, out_ptr, out_stride):
@@ -173,7 +164,7 @@ def relpose_errors(rows_list, intr, Rt_gt, Rt_est, n_inliers, thresholds=(5e-4,)
     intr [K, 8], Rt_gt / Rt_est [K, 12], n_inliers [K] (host arrays or CUDA tensors) -> (cosines float64 CUDA [K, 2]
     (rotation, translation direction; NaN where n_inliers <= 0), counts int32 CUDA [K, len(thresholds) + 1]).  No host
     sync."""
-    t = _thresholds(thresholds, 'thresholds')
+    t = check_thresholds(thresholds)
     K = len(rows_list)
     if K == 0:
         raise ValueError('relpose_errors needs at least one pair')
@@ -244,56 +235,6 @@ class _Table:
         self.k0, self.items = k0 + K, []
 
 
-def _decode(paths):
-    from PIL import Image
-    return [torch.from_numpy(np.array(Image.open(p).convert('RGB'))).pin_memory() for p in paths]
-
-
-def _eval_net(net, pairs, tab, ksize, eval_type, io_thres, ncn_thres, imsize):
-    """Patch2PixB200: both images of the next pair decode on a worker thread while the current pair runs; each pair's
-    packed rows stay on the device (match_device) until its chunk is flushed.  -> {pair index: error text}."""
-    from .eval_helper import match_device
-    from .preprocess import preprocess_image
-    dev, h = net.device, net._handle
-    failed = {}
-    empty = torch.zeros(0, 9, dtype=torch.float64, device=dev)
-    zero = torch.zeros(1, dtype=torch.float64, device=dev)
-    with ThreadPoolExecutor(max_workers=1) as pool:
-        nxt = pool.submit(_decode, [pairs[0].path0, pairs[0].path1]) if pairs else None
-        for i in range(len(pairs)):
-            cur = nxt
-            nxt = pool.submit(_decode, [pairs[i + 1].path0, pairs[i + 1].path1]) if i + 1 < len(pairs) else None
-            try:
-                im0, im1 = cur.result()
-                x0, sc0 = preprocess_image(im0, ksize, net.upsample, imsize, dev, h)
-                x1, sc1 = preprocess_image(im1, ksize, net.upsample, imsize, dev, h)
-                packed, n, _ = match_device(net, x0.unsqueeze(0), x1.unsqueeze(0), sc0, sc1, ksize, ncn_thres, True,
-                                            io_thres, eval_type, None)
-            except Exception as e:
-                failed[i] = f'{type(e).__name__}: {e}'
-                tab.add(empty, zero)
-                continue
-            tab.add(packed[:n * 9].view(n, 9), packed[n * 9:n * 9 + 1])
-    tab.flush()
-    return failed
-
-
-def _eval_callable(matcher, pairs, tab):
-    """Any callable (im0_path, im1_path) -> [N, 4] rows.  -> {pair index: error text}."""
-    from .hpatches import _as_rows
-    failed = {}
-    empty = torch.zeros(0, 4, dtype=torch.float64, device=tab.dev)
-    for i, pr in enumerate(pairs):
-        try:
-            rows = _as_rows(matcher(pr.path0, pr.path1), tab.dev)
-        except Exception as e:
-            failed[i] = f'{type(e).__name__}: {e}'
-            rows = empty
-        tab.add(rows)
-    tab.flush()
-    return failed
-
-
 def parse_record(row, pair, n_thr, failed=False):
     """One pair's Namespace(name0, name1, N, n_inliers, n_good, cos_R, cos_t, R_err, t_err, err, counts, R, t,
     match_failed) from its host table row.  Errors in degrees; +inf without a model or when the matcher raised."""
@@ -347,29 +288,37 @@ def eval_relpose(matcher, pairs, data_root, ksize=2, eval_type='fine', io_thres=
 
     -> dict(auc={t: AUC@t}, prec={e: precision@e}, n_matches: mean matches per pair, failed: [(index, name0, name1,
     error text)] of the pairs whose matcher raised, records: one Namespace per pair (parse_record), n_pairs, time)."""
-    from .model import Patch2PixB200
-    epi = _thresholds(epi_thresholds, 'epi_thresholds')
-    auc_t = [float(t) for t in _thresholds(auc_thresholds, 'auc_thresholds')]
+    epi = check_thresholds(epi_thresholds, 'epi_thresholds')
+    auc_t = [float(t) for t in check_thresholds(auc_thresholds, 'auc_thresholds')]
     if not (ransac_thres > 0 and np.isfinite(ransac_thres)):
         raise ValueError('ransac_thres must be positive')
     if not (int(chunk_pairs) >= 1):
         raise ValueError('chunk_pairs must be at least 1')
     pairs = read_pairs(pairs, data_root)
-    is_net = isinstance(matcher, Patch2PixB200)
+    run = PairRunner(matcher, ksize, eval_type, io_thres, ncn_thres, imsize)
     lprint_(f'\n>>Eval relative pose: {len(pairs)} pairs, '
-            + (f'eval_type={eval_type} ksize={ksize} io={io_thres} nc={ncn_thres} im={imsize} ' if is_net else '')
+            + (f'eval_type={eval_type} ksize={ksize} io={io_thres} nc={ncn_thres} im={imsize} ' if run.is_net else '')
             + f'rthres={ransac_thres} conf={conf}')
-    if is_net:
-        matcher.eval()
-        dev = matcher.device
-    else:
-        dev = torch.device('cuda', torch.cuda.current_device())
     start = time.time()
-    tab = _Table(dev, pairs, ransac_thres, conf, max_iters, epi, int(chunk_pairs))
-    if is_net:
-        failed = _eval_net(matcher, pairs, tab, ksize, eval_type, io_thres, ncn_thres, imsize)
-    else:
-        failed = _eval_callable(matcher, pairs, tab)
+    tab = _Table(run.dev, pairs, ransac_thres, conf, max_iters, epi, int(chunk_pairs))
+    failed = {}
+    # a failed pair adds no rows; Patch2Pix rows are the packed [n, 9] rows with their device count
+    empty = torch.zeros(0, 9 if run.is_net else 4, dtype=torch.float64, device=run.dev)
+    zero = torch.zeros(1, dtype=torch.float64, device=run.dev) if run.is_net else None
+    for i, ims in prefetch(pairs, lambda p: run.decode([p.path0, p.path1])):
+        try:
+            if isinstance(ims, Exception):
+                raise ims
+            if run.is_net:
+                packed, n = run.match(run.prepare(ims[0]), run.prepare(ims[1]))
+                item = packed[:n * 9].view(n, 9), packed[n * 9:n * 9 + 1]
+            else:
+                item = run.call(pairs[i].path0, pairs[i].path1), None
+        except Exception as e:
+            failed[i] = f'{type(e).__name__}: {e}'
+            item = empty, zero
+        tab.add(*item)
+    tab.flush()
     host = tab.table.cpu().numpy()                    # the run's one copy of the records
     runtime = time.time() - start
     records = [parse_record(host[i], p, epi.size, i in failed) for i, p in enumerate(pairs)]

@@ -42,14 +42,14 @@ import os
 import struct
 import time
 from argparse import Namespace
-from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import torch
 
 from . import _lib
 from .evaluation import qvec2rotmat, read_cameras_binary, read_images_binary
-from .localize import find_absolute_pose_batch_into, read_retrieval, write_results
+from .eval_helper import PairRunner, as_rows, prefetch
+from .localize import AbsPoseTable, read_retrieval
 
 AACHEN_THRESHOLDS = ((0.25, 2), (0.5, 5), (5, 10))
 CAMERA_CODES = {'SIMPLE_PINHOLE': 0, 'PINHOLE': 1, 'SIMPLE_RADIAL': 2, 'RADIAL': 3}
@@ -267,16 +267,6 @@ def _pair_tables(images, cams, img_cam, recs, pairs, epi_px):
     return pair_img, E, thr
 
 
-def _as_match_rows(m, dev):
-    t = m if isinstance(m, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(m, dtype=np.float64))
-    t = t.to(device=dev, dtype=torch.float64)
-    if t.numel() == 0:
-        t = t.reshape(0, 4)
-    if t.dim() != 2 or t.shape[1] != 4:
-        raise ValueError(f'matches must be [N, 4] rows (x0, y0, x1, y1), got shape {tuple(t.shape)}')
-    return t.contiguous()
-
-
 def _check(pos_args):
     for name, v in pos_args:
         if not (v > 0 and math.isfinite(v)):
@@ -367,7 +357,7 @@ def triangulate_from_matches(model_dir, pairs, matches, merge_px=4.0, epi_px=4.0
     dev = torch.device(device) if device is not None else torch.device('cuda', torch.cuda.current_device())
     cameras, images, cams, img_cam, recs = _model_tables(model_dir)
     pair_img, E, thr = _pair_tables(images, cams, img_cam, recs, pairs, epi_px)
-    rows = [_as_match_rows(m, dev) for m in matches]
+    rows = [as_rows(m, dev) for m in matches]
     offsets = np.zeros(max(len(rows), 1) + 1, dtype=np.int64)
     offsets[1:len(rows) + 1] = np.cumsum([int(r.shape[0]) for r in rows])
     offsets[len(rows) + 1:] = offsets[len(rows)]
@@ -377,56 +367,22 @@ def triangulate_from_matches(model_dir, pairs, matches, merge_px=4.0, epi_px=4.0
 
 
 # ---- matching drivers -------------------------------------------------------------------------------------------------------
-class _Runner:
-    """Runs a Patch2PixB200 (as estimate_matches_from_files would, image 0 first) or a callable (path0, path1) ->
-    [N, 4] on image pairs; a pair's result is (rows [cap, stride] device tensor, stride, n_dev device double or None,
-    n host)."""
-
-    def __init__(self, matcher, images_dir, ksize, eval_type, io_thres, imsize):
-        from .model import Patch2PixB200
-        self.matcher, self.dir = matcher, images_dir
-        self.is_net = isinstance(matcher, Patch2PixB200)
-        self.kw = (ksize, eval_type, io_thres, imsize)
-        if self.is_net:
-            matcher.eval()
-            self.dev, self.h = matcher.device, matcher._handle
-        else:
-            self.dev = torch.device('cuda', torch.cuda.current_device())
-            self.h = _lib.default_handle(self.dev)
-
-    def load(self, a, b):
-        if not self.is_net:
-            return None
-        from PIL import Image
-        return [np.asarray(Image.open(os.path.join(self.dir, n)).convert('RGB')) for n in (a, b)]
-
-    def run(self, a, b, decoded):
-        if not self.is_net:
-            from .hpatches import _as_rows
-            rows = _as_rows(self.matcher(os.path.join(self.dir, a), os.path.join(self.dir, b)), self.dev)
-            return rows, None, int(rows.shape[0])
-        from .eval_helper import match_device
-        from .preprocess import preprocess_image
-        ksize, eval_type, io_thres, imsize = self.kw
-        x0, s0 = preprocess_image(decoded[0], ksize, self.matcher.upsample, imsize, self.dev, self.h)
-        x1, s1 = preprocess_image(decoded[1], ksize, self.matcher.upsample, imsize, self.dev, self.h)
-        packed, n, _ = match_device(self.matcher, x0.unsqueeze(0), x1.unsqueeze(0), s0, s1, ksize, 0.0, True,
-                                    io_thres, eval_type, None)
-        flat = packed.reshape(-1)
-        return flat[:9 * n].view(n, 9)[:, :4], flat[9 * n:9 * n + 1], n
-
-    def each(self, pairs):
-        """Yields (index, result or exception) for pairs in order; decodes run one pair ahead on a worker thread."""
-        with ThreadPoolExecutor(max_workers=1) as pool:
-            fut = pool.submit(self.load, *pairs[0]) if pairs else None
-            for i, (a, b) in enumerate(pairs):
-                cur = fut
-                if i + 1 < len(pairs):
-                    fut = pool.submit(self.load, *pairs[i + 1])
-                try:
-                    yield i, self.run(a, b, cur.result())
-                except Exception as e:
-                    yield i, e
+def _each(run, images_dir, pairs):
+    """Yields (index, result or the exception raised) for the pairs (name0, name1) in order, decodes one pair ahead; a
+    result is (rows [cap, 4] device tensor, the device kept-row count or None, cap)."""
+    for i, ims in prefetch(pairs, lambda p: run.decode([os.path.join(images_dir, n) for n in p])):
+        try:
+            if isinstance(ims, Exception):
+                raise ims
+            if run.is_net:
+                packed, n = run.match(run.prepare(ims[0]), run.prepare(ims[1]))
+                r = packed[:9 * n].view(n, 9)[:, :4], packed[9 * n:9 * n + 1], n
+            else:
+                rows = run.call(*(os.path.join(images_dir, n) for n in pairs[i]))
+                r = rows, None, int(rows.shape[0])
+        except Exception as e:
+            r = e
+        yield i, r
 
 
 def _collect(results, dev):
@@ -452,7 +408,8 @@ def _collect(results, dev):
 
 
 def _device_rows(r):
-    """A _Runner result as rows without a host sync: rows from the device count on are NaN, which every stage drops."""
+    """A pair result of _each as rows without a host sync: rows from the device count on are NaN, which every stage
+    drops."""
     rows, n_dev, n = r
     if n_dev is None:
         return rows
@@ -473,7 +430,7 @@ def triangulate_db(matcher, images_dir, model_dir, db_pairs, chunk_pairs=512, me
     pairs = read_pairs(db_pairs) if isinstance(db_pairs, (str, os.PathLike)) else list(db_pairs)
     cameras, images, cams, img_cam, recs = _model_tables(model_dir)
     pair_img, E, thr = _pair_tables(images, cams, img_cam, recs, pairs, epi_px)
-    run = _Runner(matcher, images_dir, ksize, eval_type, io_thres, imsize)
+    run = PairRunner(matcher, ksize, eval_type, io_thres, 0.0, imsize)
     lprint_(f'\n>>Triangulate: {len(images)} images, {len(pairs)} database pairs')
     start = time.time()
     results, failed, chunk = [], [], []
@@ -491,7 +448,7 @@ def triangulate_db(matcher, images_dir, model_dir, db_pairs, chunk_pairs=512, me
             results.append((block[o:o + r[2]], r[1], r[2]))
             o += r[2]
         chunk.clear()
-    for i, r in run.each(pairs):
+    for i, r in _each(run, images_dir, pairs):
         if isinstance(r, Exception):
             failed.append((pairs[i], f'{type(r).__name__}: {r}'))
             r = None
@@ -525,7 +482,7 @@ def _localize(dev, sfm, qs, ret, per_query, results_path, ransac_thres, chunk_qu
     kp_key, kp_xy, kp_point, pts = sfm.device_arrays(dev)
     n_kp = len(sfm.kp_key)
     nq = len(ret)
-    table = torch.zeros(max(nq, 1), 13, dtype=torch.float64, device=dev)
+    table = AbsPoseTable(nq, dev)
     for k0 in range(0, nq, int(chunk_queries)):
         K = min(int(chunk_queries), nq - k0)
         items, pimg, cams = [], [], []
@@ -574,27 +531,8 @@ def _localize(dev, sfm, qs, ret, per_query, results_path, ransac_thres, chunk_qu
                                               _lib.ptr(intr_d), _lib.ptr(kp_key), _lib.ptr(kp_xy), _lib.ptr(kp_point),
                                               n_kp, _lib.ptr(pts), _lib.ptr(rows), _lib.ptr(q_off), st))
         off_h = q_off.cpu().numpy()                     # the chunk's one sync: the row offsets RANSAC is planned by
-        mask = torch.empty(int(off_h[-1]) + 1, dtype=torch.uint8, device=dev)
-        cnt_q = torch.empty(K, dtype=torch.int32, device=dev)
-        rt = torch.empty(K, 12, dtype=torch.float64, device=dev)
-        find_absolute_pose_batch_into(h, rows, 5, q_off, off_h, None, intr_d.data_ptr(), ransac_thres, None, conf,
-                                      max_iters, 0, rt.data_ptr(), mask.data_ptr(), cnt_q.data_ptr())
-        table[k0:k0 + K, :12].copy_(rt)
-        table[k0:k0 + K, 12:13].view(torch.int32)[:, 0].copy_(cnt_q)
-    host = table.cpu().numpy()
-    poses, out = {}, []
-    for i, (q, _) in enumerate(ret):
-        c = int(host[i, 12:13].view(np.int32)[0])
-        R, t = host[i, :9].reshape(3, 3).copy(), host[i, 9:12].copy()
-        if i not in failed and c <= 0:
-            failed[i] = 'no model'
-        if i in failed:
-            R, t = np.eye(3), np.zeros(3)
-        name = os.path.basename(q)
-        poses[name] = (R, t, c)
-        out.append((name, R, t))
-    write_results(results_path, out)
-    return poses
+        table.solve(k0, h, rows, q_off, off_h, None, intr_d.data_ptr(), ransac_thres, conf, max_iters)
+    return table.finish([q for q, _ in ret], failed, results_path)
 
 
 def _loc_args(ransac_thres, chunk_queries):
@@ -620,7 +558,7 @@ def localize_from_matches(sfm, queries, query_pairs, matches, results_path, rans
     for (i, d), m in zip(flat, matches):
         if d not in sfm.index:
             raise ValueError(f'query pair ({ret[i][0]} {d}): {d} is not an image of the model')
-        by_q[i].append((sfm.index[d], _as_match_rows(m, dev)))
+        by_q[i].append((sfm.index[d], as_rows(m, dev)))
     start = time.time()
     failed = {}
     poses = _localize(dev, sfm, qs, ret, lambda i: by_q[i], results_path, ransac_thres, chunk_queries, conf,
@@ -641,12 +579,12 @@ def localize_sfm(matcher, sfm, images_dir, queries, query_pairs, results_path, r
         for d in dbs:
             if d not in sfm.index:
                 raise ValueError(f'query pair ({q} {d}): {d} is not an image of the model')
-    run = _Runner(matcher, images_dir, ksize, eval_type, io_thres, imsize)
+    run = PairRunner(matcher, ksize, eval_type, io_thres, 0.0, imsize)
     lprint_(f'\n>>Localize: {len(ret)} queries, {sum(len(d) for _, d in ret)} pairs, rthres={ransac_thres}')
     start = time.time()
     flat = [(q, d) for q, dbs in ret for d in dbs]
     owner = [i for i, (_, dbs) in enumerate(ret) for _ in dbs]
-    gen = run.each(flat)
+    gen = _each(run, images_dir, flat)
 
     def per_query(i):
         got, err = [], None
