@@ -527,6 +527,51 @@ P2P_API int p2p_sfm_query_rows(p2p_handle_t h, const double* matches, long long 
                                const int32_t* kp_point, long long n_kp, const double* points, double* rows,
                                int64_t* q_offsets, void* stream);
 
+/* ---- SuperPoint keypoints and descriptors, exact nearest-neighbour matching (keypoints.cu; the Python side in
+ * patch2pix_b200/superpoint.py, the restatement in oracle/superpoint_oracle.py).
+ *
+ * p2p_sp_keypoints: logits fp32 [batch][65][hc][wc], the detector head's output.  Per image: softmax over the 65
+ * channels, dustbin dropped, depth-to-space to s [H = 8 hc][W = 8 wc] (channel c -> pixel (8 cy + c / 8, 8 cx + c % 8)),
+ * written to score_map [batch][H][W] when it is not NULL.  NMS with p = (2 nms_radius + 1)^2 max-pool, stride 1,
+ * out-of-image taps never winning: M = (s == p(s)); twice: S = p(M) > 0, s' = S ? 0 : s, M |= (s' == p(s')) & !S.
+ * A keypoint is a pixel with (M ? s : 0) > threshold and border <= x < W - border, border <= y < H - border.  With
+ * max_keypoints >= 0 an image keeps its min(max_keypoints, count) best by score, descending, exact ties in ascending
+ * flat index; with max_keypoints < 0 all, in row-major order.  Output: keypoints fp32 [.][2] (x, y) and scores fp32
+ * [.] of all images in image order, and offsets int64 [batch + 1]: image b owns rows offsets[b] .. offsets[b + 1].
+ * keypoints / scores hold batch * H * W rows (batch * min(max_keypoints, H * W) with max_keypoints >= 0).
+ * Limits: batch * H * W < 2^31, batch <= 65535, hc <= 262140, 0 <= nms_radius <= 16, border >= 0, threshold
+ * finite. */
+P2P_API int p2p_sp_keypoints(p2p_handle_t h, const float* logits, int batch, int hc, int wc, int nms_radius,
+                             float threshold, int border, int max_keypoints, float* score_map, float* keypoints,
+                             float* scores, int64_t* offsets, void* stream);
+/* p2p_sp_descriptors: desc fp32 [batch][dim][hc][wc], the raw descriptor head; keypoints / offsets as
+ * p2p_sp_keypoints wrote them, n = offsets[batch] (HOST value).  Each cell is divided by max(|cell|, 1e-12); a keypoint
+ * (x, y) samples that map bilinearly as grid_sample(align_corners=True, zero padding) at
+ * gx = (x - 3.5) / (8 wc - 4.5) * 2 - 1 (gy likewise), in fp64; the sample is divided by max(|sample|, 1e-12).
+ * Output fp32 [n][dim].  Limits: 1 <= dim <= 512. */
+P2P_API int p2p_sp_descriptors(p2p_handle_t h, const float* desc, int batch, int dim, int hc, int wc,
+                               const float* keypoints, const int64_t* offsets, long long n, float* out, void* stream);
+/* p2p_match_descriptors_batch: n_pairs pairs of descriptor sets, d0 fp32 [.][dim] with pair k's set 0 in rows
+ * offsets0[k] .. offsets0[k + 1], d1 and offsets1 likewise (offsets given on the device and, as *_host, on the
+ * host).  The similarity of rows i, j is the float64 sum over c = 0 .. dim - 1, in that order, of the exact products
+ * d0[i][c] * d1[j][c].  Row i's best column j1 has the largest similarity s1 (ties: lowest j), s2 the largest over the
+ * other columns.  Row i is accepted iff the set has a column, and: mutual = 1 -> row i is the best row of column j1
+ * (ties: lowest i); min_sim not NaN -> s1 > min_sim; ratio not NaN -> 1 - s1 < ratio * ratio * (1 - s2) in float64,
+ * true when the set has one column.  Output per row of d0: match int32 = j1 (pair-local) or -1, sim fp64 = s1 or 0.
+ * Results are exact (no tolerance), identical across runs and for a pair alone or in any batch.  Option "match_impl"
+ * 1 (default): similarities on the tensor cores (3-pass fp16 hi/lo), every decision within 2 eps of its margin redone
+ * in float64 (DESIGN.md); 0: every similarity in float64 on the CUDA cores.  Same result.  Optional outputs (NULL to
+ * skip; tensor-core path only): tc_sim [n0] / tc_idx [n0] the tensor-core best similarity and column of each row
+ * before the fix-up, eps [n_pairs] the bound of |s_tc - s_fp64| per pair, n_fixed int32 [2] the rows and columns
+ * redone in float64.  Limits: 1 <= n_pairs <= 65535, dim % 16 == 0, 16 <= dim <= 1024, fewer than 2^20 rows per set.
+ * Descriptors must be finite: a NaN or inf is not detected (that would cost a host sync) and gives unspecified
+ * matches. */
+P2P_API int p2p_match_descriptors_batch(p2p_handle_t h, const float* d0, const float* d1, const int64_t* offsets0,
+                                        const int64_t* offsets1, const int64_t* offsets0_host,
+                                        const int64_t* offsets1_host, int n_pairs, int dim, int mutual,
+                                        double min_sim, double ratio, int32_t* match, double* sim, double* tc_sim,
+                                        int32_t* tc_idx, double* eps, int32_t* n_fixed, void* stream);
+
 /* ---- bring-up / accuracy probe: C[M,N] = alpha * A[M,K] B[N,K]^T on the wgmma path with the
  * same operand format as the hot path (fp32 inputs are split to fp16 hi/lo on the device).
  * a, b, c are DEVICE fp32; K % 64 == 0. */

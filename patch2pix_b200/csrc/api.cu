@@ -124,12 +124,13 @@ struct p2p_handle_s {
   NcStackWeights ncs;           // general NeighConsensus stack (p2p_set_nc_stack_weights), beside the fixed stack above
   bool ncs_set = false;
   void* dbg_nc[4] = {nullptr, nullptr, nullptr, nullptr};   // scratch of the last p2p_neigh_consensus call (debug hook below)
+  int opt_match_impl = 1;       // p2p_match_descriptors_batch: 1 tensor-core pass + float64 fix-up, 0 float64 only
   int opt_unique_impl = 1;      // 1: rank sort over the whole GPU for lists <= 8192 rows; 0: single-block bitonic network
   int* uniq_rank = nullptr;     // zeroed scratch of the rank-sort path
   int opt_nc_l2_mode = 0;       // NC layer 2 block layout: 0 auto, 1 one haloed block per tile, 2 one block per column tap
   int opt_nc_impl = 1;          // 1: NeighConsensus on the tensor cores (nc_umma.cu); 0: fp32 CUDA-core kernels (shape-capped)
   Regressor reg[2];
-  Arena coarse, refine, feat, misc, uniq, pre, verify, sfm;
+  Arena coarse, refine, feat, misc, uniq, pre, verify, sfm, sp;
   std::vector<PreprocessCoefs> pre_coefs;   // cached resampling tables, one per image geometry
   PairFeatures pf[2];
   bool prepared = false;
@@ -493,6 +494,7 @@ int p2p_destroy(p2p_handle_t h) {
   h->pre.release();
   h->verify.release();
   h->sfm.release();
+  h->sp.release();
   for (auto& c : h->pre_coefs)
     if (c.d) cudaFree(c.d);
   for (auto& e : h->prof) { cudaEventDestroy(e.a); cudaEventDestroy(e.b); }
@@ -579,6 +581,7 @@ static int* option_slot(p2p_handle_t h, const char* key) {
   if (!strcmp(key, "nc_impl")) return &h->opt_nc_impl;
   if (!strcmp(key, "nc_l2_mode")) return &h->opt_nc_l2_mode;
   if (!strcmp(key, "unique_impl")) return &h->opt_unique_impl;
+  if (!strcmp(key, "match_impl")) return &h->opt_match_impl;
   return nullptr;
 }
 
@@ -590,6 +593,7 @@ int p2p_set_option(p2p_handle_t h, const char* key, int value) {
   if (s == &h->opt_corr_passes) P2P_REQUIRE(value == 0 || value == 1 || value == 3, "corr_passes must be 0, 1 or 3");
   if (s == &h->opt_share_windows) P2P_REQUIRE(value == 0 || value == 1, "share_windows must be 0 or 1");
   if (s == &h->opt_epi_async) P2P_REQUIRE(value == 0 || value == 1, "epi_async must be 0 or 1");
+  if (s == &h->opt_match_impl) P2P_REQUIRE(value == 0 || value == 1, "match_impl must be 0 or 1");
   if (s == &h->opt_tile_trace) {
     P2P_REQUIRE(value == 0 || value == 1, "tile_trace must be 0 or 1");
     h->traces.clear();
@@ -2037,6 +2041,64 @@ int p2p_tile_trace_read(p2p_handle_t h, int idx, int* tag, int* tiles, unsigned 
                            cudaMemcpyDeviceToHost));
   }
   return 0;
+}
+
+
+int p2p_sp_keypoints(p2p_handle_t h, const float* logits, int batch, int hc, int wc, int nms_radius, float threshold,
+                     int border, int max_keypoints, float* score_map, float* keypoints, float* scores, int64_t* offsets,
+                     void* stream) {
+  P2P_ENTER(h);
+  P2P_REQUIRE(batch >= 1 && hc >= 1 && wc >= 1 && (long long)batch * hc * wc * 64 < (1ll << 31),
+              "batch * 8hc * 8wc must be in 1 .. 2^31 - 1");
+  P2P_REQUIRE(batch <= 65535 && hc <= 65535 * 4, "batch must be <= 65535 and hc <= 262140 (launch grid limits)");
+  P2P_REQUIRE(nms_radius >= 0 && nms_radius <= kSpMaxNmsRadius, "nms_radius must be in 0..16");
+  P2P_REQUIRE(border >= 0, "border must be >= 0");
+  P2P_REQUIRE(std::isfinite(threshold), "threshold must be finite");
+  P2P_REQUIRE(logits && keypoints && scores && offsets, "null pointer");
+  return launch_sp_keypoints(h->sp, logits, batch, hc, wc, nms_radius, threshold, border, max_keypoints, score_map,
+                             keypoints, scores, (long long*)offsets, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int p2p_sp_descriptors(p2p_handle_t h, const float* desc, int batch, int dim, int hc, int wc, const float* keypoints,
+                       const int64_t* offsets, long long n, float* out, void* stream) {
+  P2P_ENTER(h);
+  P2P_REQUIRE(batch >= 1 && hc >= 1 && wc >= 1, "empty descriptor map");
+  P2P_REQUIRE((long long)batch * hc * wc < (1ll << 31), "batch * hc * wc must be < 2^31");
+  P2P_REQUIRE(dim >= 1 && dim <= kSpMaxDescDim, "dim must be in 1..512");
+  P2P_REQUIRE(n >= 0 && n < (1ll << 31), "bad keypoint count");
+  P2P_REQUIRE(desc && offsets && ((keypoints && out) || n == 0), "null pointer");
+  return launch_sp_descriptors(h->sp, desc, batch, dim, hc, wc, keypoints, (const long long*)offsets, n, out,
+                               reinterpret_cast<cudaStream_t>(stream));
+}
+
+int p2p_match_descriptors_batch(p2p_handle_t h, const float* d0, const float* d1, const int64_t* offsets0,
+                                const int64_t* offsets1, const int64_t* offsets0_host, const int64_t* offsets1_host,
+                                int n_pairs, int dim, int mutual, double min_sim, double ratio, int32_t* match,
+                                double* sim, double* tc_sim, int32_t* tc_idx, double* eps, int32_t* n_fixed,
+                                void* stream) {
+  P2P_ENTER(h);
+  P2P_REQUIRE(n_pairs >= 1 && n_pairs <= 65535, "n_pairs must be in 1..65535");
+  P2P_REQUIRE(dim >= 16 && dim <= kMatchMaxDim && dim % 16 == 0, "dim must be a multiple of 16 in 16..1024");
+  P2P_REQUIRE(mutual == 0 || mutual == 1, "mutual must be 0 or 1");
+  P2P_REQUIRE(!std::isinf(min_sim), "min_sim must be finite (NaN: no test)");
+  P2P_REQUIRE(std::isnan(ratio) || (ratio >= 0.0 && std::isfinite(ratio)), "ratio must be >= 0 (NaN: no test)");
+  P2P_REQUIRE(offsets0 && offsets1 && offsets0_host && offsets1_host, "null offsets");
+  P2P_REQUIRE(offsets0_host[0] == 0 && offsets1_host[0] == 0, "offsets must start at 0");
+  int max0 = 0, max1 = 0;
+  for (int k = 0; k < n_pairs; ++k) {
+    const int64_t a = offsets0_host[k + 1] - offsets0_host[k], b = offsets1_host[k + 1] - offsets1_host[k];
+    P2P_REQUIRE(a >= 0 && a < (1 << 20) && b >= 0 && b < (1 << 20), "every set must hold 0 .. 2^20 - 1 descriptors");
+    max0 = std::max(max0, (int)a);
+    max1 = std::max(max1, (int)b);
+  }
+  const long long n0 = offsets0_host[n_pairs], n1 = offsets1_host[n_pairs];
+  P2P_REQUIRE((d0 && match && sim) || n0 == 0, "null pointer");
+  P2P_REQUIRE(d1 || n1 == 0, "null pointer");
+  if (n0 == 0) return 0;
+  return launch_match_descriptors(h->sp, d0, d1, (const long long*)offsets0, (const long long*)offsets1, n_pairs, dim,
+                                  max0, max1, n0, n1, mutual, !std::isnan(min_sim), min_sim, !std::isnan(ratio), ratio,
+                                  h->opt_match_impl, match, sim, tc_sim, tc_idx, eps, n_fixed,
+                                  reinterpret_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

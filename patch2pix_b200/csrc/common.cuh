@@ -72,6 +72,17 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
+// Bump allocator over one scratch block: each take is padded and 256-byte aligned.
+struct Carve {
+  char* p;
+  template <typename T>
+  T* take(size_t n) {
+    T* r = (T*)p;
+    p += align_up(n * sizeof(T) + 16, 256);
+    return r;
+  }
+};
+
 // Grow-only device scratch arena owned by a handle.  Growth is a (synchronising)
 // cudaMalloc; after the first pair of a given shape the arena is stable.
 struct Arena {

@@ -266,6 +266,20 @@ int launch_sfm_query_rows(Arena& ar, const double* m4, long long M, const long l
                           const unsigned long long* qkp_key, const double* qkp_n, const double* q_intr,
                           const unsigned long long* kp_key, const double* kp_xy, const int* kp_point, long long n_kp,
                           const double* pts, double* rows, long long* q_offsets, cudaStream_t st);
+// ---- keypoints.cu: SuperPoint's keypoints and descriptors, exact nearest-neighbour matching (semantics in
+// include/p2p_b200.h, p2p_sp_* and p2p_match_descriptors_batch).  Scratch comes from `ar` (reserved here).
+constexpr int kSpMaxNmsRadius = 16;
+constexpr int kSpMaxDescDim = 512;      // descriptor channels the sampling kernel holds per warp
+constexpr int kMatchMaxDim = 1024;
+int launch_sp_keypoints(Arena& ar, const float* logits, int B, int Hc, int Wc, int r, float thr, int border, int k,
+                        float* smap_out, float* kp, float* kp_score, long long* counts, cudaStream_t st);
+int launch_sp_descriptors(Arena& ar, const float* raw, int B, int D, int Hc, int Wc, const float* kp,
+                          const long long* kp_off, long long N, float* out, cudaStream_t st);
+int launch_match_descriptors(Arena& ar, const float* d0, const float* d1, const long long* off0,
+                             const long long* off1, int K, int D, int max_n0, int max_n1, long long n0, long long n1,
+                             int mutual, int has_min, double min_sim, int has_ratio, double ratio, int impl,
+                             int* match, double* sim, double* tc_sim, int* tc_idx, double* eps_out,
+                             int* n_fixed, cudaStream_t st);
 // ---- relpose.cu: relative-pose statistics of a batch (one block per pair, pairs = B.pairs, any count): pair p writes
 // out[p * out_stride ..] = cos of the rotation and translation-direction errors of Rt_est [p] against Rt_gt [p]
 // (NaN when n_inliers[p] <= 0), then int32 [n_thr + 1]: rows with symmetric epipolar error < thr[j], rows considered.

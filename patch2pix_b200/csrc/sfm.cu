@@ -588,16 +588,6 @@ __global__ void offsets_kernel(const int* __restrict__ incl, int Q, long long* o
 }
 
 // ---- host helpers ---------------------------------------------------------------------------------------------------
-struct Carve {
-  char* p;
-  template <typename T>
-  T* take(size_t n) {
-    T* r = (T*)p;
-    p += align_up(n * sizeof(T) + 16, 256);
-    return r;
-  }
-};
-
 size_t sort_bytes(long long n, bool pairs) {
   size_t b = 0;
   if (pairs)
