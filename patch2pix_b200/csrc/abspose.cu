@@ -2,40 +2,31 @@
 // of queries, and the lift of a database cutout's matched pixels to 3D through its scan (hloc's InLoc pipeline,
 // pose_from_cluster / interpolate_scan).
 //
-// p2p_find_absolute_pose_batch enqueues, with the query as grid dimension y:
-//   abs_prep_kernel   (1 block)          effective row count, finiteness, the centroid of the world points, fp32 rows
-//                                        (world points minus the centroid, pixels minus the principal point)
-//   abs_round_kernel  (cdiv(count, 8))   per round: 3-row samples -> Grunert's P3P quartic (up to 4 poses, one thread
-//                                        per sample), every (pose, row) scored in fp32
-//   abs_select_kernel (1 block)          ransac_common.cuh's select_round on 12-double poses, the stopping bound (s = 3)
-//   abs_lo_kernel     (1 block)          Gauss-Newton on the inliers of the winner, kept while the count grows; outputs
-// The solver and scorer are their own (rows of 5 values, models of 12), so the two-view kinds of verify_common.cuh do
-// not branch on this caller.  Everything a query computes depends on its rows, threshold and cameras alone, every
-// combine runs in a fixed order and no grid size depends on the device: results are bit-reproducible, and a query's
-// result is the same alone or in a batch.  Restated in oracle/abspose_oracle.py.
-#include <algorithm>
-
+// p2p_find_absolute_pose_batch runs the RANSAC kernels of verify_common.cuh as kind 4, with the query as grid
+// dimension y and no host sync:
+//   abs_prep_kernel          (1 block)         effective row count, finiteness, the centroid of the world points, fp32
+//                                              rows (world points minus the centroid, pixels minus the principal point)
+//   verify_round_kernel<4>   (cdiv(count, 8))  per round: 3-row samples -> Grunert's P3P quartic (up to 4 poses, one
+//                                              thread per sample), every (pose, row) scored in fp32
+//   verify_select_kernel<12> (1 block)         the best of the round's 12-double poses, the stopping bound (s = 3)
+//   verify_lo_kernel<4>      (1 block)         Gauss-Newton on the inliers of the winner, kept while the count grows;
+//                                              outputs
+// This file adds what only absolute pose needs: Kind<4> (the prep, the P3P solver, the projection test and the
+// Gauss-Newton step) and the scan lift.  Everything a query computes depends on its rows, threshold and cameras alone,
+// every combine runs in a fixed order and no grid size depends on the device: results are bit-reproducible, and a
+// query's result is the same alone or in a batch.  Restated in oracle/abspose_oracle.py.
 #include <math.h>
 
 #include "kernels.h"
-#include "ransac_common.cuh"
+#include "verify_common.cuh"
 
 namespace p2p {
 namespace {
 
-constexpr int kAbsRound = 1024;      // hypotheses per round
-constexpr int kAbsSample = 3;        // rows per minimal sample
 constexpr int kAbsSlots = 4;         // P3P poses per sample
-constexpr int kAbsMinRows = 4;       // fewer rows: no rounds, no model
-constexpr int kAbsHypPerBlock = 8;   // samples solved (one thread each) and scored per block
-constexpr int kAbsThreads = 256;     // 8 warps
-constexpr int kAbsTile = 1024;       // fp32 rows staged in shared memory per scoring pass
-constexpr int kAbsLoIters = 4;       // local-optimisation refits
+constexpr int kAbsMinRows = 4;       // fewer rows: no rounds, no model; fewer inliers: no refit
 constexpr int kAbsGnSteps = 3;       // Gauss-Newton steps per refit
-constexpr int kAbsLoThreads = 256;
 constexpr int kLiftThreads = 1024;
-constexpr size_t kAbsModels = (size_t)kAbsRound * kAbsSlots * 12;   // doubles of round models per query
-constexpr size_t kAbsCounts = (size_t)kAbsRound * kAbsSlots;        // ints of round counts per query
 
 struct __align__(8) AbsRow32 {       // scoring row: world point minus the centroid, pixel minus the principal point
   float X, Y, Z, du, dv, pad;
@@ -108,11 +99,6 @@ __device__ int quartic_roots(const double (&A)[5], double (&r)[4]) {
 __device__ __forceinline__ void sub3(const double* a, const double* b, double* c) {
   for (int i = 0; i < 3; ++i) c[i] = a[i] - b[i];
 }
-__device__ __forceinline__ void cross3d(const double* a, const double* b, double* c) {
-  c[0] = a[1] * b[2] - a[2] * b[1];
-  c[1] = a[2] * b[0] - a[0] * b[2];
-  c[2] = a[0] * b[1] - a[1] * b[0];
-}
 __device__ __forceinline__ double norm3(const double* a) { return sqrt(a[0] * a[0] + a[1] * a[1] + a[2] * a[2]); }
 
 // Orthonormal frame of a triangle, columns e1 = (Q1 - Q0) / |.|, e2 = e3 x e1, e3 = (Q1 - Q0) x (Q2 - Q0) / |.|, as
@@ -121,11 +107,11 @@ __device__ bool tri_frame(const double (&Q)[3][3], double (&F)[3][3]) {
   double e1[3], d2[3], e3[3], e2[3];
   sub3(Q[1], Q[0], e1);
   sub3(Q[2], Q[0], d2);
-  cross3d(e1, d2, e3);
+  cross3(e1, d2, e3);
   const double n1 = norm3(e1), n3 = norm3(e3);
   if (!(n1 > 0.0) || !(n3 > 0.0)) return false;
   for (int i = 0; i < 3; ++i) { e1[i] /= n1; e3[i] /= n3; }
-  cross3d(e3, e1, e2);
+  cross3(e3, e1, e2);
   for (int i = 0; i < 3; ++i) { F[i][0] = e1[i]; F[i][1] = e2[i]; F[i][2] = e3[i]; }
   return true;
 }
@@ -185,25 +171,6 @@ __device__ int solve_p3p(const double (&j)[3][3], const double (&X)[3][3], doubl
   return ns;
 }
 
-// ---- scoring ------------------------------------------------------------------------------------------------------
-// fp32 projection of a pose: rows fx (R_0, t_0), fy (R_1, t_1), (R_2, t_2).
-__device__ __forceinline__ void abs_proj32(const AbsState& S, const double* m, float* p) {
-  for (int k = 0; k < 4; ++k) {
-    p[k] = (float)(S.fx * (k < 3 ? m[k] : m[9]));
-    p[4 + k] = (float)(S.fy * (k < 3 ? m[3 + k] : m[10]));
-    p[8 + k] = (float)(k < 3 ? m[6 + k] : m[11]);
-  }
-}
-
-// Depth z > 0 and squared reprojection error < th^2, as (a - du z)^2 + (b - dv z)^2 < th^2 z^2.
-__device__ __forceinline__ bool abs_inlier(const float* p, const AbsRow32& r, float th2) {
-  const float a = p[0] * r.X + p[1] * r.Y + p[2] * r.Z + p[3];
-  const float b = p[4] * r.X + p[5] * r.Y + p[6] * r.Z + p[7];
-  const float z = p[8] * r.X + p[9] * r.Y + p[10] * r.Z + p[11];
-  const float eu = a - r.du * z, ev = b - r.dv * z;
-  return z > 0.f && eu * eu + ev * ev < th2 * z * z;
-}
-
 // Bearing of row p (unit vector of ((u - cx) / fx, (v - cy) / fy, 1)) and its centred world point.
 __device__ __forceinline__ void abs_row64(const AbsState& S, const double* p, double* j, double* X) {
   const double x = (p[0] - S.cx) / S.fx, y = (p[1] - S.cy) / S.fy;
@@ -214,14 +181,9 @@ __device__ __forceinline__ void abs_row64(const AbsState& S, const double* p, do
   for (int i = 0; i < 3; ++i) X[i] = p[2 + i] - S.mean[i];
 }
 
-// ---- kernels ------------------------------------------------------------------------------------------------------
-struct Cam4 {
-  double fx, fy, cx, cy;
-};
-
-// Query q: its camera intr[4 q ..] (fx, fy, cx, cy; device), or K1 when intr is null, and its threshold px_th_dev[q]
-// (device), or px_th when px_th_dev is null.
-__global__ void __launch_bounds__(1024) abs_prep_kernel(PairBatch B, const double* __restrict__ intr, Cam4 K1,
+// Query q: its camera intr[4 q ..] (fx, fy, cx, cy; device), or K1's first view when intr is null, and its threshold
+// px_th_dev[q] (device), or px_th when px_th_dev is null.
+__global__ void __launch_bounds__(1024) abs_prep_kernel(PairBatch B, const double* __restrict__ intr, Intrinsics K1,
                                                         double px_th, const double* __restrict__ px_th_dev,
                                                         AbsRow32* __restrict__ rows32_all, AbsState* __restrict__ st_all) {
   __shared__ double red[33];
@@ -248,8 +210,8 @@ __global__ void __launch_bounds__(1024) abs_prep_kernel(PairBatch B, const doubl
   double mean[3];
   for (int k = 0; k < 3; ++k) mean[k] = block_sum_1024(sx[k], red) / (double)(m > 0 ? m : 1);
   const double* k4 = intr + 4 * (size_t)q;
-  const double fx = intr ? k4[0] : K1.fx, fy = intr ? k4[1] : K1.fy, cx = intr ? k4[2] : K1.cx,
-               cy = intr ? k4[3] : K1.cy;
+  const double fx = intr ? k4[0] : K1.fx1, fy = intr ? k4[1] : K1.fy1, cx = intr ? k4[2] : K1.cx1,
+               cy = intr ? k4[3] : K1.cy1;
   for (int r = tid; r < m; r += 1024) {
     const double* p = rows + (size_t)r * stride;
     rows32[r] = AbsRow32{(float)(p[2] - mean[0]), (float)(p[3] - mean[1]), (float)(p[4] - mean[2]), (float)(p[0] - cx),
@@ -272,85 +234,6 @@ __global__ void __launch_bounds__(1024) abs_prep_kernel(PairBatch B, const doubl
     st->row0 = pr.row0;
     st->row32 = pr.row0 - B.base;
   }
-}
-
-// Hypotheses first .. first + count - 1.  models [count * 4][12] fp64 (centred frame), counts [count * 4] (-1: no pose).
-__global__ void __launch_bounds__(kAbsThreads, 1) abs_round_kernel(const AbsState* __restrict__ st_all,
-                                                                   const AbsRow32* __restrict__ rows32_all,
-                                                                   const double* __restrict__ rows_all, int stride,
-                                                                   int first, int count, unsigned long long seed,
-                                                                   int ignore_stop, double* __restrict__ models_all,
-                                                                   int* __restrict__ counts_all) {
-  constexpr int NM = kAbsHypPerBlock * kAbsSlots, PW = NM / 8;   // models per block, per warp
-  __shared__ AbsRow32 s_rows[kAbsTile];
-  __shared__ float s_model[NM][12];
-  __shared__ int s_valid[NM];
-  const AbsState* st = st_all + blockIdx.y;
-  if (!ignore_stop && st->stop) return;
-  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  const int n = st->n;
-  const float th2 = st->th2;
-  const double* rows = rows_all + st->row0 * stride;
-  const AbsRow32* rows32 = rows32_all + st->row32;
-  double* models = models_all + blockIdx.y * kAbsModels;
-  int* counts = counts_all + blockIdx.y * kAbsCounts;
-  if (tid < kAbsHypPerBlock) {
-    const int local = blockIdx.x * kAbsHypPerBlock + tid;
-    const AbsState S = *st;
-    double out[kAbsSlots][12];
-    int nm = 0;
-    int idx[kAbsSample];
-    if (local < count && draw_sample<kAbsSample>(seed, first + local, n, idx)) {
-      double j[3][3], X[3][3];
-#pragma unroll
-      for (int k = 0; k < 3; ++k) abs_row64(S, rows + (size_t)idx[k] * stride, j[k], X[k]);
-      nm = solve_p3p(j, X, out);
-    }
-    for (int k = 0; k < kAbsSlots; ++k) {
-      const int slot = tid * kAbsSlots + k;
-      s_valid[slot] = k < nm;
-      if (k < nm) abs_proj32(S, out[k], s_model[slot]);
-      for (int e = 0; e < 12; ++e)
-        if (local < count) models[((size_t)local * kAbsSlots + k) * 12 + e] = k < nm ? out[k][e] : 0.0;
-    }
-  }
-  int cnt[PW];
-#pragma unroll
-  for (int j = 0; j < PW; ++j) cnt[j] = 0;
-  for (int t0 = 0; t0 < n; t0 += kAbsTile) {
-    const int tn = min(kAbsTile, n - t0);
-    __syncthreads();
-    for (int r = tid; r < tn; r += kAbsThreads) s_rows[r] = rows32[t0 + r];
-    __syncthreads();
-#pragma unroll
-    for (int j = 0; j < PW; ++j) {
-      const int mi = wid + 8 * j;
-      if (!s_valid[mi]) continue;
-      float p[12];
-#pragma unroll
-      for (int e = 0; e < 12; ++e) p[e] = s_model[mi][e];
-      for (int r0 = 0; r0 < tn; r0 += 32) {
-        const int r = r0 + lane;
-        const bool in = r < tn && abs_inlier(p, s_rows[r < tn ? r : 0], th2);
-        cnt[j] += __popc(__ballot_sync(0xffffffffu, in));
-      }
-    }
-  }
-  if (lane == 0) {
-#pragma unroll
-    for (int j = 0; j < PW; ++j) {
-      const int mi = wid + 8 * j;
-      const int local = blockIdx.x * kAbsHypPerBlock + mi / kAbsSlots;
-      if (local < count) counts[(size_t)blockIdx.x * NM + mi] = s_valid[mi] ? cnt[j] : -1;
-    }
-  }
-}
-
-__global__ void __launch_bounds__(1024) abs_select_kernel(AbsState* __restrict__ st, const double* __restrict__ models,
-                                                          const int* __restrict__ counts, int nm, int done, double conf,
-                                                          int max_iters) {
-  select_round<12>(st + blockIdx.y, models + blockIdx.y * kAbsModels, counts + blockIdx.y * kAbsCounts, nm, done,
-                   kAbsSample, conf, max_iters);
 }
 
 // R <- exp([w]x) R (Rodrigues), t <- t + dt.
@@ -408,141 +291,96 @@ __device__ bool solve6(const double* h, const double* g, double* x) {
   return true;
 }
 
-// Local optimisation + outputs.  Each refit runs kAbsGnSteps Gauss-Newton steps on the squared reprojection error over
-// the inliers of the current pose (left-multiplied rotation update through the exponential map, translation added);
-// the refit is kept while it has strictly more inliers.  Query q writes Rt_out[12 q ..] in world coordinates (NaN
-// without a model), count_out[q] (-1: a value is not finite) and mask_out[row0 .. row0 + n_all).
-__global__ void __launch_bounds__(kAbsLoThreads, 1) abs_lo_kernel(const AbsState* __restrict__ st_all,
-                                                                  const AbsRow32* __restrict__ rows32_all,
-                                                                  const double* __restrict__ rows_all, int stride,
-                                                                  double* __restrict__ Rt_out,
-                                                                  uint8_t* __restrict__ mask_out,
-                                                                  int* __restrict__ count_out) {
-  __shared__ double s_red[kAbsLoThreads / 32][27];
-  __shared__ double s_cur[12], s_cand[12];
-  __shared__ float s_p[12], s_pc[12];
-  __shared__ int s_cnt[kAbsLoThreads / 32], s_ok;
-  const AbsState* st = st_all + blockIdx.y;
-  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  const AbsState S = *st;
-  const int n = S.n, n_all = S.n_all;
-  const double* rows = rows_all + S.row0 * stride;
-  const AbsRow32* rows32 = rows32_all + S.row32;
-  int cur_count = S.bad ? 0 : S.best_count;
-  if (tid < 12) s_cur[tid] = S.best[tid];
-  __syncthreads();
-
-  auto count_inliers = [&](const double* m64) -> int {    // block-wide, fixed order
-    if (tid == 0) abs_proj32(S, m64, s_pc);
-    __syncthreads();
-    float p[12];
+// ---- absolute pose: kind 4 of the RANSAC kernels (verify_common.cuh) -----------------------------------------------
+// Poses live in the centred frame (R row-major, then t: x = R (X - c) + t) until write_model.  LO: each refit runs
+// kAbsGnSteps Gauss-Newton steps on the squared reprojection error over the inliers of the current pose (rotation
+// updated by left multiplication through the exponential map, translation added), each from the 21 J^T J and 6 J^T r
+// sums, and stops at a step that fails.
+template <> struct Kind<4> {
+  using State = AbsState;
+  using Row32 = AbsRow32;
+  static constexpr int kSample = 3, kSlots = kAbsSlots, kPairSlots = kAbsSlots, kLoMin = kAbsMinRows, kTile = 1024;
+  static constexpr int kModel = 12, kLoSteps = kAbsGnSteps, kLoSums = 27;
+  static void prep(dim3 grid, cudaStream_t st, const PairBatch& B, const double* intr, const Intrinsics& K1,
+                   double px_th, const double* px_th_dev, AbsRow32* rows32, AbsState* s) {
+    abs_prep_kernel<<<grid, 1024, 0, st>>>(B, intr, K1, px_th, px_th_dev, rows32, s);
+  }
+  // Element e of the pose's fp32 projection matrix: rows fx (R_0, t_0), fy (R_1, t_1), (R_2, t_2).
+  static __device__ __forceinline__ float image(const AbsState& S, const double* m, int e) {
+    const int i = e >> 2, k = e & 3;
+    const double v = k < 3 ? m[3 * i + k] : m[9 + i];
+    return (float)(i == 0 ? S.fx * v : i == 1 ? S.fy * v : v);
+  }
+  // Depth z > 0 and squared reprojection error < th^2, as (a - du z)^2 + (b - dv z)^2 < th^2 z^2.
+  static __device__ __forceinline__ bool inlier(const float* p, const AbsRow32& r, float th2) {
+    const float a = p[0] * r.X + p[1] * r.Y + p[2] * r.Z + p[3];
+    const float b = p[4] * r.X + p[5] * r.Y + p[6] * r.Z + p[7];
+    const float z = p[8] * r.X + p[9] * r.Y + p[10] * r.Z + p[11];
+    const float eu = a - r.du * z, ev = b - r.dv * z;
+    return z > 0.f && eu * eu + ev * ev < th2 * z * z;
+  }
+  static __device__ __forceinline__ int solve_sample(const AbsState& S, const double* rows, int stride,
+                                                     const int (&idx)[3], double (&out)[kAbsSlots][12]) {
+    double j[3][3], X[3][3];
 #pragma unroll
-    for (int e = 0; e < 12; ++e) p[e] = s_pc[e];
-    int c = 0;
-    for (int r = tid; r < n; r += kAbsLoThreads) c += abs_inlier(p, rows32[r], S.th2);
-    for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
-    if (lane == 0) s_cnt[wid] = c;
-    __syncthreads();
-    int tot = 0;
-    for (int w = 0; w < kAbsLoThreads / 32; ++w) tot += s_cnt[w];
-    __syncthreads();
-    return tot;
-  };
-
-  for (int it = 0; it < kAbsLoIters && cur_count >= kAbsMinRows; ++it) {
-    if (tid == 0) abs_proj32(S, s_cur, s_p);
-    if (tid < 12) s_cand[tid] = s_cur[tid];
-    __syncthreads();
-    float p[12];
-#pragma unroll
-    for (int e = 0; e < 12; ++e) p[e] = s_p[e];
-    for (int g = 0; g < kAbsGnSteps; ++g) {
-      double m[12];
-#pragma unroll
-      for (int e = 0; e < 12; ++e) m[e] = s_cand[e];
-      double acc[27];
-#pragma unroll
-      for (int e = 0; e < 27; ++e) acc[e] = 0.0;
-      for (int r = tid; r < n; r += kAbsLoThreads) {
-        if (!abs_inlier(p, rows32[r], S.th2)) continue;
-        const double* row = rows + (size_t)r * stride;
-        double X[3], P[3];
-        for (int i = 0; i < 3; ++i) X[i] = row[2 + i] - S.mean[i];
-        for (int i = 0; i < 3; ++i) P[i] = m[3 * i] * X[0] + m[3 * i + 1] * X[1] + m[3 * i + 2] * X[2];
-        const double x = P[0] + m[9], y = P[1] + m[10], z = P[2] + m[11];
-        if (!(z > 0.0)) continue;
-        const double iz = 1.0 / z;
-        const double ru = S.fx * x * iz + S.cx - row[0], rv = S.fy * y * iz + S.cy - row[1];
-        // d(x, y, z) / d(w, dt) = [-[P]x | I]; projection Jacobian [[fx/z, 0, -fx x/z^2], [0, fy/z, -fy y/z^2]]
-        const double pu[3] = {S.fx * iz, 0.0, -S.fx * x * iz * iz}, pv[3] = {0.0, S.fy * iz, -S.fy * y * iz * iz};
-        const double nPx[3][3] = {{0.0, P[2], -P[1]}, {-P[2], 0.0, P[0]}, {P[1], -P[0], 0.0}};   // -[P]x
-        double ju[6], jv[6];
-        for (int c = 0; c < 3; ++c) {
-          ju[c] = pu[0] * nPx[0][c] + pu[1] * nPx[1][c] + pu[2] * nPx[2][c];
-          jv[c] = pv[0] * nPx[0][c] + pv[1] * nPx[1][c] + pv[2] * nPx[2][c];
-          ju[3 + c] = pu[c];
-          jv[3 + c] = pv[c];
-        }
-        int e = 0;
-#pragma unroll
-        for (int i = 0; i < 6; ++i)
-#pragma unroll
-          for (int k = i; k < 6; ++k) acc[e++] += ju[i] * ju[k] + jv[i] * jv[k];
-#pragma unroll
-        for (int i = 0; i < 6; ++i) acc[21 + i] += ju[i] * ru + jv[i] * rv;
-      }
-#pragma unroll
-      for (int e = 0; e < 27; ++e) {
-        const double v = warp_sum_d(acc[e]);
-        if (lane == 0) s_red[wid][e] = v;
-      }
-      __syncthreads();
-      if (tid == 0) {
-        double hg[27], dx[6];
-        for (int e = 0; e < 27; ++e) {
-          double v = 0.0;
-          for (int w = 0; w < kAbsLoThreads / 32; ++w) v += s_red[w][e];
-          hg[e] = v;
-        }
-        s_ok = solve6(hg, hg + 21, dx);
-        if (s_ok) {
-          const double w[3] = {-dx[0], -dx[1], -dx[2]}, dt[3] = {-dx[3], -dx[4], -dx[5]};
-          double nm[12];
-          pose_update(m, w, dt, nm);
-          for (int e = 0; e < 12; ++e) s_ok &= isfinite(nm[e]);
-          if (s_ok)
-            for (int e = 0; e < 12; ++e) s_cand[e] = nm[e];
-        }
-      }
-      __syncthreads();
-      if (!s_ok) break;
+    for (int k = 0; k < 3; ++k) abs_row64(S, rows + (size_t)idx[k] * stride, j[k], X[k]);
+    return solve_p3p(j, X, out);
+  }
+  static __device__ __forceinline__ void lo_row(const AbsState& S, const double* m, const double* row,
+                                                double (&acc)[27]) {
+    double X[3], P[3];
+    for (int i = 0; i < 3; ++i) X[i] = row[2 + i] - S.mean[i];
+    for (int i = 0; i < 3; ++i) P[i] = m[3 * i] * X[0] + m[3 * i + 1] * X[1] + m[3 * i + 2] * X[2];
+    const double x = P[0] + m[9], y = P[1] + m[10], z = P[2] + m[11];
+    if (!(z > 0.0)) return;
+    const double iz = 1.0 / z;
+    const double ru = S.fx * x * iz + S.cx - row[0], rv = S.fy * y * iz + S.cy - row[1];
+    // d(x, y, z) / d(w, dt) = [-[P]x | I]; projection Jacobian [[fx/z, 0, -fx x/z^2], [0, fy/z, -fy y/z^2]]
+    const double pu[3] = {S.fx * iz, 0.0, -S.fx * x * iz * iz}, pv[3] = {0.0, S.fy * iz, -S.fy * y * iz * iz};
+    const double nPx[3][3] = {{0.0, P[2], -P[1]}, {-P[2], 0.0, P[0]}, {P[1], -P[0], 0.0}};   // -[P]x
+    double ju[6], jv[6];
+    for (int c = 0; c < 3; ++c) {
+      ju[c] = pu[0] * nPx[0][c] + pu[1] * nPx[1][c] + pu[2] * nPx[2][c];
+      jv[c] = pv[0] * nPx[0][c] + pv[1] * nPx[1][c] + pv[2] * nPx[2][c];
+      ju[3 + c] = pu[c];
+      jv[3 + c] = pv[c];
     }
-    if (!s_ok) break;
-    const int c = count_inliers(s_cand);
-    if (c <= cur_count) break;
-    cur_count = c;
-    if (tid < 12) s_cur[tid] = s_cand[tid];
-    __syncthreads();
-  }
-
-  if (tid == 0) {
-    const double nan = __longlong_as_double(0x7ff8000000000000ll);
-    const bool has = cur_count > 0;
-    for (int i = 0; i < 9; ++i) Rt_out[12 * blockIdx.y + i] = has ? s_cur[i] : nan;
-    for (int i = 0; i < 3; ++i)          // x = R (X - c) + t = R X + (t - R c)
-      Rt_out[12 * blockIdx.y + 9 + i] =
-          has ? s_cur[9 + i] - (s_cur[3 * i] * S.mean[0] + s_cur[3 * i + 1] * S.mean[1] + s_cur[3 * i + 2] * S.mean[2])
-              : nan;
-    count_out[blockIdx.y] = S.bad ? -1 : cur_count;
-    abs_proj32(S, s_cur, s_p);
-  }
-  __syncthreads();
-  float p[12];
+    int e = 0;
 #pragma unroll
-  for (int e = 0; e < 12; ++e) p[e] = s_p[e];
-  uint8_t* mask = mask_out + S.row0;
-  for (int r = tid; r < n_all; r += kAbsLoThreads) mask[r] = cur_count > 0 && r < n && abs_inlier(p, rows32[r], S.th2);
-}
+    for (int i = 0; i < 6; ++i)
+#pragma unroll
+      for (int k = i; k < 6; ++k) acc[e++] += ju[i] * ju[k] + jv[i] * jv[k];
+#pragma unroll
+    for (int i = 0; i < 6; ++i) acc[21 + i] += ju[i] * ru + jv[i] * rv;
+  }
+  static __device__ __forceinline__ bool lo_solve(const AbsState&, const double* m, const double (*red)[27],
+                                                  double* out) {
+    double hg[27], dx[6];
+    for (int e = 0; e < 27; ++e) {
+      double v = 0.0;
+      for (int w = 0; w < kLoThreads / 32; ++w) v += red[w][e];
+      hg[e] = v;
+    }
+    if (!solve6(hg, hg + 21, dx)) return false;
+    const double w[3] = {-dx[0], -dx[1], -dx[2]}, dt[3] = {-dx[3], -dx[4], -dx[5]};
+    double nm[12];
+    pose_update(m, w, dt, nm);
+    for (int e = 0; e < 12; ++e)
+      if (!isfinite(nm[e])) return false;
+    for (int e = 0; e < 12; ++e) out[e] = nm[e];
+    return true;
+  }
+  // R and t - R c in world coordinates (x = R X + t - R c), NaN without a model.
+  static __device__ __forceinline__ void write_model(const AbsState& S, const double* m, int count, int,
+                                                     double* out) {
+    if (threadIdx.x != 0) return;
+    const double nan = __longlong_as_double(0x7ff8000000000000ll);
+    const bool has = count > 0;
+    for (int i = 0; i < 9; ++i) out[i] = has ? m[i] : nan;
+    for (int i = 0; i < 3; ++i)
+      out[9 + i] = has ? m[9 + i] - (m[3 * i] * S.mean[0] + m[3 * i + 1] * S.mean[1] + m[3 * i + 2] * S.mean[2]) : nan;
+  }
+};
 
 // ---- the scan lift ------------------------------------------------------------------------------------------------
 // torch.nn.functional.grid_sample(align_corners=True) of one channel at pixel (ix, iy), bilinear: the in-bounds
@@ -621,74 +459,23 @@ __global__ void __launch_bounds__(kLiftThreads) lift_scan_kernel(const double* _
   if (tid == 0) *count_dev = (double)s_base;
 }
 
-struct AbsScratch {
-  AbsState* st;
-  AbsRow32* rows32;
-  double* models;
-  int* counts;
-};
-
-AbsScratch abs_carve(void* base, int queries, long long rows) {
-  char* p = (char*)base;
-  AbsScratch s;
-  s.st = (AbsState*)p;
-  p += align_up((size_t)queries * sizeof(AbsState), 1024);
-  s.rows32 = (AbsRow32*)p;
-  p += align_up((size_t)rows * sizeof(AbsRow32) + 16, 1024);
-  s.models = (double*)p;
-  p += align_up((size_t)queries * kAbsModels * sizeof(double), 1024);
-  s.counts = (int*)p;
-  return s;
-}
-
 }  // namespace
 
-size_t abspose_scratch_bytes(int queries, long long rows, bool rounds) {
-  return align_up((size_t)queries * sizeof(AbsState), 1024) + align_up((size_t)rows * sizeof(AbsRow32) + 16, 1024) +
-         (rounds ? align_up((size_t)queries * kAbsModels * sizeof(double), 1024) +
-                       (size_t)queries * kAbsCounts * sizeof(int)
-                 : 0);
-}
+size_t abspose_scratch_bytes(int queries, long long rows, bool rounds) { return scratch_bytes<4>(queries, rows, rounds); }
 
-int abspose_chunk_queries() {
-  const size_t per = sizeof(AbsState) + kAbsModels * sizeof(double) + kAbsCounts * sizeof(int);
-  return (int)std::min<size_t>(kMaxGridY, std::max<size_t>(1, kBatchScratchBudget / per));
-}
+int abspose_chunk_queries() { return chunk_pairs<4>(); }
 
 int launch_find_absolute_pose(const PairBatch& B, const double* intr, double px_th, const double* px_th_dev,
                               double conf, int max_iters, unsigned long long seed, void* scratch, double* Rt_out,
                               uint8_t* mask_out, int* count_out, cudaStream_t st) {
-  const AbsScratch s = abs_carve(scratch, B.pairs, B.total);
-  abs_prep_kernel<<<dim3(1, B.pairs), 1024, 0, st>>>(B, intr, Cam4{}, px_th, px_th_dev, s.rows32, s.st);
-  P2P_LAUNCH_OK();
-  for (int first = 0; first < max_iters; first += kAbsRound) {
-    const int count = min(kAbsRound, max_iters - first);
-    abs_round_kernel<<<dim3(cdiv(count, kAbsHypPerBlock), B.pairs), kAbsThreads, 0, st>>>(
-        s.st, s.rows32, B.rows, B.stride, first, count, seed, 0, s.models, s.counts);
-    P2P_LAUNCH_OK();
-    abs_select_kernel<<<dim3(1, B.pairs), 1024, 0, st>>>(s.st, s.models, s.counts, count * kAbsSlots, first + count,
-                                                         conf, max_iters);
-    P2P_LAUNCH_OK();
-  }
-  abs_lo_kernel<<<dim3(1, B.pairs), kAbsLoThreads, 0, st>>>(s.st, s.rows32, B.rows, B.stride, Rt_out, mask_out,
-                                                            count_out);
-  P2P_LAUNCH_OK();
-  return 0;
+  return find_model<4>(B, intr, {}, px_th, px_th_dev, conf, max_iters, seed, scratch, Rt_out, mask_out, count_out, st);
 }
 
 int launch_test_absolute_pose_hypotheses(const double* rows, int stride, int n, const double* intr, double px_th,
                                          unsigned long long seed, int count, void* scratch, double* models_out,
                                          int* counts_out, cudaStream_t st) {
-  const PairBatch B = single_pair(rows, stride, n, nullptr);
-  const AbsScratch s = abs_carve(scratch, 1, n);
-  abs_prep_kernel<<<1, 1024, 0, st>>>(B, nullptr, Cam4{intr[0], intr[1], intr[2], intr[3]}, px_th, nullptr, s.rows32,
-                                      s.st);
-  P2P_LAUNCH_OK();
-  abs_round_kernel<<<dim3(cdiv(count, kAbsHypPerBlock), 1), kAbsThreads, 0, st>>>(s.st, s.rows32, rows, stride, 0,
-                                                                                   count, seed, 1, models_out,
-                                                                                   counts_out);
-  P2P_LAUNCH_OK();
-  return 0;
+  const Intrinsics K{intr[0], intr[1], intr[2], intr[3], 0.0, 0.0, 0.0, 0.0};
+  return test_hypotheses<4>(rows, stride, n, K, px_th, seed, count, scratch, models_out, counts_out, st);
 }
 
 int launch_lift_scan(const double* scan, int H, int W, const double* align, const double* matches, int match_stride,

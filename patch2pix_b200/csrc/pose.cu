@@ -362,7 +362,7 @@ __device__ __forceinline__ double det3m(const double (&m)[3][3]) {
 // ---- E: kind 3 of the RANSAC kernels (verify_common.cuh) ---------------------------------------------------------
 // Camera coordinates throughout, scored as F.  kTile = 1024 rows (16 KB) leaves room for the 5-point solver's 12.8 KB
 // of shared elimination matrices: 2048 would put the round kernel 384 bytes under the 48 KB static shared-memory limit.
-template <> struct Kind<3> {
+template <> struct Kind<3> : TwoView<3> {
   static constexpr int kSample = 5, kSlots = kMaxRoots, kPairSlots = kMaxRoots, kLoMin = 8, kScore = 0, kTile = 1024;
   // Thread t < kHypPerBlock of a round block solves its hypothesis with s_M[t] as its elimination matrix.
   static __device__ int solve(const VerifyState&, const double (&p)[5][4], double (&out)[kSlots][9]) {

@@ -1,9 +1,10 @@
 // The RANSAC engine of verify.cu (F / H, kinds 0 and 1), degensac.cu (F with the DEGENSAC check: kind 0's launches plus
-// the plane-and-parallax round, kind 2) and pose.cu (E, kind 3): the state, the F / H minimal solvers, scoring, the
-// prep / round / select / local-optimisation kernels and their launch sequence (find_model).  Each translation unit
-// instantiates the kinds it launches; pose.cu defines Kind<3> before it does.
+// the plane-and-parallax round, kind 2), pose.cu (E, kind 3) and abspose.cu (absolute pose, kind 4): the two-view
+// state, the F / H minimal solvers, scoring, the prep / round / select / local-optimisation kernels and their launch
+// sequence (find_model).  Each translation unit instantiates the kinds it launches; pose.cu and abspose.cu define
+// Kind<3> and Kind<4> before they do.
 //
-// Every kernel serves a batch of pairs: pair p is blockIdx.y and owns VerifyState st[p], its rows of the concatenated
+// Every kernel serves a batch of pairs: pair p is blockIdx.y and owns the state st[p], its rows of the concatenated
 // row array (st[p].row0 ..), its fp32 rows (rows32 + st[p].row32) and its round models / counts (kPairModels /
 // kPairCounts per pair).  A pair's arithmetic does not depend on the other pairs.
 #pragma once
@@ -217,15 +218,109 @@ __device__ int solve_h4(const double (&p)[4][4], double (&out)[1][9]) {
   return 1;
 }
 
+// ---- scoring ------------------------------------------------------------------------------------------------------
+// F: dd^2 / den < th^2.  H: |pi(H x1) - x2|^2 < th^2, never with a non-positive or vanishing third coordinate.
+template <int KIND>
+__device__ __forceinline__ bool is_inlier(const float* m, float4 r, float th2) {
+  if (KIND == 0) {
+    float dd, den;
+    sampson_terms<float>(m, r.x, r.y, r.z, r.w, dd, den);
+    return dd * dd < th2 * den;
+  }
+  const float w = m[6] * r.x + m[7] * r.y + m[8];
+  const float u = m[0] * r.x + m[1] * r.y + m[2] - r.z * w, v = m[3] * r.x + m[4] * r.y + m[5] - r.w * w;
+  return w > 1e-8f && u * u + v * v < th2 * w * w;
+}
+
 // ---- the kinds ----------------------------------------------------------------------------------------------------
-// kSample rows per minimal sample, up to kSlots models per sample, kPairSlots model slots per hypothesis in a pair's
-// round buffers (F's 3 for F, H and DEGENSAC, which share one scratch layout), LO refits from kLoMin inliers, kScore
-// the inlier test (0: Sampson, F and E; 1: transfer error, H), kTile rows staged in shared memory per scoring pass.
-// solve: a minimal sample in the solvers' frame -> models in the scoring frame.  refit: the smallest eigenvector of
-// LO's normal matrix -> a model in the scoring frame (false: none).  Kind 2 is DEGENSAC's plane-and-parallax round
-// (F from 2 rows and H, no solver); kind 3, E, is defined in pose.cu.
+// What the shared kernels take from Kind<KIND>, all fixed at compile time:
+//   State, Row32           the pair state and the fp32 scoring row
+//   kSample, kSlots        rows per minimal sample, up to kSlots models per sample
+//   kPairSlots             model slots per hypothesis in a pair's round buffers (F's 3 for F, H and DEGENSAC, which
+//                          share one scratch layout)
+//   kModel                 doubles per model
+//   kLoMin                 LO refits from kLoMin inliers
+//   kTile                  rows staged in shared memory per scoring pass
+//   kLoSteps, kLoSums      per LO refit, kLoSteps accumulate-and-solve steps over kLoSums per-row sums
+//   prep                   launches the prep kernel (host)
+//   image(S, m, e)         element e of a model's fp32 scoring image
+//   inlier(m, r, th2)      the fp32 inlier test of scoring row r under an image m
+//   solve_sample           a minimal sample's row indices -> models in the scoring frame
+//   lo_row(S, c, p, acc)   adds row p's sums, linearised at the candidate c, to acc
+//   lo_solve(S, c, red)    the per-warp sums red -> the next candidate (false: none)
+//   write_model            the LO kernel's model output
+// Kind 2 is DEGENSAC's plane-and-parallax round (F from 2 rows and H, no solver); kind 3, E, is defined in pose.cu and
+// kind 4, absolute pose, in abspose.cu.
 template <int KIND> struct Kind;
-template <> struct Kind<0> {                                       // F: 7-point, up to 3 roots
+
+// What kinds 0 to 3 share: VerifyState, fp32 rows (x1, y1, x2, y2) in the scoring frame, models of 9 doubles scored
+// through their fp32 cast, samples and LO rows mapped to the solvers' frame by to_frame, and one LO step per refit: the
+// 45 sums of the normal matrix, its smallest eigenvector, then Kind<KIND>::refit.  Kind<KIND> adds kScore (the inlier
+// test, 0: Sampson, F and E; 1: transfer error, H), solve (a minimal sample in the solvers' frame -> models in the
+// scoring frame) and refit (the smallest eigenvector -> a model in the scoring frame, false: none).
+template <int KIND> struct TwoView {
+  using State = VerifyState;
+  using Row32 = float4;
+  static constexpr int kModel = 9, kLoSteps = 1, kLoSums = 45;
+  static void prep(dim3 grid, cudaStream_t st, const PairBatch& B, const double* intr, const Intrinsics& K1,
+                   double px_th, const double* px_th_dev, float4* rows32, VerifyState* s);
+  static __device__ __forceinline__ float image(const VerifyState&, const double* m, int e) { return (float)m[e]; }
+  static __device__ __forceinline__ bool inlier(const float* m, float4 r, float th2) {
+    return is_inlier<Kind<KIND>::kScore>(m, r, th2);
+  }
+  template <int S, int SL>
+  static __device__ __forceinline__ int solve_sample(const VerifyState& st, const double* rows, int stride,
+                                                     const int (&idx)[S], double (&out)[SL][9]) {
+    double p[S][4];
+#pragma unroll
+    for (int k = 0; k < S; ++k) to_frame<KIND>(st, rows + (size_t)idx[k] * stride, p[k]);
+    return Kind<KIND>::solve(st, p, out);
+  }
+  static __device__ __forceinline__ void lo_row(const VerifyState& S, const double*, const double* p,
+                                                double (&acc)[45]) {
+    double q[4];
+    to_frame<KIND>(S, p, q);
+    const double x = q[0], y = q[1], u = q[2], v = q[3];
+    if (Kind<KIND>::kScore == 0) {
+      const double a[9] = {u * x, u * y, u, v * x, v * y, v, x, y, 1.0};
+      int e = 0;
+#pragma unroll
+      for (int i = 0; i < 9; ++i)
+#pragma unroll
+        for (int j = i; j < 9; ++j) acc[e++] += a[i] * a[j];
+    } else {
+      const double a[9] = {-x, -y, -1.0, 0.0, 0.0, 0.0, u * x, u * y, u};
+      const double b[9] = {0.0, 0.0, 0.0, -x, -y, -1.0, v * x, v * y, v};
+      int e = 0;
+#pragma unroll
+      for (int i = 0; i < 9; ++i)
+#pragma unroll
+        for (int j = i; j < 9; ++j) acc[e++] += a[i] * a[j] + b[i] * b[j];
+    }
+  }
+  static __device__ __forceinline__ bool lo_solve(const VerifyState& S, const double*, const double (*red)[45],
+                                                  double* out) {
+    double M[9][9], h[9];
+    int e = 0;
+    for (int i = 0; i < 9; ++i)
+      for (int j = i; j < 9; ++j) {
+        double v = 0.0;
+        for (int w = 0; w < kLoThreads / 32; ++w) v += red[w][e];
+        M[i][j] = M[j][i] = v;
+        ++e;
+      }
+    jacobi_min_eigvec<9>(M, h);
+    return Kind<KIND>::refit(S, h, out);
+  }
+  // The model, NaN when a row is not finite, zeros without a model.
+  static __device__ __forceinline__ void write_model(const VerifyState&, const double* m, int count, int bad,
+                                                     double* out) {
+    const int t = threadIdx.x;
+    if (t < 9) out[t] = bad ? __longlong_as_double(0x7ff8000000000000ll) : (count > 0 ? m[t] : 0.0);
+  }
+};
+
+template <> struct Kind<0> : TwoView<0> {                          // F: 7-point, up to 3 roots
   static constexpr int kSample = 7, kSlots = 3, kPairSlots = 3, kLoMin = 8, kScore = 0, kTile = 2048;
   static __device__ int solve(const VerifyState& S, const double (&p)[7][4], double (&out)[3][9]) {
     double mn[3][9];
@@ -248,7 +343,7 @@ template <> struct Kind<0> {                                       // F: 7-point
     return denormalise<0>(S, h, out);
   }
 };
-template <> struct Kind<1> {                                       // H: 4-point DLT
+template <> struct Kind<1> : TwoView<1> {                          // H: 4-point DLT
   static constexpr int kSample = 4, kSlots = 1, kPairSlots = 3, kLoMin = 4, kScore = 1, kTile = 2048;
   static __device__ int solve(const VerifyState& S, const double (&p)[4][4], double (&out)[1][9]) {
     double mn[1][9];
@@ -256,24 +351,13 @@ template <> struct Kind<1> {                                       // H: 4-point
   }
   static __device__ bool refit(const VerifyState& S, double (&h)[9], double* out) { return denormalise<1>(S, h, out); }
 };
-template <> struct Kind<2> { static constexpr int kSample = 2, kSlots = 1, kPairSlots = 3, kScore = 0, kTile = 2048; };
+template <> struct Kind<2> : TwoView<2> {
+  static constexpr int kSample = 2, kSlots = 1, kPairSlots = 3, kScore = 0, kTile = 2048;
+};
 
-template <int KIND> constexpr size_t kPairModels = (size_t)kRound * Kind<KIND>::kPairSlots * 9;   // doubles per pair
-template <int KIND> constexpr size_t kPairCounts = (size_t)kRound * Kind<KIND>::kPairSlots;       // ints per pair
-
-// ---- scoring ------------------------------------------------------------------------------------------------------
-// F: dd^2 / den < th^2.  H: |pi(H x1) - x2|^2 < th^2, never with a non-positive or vanishing third coordinate.
 template <int KIND>
-__device__ __forceinline__ bool is_inlier(const float* m, float4 r, float th2) {
-  if (KIND == 0) {
-    float dd, den;
-    sampson_terms<float>(m, r.x, r.y, r.z, r.w, dd, den);
-    return dd * dd < th2 * den;
-  }
-  const float w = m[6] * r.x + m[7] * r.y + m[8];
-  const float u = m[0] * r.x + m[1] * r.y + m[2] - r.z * w, v = m[3] * r.x + m[4] * r.y + m[5] - r.w * w;
-  return w > 1e-8f && u * u + v * v < th2 * w * w;
-}
+constexpr size_t kPairModels = (size_t)kRound * Kind<KIND>::kPairSlots * Kind<KIND>::kModel;   // doubles per pair
+template <int KIND> constexpr size_t kPairCounts = (size_t)kRound * Kind<KIND>::kPairSlots;       // ints per pair
 
 // a x + b y + c with the rounding fixed as fma(a, x, b y) + c, so that the result does not depend on how the compiler
 // schedules the products of an expression it also computes elsewhere (DEGENSAC's H x1 in the tests and the models).
@@ -409,50 +493,63 @@ __global__ void __launch_bounds__(1024) verify_prep_kernel(PairBatch B, const do
   }
 }
 
-// Hypotheses first .. first + count - 1.  models [count * slots][9] fp64 (scoring frame), counts [count * slots]
+template <int KIND>
+void TwoView<KIND>::prep(dim3 grid, cudaStream_t st, const PairBatch& B, const double* intr, const Intrinsics& K1,
+                         double px_th, const double* px_th_dev, float4* rows32, VerifyState* s) {
+  verify_prep_kernel<KIND == 3><<<grid, 1024, 0, st>>>(B, intr, K1, px_th, px_th_dev, Kind<KIND>::kSample, rows32, s);
+}
+
+// Hypotheses first .. first + count - 1.  models [count * slots][kModel] fp64 (scoring frame), counts [count * slots]
 // (-1: no model in that slot).
 template <int KIND>
-__global__ void __launch_bounds__(kScoreThreads, 1) verify_round_kernel(const VerifyState* __restrict__ st_all,
-                                                                     const float4* __restrict__ rows32_all,
-                                                                     const double* __restrict__ rows_all, int stride,
-                                                                     int first, int count, unsigned long long seed,
-                                                                     int ignore_stop, double h_th2,
-                                                                     double* __restrict__ models_all,
-                                                                     int* __restrict__ counts_all) {
-  constexpr int S = Kind<KIND>::kSample, SL = Kind<KIND>::kSlots, NM = kHypPerBlock * SL, kTile = Kind<KIND>::kTile;
-  __shared__ float4 s_rows[kTile];
-  __shared__ float s_model[NM][9];
+__global__ void __launch_bounds__(kScoreThreads, 1)
+    verify_round_kernel(const typename Kind<KIND>::State* __restrict__ st_all,
+                        const typename Kind<KIND>::Row32* __restrict__ rows32_all, const double* __restrict__ rows_all,
+                        int stride, int first, int count, unsigned long long seed, int ignore_stop, double h_th2,
+                        double* __restrict__ models_all, int* __restrict__ counts_all) {
+  using K = Kind<KIND>;
+  constexpr int S = K::kSample, SL = K::kSlots, L = K::kModel, NM = kHypPerBlock * SL, kTile = K::kTile;
+  __shared__ typename K::Row32 s_rows[kTile];
+  __shared__ float s_model[NM][L];
   __shared__ int s_valid[NM];
-  const VerifyState* st = st_all + blockIdx.y;
-  if (KIND == 2 ? !st->pending : !ignore_stop && st->stop) return;
+  const typename K::State* st = st_all + blockIdx.y;
+  if constexpr (KIND == 2) {
+    if (!st->pending) return;
+  } else if (!ignore_stop && st->stop) {
+    return;
+  }
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   const int n = st->n;
   const float th2 = st->th2;
   const double* rows = rows_all + st->row0 * stride;
-  const float4* rows32 = rows32_all + st->row32;
+  const typename K::Row32* rows32 = rows32_all + st->row32;
   double* models = models_all + blockIdx.y * kPairModels<KIND>;
   int* counts = counts_all + blockIdx.y * kPairCounts<KIND>;
   if (tid < kHypPerBlock) {
     const int local = blockIdx.x * kHypPerBlock + tid;
-    double out[SL][9];
+    double out[SL][L];
     int nm = 0;
     if constexpr (KIND == 2) {
       if (local < count && parallax_model(*st, rows, stride, seed, first + local, h_th2, out[0])) nm = 1;
     } else if (local < count) {
       int idx[S];
-      if (draw_sample<S>(seed, first + local, n, idx)) {
-        double p[S][4];
-#pragma unroll
-        for (int k = 0; k < S; ++k) to_frame<KIND>(*st, rows + (size_t)idx[k] * stride, p[k]);
-        nm = Kind<KIND>::solve(*st, p, out);
-      }
+      if (draw_sample<S>(seed, first + local, n, idx)) nm = K::solve_sample(*st, rows, stride, idx, out);
     }
     for (int k = 0; k < SL; ++k) {
       const int slot = tid * SL + k;
       s_valid[slot] = k < nm;
-      for (int j = 0; j < 9; ++j) {
-        s_model[slot][j] = k < nm ? (float)out[k][j] : 0.f;
-        if (local < count) models[((size_t)local * SL + k) * 9 + j] = k < nm ? out[k][j] : 0.0;
+      if constexpr (L == 9) {                             // the image is a cast: zeros for an empty slot
+        for (int j = 0; j < L; ++j) {
+          s_model[slot][j] = k < nm ? K::image(*st, out[k], j) : 0.f;
+          if (local < count) models[((size_t)local * SL + k) * L + j] = k < nm ? out[k][j] : 0.0;
+        }
+      } else {
+        // Images of the slots that hold a model only (scoring skips the others).  Behind a select, ptxas computes
+        // every slot's image first: kind 4 then needs 217 registers and runs one block per SM instead of two.
+        if (k < nm)
+          for (int j = 0; j < L; ++j) s_model[slot][j] = K::image(*st, out[k], j);
+        if (local < count)
+          for (int j = 0; j < L; ++j) models[((size_t)local * SL + k) * L + j] = k < nm ? out[k][j] : 0.0;
       }
     }
   }
@@ -468,12 +565,12 @@ __global__ void __launch_bounds__(kScoreThreads, 1) verify_round_kernel(const Ve
     for (int j = 0; j < (NM + 7) / 8; ++j) {
       const int mi = wid + 8 * j;
       if (mi >= NM || !s_valid[mi]) continue;
-      float m[9];
+      float m[L];
 #pragma unroll
-      for (int e = 0; e < 9; ++e) m[e] = s_model[mi][e];
+      for (int e = 0; e < L; ++e) m[e] = s_model[mi][e];
       for (int r0 = 0; r0 < tn; r0 += 32) {
         const int r = r0 + lane;
-        const bool in = r < tn && is_inlier<Kind<KIND>::kScore>(m, s_rows[r < tn ? r : 0], th2);
+        const bool in = r < tn && K::inlier(m, s_rows[r < tn ? r : 0], th2);
         cnt[j] += __popc(__ballot_sync(0xffffffffu, in));
       }
     }
@@ -489,50 +586,53 @@ __global__ void __launch_bounds__(kScoreThreads, 1) verify_round_kernel(const Ve
 }
 
 // Best of this round's nm models -> state if strictly better than the best so far; then the stopping bound for samples
-// of `sample` rows.  Pair p's round models and counts start pair_slots * kRound slots after pair p - 1's.
-__global__ void __launch_bounds__(1024) verify_select_kernel(VerifyState* __restrict__ st, const double* __restrict__ models,
+// of `sample` rows.  Pair p's round models and counts start pair_slots * kRound slots after pair p - 1's; models hold
+// L doubles each.
+template <int L = 9, typename State>
+__global__ void __launch_bounds__(1024) verify_select_kernel(State* __restrict__ st, const double* __restrict__ models,
                                                              const int* __restrict__ counts, int nm, int done, int sample,
                                                              int pair_slots, double conf, int max_iters) {
   const size_t slots = (size_t)blockIdx.y * kRound * pair_slots;
-  select_round(st + blockIdx.y, models + slots * 9, counts + slots, nm, done, sample, conf, max_iters);
+  select_round<L>(st + blockIdx.y, models + slots * L, counts + slots, nm, done, sample, conf, max_iters);
 }
 
-// Local optimisation + outputs.  Refits on the inliers of the current model in the solvers' frame (F: 8-point with
-// rank-2 enforcement; H: DLT; E: 8-point projected onto the essential manifold), keeps the refit while it has strictly
-// more inliers, then writes model, mask and count.  Pair p writes model_out[9 p ..], count_out[p] and
-// mask_out[row0 .. row0 + n_all).
+// Local optimisation + outputs.  Each refit runs kLoSteps steps on the inliers of the current model (F: 8-point with
+// rank-2 enforcement; H: DLT; E: 8-point projected onto the essential manifold; absolute pose: Gauss-Newton), and is
+// kept while it has strictly more inliers; then the kernel writes model, mask and count.  Pair p writes
+// model_out[kModel p ..], count_out[p] and mask_out[row0 .. row0 + n_all).
 template <int KIND>
-__global__ void __launch_bounds__(kLoThreads, 1) verify_lo_kernel(const VerifyState* __restrict__ st_all,
-                                                               const float4* __restrict__ rows32_all,
-                                                               const double* __restrict__ rows_all, int stride,
-                                                               double* __restrict__ model_out,
-                                                               uint8_t* __restrict__ mask_out, int* __restrict__ count_out) {
-  constexpr int SC = Kind<KIND>::kScore;
-  __shared__ double s_red[kLoThreads / 32][45];
-  __shared__ double s_cur[9], s_cand[9];
-  __shared__ float s_f32[9];
+__global__ void __launch_bounds__(kLoThreads, 1)
+    verify_lo_kernel(const typename Kind<KIND>::State* __restrict__ st_all,
+                     const typename Kind<KIND>::Row32* __restrict__ rows32_all, const double* __restrict__ rows_all,
+                     int stride, double* __restrict__ model_out, uint8_t* __restrict__ mask_out,
+                     int* __restrict__ count_out) {
+  using K = Kind<KIND>;
+  constexpr int L = K::kModel;
+  __shared__ double s_red[kLoThreads / 32][K::kLoSums];
+  __shared__ double s_cur[L], s_cand[L];
+  __shared__ float s_f32[L];
   __shared__ int s_cnt[kLoThreads / 32], s_ok;
-  const VerifyState* st = st_all + blockIdx.y;
+  const typename K::State* st = st_all + blockIdx.y;
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   const int n = st->n, bad = st->bad, n_all = st->n_all;
   const float th2 = st->th2;
   const double* rows = rows_all + st->row0 * stride;
-  const float4* rows32 = rows32_all + st->row32;
-  model_out += 9 * blockIdx.y;
+  const typename K::Row32* rows32 = rows32_all + st->row32;
+  model_out += L * blockIdx.y;
   count_out += blockIdx.y;
   mask_out += st->row0;
   int cur_count = bad ? 0 : st->best_count;
-  if (tid < 9) s_cur[tid] = st->best[tid];
+  if (tid < L) s_cur[tid] = st->best[tid];
   __syncthreads();
 
   auto count_inliers = [&](const double* m64) -> int {    // block-wide, fixed order
-    if (tid < 9) s_f32[tid] = (float)m64[tid];
+    if (tid < L) s_f32[tid] = K::image(*st, m64, tid);
     __syncthreads();
-    float m[9];
+    float m[L];
 #pragma unroll
-    for (int e = 0; e < 9; ++e) m[e] = s_f32[e];
+    for (int e = 0; e < L; ++e) m[e] = s_f32[e];
     int c = 0;
-    for (int r = tid; r < n; r += kLoThreads) c += is_inlier<SC>(m, rows32[r], th2);
+    for (int r = tid; r < n; r += kLoThreads) c += K::inlier(m, rows32[r], th2);
     for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
     if (lane == 0) s_cnt[wid] = c;
     __syncthreads();
@@ -542,80 +642,55 @@ __global__ void __launch_bounds__(kLoThreads, 1) verify_lo_kernel(const VerifySt
     return tot;
   };
 
-  for (int it = 0; it < kLoIters && cur_count >= Kind<KIND>::kLoMin; ++it) {
-    if (tid < 9) s_f32[tid] = (float)s_cur[tid];
+  for (int it = 0; it < kLoIters && cur_count >= K::kLoMin; ++it) {
+    if (tid < L) s_f32[tid] = K::image(*st, s_cur, tid);
     __syncthreads();
-    float m[9];
+    float m[L];
 #pragma unroll
-    for (int e = 0; e < 9; ++e) m[e] = s_f32[e];
-    double acc[45];
+    for (int e = 0; e < L; ++e) m[e] = s_f32[e];
+    const typename K::State S = *st;                      // the frame, in registers for the row loop
+    for (int g = 0; g < K::kLoSteps; ++g) {
+      double at[L];                                       // the model this step linearises at
 #pragma unroll
-    for (int e = 0; e < 45; ++e) acc[e] = 0.0;
-    const VerifyState S = *st;                            // the frame, in registers for the row loop
-    for (int r = tid; r < n; r += kLoThreads) {
-      if (!is_inlier<SC>(m, rows32[r], th2)) continue;
-      double q[4];
-      to_frame<KIND>(S, rows + (size_t)r * stride, q);
-      const double x = q[0], y = q[1], u = q[2], v = q[3];
-      if (SC == 0) {
-        const double a[9] = {u * x, u * y, u, v * x, v * y, v, x, y, 1.0};
-        int e = 0;
+      for (int e = 0; e < L; ++e) at[e] = g == 0 ? s_cur[e] : s_cand[e];
+      double acc[K::kLoSums];
 #pragma unroll
-        for (int i = 0; i < 9; ++i)
+      for (int e = 0; e < K::kLoSums; ++e) acc[e] = 0.0;
+      for (int r = tid; r < n; r += kLoThreads)
+        if (K::inlier(m, rows32[r], th2)) K::lo_row(S, at, rows + (size_t)r * stride, acc);
 #pragma unroll
-          for (int j = i; j < 9; ++j) acc[e++] += a[i] * a[j];
-      } else {
-        const double a[9] = {-x, -y, -1.0, 0.0, 0.0, 0.0, u * x, u * y, u};
-        const double b[9] = {0.0, 0.0, 0.0, -x, -y, -1.0, v * x, v * y, v};
-        int e = 0;
-#pragma unroll
-        for (int i = 0; i < 9; ++i)
-#pragma unroll
-          for (int j = i; j < 9; ++j) acc[e++] += a[i] * a[j] + b[i] * b[j];
+      for (int e = 0; e < K::kLoSums; ++e) {
+        const double v = warp_sum_d(acc[e]);
+        if (lane == 0) s_red[wid][e] = v;
       }
+      __syncthreads();
+      if (tid == 0) s_ok = K::lo_solve(S, at, s_red, s_cand);
+      __syncthreads();
+      if (!s_ok) break;
     }
-#pragma unroll
-    for (int e = 0; e < 45; ++e) {
-      const double v = warp_sum_d(acc[e]);
-      if (lane == 0) s_red[wid][e] = v;
-    }
-    __syncthreads();
-    if (tid == 0) {
-      double M[9][9], h[9];
-      int e = 0;
-      for (int i = 0; i < 9; ++i)
-        for (int j = i; j < 9; ++j) {
-          double v = 0.0;
-          for (int w = 0; w < kLoThreads / 32; ++w) v += s_red[w][e];
-          M[i][j] = M[j][i] = v;
-          ++e;
-        }
-      jacobi_min_eigvec<9>(M, h);
-      s_ok = Kind<KIND>::refit(S, h, s_cand);
-    }
-    __syncthreads();
     if (!s_ok) break;
     const int c = count_inliers(s_cand);
     if (c <= cur_count) break;
     cur_count = c;
-    if (tid < 9) s_cur[tid] = s_cand[tid];
+    if (tid < L) s_cur[tid] = s_cand[tid];
     __syncthreads();
   }
 
-  if (tid < 9) model_out[tid] = bad ? __longlong_as_double(0x7ff8000000000000ll) : (cur_count > 0 ? s_cur[tid] : 0.0);
+  K::write_model(*st, s_cur, cur_count, bad, model_out);
   if (tid == 0) *count_out = bad ? -1 : cur_count;
-  if (tid < 9) s_f32[tid] = (float)s_cur[tid];
+  if (tid < L) s_f32[tid] = K::image(*st, s_cur, tid);
   __syncthreads();
-  float m[9];
+  float m[L];
 #pragma unroll
-  for (int e = 0; e < 9; ++e) m[e] = s_f32[e];
+  for (int e = 0; e < L; ++e) m[e] = s_f32[e];
   for (int r = tid; r < n_all; r += kLoThreads)
-    mask_out[r] = cur_count > 0 && r < n && is_inlier<SC>(m, rows32[r], th2);
+    mask_out[r] = cur_count > 0 && r < n && K::inlier(m, rows32[r], th2);
 }
 
+template <typename State, typename Row32>
 struct Scratch {
-  VerifyState* st;
-  float4* rows32;
+  State* st;
+  Row32* rows32;
   double* models;
   int* counts;
 };
@@ -623,15 +698,16 @@ struct Scratch {
 // `pairs` states, `rows` fp32 rows, then nhyp hypotheses' models and counts per pair (nhyp = kRound: pair strides
 // kPairModels / kPairCounts).
 template <int KIND>
-Scratch carve(void* base, int pairs, long long rows, int nhyp) {
+Scratch<typename Kind<KIND>::State, typename Kind<KIND>::Row32> carve(void* base, int pairs, long long rows, int nhyp) {
+  using K = Kind<KIND>;
   char* p = (char*)base;
-  Scratch s;
-  s.st = (VerifyState*)p;
-  p += align_up((size_t)pairs * sizeof(VerifyState), 1024);
-  s.rows32 = (float4*)p;
-  p += align_up((size_t)rows * sizeof(float4) + 16, 1024);
+  Scratch<typename K::State, typename K::Row32> s;
+  s.st = (typename K::State*)p;
+  p += align_up((size_t)pairs * sizeof(typename K::State), 1024);
+  s.rows32 = (typename K::Row32*)p;
+  p += align_up((size_t)rows * sizeof(typename K::Row32) + 16, 1024);
   s.models = (double*)p;
-  p += align_up((size_t)pairs * nhyp * Kind<KIND>::kPairSlots * 9 * sizeof(double), 1024);
+  p += align_up((size_t)pairs * nhyp * K::kPairSlots * K::kModel * sizeof(double), 1024);
   s.counts = (int*)p;
   return s;
 }
@@ -639,7 +715,9 @@ Scratch carve(void* base, int pairs, long long rows, int nhyp) {
 // Bytes carve<KIND> lays out for nhyp = kRound (rounds) or 0.
 template <int KIND>
 size_t scratch_bytes(int pairs, long long rows, bool rounds) {
-  return align_up((size_t)pairs * sizeof(VerifyState), 1024) + align_up((size_t)rows * sizeof(float4) + 16, 1024) +
+  using K = Kind<KIND>;
+  return align_up((size_t)pairs * sizeof(typename K::State), 1024) +
+         align_up((size_t)rows * sizeof(typename K::Row32) + 16, 1024) +
          (rounds ? align_up((size_t)pairs * kPairModels<KIND> * sizeof(double), 1024) +
                        (size_t)pairs * kPairCounts<KIND> * sizeof(int)
                  : 0);
@@ -648,12 +726,13 @@ size_t scratch_bytes(int pairs, long long rows, bool rounds) {
 // Pairs per launch within kBatchScratchBudget.
 template <int KIND>
 int chunk_pairs() {
-  const size_t per_pair = sizeof(VerifyState) + kPairModels<KIND> * sizeof(double) + kPairCounts<KIND> * sizeof(int);
+  const size_t per_pair = sizeof(typename Kind<KIND>::State) + kPairModels<KIND> * sizeof(double) +
+                          kPairCounts<KIND> * sizeof(int);
   return (int)std::min<size_t>(kMaxGridY, std::max<size_t>(1, kBatchScratchBudget / per_pair));
 }
 
-template <int KIND>
-int enqueue_round(const Scratch& s, const PairBatch& B, int first, int count, unsigned long long seed, int ignore_stop,
+template <int KIND, typename Scr>
+int enqueue_round(const Scr& s, const PairBatch& B, int first, int count, unsigned long long seed, int ignore_stop,
                   cudaStream_t st, double h_th2 = 0.0) {
   verify_round_kernel<KIND><<<dim3(cdiv(count, kHypPerBlock), B.pairs), kScoreThreads, 0, st>>>(
       s.st, s.rows32, B.rows, B.stride, first, count, seed, ignore_stop, h_th2, s.models, s.counts);
@@ -661,24 +740,25 @@ int enqueue_round(const Scratch& s, const PairBatch& B, int first, int count, un
   return 0;
 }
 
-// RANSAC for F (kind 0), H (1) or E (3): prep, then per round of kRound hypotheses a round and a select, then LO.
-// intr / K1: the pairs' cameras for E, as launch_find_essential takes them; F and H ignore them.  px_th_dev (device,
-// nullable): one threshold per pair of the launch, in place of px_th.
+// RANSAC for F (kind 0), H (1), E (3) or absolute pose (4): prep, then per round of kRound hypotheses a round and a
+// select, then LO.  intr / K1: the pairs' cameras for E and absolute pose, as launch_find_essential and
+// launch_find_absolute_pose take them; F and H ignore them.  px_th_dev (device, nullable): one threshold per pair of
+// the launch, in place of px_th.
 template <int KIND>
 int find_model(const PairBatch& B, const double* intr, const Intrinsics& K1, double px_th, const double* px_th_dev,
                double conf, int max_iters, unsigned long long seed, void* scratch, double* model_out, uint8_t* mask_out,
                int* count_out, cudaStream_t st) {
-  const Scratch s = carve<KIND>(scratch, B.pairs, B.total, kRound);
-  verify_prep_kernel<KIND == 3><<<dim3(1, B.pairs), 1024, 0, st>>>(B, intr, K1, px_th, px_th_dev, Kind<KIND>::kSample,
-                                                                    s.rows32, s.st);
+  using K = Kind<KIND>;
+  const auto s = carve<KIND>(scratch, B.pairs, B.total, kRound);
+  K::prep(dim3(1, B.pairs), st, B, intr, K1, px_th, px_th_dev, s.rows32, s.st);
   P2P_LAUNCH_OK();
   for (int first = 0; first < max_iters; first += kRound) {
     const int count = min(kRound, max_iters - first);
     int rc = enqueue_round<KIND>(s, B, first, count, seed, 0, st);
     if (rc) return rc;
-    verify_select_kernel<<<dim3(1, B.pairs), 1024, 0, st>>>(s.st, s.models, s.counts, count * Kind<KIND>::kSlots,
-                                                            first + count, Kind<KIND>::kSample, Kind<KIND>::kPairSlots,
-                                                            conf, max_iters);
+    verify_select_kernel<K::kModel><<<dim3(1, B.pairs), 1024, 0, st>>>(s.st, s.models, s.counts, count * K::kSlots,
+                                                                        first + count, K::kSample, K::kPairSlots, conf,
+                                                                        max_iters);
     P2P_LAUNCH_OK();
   }
   verify_lo_kernel<KIND><<<dim3(1, B.pairs), kLoThreads, 0, st>>>(s.st, s.rows32, B.rows, B.stride, model_out, mask_out,
@@ -692,11 +772,10 @@ template <int KIND>
 int test_hypotheses(const double* rows, int stride, int n, const Intrinsics& K, double px_th, unsigned long long seed,
                     int count, void* scratch, double* models_out, int* counts_out, cudaStream_t st) {
   const PairBatch B = single_pair(rows, stride, n, nullptr);
-  Scratch s = carve<KIND>(scratch, 1, n, 0);
+  auto s = carve<KIND>(scratch, 1, n, 0);
   s.models = models_out;
   s.counts = counts_out;
-  verify_prep_kernel<KIND == 3><<<1, 1024, 0, st>>>(B, nullptr, K, px_th, nullptr, Kind<KIND>::kSample, s.rows32,
-                                                     s.st);
+  Kind<KIND>::prep(dim3(1), st, B, nullptr, K, px_th, nullptr, s.rows32, s.st);
   P2P_LAUNCH_OK();
   return enqueue_round<KIND>(s, B, 0, count, seed, 1, st);
 }
