@@ -572,6 +572,36 @@ P2P_API int p2p_match_descriptors_batch(p2p_handle_t h, const float* d0, const f
                                         double min_sim, double ratio, int32_t* match, double* sim, double* tc_sim,
                                         int32_t* tc_idx, double* eps, int32_t* n_fixed, void* stream);
 
+/* ---- SuperGlue's optimal transport and match extraction (superglue.cu; the Python side in
+ * patch2pix_b200/superglue.py, the float64 restatement in oracle/superglue_oracle.py).
+ *
+ * p2p_sg_sinkhorn: scores fp32 [batch][n][m], alpha a DEVICE pointer to one fp32 value (SuperGlue's bin_score, read on
+ * the device, so the call makes no host sync).  These restate SuperGlue's log_optimal_transport and match extraction:
+ *   - couplings C are [n+1][m+1]: scores in the top-left block, alpha in the last row and last column;
+ *   - norm = -log(n + m);
+ *   - log_mu is norm n times, then log(m) + norm; log_nu is norm m times, then log(n) + norm;
+ *   - start with u = v = 0 and run iters times: u_i = log_mu_i - LSE_j(C_ij + v_j), then
+ *     v_j = log_nu_j - LSE_i(C_ij + u_i);
+ *   - log_assign = C + u_i + v_j - norm, written [batch][n+1][m+1] when log_assign is not NULL.
+ * Extraction uses only the top-left n x m block of log_assign:
+ *   - i0(i) is the argmax of row i, i1(j) the argmax of column j, ties to the lowest index;
+ *   - row i is mutual iff i1(i0(i)) == i (column j likewise);
+ *   - mscores0_i = exp(max of row i) if row i is mutual, else 0; mscores1_j = mscores0[i1(j)] if column j is mutual,
+ *     else 0;
+ *   - valid0_i = mutual_i && mscores0_i > match_threshold; valid1_j = mutual_j && valid0[i1(j)];
+ *   - matches0 int32 [batch][n] = valid0 ? i0 : -1, matches1 [batch][m] = valid1 ? i1 : -1;
+ *   - mscores0 keeps exp(max) for a mutual row even when it fails the threshold, as SuperGlue does.
+ * Any of log_assign, matches0/1, mscores0/1 may be NULL.  fp32 throughout; norm, log_mu and log_nu are rounded to fp32
+ * from double.  One warp computes each u_i / v_j in a fixed order, so results are bit-identical for any grid size
+ * (option "num_sms") and pair k of a batch equals its single-pair call.  One cooperative launch; scratch is a transposed
+ * copy of the scores (4 batch n m bytes) plus O(batch (n + m)), grow-only in the handle: after the first call of a
+ * shape the call makes no host sync.  Limits: batch, n, m >= 1, n, m <= 2^20, batch (n + 1) (m + 1) < 2^31,
+ * 0 <= iters <= 100000, match_threshold finite.  Scores and alpha must be finite: a NaN or inf is not detected (that
+ * would cost a host sync) and gives unspecified results.  A failed cooperative launch returns its error. */
+P2P_API int p2p_sg_sinkhorn(p2p_handle_t h, const float* scores, int batch, int n, int m, const float* alpha,
+                            int iters, float match_threshold, float* log_assign, int32_t* matches0, int32_t* matches1,
+                            float* mscores0, float* mscores1, void* stream);
+
 /* ---- bring-up / accuracy probe: C[M,N] = alpha * A[M,K] B[N,K]^T on the wgmma path with the
  * same operand format as the hot path (fp32 inputs are split to fp16 hi/lo on the device).
  * a, b, c are DEVICE fp32; K % 64 == 0. */

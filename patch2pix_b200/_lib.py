@@ -98,6 +98,7 @@ _SIGNATURES = {
     'p2p_sp_descriptors': (_I, [_P, _P, _I, _I, _I, _I, _P, _P, _LL, _P, _P]),
     'p2p_match_descriptors_batch': (_I, [_P, _P, _P, _P, _P, C.POINTER(C.c_int64), C.POINTER(C.c_int64), _I, _I, _I,
                                          C.c_double, C.c_double, _P, _P, _P, _P, _P, _P, _P]),
+    'p2p_sg_sinkhorn': (_I, [_P, _P, _I, _I, _I, _P, _I, _F, _P, _P, _P, _P, _P, _P]),
 }
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
 PROF_KINDS = ('l2norm', 'corr', 'mutual', 'nc', 'proposals', 'prep', 'gather_mid', 'conv1_mid', 'conv2_mid', 'fc_mid',

@@ -130,7 +130,7 @@ struct p2p_handle_s {
   int opt_nc_l2_mode = 0;       // NC layer 2 block layout: 0 auto, 1 one haloed block per tile, 2 one block per column tap
   int opt_nc_impl = 1;          // 1: NeighConsensus on the tensor cores (nc_umma.cu); 0: fp32 CUDA-core kernels (shape-capped)
   Regressor reg[2];
-  Arena coarse, refine, feat, misc, uniq, pre, verify, sfm, sp;
+  Arena coarse, refine, feat, misc, uniq, pre, verify, sfm, sp, sg;
   std::vector<PreprocessCoefs> pre_coefs;   // cached resampling tables, one per image geometry
   PairFeatures pf[2];
   bool prepared = false;
@@ -495,6 +495,7 @@ int p2p_destroy(p2p_handle_t h) {
   h->verify.release();
   h->sfm.release();
   h->sp.release();
+  h->sg.release();
   for (auto& c : h->pre_coefs)
     if (c.d) cudaFree(c.d);
   for (auto& e : h->prof) { cudaEventDestroy(e.a); cudaEventDestroy(e.b); }
@@ -2099,6 +2100,20 @@ int p2p_match_descriptors_batch(p2p_handle_t h, const float* d0, const float* d1
                                   max0, max1, n0, n1, mutual, !std::isnan(min_sim), min_sim, !std::isnan(ratio), ratio,
                                   h->opt_match_impl, match, sim, tc_sim, tc_idx, eps, n_fixed,
                                   reinterpret_cast<cudaStream_t>(stream));
+}
+
+int p2p_sg_sinkhorn(p2p_handle_t h, const float* scores, int batch, int n, int m, const float* alpha, int iters,
+                    float match_threshold, float* log_assign, int32_t* matches0, int32_t* matches1, float* mscores0,
+                    float* mscores1, void* stream) {
+  P2P_ENTER(h);
+  P2P_REQUIRE(batch >= 1 && n >= 1 && m >= 1, "batch, n and m must be >= 1");
+  P2P_REQUIRE(n <= kSgMaxPoints && m <= kSgMaxPoints, "n and m must be <= 2^20");
+  P2P_REQUIRE((long long)batch * (n + 1) * (m + 1) < (1ll << 31), "batch * (n + 1) * (m + 1) must be < 2^31");
+  P2P_REQUIRE(iters >= 0 && iters <= kSgMaxIters, "iters must be in 0..100000");
+  P2P_REQUIRE(std::isfinite(match_threshold), "match_threshold must be finite");
+  P2P_REQUIRE(scores && alpha, "null pointer");
+  return launch_sg_sinkhorn(h->sg, scores, batch, n, m, alpha, iters, match_threshold, log_assign, matches0, matches1,
+                            mscores0, mscores1, std::min(sms(h), h->num_sms), reinterpret_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

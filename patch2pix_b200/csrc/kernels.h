@@ -280,6 +280,14 @@ int launch_match_descriptors(Arena& ar, const float* d0, const float* d1, const 
                              int mutual, int has_min, double min_sim, int has_ratio, double ratio, int impl,
                              int* match, double* sim, double* tc_sim, int* tc_idx, double* eps_out,
                              int* n_fixed, cudaStream_t st);
+// ---- superglue.cu: SuperGlue's log-domain Sinkhorn and mutual match extraction in one cooperative launch (semantics
+// in include/p2p_b200.h, p2p_sg_sinkhorn).  Scratch (a transposed copy of the scores, u, v and the argmaxes) comes from
+// `ar` (reserved here); `sms` caps the persistent grid at that many SMs' worth of co-resident blocks.
+constexpr int kSgMaxPoints = 1 << 20;
+constexpr int kSgMaxIters = 100000;
+int launch_sg_sinkhorn(Arena& ar, const float* scores, int B, int n, int m, const float* alpha, int iters, float thr,
+                       float* log_assign, int* matches0, int* matches1, float* mscores0, float* mscores1, int sms,
+                       cudaStream_t st);
 // ---- relpose.cu: relative-pose statistics of a batch (one block per pair, pairs = B.pairs, any count): pair p writes
 // out[p * out_stride ..] = cos of the rotation and translation-direction errors of Rt_est [p] against Rt_gt [p]
 // (NaN when n_inliers[p] <= 0), then int32 [n_thr + 1]: rows with symmetric epipolar error < thr[j], rows considered.

@@ -240,11 +240,16 @@ def superpoint_nn_matcher(sp, **match_opts):
     return matcher
 
 
-def sp_patch2pix_matcher(net, sp, io_thres=0.0, imsize=None):
+def sp_patch2pix_matcher(net, sp, io_thres=0.0, imsize=None, sg=None):
     """The (path0, path1) -> [N, 4] float64 rows callable that eval_hpatches / eval_relpose / localize_* take:
-    SuperPoint + mutual nearest-neighbour matches refined by the Patch2Pix `net` (eval_helper.refine_matches)."""
+    SuperPoint + mutual nearest-neighbour matches refined by the Patch2Pix `net` (eval_helper.refine_matches).  With a
+    SuperGlue `sg`, SuperGlue's matches (superglue.superglue_matcher) are refined instead."""
     from .eval_helper import refine_matches
-    coarse = superpoint_nn_matcher(sp)
+    if sg is None:
+        coarse = superpoint_nn_matcher(sp)
+    else:
+        from .superglue import superglue_matcher
+        coarse = superglue_matcher(sp, sg)
 
     def matcher(path0, path1):
         return refine_matches(path0, path1, net, coarse, io_thres, imsize)[0]
