@@ -675,7 +675,8 @@ int launch_sfm_tracks(Arena& ar, const int* kp_of_ep, long long M, const long lo
     iota_kernel<<<grid_of(n_kp), kSfmThreads, 0, st>>>(labels, n_kp);
     P2P_LAUNCH_OK();
   }
-  if (M > 0) {
+  // without keypoints every endpoint was dropped: no match is an edge (and the jump kernel would have no blocks)
+  if (M > 0 && n_kp > 0) {
     edge_key_kernel<<<grid_of(M), kSfmThreads, 0, st>>>(kp_of_ep, M, offsets, P, first, first + n, E, thr, kp_n, k0,
                                                         counts_dev);
     P2P_LAUNCH_OK();
