@@ -157,7 +157,9 @@ P2P_API int p2p_ncnet_coarse(p2p_handle_t h, const float* feat1, const float* fe
 /* ---- proposals: Patch2Pix.cal_coarse_matches (networks/patch2pix.py:340-375, sort=False) over
  * corr_to_matches (networks/ncn/extract_ncmatches.py:6-94).  corr4d [hA*wA, hB*wB]; delta_code may be
  * NULL (ksize 1).  matches_out int64 [hB*wB + hA*wA, 4] rows (x1,y1,x2,y2): first the best A cell for
- * every B cell, then the best B cell for every A cell; scores_out fp32 same length. */
+ * every B cell, then the best B cell for every A cell; scores_out fp32 same length.  Non-finite slices give
+ * what the reference's torch.max gives: without the softmax the first NaN, else the first maximum (an all -inf
+ * slice: cell 0, score -inf); with it, a slice holding a NaN or a +inf, or only -inf, gives cell 0, score NaN. */
 P2P_API int p2p_proposals(p2p_handle_t h, const float* corr4d, const uint8_t* delta_code, int hA, int wA, int hB, int wB,
                   int ksize, int upsample, int center, int do_softmax, int64_t* matches_out, float* scores_out,
                   void* stream);
@@ -584,7 +586,10 @@ P2P_API int p2p_match_descriptors_batch(p2p_handle_t h, const float* d0, const f
  *     v_j = log_nu_j - LSE_i(C_ij + u_i);
  *   - log_assign = C + u_i + v_j - norm, written [batch][n+1][m+1] when log_assign is not NULL.
  * Extraction uses only the top-left n x m block of log_assign:
- *   - i0(i) is the argmax of row i, i1(j) the argmax of column j, ties to the lowest index;
+ *   - i0(i) is the argmax of row i, i1(j) the argmax of column j, in np.argmax's order: NaN above +inf above every
+ *     number above -inf, ties to the lowest index (an all -inf line gives 0, a line with a NaN its first NaN);
+ *   - a NaN among the terms of an LSE makes that u_i / v_j NaN, as in float64; -inf scores (masked keypoints) are
+ *     terms of exp(-inf) = 0;
  *   - row i is mutual iff i1(i0(i)) == i (column j likewise);
  *   - mscores0_i = exp(max of row i) if row i is mutual, else 0; mscores1_j = mscores0[i1(j)] if column j is mutual,
  *     else 0;

@@ -172,6 +172,33 @@ def decidable(la, threshold, tol):
     return rows, cols
 
 
+def decidable_ties(la, threshold, tol):
+    """decidable() for matrices with exact ties: duplicated keypoints make bit-identical lines, whose entries are equal
+    in float64 and in fp32 alike, and a masked (all -inf) line ties everywhere.  Such a tie resolves to the lowest index
+    on both sides, so a line's gap is taken from its maximum to the largest value strictly below it (infinite when
+    there is none).  Lines with a NaN are never decided here; compare those
+    with extract() exactly.  -> (rows [n] bool, columns [m] bool)."""
+    z = np.asarray(la, np.float64)[:-1, :-1]
+    n, m = z.shape
+
+    def gap(axis):
+        with np.errstate(invalid='ignore'):
+            top = z.max(axis)
+            below = np.where(z < np.expand_dims(top, axis), z, -np.inf).max(axis)
+            g = np.where(np.isneginf(top), np.inf, top - below)
+        return np.where(np.isnan(top), -np.inf, g)
+
+    g0, g1 = gap(1), gap(0)
+    i0, i1 = z.argmax(1), z.argmax(0)
+    with np.errstate(invalid='ignore'):
+        thr_ok = np.abs(z.max(1) - np.log(threshold)) > tol if threshold > 0 else np.ones(n, bool)
+    # a masked line's whole decision is exact: it points at 0, and that line's argmax is either a finite entry (not
+    # mutual) or, masked too, 0 (mutual iff this is line 0), with score exp(-inf) = 0
+    rows = (g0 > tol) & (g1[i0] > tol) & thr_ok | np.isneginf(z).all(1)
+    cols = (g1 > tol) & (g0[i1] > tol) & thr_ok[i1] | np.isneginf(z).all(0)
+    return rows, cols
+
+
 def sinkhorn_bound(n, m, amax, vmax, iters):
     """Bound on |log_assign - log_assign_fp64| of p2p_sg_sinkhorn (DESIGN.md, "SuperGlue's optimal transport"): each
     half-iteration adds at most delta = u (10 (A + V) + 16 K + 4 lambda + 40) to the error of u or v, with A = max |C|

@@ -743,9 +743,13 @@ int launch_neigh_consensus(const float* x, int hA, int wA, int hB, int wB, const
 // K6+K7: proposals.  score = max softmax prob = 1 / sum exp(x - max); argmax with lowest-index
 // ties; relocalise with the pooling code; scale to pixels.  Rows [0,nB): best A for every B cell
 // (softmax over A); rows [nB, nB+nA): best B for every A cell.  Row = (x1,y1,x2,y2) int64.
+// Non-finite slices follow torch.max: the argmax order puts NaN above +inf above every number, so
+// the first NaN wins and an all -inf slice gives index 0.  With the softmax, a slice holding a NaN
+// or a +inf, or only -inf, is all NaN in the reference: index 0 and a NaN score (1 / NaN).
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void better(float& v, int& i, float v2, int i2) {
-  if (v2 > v || (v2 == v && i2 < i)) {
+  const bool n2 = v2 != v2, n = v != v;
+  if (n2 != n ? n2 : (v2 > v || (!(v2 < v) && i2 < i))) {
     v = v2;
     i = i2;
   }
@@ -819,6 +823,7 @@ __global__ void __launch_bounds__(1024) proposals_dir1_kernel(const float* __res
     float tot = 0.f;
     for (int r = 0; r < R; ++r) tot += sv[r][tx];
     const float score = do_softmax ? __fdiv_rn(1.f, tot) : best;
+    if (do_softmax && score != score) bi = 0;   // the reference's softmax is all NaN there: torch.max gives 0
     emit_match(m, sc, b, bi, b, score, wA, wB, nB, code, ks, upsample, shift);
   }
 }
@@ -847,6 +852,7 @@ __global__ void __launch_bounds__(256) proposals_dir2_kernel(const float* __rest
   s = warp_sum(s);
   if (lane == 0) {
     const float score = do_softmax ? __fdiv_rn(1.f, s) : best;
+    if (do_softmax && score != score) bi = 0;
     emit_match(m, sc, nB + a, a, bi, score, wA, wB, nB, code, ks, upsample, shift);
   }
 }

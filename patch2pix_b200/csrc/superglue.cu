@@ -48,6 +48,13 @@ struct SgArgs {
   float norm, lmu_bin, lnu_bin, thr;   // norm = -log(n + m), log(m) + norm, log(n) + norm (rounded from double)
 };
 
+// max that returns NaN when either input is NaN (fmaxf returns the other input)
+__device__ __forceinline__ float fmax_nan(float a, float b) {
+  float d;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(d) : "f"(a), "f"(b));
+  return d;
+}
+
 // u_out[r] = (i < rows ? lnorm : lbin) - LSE_j(c_ij + v_j), j = 0 .. cols, for every row r = (b, i) of a pass over
 // M [B][rows][cols]; c_ij = M[b][i][j] for i < rows and j < cols, alpha otherwise (the dustbin row / column).
 __device__ __forceinline__ void lse_pass(const float* __restrict__ M, int B, int rows, int cols, float alpha,
@@ -67,9 +74,9 @@ __device__ __forceinline__ void lse_pass(const float* __restrict__ M, int B, int
         const int j = base + k * 32 + lane;
         const float c = (row != nullptr && j < cols) ? __ldcg(row + j) : alpha;
         x[k] = j <= cols ? c + vb[j] : -INFINITY;
-        cm = fmaxf(cm, x[k]);
+        cm = fmax_nan(cm, x[k]);                      // a NaN term makes cm, then s, NaN, as in float64
       }
-      if (cm == -INFINITY) continue;                  // this lane is past the row's end
+      if (cm == -INFINITY) continue;                  // past the row's end, or masked (-inf)
       if (cm > mx) {
         s *= expf(mx - cm);                           // expf(-inf) = 0 on the first chunk
         mx = cm;
@@ -83,16 +90,18 @@ __device__ __forceinline__ void lse_pass(const float* __restrict__ M, int B, int
     for (int o = 16; o > 0; o >>= 1) {
       const float om = __shfl_xor_sync(0xffffffffu, mx, o), os = __shfl_xor_sync(0xffffffffu, s, o);
       const float M2 = fmaxf(mx, om);
-      s = M2 == -INFINITY ? 0.f : s * expf(mx - M2) + os * expf(om - M2);
+      s = M2 == -INFINITY ? s + os : s * expf(mx - M2) + os * expf(om - M2);   // s + os: 0, or NaN kept
       mx = M2;
     }
     if (lane == 0) uout[r] = (i < rows ? lnorm : lbin) - (mx + logf(s));
   }
 }
 
-// Running (value, index) max with ties to the lowest index.
+// Running (value, index) max in np.argmax's order: NaN above +inf above every number above -inf, ties (NaN with NaN
+// included) to the lowest index.
 __device__ __forceinline__ void arg_combine(float& bv, int& bi, float ov, int oi) {
-  if (ov > bv || (ov == bv && oi < bi)) {
+  const bool on = ov != ov, bn = bv != bv;
+  if (on != bn ? on : (ov > bv || (!(ov < bv) && oi < bi))) {
     bv = ov;
     bi = oi;
   }
@@ -161,12 +170,14 @@ __global__ void __launch_bounds__(kSgThreads) sg_sinkhorn_kernel(SgArgs a) {
         continue;
       }
       const float* row = a.Z + ((size_t)b * n + i) * m;
+      // every lane starts as if on a -inf at a real column (its first, or 0 past m): the first element replaces it
+      // unless it is -inf too, so the index is in [0, m) for any values, and for any compare in arg_combine
       float bv = -INFINITY;
-      int bi = 0x7fffffff;
+      int bi = lane < m ? lane : 0;
       for (int j = lane; j < m; j += 32) {
         const float z = ((__ldcg(row + j) + ui) + vb[j]) - norm;
         if (out != nullptr) out[j] = z;
-        if (z > bv) {
+        if (z > bv || (z != z && bv == bv)) {         // j rises: the lane keeps its first maximum, or first NaN
           bv = z;
           bi = j;
         }
@@ -183,11 +194,11 @@ __global__ void __launch_bounds__(kSgThreads) sg_sinkhorn_kernel(SgArgs a) {
       const float vj = a.v[(size_t)b * (m + 1) + j];
       const float* ub = a.u + (size_t)b * (n + 1);
       const float* col = a.Zt + ((size_t)b * m + j) * n;
-      float bv = -INFINITY;
-      int bi = 0x7fffffff;
+      float bv = -INFINITY;                           // as for rows: the index is in [0, n) for any values
+      int bi = lane < n ? lane : 0;
       for (int i = lane; i < n; i += 32) {
         const float z = ((__ldcg(col + i) + ub[i]) + vj) - norm;
-        if (z > bv) {
+        if (z > bv || (z != z && bv == bv)) {
           bv = z;
           bi = i;
         }
