@@ -2,18 +2,18 @@
 and OpenCV.
 
 The device scores in fp32 and the oracle in fp64, so inlier decisions may differ on rows whose squared reprojection
-error lies within 1e-4 (relative) of th^2; every comparison below exempts exactly those rows and nothing else, as
-test_gpu_pose.py does."""
+error lies within the derived per-row bound of oracle/ransac_bound.py (decision_bound) of th^2; every comparison below
+exempts exactly those rows and nothing else, as test_gpu_pose.py does."""
 import numpy as np
 import pytest
 import torch
 
 from oracle import abspose_oracle as A
+from oracle import ransac_bound as RB
 from patch2pix_b200 import localize as L
 from patch2pix_b200.synth import synthetic_abspose
 
 pytestmark = pytest.mark.gpu
-BAND = 1e-4
 TH = 4.0
 
 
@@ -23,7 +23,8 @@ def _scene(seed=0, n=1000, ratio=0.5, noise=0.5):
 
 
 def _near(m, rows, intr, mean, th2):
-    return np.abs(A.errors(m, rows, intr, mean)[0] - th2) <= BAND * th2
+    e = A.errors(m, rows, intr, mean)[0]
+    return ~(np.abs(e - th2) > RB.decision_bound(4, m, rows, th2, intr, mean))
 
 
 def _well_conditioned(rows, intr, mean, hyp, seed):

@@ -1,19 +1,25 @@
 """GPU F RANSAC with the DEGENSAC degeneracy check (model 2 of p2p_find_model, p2p_test_degeneracy) against the numpy
 oracle (oracle/degensac_oracle.py), and matches2relapose_degensac against the numpy chain of geometry.py:50-71.
 
-As in test_gpu_verify.py, the device scores F in fp32 and the oracle in fp64, so inlier decisions may differ on rows whose
-Sampson error lies within 1e-4 (relative) of px_th^2; comparisons exempt exactly those rows, and the degeneracy test is
-compared on well-conditioned samples whose points are not within the same band of h_th^2."""
+As in test_gpu_verify.py, the device scores F in fp32 and the oracle in fp64, so final inlier decisions may differ on rows
+whose Sampson error lies within the derived per-row bound of oracle/ransac_bound.py of px_th^2; comparisons exempt
+exactly those rows.  The degeneracy test is compared on well-conditioned samples whose points are not within BAND of
+h_th^2 under an induced H."""
 import numpy as np
 import pytest
 import torch
 
 from oracle import degensac_oracle as D
+from oracle import ransac_bound as RB
 from oracle import verify_oracle as V
 from patch2pix_b200.synth import OFF_PLANE, PLANE, synthetic_dominant_plane, synthetic_two_view
-from test_gpu_verify import BAND, _canon, _compare_final as _compare_final_f, _dtoh, _well_conditioned
+from test_gpu_verify import _canon, _compare_final as _compare_final_f, _dtoh, _well_conditioned
 
 pytestmark = pytest.mark.gpu
+# The plane tests run in fp64 on the device (h_inlier64, with affine2's fixed rounding of H x1), so they differ from the
+# oracle's fp64 transfer error only by fp64 rounding: a relative band of 1e-4 of h_th^2 is far wider than that.  The
+# fp32 final F decisions use the derived bound instead.
+BAND = 1e-4
 
 
 def _dominant(seed, n=1000, **kw):
@@ -68,7 +74,7 @@ def _compare_final(rows, gmask, th, seed=0, **kw):
     tr = {}
     M, omask, _ = D.find_model(rows, th, seed=seed, trace=tr, **kw)
     assert M is not None
-    near = np.abs(V.errors(0, M, rows)[0] - th * th) <= BAND * th * th
+    near = ~(np.abs(V.errors(0, M, rows)[0] - th * th) > RB.decision_bound(0, M, rows, th * th))
     if tr['margin'] <= int(near.sum()):
         return False
     diff = gmask != omask

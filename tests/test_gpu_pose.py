@@ -1,18 +1,18 @@
 """GPU relative pose (p2p_find_essential / p2p_recover_pose) against the numpy oracle (oracle/pose_oracle.py) and OpenCV.
 
 The device scores in fp32 and the oracle in fp64, so inlier decisions may differ on rows whose Sampson error lies within
-1e-4 (relative) of th^2; every comparison below exempts exactly those rows and nothing else, as test_gpu_verify.py
-does."""
+the derived per-row bound of oracle/ransac_bound.py (decision_bound) of th^2; every comparison below exempts exactly
+those rows and nothing else, as test_gpu_verify.py does."""
 import numpy as np
 import pytest
 import torch
 
 from oracle import pose_oracle as P
+from oracle import ransac_bound as RB
 from patch2pix_b200.synth import synthetic_two_view
 from test_gpu_verify import _dtoh
 
 pytestmark = pytest.mark.gpu
-BAND = 1e-4
 TH = 1.5
 INTR = [500.0, 500.0, 320.0, 240.0, 500.0, 500.0, 320.0, 240.0]
 
@@ -24,7 +24,7 @@ def _scene(seed=0, n=1000, ratio=0.5, noise=0.5, **kw):
 
 def _near(E, cam, th2):
     e = P.errors(E, cam)[0]
-    return np.abs(e - th2) <= BAND * th2
+    return ~(np.abs(e - th2) > RB.decision_bound(3, E, cam, th2))
 
 
 def _canon(M):

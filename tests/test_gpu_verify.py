@@ -1,16 +1,17 @@
 """GPU match verification (p2p_find_model / p2p_sampson_distance) against the numpy oracle (oracle/verify_oracle.py).
 
-The device scores in fp32 and the oracle in fp64, so inlier decisions may differ on rows whose error lies within 1e-4
-(relative) of px_th^2; every comparison below exempts exactly those rows and nothing else."""
+The device scores in fp32 and the oracle in fp64, so inlier decisions may differ on rows whose error lies within the
+derived per-row bound of oracle/ransac_bound.py (decision_bound) of px_th^2; every comparison below exempts exactly those
+rows and nothing else."""
 import numpy as np
 import pytest
 import torch
 
+from oracle import ransac_bound as RB
 from oracle import verify_oracle as V
 from patch2pix_b200.synth import synthetic_two_view
 
 pytestmark = pytest.mark.gpu
-BAND = 1e-4
 
 
 def _scene(kind, seed=0, n=1000, ratio=0.5, noise=0.5):
@@ -20,7 +21,7 @@ def _scene(kind, seed=0, n=1000, ratio=0.5, noise=0.5):
 
 def _near(kind, model, rows, th2):
     e = V.errors(kind, model, rows)[0]
-    return np.abs(e - th2) <= BAND * th2
+    return ~(np.abs(e - th2) > RB.decision_bound(kind, model, rows, th2))
 
 
 def _canon(M):
